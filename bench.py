@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200 worker decode engine (contract: DESIGN.md §6).
+"""bench.py — headline benchmark of the H100 worker decode engine (contract: DESIGN.md §6).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Metric (BASELINE.json): "decode tokens/sec/GPU (Llama-3-8B, seq 4K) + box req/s at 1/2/4/8 peers".
 
@@ -22,6 +22,10 @@ and a saturating load (BOX_MAX_BATCH = 128 concurrent chats per peer).  Reported
 `--impl reference` times the reference arm: the reference worker's CPU path.  The reference's own implementation
 (Ollama v0.9.6) cannot be built or installed offline, so the arm runs the CPU oracle port of the same token step
 (oracle/, OpenMP over all host cores) on the same config.
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed decode loop returned (the greedy ids of all K steps,
+the last one being its last step's result) as DIR/decode_ids.npy (float64).  Inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -47,6 +51,9 @@ SEED = 1234
 METRIC = "decode tokens/sec (Llama-3-8B bf16, seq 4K; aggregate over local worker peers)"
 BOX_MAX_BATCH = int(os.environ.get("CL_BOX_MAX_BATCH", "128"))   # sequences per worker peer's decode batch (one peer, saturated: 25 req/s at 32, 46 at 64, 68 at 128)
 BOX_GEN = 256
+# KV pool of the engine: 40 GiB = 320K tokens (128 KiB per token at Llama-3-8B shapes), beside 16 GB of weights on an
+# 80 GB H100: the 4096-token timed sequence plus 128 concurrent chats of up to 2.5K tokens each
+KV_POOL_BYTES = 40 << 30
 
 
 def load_peaks():
@@ -54,15 +61,15 @@ def load_peaks():
     if p.exists():
         try:
             d = json.loads(p.read_text())
-            return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 1453.9)), "measured"
+            return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 989.0)), "measured"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, 1400.0, "fallback"
+    return 3350.0, 989.0, "datasheet"      # H100 SXM: HBM3 GB/s, dense bf16 TFLOP/s
 
 
 def ncu_traffic(kernel: str):
-    """DRAM traffic per launch of the dominant kernel from the committed ncu --set full capture (bench.py cannot run
-    ncu): profiles/ncu_traffic.json, written by tools/ncu_summary.py from the same command under the profiler."""
+    """DRAM traffic per launch of the dominant kernel from a committed `ncu --set full` capture of this build
+    (profiles/ncu_traffic.json, written by tools/ncu_summary.py; bench.py cannot run ncu itself); None without one."""
     p = ROOT / "profiles" / "ncu_traffic.json"
     try:
         return json.loads(p.read_text()).get(kernel)
@@ -129,18 +136,18 @@ class ClockSampler:
 
 
 # ---- CPU arms (the only places that execute oracle/) ---------------------------------------------------------------
-def cpu_baseline(steps_cap_s=12.0, max_tokens=64, warm=2):
+def cpu_baseline(steps_cap_s=12.0, max_tokens=64, warm=2, room=64):
     """The CPU oracle port on this box's host cores: Llama-3-8B shapes, synthetic weights, KV cache
     pre-filled to 4096 positions (timing only), greedy decode steps for about 12 s (bounded sample of the workload)."""
     from oracle import oracle as oc
     cfg = dict(oc.PRESETS[PRESET])
-    cfg["max_seq_len"] = CTX + 64
+    cfg["max_seq_len"] = CTX + room          # room = positions decoded after the pre-filled context
     threads = oc.effective_cpus()
     oc.set_threads(threads)
     t0 = time.time()
     m = oc.Model(cfg, seed=SEED)
     gen_s = time.time() - t0
-    s = m.new_seq(CTX + 64)
+    s = m.new_seq(CTX + room)
     s.fake_fill(CTX)
     tok = 17
     for _ in range(warm):
@@ -180,21 +187,26 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return 0
-    cb, m, s = cpu_baseline(steps_cap_s=0.0, max_tokens=0, warm=0)  # builds model + pre-filled cache
-    tok, t_first = 17, time.time()
+    cb, m, s = cpu_baseline(steps_cap_s=0.0, max_tokens=0, warm=0, room=args.steps + 8)  # builds model + pre-filled cache
+    tok = 17
     lg = s.forward([tok]); tok = int(lg.argmax())
-    t_tok = time.time() - t_first
     warm = max(0, min(args.warmup, 2) - 1)
     for _ in range(warm):
         lg = s.forward([tok]); tok = int(lg.argmax())
-    steps = max(3, min(args.steps, int(150.0 / max(t_tok, 1e-3))))
+    steps = args.steps
+    ids = np.empty(steps, np.int64)
     t0 = time.time()
-    for _ in range(steps):
+    for i in range(steps):
         lg = s.forward([tok]); tok = int(lg.argmax())
+        ids[i] = tok
     dt = time.time() - t0
+    if args.dump_outputs:
+        d = Path(args.dump_outputs)
+        d.mkdir(parents=True, exist_ok=True)
+        np.save(d / "decode_ids.npy", ids.astype(np.float64))
     val = steps / dt
     cb.update(value=round(val, 4), ms_per_step=round(dt / steps * 1e3, 2),
-              sample=f"{steps} greedy decode steps at ctx {CTX} (bounded from --steps {args.steps}); " + cb["sample"].split(";", 1)[-1].strip())
+              sample=f"{steps} greedy decode steps at ctx {CTX}; " + cb["sample"].split(";", 1)[-1].strip())
     line = {"impl": "reference", "metric": METRIC, "value": round(val, 4), "unit": "tokens/s", "n_gpus": args.gpus, "steps": steps,
             "warmup": warm + 1, "ms_per_step": round(dt / steps * 1e3, 2), "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
@@ -383,7 +395,7 @@ def run_box(e, rank, n_gpus, base_port):
     """Every rank: serve as a worker peer until the load generator says stop.  Rank 0 also launches the generator."""
     from crowdllama_b200 import engine as eng
     from crowdllama_b200.worker import WorkerServer
-    srv = WorkerServer(("127.0.0.1", base_port + rank), e, peer_id=f"b200-worker-{rank}", sampling=eng.greedy(BOX_GEN, ignore_eos=True))
+    srv = WorkerServer(("127.0.0.1", base_port + rank), e, peer_id=f"worker-{rank}", sampling=eng.greedy(BOX_GEN, ignore_eos=True))
     threading.Thread(target=srv.serve_forever, kwargs={"poll_interval": 0.1}, daemon=True).start()
     res, client = None, None
     if rank == 0:
@@ -418,7 +430,7 @@ def run_ours(args):
     K, W = args.steps, max(args.warmup, 3)
     t0 = time.time()
     e = eng.Engine(preset=args.preset, model_name=MODEL_NAME, device=local, seed=SEED, max_batch=BOX_MAX_BATCH, max_seqs=BOX_MAX_BATCH + 2,
-                   start_scheduler=True)
+                   kv_pool_bytes=KV_POOL_BYTES, start_scheduler=True)
     init_s = time.time() - t0
     cfg = e.cfg
     p_read, kv_tok, layer_bytes_elems = model_bytes(cfg)
@@ -426,13 +438,13 @@ def run_ours(args):
     ctx = min(args.ctx, cfg["max_seq_len"] - (K + W + KD + 8))
     ids = prompt_ids(ctx, cfg["vocab_size"])
 
-    # ---- prefill (tcgen05 path) through the C-ABI with a host prompt
+    # ---- prefill (tensor-core path) through the C-ABI with a host prompt
     s = e.seq_create()
     t0 = time.time()
     lg = e.prefill(s, ids)
     prefill_ms_first = (time.time() - t0) * 1e3
     first = int(lg.argmax())
-    time.sleep(1.0)   # let the board's power state settle after the prefill burst (r2h: sw_power_cap right after a 58 ms prefill cost 1.7 %)
+    time.sleep(1.0)   # let the board's power state settle after the prefill burst
     # ---- warm-up decode steps (also captures the CUDA graph)
     wids, _ = e.decode_greedy(s, first, W)
     nxt = int(wids[-1])
@@ -446,6 +458,10 @@ def run_ours(args):
     clocks = clk.stop()
     launches = e.stats()["kernel_launches"] - launches0
     ms_max = grp.max(ms)
+    if args.dump_outputs and rank == 0:
+        d = Path(args.dump_outputs)
+        d.mkdir(parents=True, exist_ok=True)
+        np.save(d / "decode_ids.npy", out_ids.astype(np.float64))
     value = n_gpus * K / (ms_max * 1e-3)
     mean_ctx = ctx + W + K / 2.0
     step_bytes = 2 * p_read + kv_tok * (mean_ctx + 1)
@@ -535,10 +551,10 @@ def run_ours(args):
         "data": "synthetic",
         "config": {"workload": f"configs[2]: Llama-3-8B bf16, {ctx}-token prefill then 1-token greedy decode loop, batch 1 per GPU",
                    "preset": args.preset, "ctx": ctx, "weights": f"synthetic counter-based seed {SEED}", "page_size": 32,
-                   "replicas": n_gpus, "l2": "inputs larger than L2: every step streams 15 GB of weights (L2 = 126 MB)",
+                   "replicas": n_gpus, "l2": "inputs larger than L2: every step streams 15 GB of weights (L2 = 50 MB)",
                    "decode_path": "persistent kernel" if os.environ.get("CL_MEGA", "1") != "0" else "per-op kernels"},
         "per_gpu_tokens_per_s": round(value / n_gpus, 2),
-        # the dominant kernel of the timed graph (92 % of the step), timed live
+        # the dominant kernel of the timed graph, timed live
         "roofline": {"bound": "hbm", "kernel": kern.get("name") if isinstance(kern, dict) else None,
                      "achieved": kern["achieved"] if k_ok else round(achieved, 1), "peak": hbm, "unit": "GB/s",
                      "frac": round((kern["achieved"] if k_ok else achieved) / hbm, 4), "traffic": traffic, "peak_source": peak_src,
@@ -574,6 +590,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-box", action="store_true")
     ap.add_argument("--no-extra-configs", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the timed decode loop's outputs as DIR/<name>.npy")
     ap.add_argument("--box-client", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--box-shard", default="", help=argparse.SUPPRESS)
     ap.add_argument("--workers", type=int, default=1, help=argparse.SUPPRESS)

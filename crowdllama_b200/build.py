@@ -1,10 +1,10 @@
-"""Build libclengine.so (hand-written sm_100a kernels + C-ABI) in-tree with nvcc.
+"""Build libclengine.so (hand-written sm_90a kernels + C-ABI) in-tree with nvcc.
 
     python -m crowdllama_b200.build            # incremental
     python -m crowdllama_b200.build --force
 
-Output: crowdllama_b200/lib/libclengine.so (git-ignored, travels to the GPU box with gpurun).
-nvcc cross-compiles for sm_100a without a GPU.  cudart is linked statically so the library
+Output: crowdllama_b200/lib/libclengine.so (git-ignored build product).
+nvcc cross-compiles for sm_90a (H100) without a GPU.  cudart is linked statically so the library
 carries no dependency on torch's bundled runtime.
 """
 from __future__ import annotations
@@ -22,9 +22,9 @@ LIB = HERE / "lib" / "libclengine.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOSTCXX = "/usr/bin/g++"
 
-SOURCES = ["decode_kernels.cu", "decode_mega.cu", "decode_mega_batch.cu", "attn_decode_tc.cu", "batch_kernels.cu", "engine.cu", "ops_api.cu", "prefill.cu", "gemm_tcgen05.cu", "prefill_kernels.cu", "attn_prefill_tc.cu",
+SOURCES = ["decode_kernels.cu", "decode_mega.cu", "decode_mega_batch.cu", "attn_decode_tc.cu", "batch_kernels.cu", "engine.cu", "ops_api.cu", "prefill.cu", "gemm_wgmma.cu", "prefill_kernels.cu", "attn_prefill_tc.cu",
            "host_util.cpp", "tokenizer.cpp", "weights_io.cpp", "scheduler.cpp", "capi.cpp"]
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-ccbin", HOSTCXX,
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-ccbin", HOSTCXX,
          "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function,-fvisibility=default", "--expt-relaxed-constexpr",
          "-I", str(HERE.parent / "include")]
 
@@ -51,7 +51,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(lambda s: _compile(s, force), srcs))
     if force or not LIB.exists() or any(o.stat().st_mtime > LIB.stat().st_mtime for o in objs):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-ccbin", HOSTCXX, "-cudart", "static",
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-ccbin", HOSTCXX, "-cudart", "static",
                "-o", str(LIB), *map(str, objs), "-lpthread", "-ldl", "-lrt"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode:

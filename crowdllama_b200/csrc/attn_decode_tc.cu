@@ -1,7 +1,7 @@
 // attn_decode_tc.cu — paged GQA decode attention on the tensor cores, stand-alone kernel for the BATCHED step.
 //
-// The CUDA-core kernel of decode_kernels.cu is issue-bound once many sequences share a step (ncu, B = 8, ctx 1024:
-// 9.6 M warp instructions for 33.5 MB of KV, 27 us per layer = 23 % of the step).  This is phase P1 of the
+// The CUDA-core kernel of decode_kernels.cu is issue-bound once many sequences share a step (many warp instructions per
+// byte of KV).  This is phase P1 of the
 // persistent kernel (decode_mega.cu) as a kernel of its own:
 //   grid = (n_kv, nsplit, batch), 288 threads: warp 8 streams this split's KV pages as 128B-swizzled 2-D TMA tiles
 //   (two 32-token pages = K lo|hi, V lo|hi per 32 KB ring slot), warps 0-7 take one page each:
@@ -25,8 +25,7 @@ constexpr int HD = 128, REP = 4, P = 32;
 //   <8, 4, 1>  one CTA per SM, 8 warps, 128 KB of KV in flight — few (kv head, split, sequence) items, long chains;
 //   <4, 2, 2>  two CTAs per SM, 4 warps each, 2 x 64 KB in flight — more items than SMs (B >= 19):
 //              the prologue (block table, q) and the epilogue (warp merge, split combine) of one CTA overlap the page
-//              loop of its neighbour.  B = 128 at ctx 256 is 1024 items of ~7 us each: 7 waves become 3.5
-//              (step 5.94 -> 5.56 ms; B = 64: 4.56 -> 4.31; B = 32: 3.95 -> 3.84).
+//              loop of its neighbour, and the waves of short items halve.
 constexpr uint32_t SLOT = 32 * 1024;
 constexpr int MAXS = 64;
 constexpr float LOG2E = 1.4426950408889634f;
@@ -317,8 +316,7 @@ int launch_variant(const AttnDecodeArgs& a, const CUtensorMap& kmap, const CUten
   TcArgs t{a, layer_row0};
   cudaLaunchConfig_t cfg{};
   // persistent launch (single split, more items than resident CTAs): MINB CTAs per SM walk the items instead of one CTA
-  // per item.  r2ad, ctx 256: B = 64 4.433 -> 4.384 ms per step, B = 128 5.796 -> 5.678 (CL_BATCH_ATTN_PERSIST=0 restores
-  // one CTA per item).
+  // per item (CL_BATCH_ATTN_PERSIST=0 restores one CTA per item).
   static const int persist = getenv("CL_BATCH_ATTN_PERSIST") ? atoi(getenv("CL_BATCH_ATTN_PERSIST")) : 1;
   const int n_items = a.n_kv * a.nsplit * a.batch, resident = MINB * sm_count();
   const int grid = (persist && a.nsplit == 1 && n_items > resident) ? resident : n_items;
@@ -336,7 +334,7 @@ int launch_variant(const AttnDecodeArgs& a, const CUtensorMap& kmap, const CUten
 void attn_decode_tc_plan(int n_kv, int batch, int nsplit_max, int cta_budget, int* nsplit, int* small) {
   static const int force = getenv("CL_BATCH_ATTN_SMALL") ? atoi(getenv("CL_BATCH_ATTN_SMALL")) : -1;
   const int items = n_kv * batch;
-  *small = force >= 0 ? (force != 0) : (items > cta_budget);   // r2u: B = 16 (128 items) is faster on the 8-warp shape, B >= 32 on this one
+  *small = force >= 0 ? (force != 0) : (items > cta_budget);   // small shape once the items exceed one wave
   const int budget = *small ? 2 * cta_budget : cta_budget;
   *nsplit = std::max(1, std::min(std::min(nsplit_max, MAXS), budget / std::max(items, 1)));
 }

@@ -1,23 +1,18 @@
-// attn_prefill_tc.cu — causal GQA prefill attention over the paged KV cache on the 5th-gen tensor cores.
+// attn_prefill_tc.cu — causal GQA prefill attention over the paged KV cache on the Hopper tensor cores (wgmma).
 //
-// "prefill causal attention | T x T per head, d = 128 | tensor pipe" row of SURVEY.md §8a; upstream counterpart:
-// ggml-cuda's flash_attn_ext mma tile kernel behind the Ollama server (/root/reference/pkg/crowdllama/api.go:129-139).
+// "prefill causal attention | T x T per head, d = 128 | tensor pipe" row of SURVEY.md §8a.
 // Replaces the mma.sync kernel of prefill_kernels.cu for head_dim 128 / page 32 (that one stays for head_dim 64).
 //
-// One work item = one query head x 256 consecutive query rows = two 128-row tiles (A, B) that share every K/V block.
-// Persistent CTAs (one per SM) take items round-robin from a heaviest-first order.  Per 128-token KV block j and tile X:
-//     S_X = Q_X K_j^T        tcgen05.mma  M 128 (query rows = TMEM lanes) x N 128 (tokens) x K 128 (head dim), fp32 in TMEM
-//     P_X = exp2(S_X - m)    softmax warps: tcgen05.ld one row per thread, online max / sum in registers,
-//                            P rounded to bf16 into shared memory in the K-major 128B-swizzled UMMA layout
-//     O_X += P_X V_j         tcgen05.mma  M 128 x N 128 (head dim) x K 128 (tokens); V straight from the paged cache
-//                            as an MN-major (token rows, dims contiguous) 128B-swizzled operand; O stays in TMEM
-// TMEM: S_A | S_B | O_A | O_B = 4 x 128 fp32 columns (all 512).  The running maximum is only raised when a block exceeds
-// it by more than 2^8 (then the owning warp rescales its 32 rows of O in TMEM with tcgen05.ld / tcgen05.st): softmax is
-// invariant to the reference point, p <= 256 is harmless in bf16 / fp32, and after the first blocks of a row the
-// correction almost never runs.
-// Warp roles (320 threads): warp 0 = TMA producer (Q tiles; K / V pages through a 3 x 32 KB ring, 2-D tensor maps over the
-// whole pool, 128B swizzle), warp 1 = MMA issuer (one elected thread; tcgen05.commit -> mbarriers), warps 2-5 = softmax
-// group of tile A, warps 6-9 = tile B.  While one group runs its exponentials the tensor core works for the other.
+// One work item = one query head x 128 consecutive query rows.  Persistent CTAs (one per SM) take items round-robin from a
+// heaviest-first order.  Each of the two consumer warpgroups owns 64 of the 128 rows; per 64-token KV block j:
+//     S = Q K_j^T            wgmma m64 n64 k16 x 8 (head dim), Q and K K-major 128B-swizzled tiles, fp32 in registers
+//     P = exp2(S - m)        online softmax on the accumulator fragments (row maximum over the 4 lanes of a row),
+//                            P rounded to bf16 straight into the A-operand fragments of the next MMA
+//     O += P V_j             wgmma m64 n64 k16 x 4 (tokens) x 2 (head-dim halves), A = P from registers, V straight from
+//                            the paged cache as an MN-major (token rows, dims contiguous) 128B-swizzled operand
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread: the Q tile, K / V pages through a 4 x 32 KB ring,
+// 2-D tensor maps over the whole pool), warpgroups 1-2 = MMA + softmax.  While one warpgroup runs its exponentials the
+// tensor core works for the other.
 // Numerics (cl-llama v1, DESIGN.md §3): q, K, V bf16; scores, softmax, accumulation fp32; P rounded to bf16 before P.V
 // (the documented deviation of the prefill path); output rounded to bf16 = the o-projection's GEMM operand.
 #include <cuda.h>
@@ -26,23 +21,25 @@
 
 #include "common.cuh"
 #include "kernels.h"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace cl {
 
 namespace {
 
-using namespace tc;
+using namespace wg;
 
 constexpr int HD = 128;                 // head dim
-constexpr int TQ = 128;                 // query rows per tile
-constexpr int TKV = 128;                // tokens per KV block
+constexpr int TQ = 128;                 // query rows per item (two warpgroups of 64)
+constexpr int TKV = 64;                 // tokens per KV block
 constexpr int PAGE = 32;
-constexpr uint32_t TILE_BYTES = 32768;  // a [128][128] bf16 operand tile = two [128 rows][128 B] swizzled slabs
-constexpr uint32_t SLAB = 16384;
-constexpr int NRING = 3;
+constexpr uint32_t Q_BYTES = TQ * HD * 2;     // two [128 rows][128 B] swizzled slabs (dims 0-63 | 64-127)
+constexpr uint32_t Q_SLAB = TQ * 128;
+constexpr uint32_t KV_SLAB = TKV * 128;       // [64 tokens][128 B]
+constexpr uint32_t KV_TILE = 2 * KV_SLAB;     // K or V of one block: 16 KB
+constexpr uint32_t SLOT = 2 * KV_TILE;        // K | V
+constexpr int NRING = 4;
 constexpr int MAX_BT = 320;             // block-table entries staged in shared memory (10240 tokens)
-constexpr float RESCALE_LOG2 = 8.0f;
 
 struct AttnTcParams {
   const int* block_table;               // this sequence
@@ -53,346 +50,193 @@ struct AttnTcParams {
   float scale2;                         // 1/sqrt(HD) * log2(e)
 };
 
-// MN-major, 128B-swizzled operand (V: rows = tokens = K of the MMA, 64 dims = one 128-byte row):
-// SBO = 1024 B between 8-token groups, LBO = 16384 B between the two 64-dim halves
-__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)(SLAB >> 4) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-constexpr uint32_t IDESC_S = make_idesc(TQ, TKV);                  // A = Q (K-major), B = K (K-major)
-constexpr uint32_t IDESC_PV = make_idesc(TQ, HD) | (1u << 16);     // A = P (K-major), B = V (MN-major)
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-        "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-        "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-// work item -> (first query row, head); heaviest (latest rows) first, heads fastest
-struct Item { int q0, head, nblk[2]; };
-__device__ __forceinline__ bool get_item(const AttnTcParams& p, int idx, int n_pairs, Item* it) {
-  if (idx >= n_pairs * p.n_heads) return false;
-  const int pr = n_pairs - 1 - idx / p.n_heads;
+// work item -> (first query row, head, KV blocks); heaviest (latest rows) first, heads fastest
+struct Item { int q0, head, nblk; };
+__device__ __forceinline__ bool get_item(const AttnTcParams& p, int idx, int n_tiles, Item* it) {
+  if (idx >= n_tiles * p.n_heads) return false;
   it->head = idx % p.n_heads;
-  it->q0 = pr * 2 * TQ;
-#pragma unroll
-  for (int x = 0; x < 2; ++x) {
-    const int r0 = it->q0 + x * TQ;
-    const int last = min(r0 + TQ, p.T) - 1;                         // last real query row of the tile
-    it->nblk[x] = r0 < p.T ? (p.pos0 + last) / TKV + 1 : 0;         // KV blocks 0 .. nblk-1 hold keys <= its position
-  }
+  it->q0 = (n_tiles - 1 - idx / p.n_heads) * TQ;
+  const int last = min(it->q0 + TQ, p.T) - 1;                      // last real query row of the item
+  it->nblk = (p.pos0 + last) / TKV + 1;                            // KV blocks 0 .. nblk-1 hold keys <= its position
   return true;
 }
 
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(384, 1)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                        const __grid_constant__ CUtensorMap map_v, const AttnTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* q_s = base;                                  // [2][32 KB]
-  uint8_t* p_s = base + 2 * TILE_BYTES;                 // [2][32 KB]
-  uint8_t* ring = base + 4 * TILE_BYTES;                // [NRING][32 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + (4 + NRING) * TILE_BYTES);
-  uint64_t* q_full = bars;            // [2]
-  uint64_t* q_empty = bars + 2;       // [2]
-  uint64_t* s_full = bars + 4;        // [2]
-  uint64_t* p_full = bars + 6;        // [2]
-  uint64_t* o_full = bars + 8;        // [2]
-  uint64_t* o_empty = bars + 10;      // [2]
-  uint64_t* kv_full = bars + 12;      // [NRING]
-  uint64_t* kv_empty = bars + 12 + NRING;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12 + 2 * NRING);
-  int* bt_s = reinterpret_cast<int*>(tmem_slot + 2);    // [MAX_BT]
+  uint8_t* q_s = base;                                  // [2 slabs][128 rows][128 B]
+  uint8_t* ring = base + Q_BYTES;                       // [NRING][K lo | K hi | V lo | V hi]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)NRING * SLOT);
+  uint64_t* q_full = bars;
+  uint64_t* q_empty = bars + 1;
+  uint64_t* kv_full = bars + 2;                         // [NRING]
+  uint64_t* kv_empty = kv_full + NRING;                 // [NRING]
+  int* bt_s = reinterpret_cast<int*>(kv_empty + NRING); // [MAX_BT]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_pairs = (p.T + 2 * TQ - 1) / (2 * TQ);
+  const int n_tiles = (p.T + TQ - 1) / TQ;
   const int g_rep = p.n_heads / p.n_kv;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&map_q); prefetch_tmap(&map_k); prefetch_tmap(&map_v);
-    for (int x = 0; x < 2; ++x) {
-      mbar_init(&q_full[x], 1); mbar_init(&q_empty[x], 1); mbar_init(&s_full[x], 1);
-      mbar_init(&p_full[x], 128); mbar_init(&o_full[x], 1); mbar_init(&o_empty[x], 128);
-    }
-    for (int i = 0; i < NRING; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
+    mbar_init(q_full, 1); mbar_init(q_empty, 2);        // one arrival per consumer warpgroup
+    for (int i = 0; i < NRING; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 2); }
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < p.n_bt && i < MAX_BT; i += blockDim.x) bt_s[i] = p.block_table[i];
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ======================================= TMA producer =======================================
-    if (lane == 0) {
-      uint32_t ring_it = 0, na[2] = {0u, 0u};                       // na[x]: items so far in which tile x was active
+    if (warp == 0 && lane == 0) {
+      uint32_t ring_it = 0, nq = 0;
       Item it;
-      for (int idx = blockIdx.x; get_item(p, idx, n_pairs, &it); idx += gridDim.x) {
+      for (int idx = blockIdx.x; get_item(p, idx, n_tiles, &it); idx += gridDim.x, ++nq) {
         const int g = it.head / g_rep;
-        for (int x = 0; x < 2; ++x) {
-          if (it.nblk[x] == 0) continue;
-          mbar_wait(&q_empty[x], (na[x] & 1u) ^ 1u);                // the previous active item's last S of this tile has completed
-          ++na[x];
-          mbar_arrive_expect_tx(&q_full[x], TILE_BYTES);
-          uint8_t* dst = q_s + x * TILE_BYTES;
-          tma_load_2d(dst, &map_q, it.head * HD, it.q0 + x * TQ, &q_full[x]);
-          tma_load_2d(dst + SLAB, &map_q, it.head * HD + 64, it.q0 + x * TQ, &q_full[x]);
-        }
-        const int nmax = it.nblk[1] > it.nblk[0] ? it.nblk[1] : it.nblk[0];
-        for (int j = 0; j < nmax; ++j) {
-          for (int kv = 0; kv < 2; ++kv) {                          // ring order: K_0, V_0, K_1, V_1, ...
-            const int slot = (int)(ring_it % NRING);
-            mbar_wait(&kv_empty[slot], ((ring_it / NRING) & 1u) ^ 1u);
-            mbar_arrive_expect_tx(&kv_full[slot], TILE_BYTES);
-            uint8_t* dst = ring + (size_t)slot * TILE_BYTES;
-            const CUtensorMap* mp = kv ? &map_v : &map_k;
+        mbar_wait(q_empty, (nq & 1u) ^ 1u);                        // both warpgroups are past the previous item's last S
+        mbar_arrive_expect_tx(q_full, Q_BYTES);
+        tma_load_2d(q_s, &map_q, it.head * HD, it.q0, q_full);
+        tma_load_2d(q_s + Q_SLAB, &map_q, it.head * HD + 64, it.q0, q_full);
+        for (int j = 0; j < it.nblk; ++j, ++ring_it) {
+          const int slot = (int)(ring_it % NRING);
+          mbar_wait(&kv_empty[slot], ((ring_it / NRING) & 1u) ^ 1u);
+          mbar_arrive_expect_tx(&kv_full[slot], SLOT);
+          uint8_t* dst = ring + (size_t)slot * SLOT;
 #pragma unroll
-            for (int i = 0; i < TKV / PAGE; ++i) {
-              int pi = j * (TKV / PAGE) + i;
-              if (pi >= p.n_bt) pi = 0;                             // past the sequence: any valid page (its keys are masked, P = 0)
-              const long long row = p.layer_row0 + ((long long)bt_s[pi] * p.n_kv + g) * PAGE;
-              tma_load_2d(dst + i * 4096, mp, 0, (int)row, &kv_full[slot]);
-              tma_load_2d(dst + SLAB + i * 4096, mp, 64, (int)row, &kv_full[slot]);
-            }
-            ++ring_it;
+          for (int i = 0; i < TKV / PAGE; ++i) {
+            int pi = j * (TKV / PAGE) + i;
+            if (pi >= p.n_bt) pi = 0;                               // past the sequence: any valid page (its keys are masked)
+            const long long row = p.layer_row0 + ((long long)bt_s[pi] * p.n_kv + g) * PAGE;
+            uint8_t* d = dst + i * (PAGE * 128);
+            tma_load_2d(d, &map_k, 0, (int)row, &kv_full[slot]);
+            tma_load_2d(d + KV_SLAB, &map_k, 64, (int)row, &kv_full[slot]);
+            tma_load_2d(d + KV_TILE, &map_v, 0, (int)row, &kv_full[slot]);
+            tma_load_2d(d + KV_TILE + KV_SLAB, &map_v, 64, (int)row, &kv_full[slot]);
           }
         }
       }
-    }
-  } else if (warp == 1) {
-    // ======================================= MMA issuer =======================================
-    uint32_t ring_it = 0, np[2] = {0u, 0u}, na[2] = {0u, 0u};       // np[x]: p_full phases consumed; na[x]: active items so far
-    Item it;
-    for (int idx = blockIdx.x; get_item(p, idx, n_pairs, &it); idx += gridDim.x) {
-      const int nmax = it.nblk[1] > it.nblk[0] ? it.nblk[1] : it.nblk[0];
-      // S of block jj for both tiles from ring entry K_jj (ring index r_k); releases the K slot and, after a tile's
-      // last S, its Q tile
-      auto issue_s = [&](int jj, uint32_t r_k, int only) {
-        const uint32_t kaddr = smem_u32(ring + (size_t)(r_k % NRING) * TILE_BYTES);
-        for (int x = 0; x < 2; ++x) {
-          if (only >= 0 && x != only) continue;
-          if (jj >= it.nblk[x]) continue;
-          if (lane == 0) {
-            const uint32_t qaddr = smem_u32(q_s + x * TILE_BYTES);
-#pragma unroll
-            for (int k = 0; k < HD / UK; ++k) {
-              const uint32_t off = (uint32_t)(k >> 2) * SLAB + (uint32_t)(k & 3) * 32u;
-              umma_f16(tmem_base + (uint32_t)(x * TKV), make_smem_desc(qaddr + off), make_smem_desc(kaddr + off), IDESC_S, k ? 1u : 0u);
-            }
-            umma_commit(&s_full[x]);
-            if (jj == it.nblk[x] - 1) umma_commit(&q_empty[x]);
-          }
-          __syncwarp();
-        }
-      };
-      uint32_t oe_par[2];
-      for (int x = 0; x < 2; ++x) {
-        oe_par[x] = (na[x] & 1u) ^ 1u;
-        if (it.nblk[x]) { mbar_wait(&q_full[x], na[x] & 1u); ++na[x]; }
-      }
-      tc_fence_after();
-      // prologue: S(0) of both tiles
-      uint32_t r_k = ring_it;                                       // ring index of K_0
-      mbar_wait(&kv_full[r_k % NRING], (r_k / NRING) & 1u);
-      tc_fence_after();
-      issue_s(0, r_k, -1);
-      if (lane == 0) umma_commit(&kv_empty[r_k % NRING]);
-      __syncwarp();
-      for (int j = 0; j < nmax; ++j) {
-        const uint32_t r_v = ring_it + 2 * j + 1, r_kn = r_v + 1;   // V_j, K_{j+1}
-        mbar_wait(&kv_full[r_v % NRING], (r_v / NRING) & 1u);
-        if (j + 1 < nmax) mbar_wait(&kv_full[r_kn % NRING], (r_kn / NRING) & 1u);
-        tc_fence_after();
-        const uint32_t vaddr = smem_u32(ring + (size_t)(r_v % NRING) * TILE_BYTES);
-        for (int x = 0; x < 2; ++x) {
-          if (j >= it.nblk[x]) continue;
-          mbar_wait(&p_full[x], np[x] & 1u);                        // P_j written, S_x read, O_x(j-1) settled
-          ++np[x];
-          if (j == 0) mbar_wait(&o_empty[x], oe_par[x]);            // the previous active item's epilogue has read O_x
-          tc_fence_after();
-          issue_s(j + 1, r_kn, x);                                  // first: the other group's next scores start early
-          if (lane == 0) {
-            const uint32_t paddr = smem_u32(p_s + x * TILE_BYTES);
-#pragma unroll
-            for (int k = 0; k < TKV / UK; ++k) {
-              const uint64_t adesc = make_smem_desc(paddr + (uint32_t)(k >> 2) * SLAB + (uint32_t)(k & 3) * 32u);
-              const uint64_t bdesc = make_smem_desc_mn(vaddr + (uint32_t)k * (UK * 128u));
-              umma_f16(tmem_base + (uint32_t)(2 * TKV + x * HD), adesc, bdesc, IDESC_PV, (j | k) ? 1u : 0u);
-            }
-            umma_commit(&o_full[x]);
-          }
-          __syncwarp();
-        }
-        if (lane == 0) {
-          umma_commit(&kv_empty[r_v % NRING]);
-          if (j + 1 < nmax) umma_commit(&kv_empty[r_kn % NRING]);
-        }
-        __syncwarp();
-      }
-      ring_it += 2u * (uint32_t)nmax;
     }
   } else {
-    // ======================================= softmax groups =======================================
-    const int x = (warp - 2) >> 2;                                  // tile A: warps 2-5, tile B: warps 6-9
-    const int qd = warp & 3;                                        // TMEM lane quarter this warp may access
-    const int r = qd * 32 + lane;                                   // row of the tile = TMEM lane
-    const uint32_t t_s = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(x * TKV);
-    const uint32_t t_o = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(2 * TKV + x * HD);
-    uint8_t* prow = p_s + x * TILE_BYTES + r * 128;
-    const int sw = r & 7;
-    uint32_t ns = 0, no = 0;                                        // s_full / o_full phases consumed
+    // ======================================= consumer warpgroups =======================================
+    const int m0 = (warp >> 2) * 64 - 64;                          // rows m0 .. m0 + 63 of the item
+    const int wq = warp & 3, rq = lane >> 2, cq = lane & 3;
+    const bool leader = wq == 0 && lane == 0;
+    const uint32_t qaddr = smem_u32(q_s) + (uint32_t)m0 * 128u;
+    uint32_t ring_it = 0, nq = 0;
     Item it;
-    for (int idx = blockIdx.x; get_item(p, idx, n_pairs, &it); idx += gridDim.x) {
-      const int nb = it.nblk[x];
-      if (nb == 0) continue;
-      const int qrow = it.q0 + x * TQ + r;
-      const int qabs = p.pos0 + qrow;
-      float m_ref = 0.f, l = 0.f;
-      for (int j = 0; j < nb; ++j) {
-        mbar_wait(&s_full[x], ns & 1u);
-        ++ns;
-        tc_fence_after();
-        const int k0 = j * TKV;
-        const bool masked = k0 + TKV - 1 > p.pos0 + it.q0 + x * TQ;   // some key of the block lies above some row's diagonal
-        float mb = -INFINITY, sum = 0.f;
-        // half a row of S (64 tokens): scaled scores, running block maximum, p = 2^(s - mref) rounded to bf16 pairs
-        auto compute_half = [&](int hh, float mref, uint32_t (&pk)[32]) {
+    for (int idx = blockIdx.x; get_item(p, idx, n_tiles, &it); idx += gridDim.x, ++nq) {
+      int qabs[2];                                                  // positions of this thread's two rows
 #pragma unroll
-          for (int cc = 0; cc < 2; ++cc) {
-            const int c = hh * 2 + cc;
-            uint32_t v[32];
-            tmem_ld32(t_s + (uint32_t)(c * 32), v);
-            tmem_ld_wait();
+      for (int h = 0; h < 2; ++h) qabs[h] = p.pos0 + it.q0 + m0 + wq * 16 + h * 8 + rq;
+      float o[2][32];                                               // head-dim halves 0-63 | 64-127
 #pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              float a = __uint_as_float(v[i]) * p.scale2, b = __uint_as_float(v[i + 1]) * p.scale2;
-              if (masked) {
-                a = (k0 + c * 32 + i <= qabs) ? a : -INFINITY;
-                b = (k0 + c * 32 + i + 1 <= qabs) ? b : -INFINITY;
-              }
-              mb = fmaxf(mb, fmaxf(a, b));
-              const float p0 = ex2_approx(a - mref), p1 = ex2_approx(b - mref);
-              sum += p0 + p1;
-              pk[(cc * 32 + i) >> 1] = pack_bf16(p0, p1);
-            }
-          }
-        };
-        // -> shared memory, K-major 128B-swizzled UMMA layout: token c of the block lives in slab c/64 (= hh),
-        // 16-byte chunk ((c%64)/8) ^ (row & 7) of this row's 128 bytes
-        auto store_half = [&](int hh, const uint32_t (&pk)[32]) {
+      for (int i = 0; i < 32; ++i) { o[0][i] = 0.f; o[1][i] = 0.f; }
+      float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+      mbar_wait(q_full, nq & 1u);
+      for (int j = 0; j < it.nblk; ++j, ++ring_it) {
+        const int slot = (int)(ring_it % NRING);
+        mbar_wait(&kv_full[slot], (ring_it / NRING) & 1u);
+        const uint32_t kaddr = smem_u32(ring + (size_t)slot * SLOT), vaddr = kaddr + KV_TILE;
+        float s[32];
+        fence_regs(s);
+        fence();
 #pragma unroll
-          for (int ch = 0; ch < 8; ++ch)
-            *reinterpret_cast<uint4*>(prow + hh * SLAB + ((ch ^ sw) << 4)) = make_uint4(pk[ch * 4], pk[ch * 4 + 1], pk[ch * 4 + 2], pk[ch * 4 + 3]);
-        };
-        float corr = 1.0f;
-        uint32_t pk[32];
-        if (j == 0) {
-          // no reference yet: maximum first (block 0 holds key 0 <= every position: finite).  The P buffer is free: this
-          // group waited for the previous item's last P.V in its epilogue.
-          float m0 = -INFINITY;
-#pragma unroll
-          for (int c = 0; c < TKV / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld32(t_s + (uint32_t)(c * 32), v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float a = __uint_as_float(v[i]) * p.scale2;
-              if (!masked || k0 + c * 32 + i <= qabs) m0 = fmaxf(m0, a);
-            }
-          }
-          m_ref = m0;
-          compute_half(0, m_ref, pk); store_half(0, pk);
-          compute_half(1, m_ref, pk); store_half(1, pk);
-        } else {
-          // optimistic single pass against the running reference: the first half's exponentials overlap P.V of block
-          // j-1; its stores need the P buffer, i.e. P.V(j-1) complete
-          compute_half(0, m_ref, pk);
-          mbar_wait(&o_full[x], no & 1u);                           // P.V of block j-1 done: P buffer free, O_x stable
-          ++no;
-          tc_fence_after();
-          store_half(0, pk);
-          compute_half(1, m_ref, pk); store_half(1, pk);
-          const bool raise = mb > m_ref + RESCALE_LOG2;
-          if (__any_sync(0xffffffffu, raise)) {                     // rare: a row outgrew its reference by 2^8
-            if (raise) { corr = ex2_approx(m_ref - mb); m_ref = mb; }
-            mb = -INFINITY; sum = 0.f;
-            compute_half(0, m_ref, pk); store_half(0, pk);          // redo the block against the new reference
-            compute_half(1, m_ref, pk); store_half(1, pk);
-#pragma unroll 1
-            for (int c = 0; c < HD / 32; ++c) {                     // and move this warp's 32 rows of O to it
-              uint32_t v[32];
-              tmem_ld32(t_o + (uint32_t)(c * 32), v);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * corr);
-              tmem_st32(t_o + (uint32_t)(c * 32), v);
-            }
-            tmem_st_wait();
-          }
+        for (int k = 0; k < HD / UK; ++k) {
+          const uint32_t off = (uint32_t)(k & 3) * 32u;           // 32 bytes per MMA K inside the 64-dim slab k / 4
+          mma_ss<TKV>(s, make_desc(qaddr + (uint32_t)(k >> 2) * Q_SLAB + off), make_desc(kaddr + (uint32_t)(k >> 2) * KV_SLAB + off),
+                      k ? 1u : 0u);
         }
-        l = l * corr + sum;
-        fence_proxy_async();
-        tc_fence_before();
-        mbar_arrive(&p_full[x]);
+        commit();
+        wait<0>();
+        fence_regs(s);
+        if (j == it.nblk - 1) {                                     // last S of the item: the Q tile may be replaced
+          asm volatile("bar.sync %0, 128;" ::"r"(warp >> 2) : "memory");
+          if (leader) mbar_arrive(q_empty);
+        }
+        // scaled, masked scores; block maximum per row (4 lanes share a row)
+        const int k0 = j * TKV;
+        float mb[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int i = 0; i < TKV / 8; ++i)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int h = e >> 1, key = k0 + i * 8 + 2 * cq + (e & 1);
+            const float v = key <= qabs[h] ? s[4 * i + e] * p.scale2 : -INFINITY;
+            s[4 * i + e] = v;
+            mb[h] = fmaxf(mb[h], v);
+          }
+        float corr[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          mb[h] = fmaxf(mb[h], __shfl_xor_sync(0xffffffffu, mb[h], 1));
+          mb[h] = fmaxf(mb[h], __shfl_xor_sync(0xffffffffu, mb[h], 2));
+          const float mn = fmaxf(m_run[h], mb[h]);                  // finite: block 0 holds key 0 <= every position
+          corr[h] = ex2_approx(m_run[h] - mn);
+          m_run[h] = mn;
+          l_run[h] *= corr[h];
+        }
+        // P = 2^(s - m) -> bf16 A fragments (16-token k-step kk = accumulator column groups 2 kk, 2 kk + 1)
+        uint32_t pa[TKV / 16][4];
+#pragma unroll
+        for (int i = 0; i < TKV / 8; ++i) {
+          const float p0 = ex2_approx(s[4 * i] - m_run[0]), p1 = ex2_approx(s[4 * i + 1] - m_run[0]);
+          const float p2 = ex2_approx(s[4 * i + 2] - m_run[1]), p3 = ex2_approx(s[4 * i + 3] - m_run[1]);
+          l_run[0] += p0 + p1;
+          l_run[1] += p2 + p3;
+          pa[i >> 1][(i & 1) * 2] = pack_bf16(p0, p1);
+          pa[i >> 1][(i & 1) * 2 + 1] = pack_bf16(p2, p3);
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const float c = corr[(i >> 1) & 1];
+          o[0][i] *= c;
+          o[1][i] *= c;
+        }
+        fence_regs(o[0]);
+        fence_regs(o[1]);
+        fence();
+#pragma unroll
+        for (int kk = 0; kk < TKV / UK; ++kk)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+            mma_rs_tb<64>(o[hh], pa[kk], make_desc(vaddr + (uint32_t)hh * KV_SLAB + (uint32_t)kk * (UK * 128u), KV_SLAB), 1u);
+        commit();
+        wait<0>();
+        fence_regs(o[0]);
+        fence_regs(o[1]);
+        asm volatile("bar.sync %0, 128;" ::"r"(warp >> 2) : "memory");
+        if (leader) mbar_arrive(&kv_empty[slot]);
       }
       // epilogue: O / l -> bf16 -> out[qrow][head * HD ..]
-      mbar_wait(&o_full[x], no & 1u);
-      ++no;
-      tc_fence_after();
-      const float inv = 1.0f / l;
-      __nv_bfloat16* orow = p.out + (size_t)qrow * ((size_t)p.n_heads * HD) + (size_t)it.head * HD;
-#pragma unroll 1
-      for (int c = 0; c < HD / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld32(t_o + (uint32_t)(c * 32), v);
-        tmem_ld_wait();
-        if (qrow < p.T) {
 #pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            uint4 w;
-            w.x = pack_bf16(__uint_as_float(v[i]) * inv, __uint_as_float(v[i + 1]) * inv);
-            w.y = pack_bf16(__uint_as_float(v[i + 2]) * inv, __uint_as_float(v[i + 3]) * inv);
-            w.z = pack_bf16(__uint_as_float(v[i + 4]) * inv, __uint_as_float(v[i + 5]) * inv);
-            w.w = pack_bf16(__uint_as_float(v[i + 6]) * inv, __uint_as_float(v[i + 7]) * inv);
-            *reinterpret_cast<uint4*>(orow + c * 32 + i) = w;
-          }
+      for (int h = 0; h < 2; ++h) {
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+        const float inv = 1.0f / l_run[h];
+        const int qrow = it.q0 + m0 + wq * 16 + h * 8 + rq;
+        if (qrow < p.T) {
+          __nv_bfloat16* orow = p.out + (size_t)qrow * ((size_t)p.n_heads * HD) + (size_t)it.head * HD;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+              *reinterpret_cast<uint32_t*>(orow + hh * 64 + i * 8 + 2 * cq) =
+                  pack_bf16(o[hh][4 * i + 2 * h] * inv, o[hh][4 * i + 2 * h + 1] * inv);
         }
       }
-      tc_fence_before();
-      mbar_arrive(&o_empty[x]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
-constexpr size_t kSmem = (size_t)(4 + NRING) * TILE_BYTES + (12 + 2 * NRING) * 8 + 8 + MAX_BT * 4 + 1024;
+constexpr size_t kSmem = (size_t)Q_BYTES + (size_t)NRING * SLOT + (2 + 2 * NRING) * 8 + MAX_BT * 4 + 1024;
 
 }  // namespace
 
@@ -417,9 +261,9 @@ int launch_attn_prefill_tc(const AttnPrefillArgs& a, const CUtensorMap& kmap, co
   AttnTcParams p;
   p.block_table = a.block_table; p.n_bt = (a.pos0 + a.T + PAGE - 1) / PAGE; p.pos0 = a.pos0; p.T = a.T; p.n_heads = a.n_heads; p.n_kv = a.n_kv;
   p.layer_row0 = layer_row0; p.out = a.out; p.scale2 = 1.4426950408889634f / sqrtf((float)HD);
-  const int items = ((a.T + 2 * TQ - 1) / (2 * TQ)) * a.n_heads;
+  const int items = ((a.T + TQ - 1) / TQ) * a.n_heads;
   const int grid = items < sm_count() ? items : sm_count();
-  attn_prefill_tc_kernel<<<grid, 320, kSmem, st>>>(qmap, kmap, vmap, p);
+  attn_prefill_tc_kernel<<<grid, 384, kSmem, st>>>(qmap, kmap, vmap, p);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -1,6 +1,6 @@
 // batch_kernels.cu — glue kernels of the BATCHED decode step (continuous batching, B >= 2 sequences).
-// The weight projections of a batched step run on the tensor cores (gemm_tcgen05.cu, token tile 32,
-// split-K so that ~148 CTAs stream the weights); everything here is per-sequence element-wise work
+// The weight projections of a batched step run on the tensor cores (gemm_wgmma.cu, token tile 32,
+// split-K so that every SM streams weights); everything here is per-sequence element-wise work
 // between those GEMMs.  Sequences live in "slots"; slots[b] maps batch index -> slot.
 #include "common.cuh"
 #include "kernels.h"

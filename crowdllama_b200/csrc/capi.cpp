@@ -15,7 +15,7 @@ const char* cl_strerror(int status) {
   switch (status) {
     case CL_OK: return "ok";
     case CL_ERR_INVALID_ARG: return "invalid argument";
-    case CL_ERR_NO_DEVICE: return "no sm_100 CUDA device (no CPU fallback)";
+    case CL_ERR_NO_DEVICE: return "no sm_90 CUDA device (no CPU fallback)";
     case CL_ERR_CUDA: return "CUDA error";
     case CL_ERR_OOM: return "out of device memory or KV pages";
     case CL_ERR_UNKNOWN_MODEL: return "model not served by this engine";

@@ -1,4 +1,4 @@
-// common.cuh — device helpers shared by the sm_100a kernels of libclengine.so.
+// common.cuh — device helpers shared by the sm_90a kernels of libclengine.so.
 // Numerics contract "cl-llama v1": see DESIGN.md §3 (bf16 weights / KV, fp32 residual stream,
 // bf16-rounded GEMV inputs, fp32 accumulation).
 #pragma once
@@ -31,11 +31,12 @@ __device__ __forceinline__ uint4 ldg_stream(const void* p) {
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
 }
-// 256-bit streaming load (sm_100: LDG.E.NA.EFL2.256) — 32 bytes per lane, L2 evict-first
+// 32 bytes per lane as two 128-bit streaming loads (Hopper has no 256-bit load)
 struct u32x8 { uint32_t v[8]; };
 __device__ __forceinline__ u32x8 ldg_stream256(const void* p) {
   u32x8 r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.nc.L1::no_allocate.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7])
                : "l"(p));
   return r;

@@ -1,4 +1,4 @@
-// decode_kernels.cu — single-token (and small-batch) decode kernels for sm_100a.
+// decode_kernels.cu — single-token (and small-batch) decode kernels for sm_90a.
 //
 // These implement the arithmetic that the reference reaches through callOllamaAPI
 // (/root/reference/pkg/crowdllama/api.go:108-160 -> ollama v0.9.6 llama.cpp decode loop; SURVEY.md
@@ -28,7 +28,7 @@ int sm_count() {
     const char* cv = getenv("CL_CARVEOUT_MAX");
     if (cv && *cv == '0') g_carveout_max = false;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -415,8 +415,7 @@ static cudaError_t launch_ring(const GemvArgs& a, cudaStream_t st, bool pdl) {
     case 2048: return launch_ring_inst<EPI, NORM, 2, 4, 2, 6>(a, st, pdl);
     case 4096:
       // q|k|v and o-proj share the SM with the attention kernel (128 KB KV ring) under PDL: 4 stages (64 KB)
-      // (4 stages measured 2.5 us slower per kernel than 6: 64 KB in flight per SM is below the
-      //  bandwidth-latency product; see profiles/README.md)
+      // (fewer bytes in flight per SM than the bandwidth-latency product needs)
       return launch_ring_inst<EPI, NORM, 2, 4, 4, 6>(a, st, pdl);
     case 8192: return launch_ring_inst<EPI, NORM, 1, 8, 4, 4>(a, st, pdl);
     case 14336: return launch_ring_inst<EPI, NORM, 1, 8, 7, 3>(a, st, pdl);
@@ -890,7 +889,7 @@ __global__ void synth_bf16_kernel(__nv_bfloat16* out, int64_t n, int k_cols, int
 int launch_synth_bf16(__nv_bfloat16* out, int64_t n_logical, int k_cols, int row_mult, int row_off, uint64_t seed,
                       int key, float scale, cudaStream_t st, int rope_hd) {
   int blocks = (int)((n_logical + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > sm_count() * 16) blocks = sm_count() * 16;
   if (blocks < 1) blocks = 1;
   synth_bf16_kernel<<<blocks, 256, 0, st>>>(out, n_logical, k_cols, row_mult, row_off, seed, key, scale, rope_hd);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;

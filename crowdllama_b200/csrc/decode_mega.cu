@@ -1,10 +1,10 @@
 // decode_mega.cu — the whole transformer stack of ONE decode token as a single persistent kernel.
 //
 // Why: with one kernel per op (decode_kernels.cu) the weight stream stops at every kernel boundary:
-// profiles/README.md (CL_TIMELINE) shows ~33 us of a 92 us layer spent in dependency release
-// (2.5-5 us x 5 boundaries), x/RMSNorm prologues (1-2.5 us x 5) and the attention latency chain,
+// a CL_TIMELINE trace shows a large share of each layer spent in dependency release at 5 boundaries,
+// x/RMSNorm prologues and the attention latency chain,
 // during which at most 96 KB/SM of prefetched weights keep HBM busy.  Here:
-//   * grid = one CTA per SM (148), 288 threads: warp 8 is the producer, warps 0..7 consume;
+//   * grid = one CTA per SM, 288 threads: warp 8 is the producer, warps 0..7 consume;
 //   * the producer streams EVERY byte the CTA will need — q|k|v rows, this CTA's KV pages, o rows,
 //     gate|up rows, down rows, layer after layer — through ONE 6 x 32 KB shared-memory ring with
 //     1-D TMA bulk copies; it never waits for activations (only for free slots, and once per layer for
@@ -77,8 +77,8 @@ __device__ __forceinline__ void grid_barrier(unsigned* cnt, int tid, volatile in
 constexpr int CH = 1;
 
 // ---- L2 lookahead.  Whenever a producer finds its ring full (the consumers sit in an epilogue, a grid barrier,
-// a norm prologue or attention: ~24 us per layer with HBM idle) it pulls weight tiles that lie AHEAD of every
-// CTA's ring into the 126 MB L2 with cp.async.bulk.prefetch.L2.  All weight tiles of the step form one sequence
+// a norm prologue or attention, with HBM idle) it pulls weight tiles that lie AHEAD of every
+// CTA's ring into the L2 (50 MB on H100) with cp.async.bulk.prefetch.L2.  All weight tiles of the step form one sequence
 // in consumption order (per layer: q|k|v, o, gate|up, down); `ctr` is the global prefetch frontier in that
 // numbering.  The frontier is kept between (own demand position + min_ahead) and (+ budget) tiles, so the
 // lookahead never outgrows L2.  When the consumers resume, the ring refills from L2 faster than HBM could feed
@@ -124,12 +124,12 @@ __device__ __forceinline__ void lookahead_step(Lookahead& la, const MegaArgs& a,
   }
 }
 // wait for a free ring slot; while blocked, run the L2 lookahead.  Then cap the number of copies IN FLIGHT:
-// tools/bench_barrier.cu shows that ~3 x 32 KB per SM already saturate HBM (7.4 TB/s), while every further tile in
+// a few 32 KB copies per SM already saturate HBM (tools/bench_barrier.cu measures it), while every further tile in
 // flight only deepens the queues in front of the L2 slices — and the grid barriers' red/poll round trips wait in
-// those queues (1.2 us idle, 4.4 us with 3 tiles in flight, 12 us with 6).  The ring still fills all NS slots.
+// those queues.  The ring still fills all NS slots.
 __device__ __forceinline__ void wait_slot(Ring& r, int st, Lookahead& la, const MegaArgs& a, unsigned mypos) {
   // (try_wait, not test_wait: a tightly polling producer warp measurably slows the two consumer warps that share
-  // its scheduler — 2.83 -> 2.86 ms/token)
+  // its scheduler)
   for (uint32_t spins = 0; !mbar_try_wait(&r.empty[st], r.parity() ^ 1u); ++spins) {
     lookahead_step(la, a, mypos);
     if (spins > (1u << 22)) __trap();
@@ -489,7 +489,6 @@ __global__ void __launch_bounds__(288, 1) decode_mega_kernel(const __grid_consta
           float rs = 0.f;
           // P is split into two bf16 terms (hi + lo) so that P.V keeps ~fp32 accuracy: a single bf16 P would put a
           // 2^-9 relative error on every attention output, which the bf16 rounding points downstream amplify
-          // (profiles/README.md, "parity vs depth")
           uint32_t pf[2][4], pl[2][4];
 #pragma unroll
           for (int nj = 0; nj < 4; ++nj) {
@@ -561,7 +560,7 @@ __global__ void __launch_bounds__(288, 1) decode_mega_kernel(const __grid_consta
       const int PS = HD + 2;
       const int c0 = (int)(((long long)a.q_dim * blockIdx.x) / gridDim.x), c1 = (int)(((long long)a.q_dim * (blockIdx.x + 1)) / gridDim.x);
       const float* pbase = a.part + (size_t)slot * a.n_kv * a.nsplit * REP * PS;
-      constexpr int MAXR = 4;   // 4 rounds x 8 warps = 32 outputs >= ceil(4096 / 148)
+      constexpr int MAXR = 4;   // 4 rounds x 8 warps = 32 outputs >= ceil(4096 / 132)
       float mv[MAXR], lv[MAXR], av[MAXR];
 #pragma unroll
       for (int q = 0; q < MAXR; ++q) {
@@ -670,7 +669,7 @@ bool mega_prepare_device() {
 
 int launch_decode_mega(const MegaArgs& a, cudaStream_t st) {
   if (!mega_prepare_device()) return -1;
-  // default on: measured identical to the plain launch (r2a: 355.6 vs 355.7 tok/s), and a grid that cannot be fully
+  // default on: no slower than the plain launch, and a grid that cannot be fully
   // resident fails at launch instead of trapping in a barrier
   static const bool coop = !(getenv("CL_MEGA_COOP") && atoi(getenv("CL_MEGA_COOP")) == 0);
   if (coop) {

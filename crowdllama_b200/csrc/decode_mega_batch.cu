@@ -1,14 +1,14 @@
 // decode_mega_batch.cu — one BATCHED decode step (B = 2..32 sequences) of the whole transformer stack as a single
 // persistent kernel: the continuous-batching inner loop of the worker (scheduler.cpp) without ~10 kernel launches per
-// layer.  Same idea as decode_mega.cu (B = 1), with the projections on the 5th-gen tensor cores:
+// layer.  Same idea as decode_mega.cu (B = 1), with the projections on the tensor cores (wgmma):
 //
 //   grid = one CTA per SM, 352 threads: warp 0 = TMA producer of W / KV tiles, warp 10 = TMA producer of the token operand,
-//   warp 1 = tcgen05 MMA issuer, warps 2-9 = consumers
-//   (GEMM epilogues: TMEM -> fp32 split-K partials; paged tensor-core attention; per-token reductions).
-//   Projections are Y[n][b] = sum_k W[n][k] X[b][k] with W tile [128 rows x 64 k] = UMMA A (16 KB, 2-D TMA, 128B
-//   swizzle), the B <= 32 token columns [32 x 64 k] = UMMA B (4 KB), accumulators [128 lanes x 32 columns] in TMEM.
+//   warps 2-9 = consumers (paged tensor-core attention; per-token reductions); consumer warps 4-7 form warpgroup 1, which
+//   also runs the projections' MMAs and writes their fp32 split-K partials (warp 1 is idle).
+//   Projections are Y[n][b] = sum_k W[n][k] X[b][k] with W tile [128 rows x 64 k] = MMA A (16 KB, 2-D TMA, 128B
+//   swizzle, two m64 halves), the B <= 32 token columns [32 x 64 k] = MMA B (4 KB), accumulators in registers.
 //   Every projection is cut into (row tile, k split) units — split counts from the engine's pick_splits — so that all
-//   148 SMs stream weights; fp32 partials go to a workspace and are folded in FIXED order by the next phase
+//   SMs stream weights; fp32 partials go to a workspace and are folded in FIXED order by the next phase
 //   (deterministic run to run).
 //   The producer streams W k-blocks, this CTA's KV pages and again W k-blocks through ONE ring of 16 KB slots in
 //   program order and never waits for activations with W: at a phase boundary it first primes the ring with the next
@@ -21,7 +21,7 @@
 //   AT  attention unit (b, kv head, split): q / k / v from the partials (+RoPE, K/V append into the paged cache),
 //       mma.sync m16n8k16 over TMA-swizzled pages (P = hi + lo bf16), the last split to finish combines -> bf16 attn_b
 //   G1  o partials   R1  h_b += ..., xn_b = norm   G2  gate|up partials   R2  act = bf16(SiLU(g) u)   G3  down partials
-// then the final norm; the LM head follows as a separate tcgen05 GEMM launch (gemm_tcgen05.cu).
+// then the final norm; the LM head follows as a separate GEMM launch (gemm_wgmma.cu).
 // Built for the Llama-3-8B / Mistral-7B layer shape (d 4096, d_ff 14336, head_dim 128, 4 q heads per kv head, page 32).
 #include <cuda.h>
 
@@ -29,25 +29,23 @@
 
 #include "common.cuh"
 #include "kernels.h"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace cl {
 
 namespace {
 
-using namespace tc;
+using namespace wg;
 
 constexpr int D = 4096, F = 14336, HD = 128, REP = 4, P = 32, HALF = HD / 2;
-constexpr int BT = 32;                       // token columns (UMMA N)
+constexpr int BT = 32;                       // token columns (MMA N)
 constexpr int NSW = 6;                       // W / KV ring slots of 16 KB (at most max_flight of them in flight)
 constexpr uint32_t WSLOT = 16384;
 constexpr int NSX = 25;                      // resident X tiles of 4 KB: the k range of one split (<= 25 k-blocks)
 constexpr uint32_t XSLOT = 4096;
-constexpr int NACC = 4;                      // TMEM accumulator sets of 32 columns
 constexpr int NC = 8;                        // consumer warps
 constexpr int MAXS = 32;                     // max KV splits per (sequence, kv head)
 constexpr float LOG2E = 1.4426950408889634f;
-constexpr uint32_t IDESC = make_idesc(BM, BT);
 
 struct Proj {                                // one projection of one layer
   const CUtensorMap* wmap;                   // device-resident tensor map of W [N][K], box {64, 128}
@@ -58,10 +56,9 @@ __device__ __forceinline__ void bar_consumers() { asm volatile("bar.sync 1, 256;
 
 // grid-wide barrier among the consumer warps of all CTAs (producer / MMA warps do not take part)
 // pause: while this CTA's consumers sit in the barrier its producer issues no new bulk copy — the barrier's red / poll round
-// trips queue behind bulk traffic in front of the L2 slices (tools/bench_barrier.cu: 1.2 us idle, 3.1 us with 2 x 32 KB in
-// flight per SM, 12 us with 6)
+// trips queue behind bulk traffic in front of the L2 slices (tools/bench_barrier.cu)
 // pause[1] counts the barriers this CTA has left: its producer waits for "barrier n passed" on that shared-memory word
-// instead of adding 148 more pollers to the global counter.
+// instead of adding one more poller per SM to the global counter.
 __device__ __forceinline__ void grid_barrier(unsigned* cnt, int ctid, volatile int* pause) {
   bar_consumers();
   if (ctid == 0) {
@@ -134,11 +131,8 @@ __global__ void __launch_bounds__(352, 1) decode_mega_batch_kernel(const __grid_
   uint64_t* w_full = bars;                   // [NSW]
   uint64_t* w_empty = w_full + NSW;          // [NSW]
   uint64_t* x_full = w_empty + NSW;          // [NSX]  tile i of this GEMM phase's token operand has landed
-  uint64_t* t_full = x_full + NSX;           // [NACC]
-  uint64_t* t_empty = t_full + NACC;         // [NACC]
-  uint64_t* kv_ready = t_empty + NACC;       // [1]  consumers -> producer: the current token's K/V rows are in the cache
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(kv_ready + 1);
-  float* red_m = reinterpret_cast<float*>(tmem_slot + 2);    // [NC][REP]
+  uint64_t* kv_ready = x_full + NSX;         // [1]  consumers -> producer: the current token's K/V rows are in the cache
+  float* red_m = reinterpret_cast<float*>(kv_ready + 1);     // [NC][REP]
   float* red_l = red_m + NC * REP;                           // [NC][REP]
   float* red_acc = red_l + NC * REP;                         // [NC][REP][HD]
   float* qs = red_acc + NC * REP * HD;                       // [REP][HD]   roped, bf16-rounded query of the unit
@@ -154,19 +148,11 @@ __global__ void __launch_bounds__(352, 1) decode_mega_batch_kernel(const __grid_
   if (threadIdx.x == 0) {
     for (int i = 0; i < NSW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 1); }
     for (int i = 0; i < NSX; ++i) mbar_init(&x_full[i], 1);
-    for (int i = 0; i < NACC; ++i) { mbar_init(&t_full[i], 1); mbar_init(&t_empty[i], 4); }
     mbar_init(kv_ready, 1);
     pause_s[0] = 0; pause_s[1] = 0;
     fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(NACC * BT) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // the four projections of layer l, then the LM head (l == n_layers, j == 0)
   auto proj = [&](int l, int j) -> Proj {
@@ -300,93 +286,69 @@ __global__ void __launch_bounds__(352, 1) decode_mega_batch_kernel(const __grid_
         dbg[3] = c_xempty; dbg[4] = c_phase;
       }
     }
-  } else if (warp == 1) {
-    // =============================================== MMA issuer ===============================================
-    uint32_t wit = 0, gp = 0, tn = 0;               // ring items consumed; GEMM phases; units issued (accumulator = tn % NACC)
-    long long m_w = 0, m_x = 0, m_t = 0;            // diagnostics: cycles blocked on W tiles / X tiles / a free accumulator
-    auto gemm_units = [&](int l, int j) {
-      const Proj pr = proj(l, j);
-      const GemmPlan g = gemm_plan(pr);
-      bool first = true;                            // the X tiles are waited for once, by the phase's first unit
-      for (int rt = g.m; rt < g.RT && g.nk > 0; rt += g.M, ++tn) {
-        const int acc = (int)(tn % NACC);
-        { const long long t0 = clock64(); mbar_wait(&t_empty[acc], ((tn / NACC) & 1u) ^ 1u); m_t += clock64() - t0; }
-        tc_fence_after();
-        const uint32_t d_addr = tmem_base + (uint32_t)(acc * BT);
-        for (int kb = 0; kb < g.nk; ++kb) {
-          const int s = (int)(wit % NSW);
-          const long long t0 = clock64();
-          mbar_wait(&w_full[s], (wit / NSW) & 1u);
-          const long long t1 = clock64();
-          if (first) mbar_wait(&x_full[kb], gp & 1u);
-          m_w += t1 - t0; m_x += clock64() - t1;
-          tc_fence_after();
-          if (lane == 0) {
-            const uint64_t adesc = make_smem_desc(smem_u32(wring + (size_t)s * WSLOT));
-            const uint64_t bdesc = make_smem_desc(smem_u32(xres + (size_t)kb * XSLOT));
-#pragma unroll
-            for (int k = 0; k < BK / UK; ++k) umma_f16(d_addr, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, (kb | k) != 0 ? 1u : 0u);
-            umma_commit(&w_empty[s]);
-            if (kb == g.nk - 1) umma_commit(&t_full[acc]);
-          }
-          __syncwarp();
-          ++wit;
-        }
-        first = false;
-      }
-      // observe EVERY x_full barrier in EVERY phase (tiles beyond this split's range, or all of them when this CTA has no
-      // unit in the phase): a warp that skipped a phase of a barrier would pass its next wait on stale parity
-      for (int i = first ? 0 : g.nk; i < NSX; ++i) mbar_wait(&x_full[i], gp & 1u);
-      ++gp;
-    };
-    for (int l = 0; l < a.n_layers; ++l) {
-      gemm_units(l, 0);
-      // the attention pages pass through the same ring: observe their barriers in order (never skip a phase of a slot
-      // — see the attention loop), without touching the data
-      for (int i = 0; i < att_pages; ++i, ++wit) mbar_wait(&w_full[wit % NSW], (wit / NSW) & 1u);
-      gemm_units(l, 1);
-      gemm_units(l, 2);
-      gemm_units(l, 3);
-    }
-    if (a.tl != nullptr && blockIdx.x == 0 && lane == 0) {
-      long long* dbg = a.tl + (size_t)a.n_layers * 16 + 8;
-      dbg[0] = m_w; dbg[1] = m_x; dbg[2] = m_t;
-    }
   } else if (warp >= 2 && warp < 2 + NC) {
     // =============================================== consumers ===============================================
     const int cw = warp - 2, ctid = cw * 32 + lane;          // consumer warp 0..7, consumer thread 0..255
-    uint32_t wit = 0, tn = 0, att_n = 0;
-    // ---- split-K epilogue: warps 2-5 own the TMEM lane quarters (warp % 4); partial[ks][b][n] fp32
-    auto gemm_epilogue = [&](int l, int j) {
+    uint32_t wit = 0, att_n = 0, gp = 0;                     // ring items consumed; attention units; GEMM phases
+    // ---- projections: warpgroup 1 (warps 4-7) runs the MMAs of this CTA's units and writes the split-K partials
+    // partial[ks][b][n] fp32 (LM head: the logits); the other consumer warps only keep the ring count
+    auto gemm_units = [&](int l, int j) {
       const Proj pr = proj(l, j);
       const GemmPlan g = gemm_plan(pr);
-      for (int rt = g.m; rt < g.RT && g.nk > 0; rt += g.M, ++tn) {
-        wit += (uint32_t)g.nk;
-        if (cw >= 4) continue;
-        const int acc = (int)(tn % NACC);
-        mbar_wait(&t_full[acc], (tn / NACC) & 1u);
-        tc_fence_after();
-        const int qd = warp & 3;
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(acc * BT), v);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&t_empty[acc]);
-        const int n = rt * BM + qd * 32 + lane;
-        if (n < pr.N) {
-          if (l == a.n_layers) {                     // LM head: logits[slot][n]
+      const bool mma = warp >= 4 && warp < 8;
+      const int wq = warp & 3, rq = lane >> 2, cq = lane & 3;
+      bool first = true;                            // the X tiles are waited for once, by the phase's first unit
+      for (int rt = g.m; rt < g.RT && g.nk > 0; rt += g.M) {
+        if (!mma) { wit += (uint32_t)g.nk; continue; }
+        float acc[2][BT / 2];                       // W rows 0-63 | 64-127 of the tile
 #pragma unroll
-            for (int b = 0; b < BT; ++b)
-              if (b < a.B) a.logits[(size_t)a.slots[b] * a.vocab + n] = __uint_as_float(v[b]);
-          } else {
-            float* dst = a.part + (size_t)g.ks * BT * pr.N + n;
+        for (int i = 0; i < BT / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+        int prev = -1;
+        for (int kb = 0; kb < g.nk; ++kb, ++wit) {
+          const int s = (int)(wit % NSW);
+          mbar_wait(&w_full[s], (wit / NSW) & 1u);
+          if (first) mbar_wait(&x_full[kb], gp & 1u);
+          const uint32_t wa = smem_u32(wring + (size_t)s * WSLOT), xa = smem_u32(xres + (size_t)kb * XSLOT);
+          fence_regs(acc[0]); fence_regs(acc[1]);
+          fence();
 #pragma unroll
-            for (int b = 0; b < BT; ++b)
-              if (b < a.B) dst[(size_t)b * pr.N] = __uint_as_float(v[b]);
-          }
+          for (int k = 0; k < BK / UK; ++k)
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf)
+              mma_ss<BT>(acc[hf], make_desc(wa + (uint32_t)hf * 8192u + (uint32_t)k * 32u), make_desc(xa + (uint32_t)k * 32u), 1u);
+          commit();
+          wait<1>();                                // the previous k-block's MMAs are done: release its slot
+          fence_regs(acc[0]); fence_regs(acc[1]);
+          if (prev >= 0 && ctid == 64) mbar_arrive(&w_empty[prev]);
+          prev = s;
         }
+        wait<0>();
+        fence_regs(acc[0]); fence_regs(acc[1]);
+        if (prev >= 0 && ctid == 64) mbar_arrive(&w_empty[prev]);
+        first = false;
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int n = rt * BM + hf * 64 + wq * 16 + h * 8 + rq;
+            if (n >= pr.N) continue;
+#pragma unroll
+            for (int i = 0; i < BT / 8; ++i)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int b = i * 8 + 2 * cq + e;
+                if (b >= a.B) continue;
+                const float v = acc[hf][4 * i + 2 * h + e];
+                if (l == a.n_layers) a.logits[(size_t)a.slots[b] * a.vocab + n] = v;     // LM head: logits[slot][n]
+                else a.part[((size_t)g.ks * BT + b) * pr.N + n] = v;
+              }
+          }
       }
+      // observe EVERY x_full barrier in EVERY phase (tiles beyond this split's range, or all of them when this CTA has no
+      // unit in the phase): a warp that skipped a phase of a barrier would pass its next wait on stale parity
+      if (mma)
+        for (int i = first ? 0 : g.nk; i < NSX; ++i) mbar_wait(&x_full[i], gp & 1u);
+      ++gp;
     };
     // ---- h_b += sum_s partial[s][b][:] (fixed order; n_split == 0: nothing to add); xn_b = bf16(rmsnorm(h_b) * gain)
     auto resid_norm = [&](const float* gain, int n_split) {
@@ -448,7 +410,7 @@ __global__ void __launch_bounds__(352, 1) decode_mega_batch_kernel(const __grid_
       grid_barrier(bars_l + 0, ctid, pause_s);
       CL_STAMP(1);
       // ------------------------------------------------------------------ G0: q|k|v partials
-      gemm_epilogue(l, 0);
+      gemm_units(l, 0);
       CL_STAMP(2);
       grid_barrier(bars_l + 1, ctid, pause_s);
       CL_STAMP(3);
@@ -667,7 +629,7 @@ __global__ void __launch_bounds__(352, 1) decode_mega_batch_kernel(const __grid_
       grid_barrier(bars_l + 2, ctid, pause_s);
       CL_STAMP(5);
       // ------------------------------------------------------------------ G1: o partials
-      gemm_epilogue(l, 1);
+      gemm_units(l, 1);
       CL_STAMP(6);
       grid_barrier(bars_l + 3, ctid, pause_s);
       CL_STAMP(7);
@@ -677,7 +639,7 @@ __global__ void __launch_bounds__(352, 1) decode_mega_batch_kernel(const __grid_
       grid_barrier(bars_l + 4, ctid, pause_s);
       CL_STAMP(9);
       // ------------------------------------------------------------------ G2: gate|up partials
-      gemm_epilogue(l, 2);
+      gemm_units(l, 2);
       CL_STAMP(10);
       grid_barrier(bars_l + 5, ctid, pause_s);
       CL_STAMP(11);
@@ -698,24 +660,18 @@ __global__ void __launch_bounds__(352, 1) decode_mega_batch_kernel(const __grid_
       grid_barrier(bars_l + 6, ctid, pause_s);
       CL_STAMP(13);
       // ------------------------------------------------------------------ G3: down partials
-      gemm_epilogue(l, 3);
+      gemm_units(l, 3);
       CL_STAMP(14);
       // its barrier (bars_l + 7) is taken at the top of the next layer / before the final norm
     }
     grid_barrier(a.bars + (size_t)(a.n_layers - 1) * 8 + 7, ctid, pause_s);
     resid_norm(a.final_norm, a.s_dn);                 // xn = final norm: the LM head (K = 64 k-blocks, more than the resident
-                                                      // operand holds) runs as a plain tcgen05 GEMM launch after this kernel
+                                                      // operand holds) runs as a plain GEMM launch after this kernel
 #undef CL_STAMP
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(NACC * BT) : "memory");
   }
 }
 
-constexpr size_t kSmem = (size_t)NSW * WSLOT + (size_t)NSX * XSLOT + (2 * NSW + NSX + 2 * NACC + 1) * 8 + 8 +
+constexpr size_t kSmem = (size_t)NSW * WSLOT + (size_t)NSX * XSLOT + (2 * NSW + NSX + 1) * 8 +
                          (2 * NC * REP + NC * REP * HD + REP * HD + 2 * MAXS * REP + REP + NC + 8) * 4 + 1024 + 64;
 
 bool g_ready[64] = {false}, g_ok[64] = {false};

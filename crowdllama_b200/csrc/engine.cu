@@ -1,5 +1,5 @@
 // engine.cu — the worker-side decode engine: weights, paged KV cache, the token step (CUDA graph
-// of hand-written sm_100a kernels), prefill, and the token-level entry points of the C-ABI.
+// of hand-written sm_90a kernels), prefill, and the token-level entry points of the C-ABI.
 //
 // Replaces, behind crowdllama.UnifiedAPIHandler (/root/reference/pkg/crowdllama/api.go:19), the
 // whole chain WorkerAPIHandler -> callOllamaAPI -> embedded Ollama server -> llama.cpp runner
@@ -87,8 +87,8 @@ int Engine::init(const cl_engine_config& c) {
   CL_CUDA_OK(cudaSetDevice(device_));
   cudaDeviceProp prop{};
   CL_CUDA_OK(cudaGetDeviceProperties(&prop, device_));
-  if (prop.major != 10) {
-    set_last_error(std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) + ", kernels are built for sm_100a only");
+  if (prop.major != 9) {
+    set_last_error(std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) + ", kernels are built for sm_90a only");
     return CL_ERR_NO_DEVICE;
   }
   snprintf(gpu_name_, sizeof gpu_name_, "%s", prop.name);
@@ -103,7 +103,7 @@ int Engine::init(const cl_engine_config& c) {
   use_pdl_ = env_int("CL_PDL", 1) != 0;
   pdl_early_ = env_int("CL_PDL_EARLY", 1);
   skip_attn_ = env_int("CL_SKIP_ATTN", 0) != 0;   // timing experiments only (wrong results)
-  use_flags_ = env_int("CL_FLAGS", 0) != 0;      // measured slower than griddepcontrol.wait (profiles/README.md)
+  use_flags_ = env_int("CL_FLAGS", 0) != 0;      // measured slower than griddepcontrol.wait
   want_timeline_ = env_int("CL_TIMELINE", 0) != 0;
   gemv_variant_ = c.decode_path == 1 ? 0 : 1;
   gemv_variant_ = env_int("CL_GEMV_VARIANT", gemv_variant_);
@@ -171,10 +171,9 @@ int Engine::init(const cl_engine_config& c) {
   {
     // Advertised throughput = CAPACITY, and load-INDEPENDENT: what this worker can deliver with a full batch, estimated
     // from the device's memory bandwidth and the model's bytes per token (70 % of the HBM roofline of one decode step x
-    // max_batch).  Round 1 advertised the measured decode steps/s x max_batch; a step at B = 32 takes 1.6x as long as at
+    // max_batch).  Round 1 advertised the measured decode steps/s x max_batch; a step at B = 32 takes longer than at
     // B = 1, so busy workers advertised LESS than idle ones, crossed a half-octave bucket, and FindBestWorker's strict
-    // maximum (manager.go:369-377) sent every request of a refresh interval to one idle worker (8 peers, r2k: 96 of 192
-    // requests on one worker).  Identical GPUs now advertise identical numbers and tie, which is what the reference's
+    // maximum (manager.go:369-377) sent every request of a refresh interval to one idle worker.  Identical GPUs now advertise identical numbers and tie, which is what the reference's
     // constants (peer.go:319-343) did; the measured rate stays available as cl_stats.measured_tokens_per_sec.
     const double params = (double)cfg.n_layers * ((double)qkv_dim_ * cfg.d_model + (double)cfg.d_model * q_dim_ + 3.0 * cfg.d_ff * cfg.d_model) +
                           (double)cfg.vocab_size * cfg.d_model;
@@ -332,8 +331,8 @@ int Engine::alloc_state() {
     CL_CUDA_OK(cudaMemsetAsync(d_timeline_, 0, (size_t)(cfg.n_layers * 5 + 1) * 4 * 8, stream_));
   }
   batch_gemm_min_ = env_int("CL_BATCH_GEMM_MIN", 2);
-  // token tile of the projections = 32 / 64 / 128 rows (gemm_tcgen05.cu picks it from the step's batch size)
-  use_batch_gemm_ = env_int("CL_BATCH_GEMM", 1) != 0 && max_batch_ >= 2 && gemm_tcgen05_supported(max_batch_, cfg.d_model, cfg.d_model) &&
+  // token tile of the projections = 32 / 64 / 128 rows (gemm_wgmma.cu picks it from the step's batch size)
+  use_batch_gemm_ = env_int("CL_BATCH_GEMM", 1) != 0 && max_batch_ >= 2 && gemm_tc_supported(max_batch_, cfg.d_model, cfg.d_model) &&
                     max_batch_ <= 128;
   if (use_batch_gemm_) {
     bws_.reset(new BatchWs());
@@ -432,7 +431,7 @@ int Engine::ensure_capacity(cl_seq_t s, int n_tokens) {
 // ---- one token step for the sequences listed in d_slots_[0..B) -----------------------------------
 int Engine::enqueue_step(int B, bool tail) {
   if (B >= 2 && tail && use_batch_mega_ && have_kv_maps_ && bws_) return enqueue_step_batch_mega(B);
-  if (B >= batch_gemm_min_ && tail && use_batch_gemm_ && bws_) return enqueue_step_batched(B);   // from B = 2: 3.58 vs 3.94 ms at ctx 256, 3.72 vs 4.29 at ctx 4096 against two GEMV passes (r2p)
+  if (B >= batch_gemm_min_ && tail && use_batch_gemm_ && bws_) return enqueue_step_batched(B);   // from B = 2: faster than two GEMV passes
   const int d = cfg.d_model, F = cfg.d_ff, L_ = cfg.n_layers;
   int n = 0, r;
 #define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } n += r; } while (0)
@@ -531,10 +530,10 @@ int Engine::enqueue_step(int B, bool tail) {
   return n;
 }
 
-// ---- batched token step (B >= 2): tensor-core projections (tcgen05, split-K) + per-sequence glue -----
+// ---- batched token step (B >= 2): tensor-core projections (wgmma, split-K) + per-sequence glue -----
 // split-K count of a batched-decode projection: the launch is as slow as its busiest CTA, i.e.
-// rounds(= ceil(tiles * s / SMs)) x k-blocks per unit.  224 gate|up tiles on 148 SMs cost 2 x 64 k-blocks unsplit but
-// 8 x 13 with 5 splits (ideal 96.9); down 56 -> 50 with 9.  Among the counts within 10 % of the best the smallest wins
+// rounds(= ceil(tiles * s / SMs)) x k-blocks per unit.  224 gate|up tiles on 132 SMs cost 2 x 64 k-blocks unsplit but
+// 9 x 13 with 5 splits.  Among the counts within 10 % of the best the smallest wins
 // (fewer partials for the consumer kernel to sum).
 int pick_splits_public(int n_rows, int K) { return pick_splits(n_rows, K); }
 static int pick_splits(int n_rows, int K) {

@@ -19,11 +19,11 @@
 namespace cl {
 
 // Defaults of the features added in round 2.  Each has an environment switch; the default is turned on only after a GPU run
-// of the parity tests and the benchmark with it (profiles/README.md records the run).
+// of the parity tests and the benchmark with it.
 constexpr int kDefaultSchedPrefillChunk = 1024; // CL_SCHED_PREFILL_CHUNK: admission token budget per scheduler iteration (0 = whole prompts); validated r2e
-constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts up to this many tokens take the split-K path (0 = off); validated r2e (128 tokens: 12.1 -> 6.3 ms)
-constexpr int kDefaultPrefillFused = 1;         // CL_PREFILL_FUSED bit mask: 1 = SiLU*mul (validated r2h: 63.2 -> 58.5 ms per 4096-token prefill), 2 = RoPE + cache scatter (correct but slower: r2g) fused into the prefill GEMM epilogues
-constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi; validated r2v: 64 clients x 146-token prompts 38.5 -> 47.4 req/s)
+constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts up to this many tokens take the split-K path (0 = off)
+constexpr int kDefaultPrefillFused = 1;         // CL_PREFILL_FUSED bit mask: 1 = SiLU*mul, 2 = RoPE + cache scatter (correct, measured slower) fused into the prefill GEMM epilogues
+constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi)
 constexpr int kDefaultSchedLingerUs = 1000;     // CL_SCHED_LINGER_US: with an empty batch, keep collecting while requests arrive within this gap (max 8x in total)
 constexpr int kDefaultBatchMega = 0;            // CL_BATCH_MEGA: persistent batched decode kernel for B >= 2
 
@@ -187,14 +187,14 @@ class Engine {
   int alloc_state();
   int ensure_capacity(cl_seq_t s, int n_tokens);  // reserve pages + upload block table row
   int enqueue_step(int B, bool tail);              // kernels of one token step for d_slots_[0..B)
-  int enqueue_step_batched(int B);                 // B >= 2: tcgen05 projections + per-sequence glue kernels
+  int enqueue_step_batched(int B);                 // B >= 2: wgmma projections + per-sequence glue kernels
   int run_step_graph(int B);
   bool ensure_graph(int B);
   void precapture_graphs();                       // graph launch (or eager enqueue)
   int read_logits(int slot, float* out);
   int prefill_tokenwise(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
   int prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
-  int ensure_prefill_ws(int tokens);  // tcgen05 path (prefill.cu)
+  int ensure_prefill_ws(int tokens);  // tensor-core path (prefill.cu)
   int prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_out);    // short prompts: split-K projections (prefill.cu)
   bool prefill_path_ok() const;
   int set_single_slot(cl_seq_t s);

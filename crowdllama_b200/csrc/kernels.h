@@ -1,4 +1,4 @@
-// kernels.h — host-side launch interface of the sm_100a kernels (internal to libclengine.so).
+// kernels.h — host-side launch interface of the sm_90a kernels (internal to libclengine.so).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -212,13 +212,13 @@ struct PerDeviceOnce {
   void mark() { *slot() = true; }
 };
 
-// ---- prefill path (prefill_kernels.cu / gemm_tcgen05.cu) -----------------------------------------
+// ---- prefill path (prefill_kernels.cu / gemm_wgmma.cu) -----------------------------------------
 // X bf16 [T][K] row-major, W bf16 [N][K] row-major -> Y fp32 [T][N] (+= resid when resid != nullptr)
 // k_splits > 1: split-K, partial s is written to Y + s*T*N (no residual); the consumer sums the partials
 int launch_gemm_bf16(const __nv_bfloat16* X, const __nv_bfloat16* W, float* Y, const float* resid, int T, int N, int K,
                      cudaStream_t st, int k_splits = 1, bool pdl = false);
-bool gemm_tcgen05_supported(int T, int N, int K);
-// fused prefill epilogues of the tcgen05 GEMM (gemm_tcgen05.cu): the fp32 result never leaves the SM
+bool gemm_tc_supported(int T, int N, int K);
+// fused prefill epilogues of the wgmma GEMM (gemm_wgmma.cu): the fp32 result never leaves the SM
 struct GemmEpi {
   int kind = 0;                              // 1: gate|up rows interleaved (2i gate, 2i+1 up) -> act[t][i] = bf16(silu(g) * u)
                                              // 2: q|k|v rows rope-pair-interleaved, head_dim 128 -> RoPE at pos0 + t, bf16, q_out / paged cache
@@ -249,7 +249,7 @@ struct AttnPrefillArgs {
   __nv_bfloat16* out;                // [T][H*D]
 };
 int launch_attn_prefill(const AttnPrefillArgs& a, cudaStream_t st);
-// tcgen05 variant (attn_prefill_tc.cu): head_dim 128, page 32; kmap / vmap = pool-wide 2-D tensor maps (box {64, 32})
+// wgmma variant (attn_prefill_tc.cu): head_dim 128, page 32; kmap / vmap = pool-wide 2-D tensor maps (box {64, 32})
 bool attn_prefill_tc_supported(int n_heads, int n_kv, int head_dim, int page_size, int pos0, int T);
 int launch_attn_prefill_tc(const AttnPrefillArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st);
 // act = bf16(silu(gu[:, 2i]) * gu[:, 2i+1])

@@ -58,7 +58,7 @@ int run_gemv(int device, int variant, int epi, bool norm, const uint16_t* w, con
   CL_CUDA_OK(cudaDeviceSynchronize());
   CL_CUDA_OK(cudaMemcpy(y, dy.p, (size_t)out_n * 4, cudaMemcpyDeviceToHost));
   if (iters > 0 && ms && epi != EPI_RESID) {
-    // timing loop: rotate over enough weight copies to exceed the 126 MB L2
+    // timing loop: rotate over enough weight copies (256 MB) to exceed the L2 (50 MB on H100)
     const size_t wbytes = (size_t)n_rows * k * 2;
     int copies = (int)std::min<size_t>(16, (256ull << 20) / wbytes + 1);
     std::vector<DevBuf> extra(copies > 1 ? copies - 1 : 0);

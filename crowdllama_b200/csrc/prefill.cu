@@ -1,5 +1,5 @@
 // prefill.cu — prompt (prefill) path of the engine: chunks of up to prefill_chunk_tokens_ tokens go
-// through tcgen05 GEMMs (gemm_tcgen05.cu) and the causal paged attention kernel
+// through wgmma GEMMs (gemm_wgmma.cu) and the causal paged attention kernel
 // (prefill_kernels.cu); the last position's logits come from the decode LM-head GEMV so that
 // prefill and decode share one logits/argmax tail.  Also: cl_op_gemm_bf16 / cl_op_attn_prefill.
 #include <algorithm>
@@ -21,7 +21,7 @@ bool Engine::prefill_path_ok() const {
     const char* v = getenv("CL_PREFILL_TCGEN05");
     disabled = (v && *v == '0') ? 1 : 0;
   }
-  return !disabled && gemm_tcgen05_supported(16, cfg.d_model, cfg.d_model);
+  return !disabled && gemm_tc_supported(16, cfg.d_model, cfg.d_model);
 }
 
 // split-K rule shared with the batched decode step (engine.cu)
@@ -70,8 +70,8 @@ struct PrefillProfiler {
 };
 
 // Short prompts (prefill_min_tokens_ <= n <= 256, e.g. a 128-token chat): one token tile per W row tile means only
-// N/128 CTAs stream the weights of a projection (48 for q|k|v, 32 for o and down) — 11 ms for 128 tokens where the
-// weight stream alone needs 2.4.  Same recipe as the batched decode step: split-K so that ~148 CTAs share every
+// N/128 CTAs stream the weights of a projection (48 for q|k|v, 32 for o and down), far below the
+// machine's weight-streaming rate.  Same recipe as the batched decode step: split-K so that all SMs share every
 // projection's weights, fp32 partials in a workspace, the per-row glue kernels (batch_kernels.cu) fold them in fixed
 // order into the residual stream / RoPE / SiLU.  Rows are the prompt's tokens, attention is the causal prefill kernel.
 int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_out) {
@@ -110,7 +110,7 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
 #define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } launches += r; pp.mark(#call); } while (0)
   // programmatic dependent launch between the GEMMs and the per-row glue kernels, as in the batched decode step (the two
   // prefill kernels in between are launched normally and order the stream)
-  static const bool small_pdl = !getenv("CL_SMALL_PDL") || atoi(getenv("CL_SMALL_PDL")) != 0;   // 146 tokens: 6.41 -> 5.90 ms (r2q)
+  static const bool small_pdl = !getenv("CL_SMALL_PDL") || atoi(getenv("CL_SMALL_PDL")) != 0;
   const bool bp = small_pdl && use_pdl_;
   pp.mark("start");
   CL_LAUNCH(launch_embed_rows(embed_, d, d_prompt_, w.h, T, stream_));
@@ -273,12 +273,11 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
 
 
 // Several prompts in ONE pass of the tile path (admission of a burst of short chats): the rows of all prompts are
-// concatenated, so every projection streams its weights once for all of them and runs on full 128 x 256 tiles —
-// 64 prompts of 130 tokens cost 64 x 6.0 ms one by one (the split-K short-prompt path streams all weights per prompt)
-// against about 2.3 ms each in passes of 1024-4096 rows.  Everything row-wise (embedding, RMSNorm, the four GEMMs,
+// concatenated, so every projection streams its weights once for all of them and runs on full tiles (the split-K
+// short-prompt path streams all weights once per prompt).  Everything row-wise (embedding, RMSNorm, the four GEMMs,
 // SiLU) is unchanged; RoPE + cache scatter and the causal attention run per sequence on its row range (pointer
 // offsets into the same workspace; each sequence has its own position offset and block table); the last row of every
-// sequence goes through the batched LM head of the decode step (final norm + tcgen05 GEMM + argmax), which leaves
+// sequence goes through the batched LM head of the decode step (final norm + wgmma GEMM + argmax), which leaves
 // d_tok_ / d_pos_ of every slot ready for the first decode step.  A row's results do not depend on the other rows of
 // the pass: logits and cache contents are bit-identical to prefill_chunked on each prompt alone (tests/test_gpu_prefill.py).
 int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* ids, const int* lens, float* logits_out) {
@@ -421,7 +420,7 @@ int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, 
   if (!x || !w || !y || t <= 0 || n <= 0 || k <= 0) return CL_ERR_INVALID_ARG;
   int rc = check_device(device);
   if (rc) return rc;
-  if (!gemm_tcgen05_supported(t, n, k)) { set_last_error("shape not supported by the tcgen05 GEMM (K % 8)"); return CL_ERR_INVALID_ARG; }
+  if (!gemm_tc_supported(t, n, k)) { set_last_error("shape not supported by the wgmma GEMM (K % 8)"); return CL_ERR_INVALID_ARG; }
   DevBuf dx, dw, dy;
   CL_CUDA_OK(dx.upload(x, (size_t)t * k * 2));
   CL_CUDA_OK(dw.upload(w, (size_t)n * k * 2));
@@ -453,7 +452,7 @@ int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, 
   return CL_OK;
 }
 
-// variant: -1 auto (tcgen05 kernel when the shape allows, CL_PREFILL_ATTN_TC=0 forces the other), 0 mma.sync kernel, 1 tcgen05 kernel
+// variant: -1 auto (wgmma kernel when the shape allows, CL_PREFILL_ATTN_TC=0 forces the other), 0 mma.sync kernel, 1 wgmma kernel
 static int attn_prefill_impl(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t, int32_t n_heads, int32_t n_kv,
                              int32_t head_dim, int variant, int iters, float* out, float* ms) {
   if (!q || !k || !v || !out || t <= 0) return CL_ERR_INVALID_ARG;
@@ -487,7 +486,7 @@ static int attn_prefill_impl(int device, const uint16_t* q, const uint16_t* k, c
   bool tc = variant != 0 && attn_prefill_tc_supported(n_heads, n_kv, HD, P, 0, t);
   if (variant == 1 && !tc && head_dim == 128) tc = (t + P - 1) / P <= 320;          // explicit request overrides the env switch
   if (tc) tc = make_tmap_2d_bf16(&km, dk.p, (uint64_t)n_pages * n_kv * P, HD, 64, 32) && make_tmap_2d_bf16(&vm, dv.p, (uint64_t)n_pages * n_kv * P, HD, 64, 32);
-  if (variant == 1 && !tc) { set_last_error("tcgen05 prefill attention does not support this shape"); return CL_ERR_INVALID_ARG; }
+  if (variant == 1 && !tc) { set_last_error("wgmma prefill attention does not support this shape"); return CL_ERR_INVALID_ARG; }
   auto run = [&]() { return tc ? launch_attn_prefill_tc(a, km, vm, 0, nullptr) : launch_attn_prefill(a, nullptr); };
   if (run() < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("prefill attention launch failed"); return CL_ERR_CUDA; }
   if (launch_bf16_to_f32(dout.as<__nv_bfloat16>(), dout32.as<float>(), (int64_t)t * qd, nullptr) < 0) return CL_ERR_CUDA;

@@ -3,7 +3,7 @@
 // (Upstream counterparts, SURVEY.md §2.2: ggml-cuda rms_norm / rope / cpy / flash_attn_ext / silu.)
 //
 // The attention kernel is a FlashAttention-2 style mma.sync (m16n8k16 bf16) kernel: it is the
-// round-1 baseline for prompts; the tcgen05 version is the planned replacement (DESIGN.md §7).
+// round-1 baseline for prompts; attn_prefill_tc.cu replaces it for head_dim 128.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -115,7 +115,7 @@ __global__ void silu_mul_bf16_kernel(const float* __restrict__ gu, __nv_bfloat16
 }
 int launch_silu_mul_bf16(const float* gu, __nv_bfloat16* act, int T, int d_ff, cudaStream_t st) {
   const int64_t total = (int64_t)T * d_ff;
-  int blocks = (int)std::min<int64_t>((total / 2 + 255) / 256, 148 * 16);
+  int blocks = (int)std::min<int64_t>((total / 2 + 255) / 256, (int64_t)sm_count() * 16);
   if (blocks < 1) blocks = 1;
   silu_mul_bf16_kernel<<<blocks, 256, 0, st>>>(gu, act, total);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;

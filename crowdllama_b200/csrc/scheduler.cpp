@@ -244,7 +244,7 @@ void Engine::scheduler_main() {
     std::lock_guard<std::mutex> elk(mu_);
     // ---- admission.  A prompt is prefilled in chunks of sched_prefill_chunk_ tokens, ONE chunk per scheduler iteration,
     // interleaved with the decode steps of the running batch: an admit never stalls active sequences for more than one
-    // chunk (a 4096-token prompt used to hold every running request for the whole ~85 ms prefill).
+    // chunk (a 4096-token prompt used to hold every running request for its whole prefill).
     // Several short prompts may be admitted in one iteration as long as their tokens fit the same budget (a burst of
     // 128-token chats fills the batch in a few iterations instead of one request per decode step).
     int budget = sched_prefill_chunk_ > 0 ? sched_prefill_chunk_ : (1 << 30);   // 0: unlimited = whole prompts, as in round 1
@@ -439,9 +439,9 @@ void Engine::scheduler_main() {
     int rc = run_step_graph(B);
     if (rc == CL_OK) {
       cudaMemcpyAsync(toks.data(), d_tok_, (size_t)max_seqs_ * 4, cudaMemcpyDeviceToHost, stream_);
-      // Batched steps last 3.5-6 ms: wait on a blocking-sync event instead of spinning in cudaStreamSynchronize, so that
+      // Batched steps last milliseconds: wait on a blocking-sync event instead of spinning in cudaStreamSynchronize, so that
       // eight worker processes on one box do not burn eight host cores (the box's cgroup quota is 16) while their GPUs
-      // work.  Single-sequence steps (2.8 ms, latency matters) keep the spinning wait.
+      // work.  Single-sequence steps (latency matters) keep the spinning wait.
       if (B >= 2 && sched_blocking_sync_ && step_done_ev_) {
         if (cudaEventRecord(step_done_ev_, stream_) != cudaSuccess || cudaEventSynchronize(step_done_ev_) != cudaSuccess) rc = CL_ERR_CUDA;
       } else if (cudaStreamSynchronize(stream_) != cudaSuccess) rc = CL_ERR_CUDA;

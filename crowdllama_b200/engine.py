@@ -1,7 +1,7 @@
 """ctypes binding of libclengine.so — the same C-ABI a Go cgo shim binds (include/clengine.h).
 
 There is no CPU fallback anywhere in this package: if the shared library is missing the import
-of the binding fails loudly, and if no sm_100 device is visible `Engine(...)` raises
+of the binding fails loudly, and if no sm_90 device is visible `Engine(...)` raises
 `EngineError(CL_ERR_NO_DEVICE)`.
 """
 from __future__ import annotations
@@ -573,7 +573,7 @@ def op_attn_prefill(q_bf16, k_bf16, v_bf16, n_heads, n_kv, head_dim, device=0):
 
 
 def op_attn_prefill_variant(q_bf16, k_bf16, v_bf16, n_heads, n_kv, head_dim, variant, iters=0, device=0):
-    """variant 0: mma.sync kernel, 1: tcgen05 kernel, -1: auto.  Returns (out, ms per launch or None)."""
+    """variant 0: mma.sync kernel, 1: wgmma kernel, -1: auto.  Returns (out, ms per launch or None)."""
     q = np.ascontiguousarray(q_bf16, dtype=np.uint16)
     k = np.ascontiguousarray(k_bf16, dtype=np.uint16)
     v = np.ascontiguousarray(v_bf16, dtype=np.uint16)

@@ -202,7 +202,7 @@ def make_server(worker_addrs, port: int = 9001, host: str = "127.0.0.1", seed: i
 def main():
     """python -m crowdllama_b200.gateway --port 9001 --worker 127.0.0.1:9101 --worker 127.0.0.1:9102 ..."""
     import argparse
-    ap = argparse.ArgumentParser(description="Ollama-compatible gateway stand-in in front of B200 worker peers")
+    ap = argparse.ArgumentParser(description="Ollama-compatible gateway stand-in in front of GPU worker peers")
     ap.add_argument("--host", default="127.0.0.1")
     ap.add_argument("--port", type=int, default=9001)                      # the reference gateway's default port
     ap.add_argument("--worker", action="append", default=[], help="host:port of a worker peer (repeatable)")

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's handler interface for the hot path.
 
   UnifiedAPIHandler        /root/reference/pkg/crowdllama/api.go:19
-  WorkerAPIHandler         api.go:45-96   -> worker_api_handler(engine): the B200 engine behind the
+  WorkerAPIHandler         api.go:45-96   -> worker_api_handler(engine): the GPU engine behind the
                                              same closure shape (the Go cgo shim in go/b200handler
                                              does exactly this around cl_generate)
   DefaultAPIHandler        api.go:163-189 -> default_api_handler (consumer echo)
@@ -81,7 +81,7 @@ def worker_api_handler(engine: "eng.Engine", sampling: "eng.Sampling | None" = N
         try:
             r = engine.generate(generate_req.model, generate_req.prompt, merge_sampling(sampling, generate_req.options))
         except eng.EngineError as ex:                                # api.go:63-68 wraps the backend error
-            raise HandlerError(f"failed to call B200 engine: {ex}") from ex
+            raise HandlerError(f"failed to call GPU engine: {ex}") from ex
         return _response(generate_req.model, r.text, True, r.done_reason)
 
     def stream(ctx, req: BaseMessage, emit) -> None:
@@ -100,7 +100,7 @@ def worker_api_handler(engine: "eng.Engine", sampling: "eng.Sampling | None" = N
             r = engine.generate_stream(generate_req.model, generate_req.prompt, merge_sampling(sampling, generate_req.options),
                                        on_text)
         except eng.EngineError as ex:
-            raise HandlerError(f"failed to call B200 engine: {ex}") from ex
+            raise HandlerError(f"failed to call GPU engine: {ex}") from ex
         emit(_response(generate_req.model, "", True, r.done_reason))
 
     handler.stream = stream
@@ -114,7 +114,7 @@ def worker_api_handler_bytes(engine: "eng.Engine", sampling: "eng.Sampling | Non
     def _wrap(ex):
         if ex.status == eng.CL_ERR_BAD_MESSAGE:
             return HandlerError("expected GenerateRequest, got different message type")
-        return HandlerError(f"failed to call B200 engine: {ex}")
+        return HandlerError(f"failed to call GPU engine: {ex}")
 
     def handler(ctx, req: BaseMessage) -> BaseMessage:
         try:

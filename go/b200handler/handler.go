@@ -1,4 +1,4 @@
-// Package b200handler is the cgo shim that drops the B200 engine into CrowdLlama's worker path.
+// Package b200handler is the cgo shim that drops the GPU engine into CrowdLlama's worker path.
 //
 // It builds a crowdllama.UnifiedAPIHandler (pkg/crowdllama/api.go:19) with the same contract as
 // crowdllama.WorkerAPIHandler (api.go:45-96), replacing the HTTP round trip to Ollama
@@ -37,7 +37,7 @@ type Engine struct {
 	model string
 }
 
-// Config mirrors the CROWDLLAMA_* knobs added for the B200 worker (pkg/config/config.go:58-79 style).
+// Config mirrors the CROWDLLAMA_* knobs added for the GPU worker (pkg/config/config.go:58-79 style).
 type Config struct {
 	Device     int    // CROWDLLAMA_B200_DEVICE
 	ModelName  string // name advertised in Resource.SupportedModels and matched exactly (manager.go:349-354), e.g. "llama3:8b"
@@ -132,7 +132,7 @@ func (e *Engine) Handler() crowdllama.UnifiedAPIHandler {
 			return nil, ctx.Err()
 		}
 		if last == nil || !last.Done {
-			return nil, fmt.Errorf("failed to call B200 engine: no final response frame")
+			return nil, fmt.Errorf("failed to call GPU engine: no final response frame")
 		}
 		last.Response = string(text) // api.go:80: the full assistant text in ONE message (the reference never streams, api.go:155)
 		return &llamav1.BaseMessage{Message: &llamav1.BaseMessage_GenerateResponse{GenerateResponse: last}}, nil
@@ -168,7 +168,7 @@ func (e *Engine) HandleStream(ctx context.Context, req *llamav1.BaseMessage, emi
 	defer C.free(buf)
 	if rc := C.cl_handle_message_stream(e.h, (*C.uint8_t)(buf), C.size_t(len(raw)), nil,
 		C.cl_frame_cb(C.goFrameCallback), unsafe.Pointer(&h)); rc != C.CL_OK {
-		return fmt.Errorf("failed to call B200 engine: %w", lastErr(rc))
+		return fmt.Errorf("failed to call GPU engine: %w", lastErr(rc))
 	}
 	return emitErr
 }

@@ -1,5 +1,5 @@
 /*
- * clengine.h — C-ABI of the B200-native CrowdLlama worker decode engine (libclengine.so).
+ * clengine.h — C-ABI of the H100-native (sm_90a) CrowdLlama worker decode engine (libclengine.so).
  *
  * This is the drop-in boundary for the ONE hot path this repository accelerates: the
  * worker-side model step that the reference reaches through
@@ -20,7 +20,7 @@
  *   - cl_generate(), cl_generate_ids(), cl_engine_stats() are thread-safe and re-entrant (one goroutine per inbound
  *     libp2p stream calls the handler concurrently: /root/reference/pkg/peer/peer.go:177-182).
  *     The token-level cl_seq_* / cl_prefill / cl_decode_step calls are serialised internally by one engine lock.
- *   - there is NO CPU fallback: if no sm_100 device is present cl_engine_create fails with
+ *   - there is NO CPU fallback: if no sm_90 (compute capability 9.x) device is present cl_engine_create fails with
  *     CL_ERR_NO_DEVICE.
  */
 #ifndef CLENGINE_H_
@@ -38,7 +38,7 @@ extern "C" {
 typedef enum cl_status {
   CL_OK = 0,
   CL_ERR_INVALID_ARG = -1,
-  CL_ERR_NO_DEVICE = -2,     /* no CUDA device / not sm_100 */
+  CL_ERR_NO_DEVICE = -2,     /* no CUDA device / not sm_90 */
   CL_ERR_CUDA = -3,          /* CUDA runtime error; see cl_last_error() */
   CL_ERR_OOM = -4,           /* device memory or KV pages exhausted */
   CL_ERR_UNKNOWN_MODEL = -5, /* model name not served by this engine */
@@ -298,14 +298,14 @@ int cl_op_qkv_rope_append(int device, int variant, const uint16_t* w_qkv, const 
 int cl_op_attn_decode(int device, const float* q, const uint16_t* k_cache, const uint16_t* v_cache,
                       int32_t ctx_len, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size,
                       float* out);
-/* prefill GEMM on tcgen05: Y[t][n] = sum_k X[t][k] W[n][k]; X,W bf16, Y fp32 */
+/* prefill GEMM on the tensor cores (wgmma): Y[t][n] = sum_k X[t][k] W[n][k]; X,W bf16, Y fp32 */
 int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, int32_t t,
                     int32_t n, int32_t k, int32_t iters, float* ms);
 /* causal prefill attention: q [t][n_heads][d], k,v [t][n_kv][d] bf16 (roped), out bf16-rounded fp32 */
 int cl_op_attn_prefill(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v,
                        int32_t t, int32_t n_heads, int32_t n_kv, int32_t head_dim, float* out);
 /* the same with the kernel chosen explicitly — variant 0: mma.sync kernel (prefill_kernels.cu, any head_dim 64|128),
- * 1: tcgen05 kernel (attn_prefill_tc.cu, head_dim 128), -1: what the engine would pick — and an optional timing loop */
+ * 1: wgmma kernel (attn_prefill_tc.cu, head_dim 128), -1: what the engine would pick — and an optional timing loop */
 int cl_op_attn_prefill_variant(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t,
                                int32_t n_heads, int32_t n_kv, int32_t head_dim, float* out, int32_t iters, float* ms);
 /* synthetic weight generator (device kernel) -> host copy, for known-answer tests */

@@ -102,7 +102,7 @@ def _ids_match(ids, ref, margins):
 @pytest.mark.parametrize("batch_gemm", ["1", "0"])
 def test_batched_decode_matches_single_and_oracle(monkeypatch, batch_gemm):
     """Continuous-batching inner loop: B sequences of different lengths advance together.  CL_BATCH_GEMM=1 is
-    the tensor-core path (tcgen05 split-K projections + glue kernels), 0 the per-sequence GEMV kernels."""
+    the tensor-core path (wgmma split-K projections + glue kernels), 0 the per-sequence GEMV kernels."""
     monkeypatch.setenv("CL_BATCH_GEMM", batch_gemm)
     monkeypatch.setenv("CL_BATCH_GEMM_MIN", "2")
     cfg = oc.PRESETS["tiny-test"]
@@ -267,7 +267,7 @@ def test_engine_with_a_tokenizer_json(name):
 
 @pytest.mark.parametrize("preset", ["tinyllama-1.1b", "llama3.2-1b"])
 def test_tinyllama_shapes_match_oracle(preset):
-    """Model shapes outside the persistent kernels (head_dim 64): per-op decode kernels + tcgen05 prefill.  llama3.2-1b
+    """Model shapes outside the persistent kernels (head_dim 64): per-op decode kernels + wgmma prefill.  llama3.2-1b
     adds the "llama3" rotary frequency scaling and a 128K vocabulary (6 layers of the 16 keep the test short)."""
     cfg = dict(oc.PRESETS[preset])
     cfg["max_seq_len"] = 256

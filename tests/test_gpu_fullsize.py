@@ -16,7 +16,7 @@ def _prompt(n, vocab, salt=0):
 
 
 def test_llama3_8b_full_model_matches_oracle():
-    """Full 32-layer Llama-3-8B shapes, seeded synthetic weights (bit-identical on both sides): tcgen05 prefill
+    """Full 32-layer Llama-3-8B shapes, seeded synthetic weights (bit-identical on both sides): wgmma prefill
     + persistent decode kernel vs the CPU oracle, teacher-forced; then run-to-run determinism of greedy decode."""
     cfg = dict(oc.PRESETS["llama3-8b"])
     cfg["max_seq_len"] = 256
@@ -41,7 +41,7 @@ def test_llama3_8b_full_model_matches_oracle():
             tok = int(lo.argmax())
         print(f"llama3-8b full: max |dlogit| {max(errs):.4g} over prefill + 5 decode steps, near-tie mismatches {mism}")
         # stated fp tolerance on logits (DESIGN.md §2): 0.05 + 0.03*sqrt(L) — bf16 rounding of every GEMV input makes
-        # last-bit differences in fp32 summation order grow ~1e-3*sqrt(L) relative (measured: profiles/README.md)
+        # last-bit differences in fp32 summation order grow ~1e-3*sqrt(L) relative
         assert max(errs) < 0.05 + 0.03 * np.sqrt(cfg["n_layers"])
         hid = e.debug_hidden()
         ho = m.hidden(cfg["n_layers"])

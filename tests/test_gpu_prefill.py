@@ -1,4 +1,4 @@
-"""Prefill path parity: tcgen05 GEMM, causal paged attention, and the engine's chunked prefill vs the oracle."""
+"""Prefill path parity: tensor-core GEMM, causal paged attention, and the engine's chunked prefill vs the oracle."""
 import numpy as np
 import pytest
 
@@ -40,13 +40,13 @@ def test_attn_prefill_matches_oracle(n_heads, n_kv, hd, t):
 
 
 @pytest.mark.parametrize("variant", [0, 1])
-@pytest.mark.parametrize("t,n_heads,n_kv", [(1, 4, 1), (127, 4, 1), (128, 8, 2), (129, 4, 4), (255, 4, 1), (257, 8, 2), (640, 4, 1), (1000, 8, 2),
-                                            (2049, 4, 1)])
+@pytest.mark.parametrize("t,n_heads,n_kv", [(1, 4, 1), (127, 4, 1), (128, 8, 2), (129, 4, 4), (193, 4, 1), (255, 4, 1), (257, 8, 2), (640, 4, 1),
+                                            (1000, 8, 2), (2049, 4, 1)])
 def test_attn_prefill_kernels_head_dim_128(variant, t, n_heads, n_kv):
-    """Both prefill attention kernels at head_dim 128 — variant 1 = tcgen05 (S and O in TMEM, K/V pages by 2-D TMA,
+    """Both prefill attention kernels at head_dim 128 — variant 1 = wgmma (S and O in registers, K/V pages by 2-D TMA,
     V as an MN-major operand), variant 0 = the mma.sync kernel — against the oracle's per-position attention: ragged
-    lengths around the 128-row tile / 256-row item / 128-token block boundaries, reversed page order, GQA 1:1 ... 4:1.
-    Score scale ~ N(0, 4): rows whose maximum moves by more than 2^8 between blocks exercise the TMEM rescale path."""
+    lengths around the 128-row item and 64-token KV block boundaries (127 / 128 / 129, 193 inside an item, 255 / 257, ...), reversed page order, GQA 1:1 ... 4:1.
+    Score scale ~ N(0, 4): row maxima move between blocks and exercise the online-softmax rescale."""
     rng = np.random.default_rng(t * 5 + n_heads + n_kv)
     hd = 128
     q = _rand_bf16(rng, (t, n_heads * hd), 2.0)
@@ -79,7 +79,7 @@ def test_engine_chunked_prefill_matches_oracle(monkeypatch, n_prompt, path):
         so = m.new_seq()
         lo = so.forward(p)
         s = e.seq_create()
-        lg = e.prefill(s, p)                       # >= 16 tokens -> tcgen05 path
+        lg = e.prefill(s, p)                       # >= 16 tokens -> tensor-core path
         assert np.abs(lg - lo).max() < 0.125
         # decode continues from the prefix the prefill kernels wrote into the paged cache
         tok = int(lo.argmax())
@@ -98,7 +98,7 @@ def test_engine_chunked_prefill_matches_oracle(monkeypatch, n_prompt, path):
 
 @pytest.mark.parametrize("fused", ["3", "0"])
 def test_prefill_paths_agree_on_llama_shapes(monkeypatch, fused):
-    """Token-wise (decode kernels), full-tile (tcgen05; fused = RoPE / SiLU in the GEMM epilogues) and short-prompt
+    """Token-wise (decode kernels), full-tile (wgmma; fused = RoPE / SiLU in the GEMM epilogues) and short-prompt
     (split-K) prefill of the same prompts give the same logits within tolerance at Llama-3-8B layer shapes (2 layers);
     the short-prompt path is also compared with the oracle directly."""
     monkeypatch.setenv("CL_PREFILL_SMALL_MAX", "256")
@@ -123,10 +123,10 @@ def test_prefill_paths_agree_on_llama_shapes(monkeypatch, fused):
             e.seq_free(ss)
         p = _prompt(300, cfg["vocab_size"])
         s1 = e.seq_create()
-        a = e.prefill(s1, p)                       # tcgen05
+        a = e.prefill(s1, p)                       # tensor-core tile path
         s2 = e.seq_create()
         b = None
-        for i in range(0, 300, 10):                # 10-token pieces stay below the tcgen05 threshold
+        for i in range(0, 300, 10):                # 10-token pieces stay below the tile-path threshold
             b = e.prefill(s2, p[i:i + 10])
         assert np.abs(a - b).max() < 0.125
         assert int(a.argmax()) == int(b.argmax()) or np.sort(b)[-1] - np.sort(b)[-2] < 2e-2
@@ -134,8 +134,8 @@ def test_prefill_paths_agree_on_llama_shapes(monkeypatch, fused):
 
 @pytest.mark.parametrize("t2", [150, 300])
 def test_prefill_continuation_at_an_unaligned_position_llama_shapes(monkeypatch, t2):
-    """Multi-turn / chunked prompts: a second prefill appended at a position that is no multiple of the 128-token KV
-    block (pos0 = 105) — the tcgen05 attention's diagonal then cuts through blocks, and keys come from pages written
+    """Multi-turn / chunked prompts: a second prefill appended at a position that is no multiple of the 64-token KV
+    block (pos0 = 105) — the wgmma attention's diagonal then cuts through blocks, and keys come from pages written
     by an earlier prefill and by decode steps.  t2 = 150 takes the short-prompt path, 300 the full-tile path."""
     monkeypatch.setenv("CL_PREFILL_SMALL_MAX", "256")
     monkeypatch.setenv("CL_PREFILL_FUSED", "3")
@@ -172,8 +172,8 @@ def test_multi_prompt_prefill_is_bit_identical_to_one_prompt_at_a_time(monkeypat
     """Engine::prefill_multi (cl_prefill_batch): several prompts as the rows of ONE tile-path pass.  A row's results do
     not depend on its neighbours, so the cached K / V of every position and the greedy continuation must equal, bit for
     bit, the same prompts prefilled alone through the tile path (CL_PREFILL_SMALL_MAX=0) — at Llama-3-8B layer shapes
-    (tcgen05 attention) and on the tiny preset (head_dim 64).  The last-position logits come from the batched LM head
-    (tcgen05 GEMM) instead of the single-sequence GEMV: same bf16 inputs, another summation order (<= 2e-4)."""
+    (wgmma attention) and on the tiny preset (head_dim 64).  The last-position logits come from the batched LM head
+    (wgmma GEMM) instead of the single-sequence GEMV: same bf16 inputs, another summation order (<= 2e-4)."""
     monkeypatch.setenv("CL_PREFILL_SMALL_MAX", "0")
     for preset, layers, lens in (("llama3-8b", 2, [130, 17, 256, 33, 64, 300, 129]), ("tiny-test", 2, [40, 16, 97, 31])):
         cfg = dict(oc.PRESETS[preset])

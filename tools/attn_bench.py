@@ -1,4 +1,4 @@
-"""Prefill attention microbenchmark: both kernels (0 = mma.sync, 1 = tcgen05) at Llama-3-8B head geometry.
+"""Prefill attention microbenchmark: both kernels (0 = mma.sync, 1 = wgmma) at Llama-3-8B head geometry.
     python tools/attn_bench.py [T ...]      -> one JSON line per (T, variant): ms per launch, causal TFLOP/s"""
 import json
 import sys

@@ -1,4 +1,4 @@
-// Stand-alone microbenchmark: cost of one grid-wide barrier among 148 persistent CTAs on sm_100a, idle and
+// Stand-alone microbenchmark: cost of one grid-wide barrier among persistent CTAs (one per SM, sm_90a), idle and
 // under a saturating background stream (a producer warp per CTA pulling 32 KB bulk copies, like the decode
 // megakernel).  Variants of the arrive/poll protocol are compared.  Build + run: tools/bench_barrier.sh
 #include <cuda_runtime.h>

@@ -1,7 +1,6 @@
-"""tcgen05 GEMM microbenchmark at the Llama-3-8B prefill shapes (T tokens): ms and TFLOP/s per projection.
-    CL_GEMM_MT=1|2 python tools/gemm_bench.py [T]"""
+"""wgmma GEMM microbenchmark at the Llama-3-8B prefill shapes (T tokens): ms and TFLOP/s per projection.
+    python tools/gemm_bench.py [T] [iters]"""
 import json
-import os
 import sys
 from pathlib import Path
 
@@ -21,5 +20,5 @@ for name, n, k in (("qkv", 6144, 4096), ("o", 4096, 4096), ("gate|up", 28672, 40
     _, ms = eng.op_gemm_bf16(x, w, iters=ITERS)
     fl = 2.0 * T * n * k
     tot_ms += ms; tot_fl += fl
-    print(json.dumps({"mt": os.environ.get("CL_GEMM_MT", "2"), "T": T, "iters": ITERS, "proj": name, "n": n, "k": k, "ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}), flush=True)
-print(json.dumps({"mt": os.environ.get("CL_GEMM_MT", "2"), "T": T, "layer_ms": round(tot_ms, 4), "tflops": round(tot_fl / tot_ms / 1e9, 1)}), flush=True)
+    print(json.dumps({"T": T, "iters": ITERS, "proj": name, "n": n, "k": k, "ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}), flush=True)
+print(json.dumps({"T": T, "layer_ms": round(tot_ms, 4), "tflops": round(tot_fl / tot_ms / 1e9, 1)}), flush=True)

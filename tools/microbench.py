@@ -15,7 +15,7 @@ from crowdllama_b200 import engine as eng  # noqa: E402
 
 OUT = ROOT / "gpurun_out"
 OUT.mkdir(exist_ok=True)
-HBM = 6572.2
+HBM = 3350.0   # H100 SXM data sheet, GB/s
 
 
 def emit(f, **kw):
@@ -68,7 +68,7 @@ def decode_sweep(f, preset="llama3-8b", ctx=4096, steps=128):
                 t0 = time.time()
                 # fill the cache cheaply: the prompt goes through the (slow, exact) token-wise path only
                 # for a short prefix; the rest of the context is decode steps on device
-                lg = e.prefill(s, prompt[:ctx - 64])          # tcgen05 prefill
+                lg = e.prefill(s, prompt[:ctx - 64])          # tensor-core prefill
                 t_prefill = time.time() - t0
                 ids, ms_fill = e.decode_greedy(s, int(lg.argmax()), 64)
                 t_fill = time.time() - t0
@@ -85,7 +85,7 @@ def decode_sweep(f, preset="llama3-8b", ctx=4096, steps=128):
 
 
 def gemm_sweep(f):
-    """Prefill projections on tcgen05 (cl_op_gemm_bf16, T = 4096 tokens)."""
+    """Prefill projections on wgmma (cl_op_gemm_bf16, T = 4096 tokens)."""
     rng = np.random.default_rng(0)
     T = 4096
     for name, n, k in [("qkv", 6144, 4096), ("o", 4096, 4096), ("gateup", 28672, 4096), ("down", 4096, 14336)]:
@@ -94,9 +94,9 @@ def gemm_sweep(f):
         try:
             _, ms = eng.op_gemm_bf16(x, w, iters=10)
             tf = 2.0 * T * n * k / (ms * 1e-3) / 1e12
-            emit(f, bench="gemm_tcgen05", shape=name, t=T, n=n, k=k, ms=round(ms, 4), tflops=round(tf, 1), frac_of_sustained=round(tf / 1453.9, 3))
+            emit(f, bench="gemm_wgmma", shape=name, t=T, n=n, k=k, ms=round(ms, 4), tflops=round(tf, 1), frac_of_peak=round(tf / 989.0, 3))
         except Exception as ex:  # noqa: BLE001
-            emit(f, bench="gemm_tcgen05", shape=name, error=str(ex))
+            emit(f, bench="gemm_wgmma", shape=name, error=str(ex))
 
 
 def batch_sweep(f, preset="llama3-8b", ctx=1024, steps=64):

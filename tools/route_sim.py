@@ -1,7 +1,7 @@
 """Closed-loop routing simulation behind the two-level Load rule (router.advertised_load).
 
-N identical workers, each decoding up to `max_batch` requests at once (step time grows with the batch, measured on one
-B200: 2.8 ms at B = 1, 4.6 ms at B = 32), requests of 256 tokens, a gateway that applies FindBestWorker
+N identical workers, each decoding up to `max_batch` requests at once (step time grows with the batch, fitted to one
+H100 SXM: 5.5 ms at B = 1, 7.5 ms at B = 63, 9.8 ms at B = 126), requests of 256 tokens, a gateway that applies FindBestWorker
 (manager.go:338-387: strict max of T / (1 + Load), random order) to metadata that is refreshed every `refresh` seconds.
 Prints requests/s for a set of Load thresholds: Load = 1 iff (active + queued) / max_batch >= threshold.
 
@@ -39,7 +39,7 @@ def simulate(n_workers, conc, refresh, thr, seconds, max_batch=32, gen=256, seed
             b = min(len(q), max_batch)
             if not b:
                 continue
-            acc[w] += dt / ((2.8 + 0.056 * b) * 1e-3)
+            acc[w] += dt / ((5.5 + 0.034 * b) * 1e-3)
             k = int(acc[w]); acc[w] -= k
             if k:
                 for i in range(b):
@@ -61,7 +61,7 @@ if __name__ == "__main__":
     ap.add_argument("--refresh", type=float, default=2.0)
     ap.add_argument("--seconds", type=float, default=60.0)
     a = ap.parse_args()
-    ideal = a.workers * min(32, a.concurrency / a.workers) / (256 * (2.8 + 0.056 * min(32, a.concurrency / a.workers)) * 1e-3)
+    ideal = a.workers * min(32, a.concurrency / a.workers) / (256 * (5.5 + 0.034 * min(32, a.concurrency / a.workers)) * 1e-3)
     print(f"{a.workers} workers, {a.concurrency} closed-loop clients, metadata refresh {a.refresh}s; perfectly balanced: {ideal:.1f} req/s")
     for thr in (1.0, 1.25, 1.5, 2.0, 1e9):
         r = [simulate(a.workers, a.concurrency, a.refresh, thr, a.seconds, seed=s) for s in range(3)]

@@ -1,8 +1,8 @@
-"""profiles/sass_summary.txt: per kernel, how often the SASS mnemonics that prove (or disprove) a Blackwell-native kernel
-occur — UTCHMMA / UTCBAR / LDTM / STTM (tcgen05 + TMEM), UTMALDG / UBLKCP / UBLKPF (TMA), HMMA (mma.sync), LDGSTS
-(cp.async), MUFU.EX2 — from `cuobjdump -sass` of the objects libclengine.so is linked from.
+"""Per kernel, how often the SASS mnemonics that prove (or disprove) a Hopper-native kernel occur — HGMMA / WARPGROUP
+(wgmma), UTMALDG / UBLKCP / UBLKPF (TMA), HMMA (mma.sync), LDGSTS (cp.async), MUFU.EX2 — from `cuobjdump -sass` of the
+objects libclengine.so is linked from.
 
-    python tools/sass_summary.py [profiles/sass_summary.txt]
+    python tools/sass_summary.py [sass_summary.txt]
 """
 import collections
 import re
@@ -12,7 +12,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
 OBJ = ROOT / "crowdllama_b200" / "lib" / "obj"
-PAT = ["UTCHMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UBLKCP", "UBLKPF", "HMMA", "LDGSTS", "MUFU.EX2", "SYNCS", "LDSM"]
+PAT = ["HGMMA", "WARPGROUP", "UTMALDG", "UBLKCP", "UBLKPF", "HMMA", "LDGSTS", "MUFU.EX2", "SYNCS", "LDSM"]
 
 
 def demangle(names):
@@ -21,7 +21,7 @@ def demangle(names):
 
 
 def main(dst):
-    lines = ["# SASS mnemonic counts per kernel (cuobjdump -sass of crowdllama_b200/lib/obj/*.o, sm_100a); 0 = absent; kernels without any",
+    lines = ["# SASS mnemonic counts per kernel (cuobjdump -sass of crowdllama_b200/lib/obj/*.o, sm_90a); 0 = absent; kernels without any",
              "# of these mnemonics are omitted",
              "# " + " ".join(f"{p:>8s}" for p in PAT) + "  kernel  [object]"]
     for obj in sorted(OBJ.glob("*.cu.o")):

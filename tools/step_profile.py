@@ -1,5 +1,5 @@
 """Workload for ncu: Llama-3-8B, 4096-token prefill, then a few eager (non-graph) decode steps.
-Usage under gpurun (see profiles/README.md):
+Usage (Nsight Compute on the GPU machine):
   CL_GRAPH=0 ncu --metrics gpu__time_duration.sum --clock-control none -k regex:'gemv|attn_decode|step_|embed_kernel' \
       -s 164 -c 330 --csv --log-file gpurun_out/launches.csv python tools/step_profile.py 3
 """
