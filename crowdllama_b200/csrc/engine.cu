@@ -102,8 +102,6 @@ int Engine::init(const cl_engine_config& c) {
   use_graph_ = c.use_cuda_graph >= 0 && env_int("CL_GRAPH", 1) != 0;
   use_pdl_ = env_int("CL_PDL", 1) != 0;
   pdl_early_ = env_int("CL_PDL_EARLY", 1);
-  skip_attn_ = env_int("CL_SKIP_ATTN", 0) != 0;   // timing experiments only (wrong results)
-  use_flags_ = env_int("CL_FLAGS", 0) != 0;      // measured slower than griddepcontrol.wait
   want_timeline_ = env_int("CL_TIMELINE", 0) != 0;
   gemv_variant_ = c.decode_path == 1 ? 0 : 1;
   gemv_variant_ = env_int("CL_GEMV_VARIANT", gemv_variant_);
@@ -323,7 +321,7 @@ int Engine::alloc_state() {
   DMALLOC(d_tail_cnt_, S * 4);
   DMALLOC(d_ids_ring_, (size_t)ring_steps_ * max_batch_ * 4);
   DMALLOC(d_step_counter_, 4);
-  n_sync_ = std::max(cfg.n_layers * 5 + 1 + cfg.n_layers * max_batch_, cfg.n_layers * 10 + 4);   // megakernel: 6 barriers + 4 tile counters per layer + lookahead frontier
+  n_sync_ = cfg.n_layers * 10 + 1;   // persistent kernel: 6 grid barriers + 4 tile counters per layer + the lookahead frontier
   DMALLOC(d_sync_, (size_t)n_sync_ * 4);
   CL_CUDA_OK(cudaMemsetAsync(d_sync_, 0, (size_t)n_sync_ * 4, stream_));
   if (want_timeline_) {
@@ -336,7 +334,7 @@ int Engine::alloc_state() {
                     max_batch_ <= 128;
   if (use_batch_gemm_) {
     bws_.reset(new BatchWs());
-    const size_t Bm = std::max(max_batch_, 32), widest = std::max<size_t>((size_t)qkv_dim_, std::max<size_t>(2 * (size_t)cfg.d_ff, d));   // 32 rows: the persistent batched kernel's token tile
+    const size_t Bm = max_batch_, widest = std::max<size_t>((size_t)qkv_dim_, std::max<size_t>(2 * (size_t)cfg.d_ff, d));
     DMALLOC(bws_->xn, Bm * d * 2);
     DMALLOC(bws_->attn, Bm * q_dim_ * 2);
     DMALLOC(bws_->act, Bm * (size_t)cfg.d_ff * 2);
@@ -351,37 +349,6 @@ int Engine::alloc_state() {
     }
     DMALLOC(bws_->part, part_floats * 4);
     DMALLOC(bws_->logits, Bm * (size_t)cfg.vocab_size * 4);
-    // persistent batched step: tensor maps of every weight matrix (device array) and of the three token operands
-    use_batch_mega_ = env_int("CL_BATCH_MEGA", kDefaultBatchMega) != 0 && cfg.head_dim == 128 && page_size_ == 32 && max_batch_ <= 32 &&
-                      batch_mega_supported(cfg.d_model, cfg.d_ff, cfg.head_dim, cfg.n_heads, cfg.n_kv_heads, page_size_, cfg.vocab_size);
-    if (use_batch_mega_) {
-      auto kbp = [&](int N, int K) { const int nkb = K / 64, sp = pick_splits(N, K); return (nkb + sp - 1) / sp; };
-      if (kbp(qkv_dim_, cfg.d_model) > 25 || kbp(cfg.d_model, q_dim_) > 25 || kbp(2 * cfg.d_ff, cfg.d_model) > 25 || kbp(cfg.d_model, cfg.d_ff) > 25)
-        use_batch_mega_ = false;   // a split's token operand must fit the kernel's 25 resident tiles
-    }
-    if (use_batch_mega_) {
-      std::vector<CUtensorMap> wm((size_t)cfg.n_layers * 4 + 1);
-      std::vector<BatchMegaLayer> bl(cfg.n_layers);
-      bool ok = batch_mega_prepare_device();
-      for (int l = 0; l < cfg.n_layers && ok; ++l) {
-        const auto& L = layers_[l];
-        ok = make_wmap(&wm[(size_t)l * 4 + 0], L.wqkv, qkv_dim_, cfg.d_model) && make_wmap(&wm[(size_t)l * 4 + 1], L.wo, cfg.d_model, q_dim_) &&
-             make_wmap(&wm[(size_t)l * 4 + 2], L.wgu, 2 * cfg.d_ff, cfg.d_model) && make_wmap(&wm[(size_t)l * 4 + 3], L.wdown, cfg.d_model, cfg.d_ff);
-        bl[l] = BatchMegaLayer{L.attn_norm, L.ffn_norm, kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_};
-      }
-      ok = ok && make_wmap(&wm[(size_t)cfg.n_layers * 4], lm_head_, cfg.vocab_size, cfg.d_model) &&
-           make_tmap_2d_bf16(&bm_map_xn_, bws_->xn, 32, cfg.d_model, 64, 32) && make_tmap_2d_bf16(&bm_map_attn_, bws_->attn, 32, q_dim_, 64, 32) &&
-           make_tmap_2d_bf16(&bm_map_act_, bws_->act, 32, cfg.d_ff, 64, 32);
-      if (ok) {
-        DMALLOC(d_bm_wmaps_, wm.size() * sizeof(CUtensorMap));
-        DMALLOC(d_bm_layers_, bl.size() * sizeof(BatchMegaLayer));
-        CL_CUDA_OK(cudaMemcpy(d_bm_wmaps_, wm.data(), wm.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-        CL_CUDA_OK(cudaMemcpy(d_bm_layers_, bl.data(), bl.size() * sizeof(BatchMegaLayer), cudaMemcpyHostToDevice));
-      } else {
-        fprintf(stderr, "[clengine] persistent batched decode kernel unavailable on this device / shape: using the per-kernel batched step\n");
-        use_batch_mega_ = false;
-      }
-    }
   }
   prompt_cap_ = cfg.max_seq_len;
   DMALLOC(d_prompt_, (size_t)prompt_cap_ * 4);
@@ -428,24 +395,57 @@ int Engine::ensure_capacity(cl_seq_t s, int n_tokens) {
   return CL_OK;
 }
 
+// ---- per-launch event profiler (CL_PREFILL_PROFILE, CL_STEP_PROFILE) ----------------------------
+LaunchProfiler::LaunchProfiler(cudaStream_t st, const char* env) : st_(st) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  cudaStreamIsCapturing(st, &cap);
+  on_ = env && env_int(env, 0) != 0 && cap == cudaStreamCaptureStatusNone;
+  mark("start");
+}
+
+void LaunchProfiler::mark(const char* call) {
+  if (!on_) return;
+  cudaEvent_t e;
+  cudaEventCreate(&e);
+  cudaEventRecord(e, st_);
+  ev_.push_back(e);
+  name_.push_back(call);
+}
+
+void LaunchProfiler::report(const char* tag, int key_width, const std::string& head) {
+  if (!on_ || ev_.size() < 2) return;
+  cudaStreamSynchronize(st_);
+  std::map<std::string, std::pair<double, int>> acc;
+  double total = 0.0;
+  for (size_t i = 1; i < ev_.size(); ++i) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ev_[i - 1], ev_[i]);
+    const std::string full(name_[i]);
+    std::string key = full.substr(0, full.find('('));
+    auto has = [&](const char* arg) { return full.find(arg) != std::string::npos; };
+    if (key == "launch_gemm_bf16_epi") key += has("L.wqkv") ? ":qkv+rope" : ":gate|up+silu";
+    if (key == "launch_gemm_bf16")     // split by projection: the weight argument names it
+      key += has("L.wqkv") ? ":qkv" : has("L.wo") ? ":o" : has("L.wgu") ? ":gate|up" : has("lm_head_") ? ":lm_head" : ":down";
+    acc[key].first += ms; acc[key].second += 1;
+    total += ms;
+  }
+  fprintf(stderr, "[%s] %s, %zu launches, %.3f ms on the device\n", tag, head.c_str(), ev_.size() - 1, total);
+  for (auto& kv : acc)
+    fprintf(stderr, "[%s]   %-*s n=%4d total %8.3f ms  mean %8.2f us\n", tag, key_width, kv.first.c_str(), kv.second.second, kv.second.first,
+            1e3 * kv.second.first / kv.second.second);
+  for (auto e : ev_) cudaEventDestroy(e);
+  ev_.clear(); name_.clear();
+}
+
 // ---- one token step for the sequences listed in d_slots_[0..B) -----------------------------------
-int Engine::enqueue_step(int B, bool tail) {
-  if (B >= 2 && tail && use_batch_mega_ && have_kv_maps_ && bws_) return enqueue_step_batch_mega(B);
-  if (B >= batch_gemm_min_ && tail && use_batch_gemm_ && bws_) return enqueue_step_batched(B);   // from B = 2: faster than two GEMV passes
+int Engine::enqueue_step(int B) {
+  if (B >= batch_gemm_min_ && use_batch_gemm_ && bws_) return enqueue_step_batched(B);   // from B = 2: faster than two GEMV passes
   const int d = cfg.d_model, F = cfg.d_ff, L_ = cfg.n_layers;
-  int n = 0, r;
-#define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } n += r; } while (0)
-  // StepSync: counter-based dependencies inside the step (kernels.h).  Only with PDL (the consumers must
-  // already be resident to profit) and never for the first kernel after embed / the tail (stream order).
-  const bool flags = use_flags_ && use_pdl_;
-  const bool defer_combine = flags && gemv_variant_ == 1 && gemv_variant_supported(1, d, q_dim_) && nsplit_ <= 32 &&
-                             (q_dim_ + sm_count() - 1) / sm_count() <= 64;
-  auto cnt = [&](int l, int k) -> unsigned* { return flags ? d_sync_ + (size_t)l * 5 + k : nullptr; };
+  int launches = 0;
+  LaunchProfiler prof(stream_, nullptr);
   auto tl = [&](int l, int k) -> long long* { return d_timeline_ ? d_timeline_ + ((size_t)l * 5 + k) * 4 : nullptr; };
-  const unsigned* prev_cnt = nullptr;
-  int prev_n = 0, nc = 0;
   CL_LAUNCH(launch_embed(embed_, d, d_tok_, d_h_, d, d_slots_, B, stream_));
-  const bool mega = use_mega_ && B == 1 && !skip_attn_ && d_mega_layers_ != nullptr;
+  const bool mega = use_mega_ && B == 1 && d_mega_layers_ != nullptr;
   if (probe_ev_) cudaEventRecord(probe_ev_[probe_idx_], stream_);
   if (mega) {
     MegaArgs m;
@@ -466,9 +466,8 @@ int Engine::enqueue_step(int B, bool tail) {
     g.qkv.rope = rope_; g.qkv.pos = d_pos_; g.qkv.block_tables = d_bt_; g.qkv.bt_stride = max_pages_per_seq_;
     g.qkv.kpool = kpool_ + (size_t)l * kv_layer_elems_; g.qkv.vpool = vpool_ + (size_t)l * kv_layer_elems_;
     g.qkv.n_heads = cfg.n_heads; g.qkv.n_kv = cfg.n_kv_heads; g.qkv.head_dim = cfg.head_dim; g.qkv.page_size = page_size_;
-    g.sync.wait = prev_cnt; g.sync.n_wait = (unsigned)prev_n; g.sync.signal = cnt(l, 0); g.tl = tl(l, 0);
-    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_QKV, true, g, stream_, use_pdl_, &nc));
-    prev_cnt = cnt(l, 0); prev_n = nc;
+    g.tl = tl(l, 0);
+    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_QKV, true, g, stream_, use_pdl_));
     // (2) paged GQA attention over tokens 0..pos
     AttnDecodeArgs a;
     a.q = d_q_; a.q_stride = q_dim_;
@@ -476,58 +475,51 @@ int Engine::enqueue_step(int B, bool tail) {
     a.block_tables = d_bt_; a.bt_stride = max_pages_per_seq_; a.pos = d_pos_;
     a.out = d_attn_; a.out_stride = q_dim_; a.part = d_attn_part_; a.counters = d_attn_cnt_;
     a.slots = d_slots_; a.batch = B; a.n_heads = cfg.n_heads; a.n_kv = cfg.n_kv_heads; a.head_dim = cfg.head_dim;
-    a.page_size = page_size_; a.nsplit = nsplit_; a.pdl_early = pdl_early_;
-    a.sync.wait = prev_cnt; a.sync.n_wait = (unsigned)prev_n;
-    a.sync.signal = defer_combine ? cnt(l, 1) : nullptr; a.tl = tl(l, 1);
-    if (!skip_attn_) CL_LAUNCH(launch_attn_decode(a, stream_, use_pdl_));
-    // (3) o projection + residual (prologue: cross-split combine of the attention partials when deferred)
+    a.page_size = page_size_; a.nsplit = nsplit_; a.pdl_early = pdl_early_; a.tl = tl(l, 1);
+    CL_LAUNCH(launch_attn_decode(a, stream_, use_pdl_));
+    // (3) o projection + residual
     GemvArgs o;
     o.slots = d_slots_; o.batch = B; o.pdl_early = pdl_early_;
-    o.W = L.wo; o.N = d; o.K = q_dim_; o.x = d_attn_; o.x_stride = q_dim_; o.y = d_h_; o.resid = d_h_; o.y_stride = d;
-    if (defer_combine && !skip_attn_) {
-      o.sync.wait = cnt(l, 1); o.sync.n_wait = (unsigned)(cfg.n_kv_heads * nsplit_ * B);
-      o.comb.part = d_attn_part_; o.comb.nsplit = nsplit_; o.comb.n_kv = cfg.n_kv_heads; o.comb.rep = cfg.n_heads / cfg.n_kv_heads;
-      o.comb.head_dim = cfg.head_dim; o.comb.x_out = d_attn_; o.comb.phase = d_sync_ + (size_t)L_ * 5 + 1 + (size_t)l * max_batch_;
-    } else {
-      // the attention kernel combined in-kernel and publishes nothing: fall back to grid completion
-      o.sync.wait = nullptr;
-    }
-    o.sync.signal = cnt(l, 2); o.tl = tl(l, 2);
-    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_RESID, false, o, stream_, use_pdl_, &nc));
-    prev_cnt = cnt(l, 2); prev_n = nc;
+    o.W = L.wo; o.N = d; o.K = q_dim_; o.x = d_attn_; o.x_stride = q_dim_; o.y = d_h_; o.resid = d_h_; o.y_stride = d; o.tl = tl(l, 2);
+    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_RESID, false, o, stream_, use_pdl_));
     // (4) RMSNorm + gate/up + SiLU*mul
     GemvArgs u;
     u.slots = d_slots_; u.batch = B; u.pdl_early = pdl_early_;
     u.W = L.wgu; u.N = 2 * F; u.K = d; u.h = d_h_; u.gain = L.ffn_norm; u.eps = cfg.rms_eps; u.y = d_act_;
-    u.x_stride = d; u.y_stride = F;
-    u.sync.wait = prev_cnt; u.sync.n_wait = (unsigned)prev_n; u.sync.signal = cnt(l, 3); u.tl = tl(l, 3);
-    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_GATEUP, true, u, stream_, use_pdl_, &nc));
-    prev_cnt = cnt(l, 3); prev_n = nc;
+    u.x_stride = d; u.y_stride = F; u.tl = tl(l, 3);
+    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_GATEUP, true, u, stream_, use_pdl_));
     // (5) down projection + residual
     GemvArgs w;
     w.slots = d_slots_; w.batch = B; w.pdl_early = pdl_early_;
-    w.W = L.wdown; w.N = d; w.K = F; w.x = d_act_; w.x_stride = F; w.y = d_h_; w.resid = d_h_; w.y_stride = d;
-    w.sync.wait = prev_cnt; w.sync.n_wait = (unsigned)prev_n; w.sync.signal = cnt(l, 4); w.tl = tl(l, 4);
-    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_RESID, false, w, stream_, use_pdl_, &nc));
-    prev_cnt = cnt(l, 4); prev_n = nc;
+    w.W = L.wdown; w.N = d; w.K = F; w.x = d_act_; w.x_stride = F; w.y = d_h_; w.resid = d_h_; w.y_stride = d; w.tl = tl(l, 4);
+    CL_LAUNCH(launch_gemv(gemv_variant_, EPI_RESID, false, w, stream_, use_pdl_));
   }
   if (probe_ev_) cudaEventRecord(probe_ev_[probe_idx_ + 1], stream_);
+  CL_LAUNCH(enqueue_lm_head(B, use_pdl_ && !mega));
+  CL_LAUNCH(enqueue_step_tail(B));
+  return launches;
+}
+
+// The LM head of a single-slot step or prefill: final RMSNorm + GEMV of d_h_ into d_logits_.
+int Engine::enqueue_lm_head(int B, bool pdl) {
   GemvArgs lm;
   lm.slots = d_slots_; lm.batch = B; lm.pdl_early = pdl_early_;
-  lm.W = lm_head_; lm.N = cfg.vocab_size; lm.K = d; lm.h = d_h_; lm.gain = final_norm_; lm.eps = cfg.rms_eps;
-  lm.y = d_logits_; lm.x_stride = d; lm.y_stride = cfg.vocab_size;
-  lm.sync.wait = prev_cnt; lm.sync.n_wait = (unsigned)prev_n; lm.tl = tl(L_, 0);
-  CL_LAUNCH(launch_gemv(gemv_variant_, EPI_STORE, true, lm, stream_, use_pdl_ && !mega));
-  if (tail) {
-    StepTailArgs t;
-    t.logits = d_logits_; t.vocab = cfg.vocab_size; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
-    t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
-    t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = B;
-    t.sync_counters = d_sync_; t.n_sync_counters = n_sync_;
-    CL_LAUNCH(launch_step_tail(t, stream_));
-  }
-#undef CL_LAUNCH
-  return n;
+  lm.W = lm_head_; lm.N = cfg.vocab_size; lm.K = cfg.d_model; lm.h = d_h_; lm.gain = final_norm_; lm.eps = cfg.rms_eps;
+  lm.y = d_logits_; lm.x_stride = cfg.d_model; lm.y_stride = cfg.vocab_size;
+  lm.tl = d_timeline_ ? d_timeline_ + (size_t)cfg.n_layers * 5 * 4 : nullptr;
+  return launch_gemv(gemv_variant_, EPI_STORE, true, lm, stream_, pdl);
+}
+
+// The tail of every decode step and prefill: greedy id of d_logits_ for d_slots_[0..B) into d_tok_ and the id ring,
+// d_pos_ += 1.  It also zeroes the persistent kernel's counters.  They are zero whenever no step is running, so the
+// zeroing is needed only behind the persistent kernel and harmless everywhere else.
+int Engine::enqueue_step_tail(int B) {
+  StepTailArgs t;
+  t.logits = d_logits_; t.vocab = cfg.vocab_size; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
+  t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
+  t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = B;
+  t.sync_counters = d_sync_; t.n_sync_counters = n_sync_;
+  return launch_step_tail(t, stream_);
 }
 
 // ---- batched token step (B >= 2): tensor-core projections (wgmma, split-K) + per-sequence glue -----
@@ -552,58 +544,10 @@ static int pick_splits(int n_rows, int K) {
   return 1;
 }
 
-// ---- batched token step as ONE persistent kernel (decode_mega_batch.cu): embed -> kernel (all layers + LM head) -> tail
-int Engine::enqueue_step_batch_mega(int B) {
-  int n = 0, r;
-#define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } n += r; } while (0)
-  const int d = cfg.d_model, F = cfg.d_ff, V = cfg.vocab_size;
-  CL_LAUNCH(launch_embed(embed_, d, d_tok_, d_h_, d, d_slots_, B, stream_));
-  BatchMegaArgs m;
-  m.layers = d_bm_layers_; m.wmaps = d_bm_wmaps_; m.n_layers = cfg.n_layers; m.B = B; m.n_kv = cfg.n_kv_heads;
-  m.nsplit = std::max(1, std::min(std::min(nsplit_, 32), sm_count() / (cfg.n_kv_heads * B)));
-  m.q_dim = q_dim_; m.qkv_dim = qkv_dim_; m.vocab = V;
-  m.s_qkv = pick_splits(qkv_dim_, d); m.s_o = pick_splits(d, q_dim_); m.s_gu = pick_splits(2 * F, d); m.s_dn = pick_splits(d, F);
-  m.eps = cfg.rms_eps; m.rope = rope_; m.pos = d_pos_; m.block_tables = d_bt_; m.bt_stride = max_pages_per_seq_; m.slots = d_slots_;
-  m.h = d_h_; m.xn = bws_->xn; m.attn = bws_->attn; m.act = bws_->act; m.part = bws_->part; m.att_part = d_attn_part_; m.att_cnt = d_attn_cnt_;
-  m.logits = d_logits_; m.final_norm = final_norm_; m.bars = d_sync_;
-  m.kv_layer_rows = (long long)n_pages_ * cfg.n_kv_heads * page_size_;
-  m.tl = d_timeline_;
-  m.max_flight = env_int("CL_BMEGA_MAX_FLIGHT", 4); m.pause_in_barrier = env_int("CL_BMEGA_PAUSE", 1);
-  m.map_xn = bm_map_xn_; m.map_attn = bm_map_attn_; m.map_act = bm_map_act_; m.kmap = kmap_; m.vmap = vmap_;
-  CL_LAUNCH(launch_decode_mega_batch(m, stream_));
-  CL_LAUNCH(launch_gemm_bf16(bws_->xn, lm_head_, bws_->logits, nullptr, B, V, d, stream_, 1, false));
-  CL_LAUNCH(launch_batch_scatter_rows(bws_->logits, V, d_logits_, V, d_slots_, B, stream_));
-  StepTailArgs t;
-  t.logits = d_logits_; t.vocab = V; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
-  t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
-  t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = B;
-  t.sync_counters = d_sync_; t.n_sync_counters = n_sync_;
-  CL_LAUNCH(launch_step_tail(t, stream_));
-#undef CL_LAUNCH
-  return n;
-}
-
 int Engine::enqueue_step_batched(int B) {
   const int d = cfg.d_model, F = cfg.d_ff, L_ = cfg.n_layers, V = cfg.vocab_size;
-  int n = 0, r;
-  // CL_STEP_PROFILE=1 (eager launches only, CL_GRAPH=0): a CUDA event after every launch; per-kernel-class device time of
-  // the step — gap before the kernel included — goes to stderr
-  const bool prof_env = env_int("CL_STEP_PROFILE", 0) != 0;
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(stream_, &cap);
-  const bool prof = prof_env && cap == cudaStreamCaptureStatusNone;
-  std::vector<cudaEvent_t> pev;
-  std::vector<const char*> pname;
-  auto mark = [&](const char* name) {
-    if (!prof) return;
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, stream_);
-    pev.push_back(e);
-    pname.push_back(name);
-  };
-  mark("start");
-#define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } n += r; mark(#call); } while (0)
+  int launches = 0;
+  LaunchProfiler prof(stream_, "CL_STEP_PROFILE");   // eager launches only (CL_GRAPH=0)
   BatchWs& w = *bws_;
   static const int batch_attn_ctas = env_int("CL_BATCH_ATTN_CTAS", sm_count());
   static const bool bpdl_env = env_int("CL_BATCH_PDL", 1) != 0;
@@ -644,33 +588,9 @@ int Engine::enqueue_step_batched(int B) {
   CL_LAUNCH(launch_batch_resid_norm(d_h_, d, pending, pending_s, B, final_norm_, cfg.rms_eps, w.xn, d_slots_, stream_, bp));
   CL_LAUNCH(launch_gemm_bf16(w.xn, lm_head_, w.logits, nullptr, B, V, d, stream_, 1, bp));
   CL_LAUNCH(launch_batch_scatter_rows(w.logits, V, d_logits_, V, d_slots_, B, stream_));
-  StepTailArgs t;
-  t.logits = d_logits_; t.vocab = V; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
-  t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
-  t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = B;
-  t.sync_counters = d_sync_; t.n_sync_counters = n_sync_;
-  CL_LAUNCH(launch_step_tail(t, stream_));
-#undef CL_LAUNCH
-  if (prof && pev.size() > 1) {
-    cudaStreamSynchronize(stream_);
-    std::map<std::string, std::pair<double, int>> acc;
-    double total = 0.0;
-    for (size_t i = 1; i < pev.size(); ++i) {
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, pev[i - 1], pev[i]);
-      const std::string full(pname[i]);
-      std::string key = full.substr(0, full.find('('));
-      if (key == "launch_gemm_bf16")
-        key += full.find("L.wqkv") != std::string::npos ? ":qkv" : full.find("L.wo") != std::string::npos ? ":o" : full.find("L.wgu") != std::string::npos ? ":gate|up"
-               : full.find("lm_head_") != std::string::npos ? ":lm_head" : ":down";
-      acc[key].first += ms; acc[key].second += 1;
-      total += ms;
-    }
-    fprintf(stderr, "[step profile] B=%d, %zu launches, %.3f ms on the device\n", B, pev.size() - 1, total);
-    for (auto& kv : acc) fprintf(stderr, "[step profile]   %-34s n=%4d total %8.3f ms  mean %8.2f us\n", kv.first.c_str(), kv.second.second, kv.second.first, 1e3 * kv.second.first / kv.second.second);
-    for (auto e : pev) cudaEventDestroy(e);
-  }
-  return n;
+  CL_LAUNCH(enqueue_step_tail(B));
+  prof.report("step profile", 34, "B=" + std::to_string(B));
+  return launches;
 }
 
 // Capture + instantiate + upload the step graph of batch size B (no launch).  Returns true if graphs_[B] exists afterwards.
@@ -681,7 +601,7 @@ bool Engine::ensure_graph(int B) {
     cudaGraph_t g = nullptr;
     cudaGraphExec_t ex = nullptr;
     cudaError_t e = cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal);
-    int n = e == cudaSuccess ? enqueue_step(B, true) : -1;
+    int n = e == cudaSuccess ? enqueue_step(B) : -1;
     cudaError_t e2 = cudaStreamEndCapture(stream_, &g);
     if (e == cudaSuccess && n > 0 && e2 == cudaSuccess && g) e = cudaGraphInstantiate(&ex, g, 0);
     else e = cudaErrorUnknown;
@@ -725,7 +645,7 @@ int Engine::run_step_graph(int B) {
       return CL_OK;
     }
   }
-  const int n = enqueue_step(B, true);
+  const int n = enqueue_step(B);
   if (n < 0) return n;
   launches_ += n;
   return CL_OK;
@@ -950,7 +870,7 @@ int Engine::time_dominant_kernel(cl_seq_t s, int32_t first_id, int n_steps, floa
   CL_CUDA_OK(cudaEventRecord(ev[2 * n_steps], stream_));
   for (int i = 0; i < n_steps && rc == CL_OK; ++i) {
     probe_idx_ = 2 * i;
-    const int n = enqueue_step(1, true);
+    const int n = enqueue_step(1);
     if (n < 0) rc = n; else launches_ += n;
   }
   probe_ev_ = nullptr;

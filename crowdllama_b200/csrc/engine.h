@@ -25,7 +25,6 @@ constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts
 constexpr int kDefaultPrefillFused = 1;         // CL_PREFILL_FUSED bit mask: 1 = SiLU*mul, 2 = RoPE + cache scatter (correct, measured slower) fused into the prefill GEMM epilogues
 constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi)
 constexpr int kDefaultSchedLingerUs = 1000;     // CL_SCHED_LINGER_US: with an empty batch, keep collecting while requests arrive within this gap (max 8x in total)
-constexpr int kDefaultBatchMega = 0;            // CL_BATCH_MEGA: persistent batched decode kernel for B >= 2
 
 void set_last_error(const std::string& s);
 const char* get_last_error();
@@ -37,6 +36,33 @@ const char* get_last_error();
       ::cl::set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                   \
       return CL_ERR_CUDA;                                                                         \
     }                                                                                             \
+  } while (0)
+
+// CL_PREFILL_PROFILE / CL_STEP_PROFILE = 1 (eager launches only): a CUDA event after every launch; report() prints the
+// device time per kernel class, gap before each kernel included, to stderr.  Off while the stream is being captured.
+class LaunchProfiler {
+ public:
+  LaunchProfiler(cudaStream_t st, const char* env);   // env == nullptr: never on
+  void mark(const char* call);                        // call: the launcher expression, its name up to '(' is the class
+  void report(const char* tag, int key_width, const std::string& head);   // "[tag] head, N launches, T ms on the device"
+
+ private:
+  bool on_ = false;
+  cudaStream_t st_ = nullptr;
+  std::vector<cudaEvent_t> ev_;
+  std::vector<const char*> name_;
+};
+
+// Enqueue one launcher call (kernels.h) inside an Engine member that keeps `int launches` and `LaunchProfiler prof`.
+#define CL_LAUNCH(call)                                                                                     \
+  do {                                                                                                      \
+    const int r_ = (call);                                                                                  \
+    if (r_ < 0) {                                                                                           \
+      ::cl::set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError()));             \
+      return CL_ERR_CUDA;                                                                                   \
+    }                                                                                                       \
+    launches += r_;                                                                                         \
+    prof.mark(#call);                                                                                       \
   } while (0)
 
 // ---- paged-KV allocator: host-side free list + per-owner page lists (no GPU needed) -----------
@@ -186,8 +212,10 @@ class Engine {
   int fill_synthetic(uint64_t seed);
   int alloc_state();
   int ensure_capacity(cl_seq_t s, int n_tokens);  // reserve pages + upload block table row
-  int enqueue_step(int B, bool tail);              // kernels of one token step for d_slots_[0..B)
+  int enqueue_step(int B);                         // kernels of one token step for d_slots_[0..B)
   int enqueue_step_batched(int B);                 // B >= 2: wgmma projections + per-sequence glue kernels
+  int enqueue_lm_head(int B, bool pdl);            // final norm + LM-head GEMV of d_h_ -> d_logits_ for d_slots_[0..B)
+  int enqueue_step_tail(int B);                    // argmax of d_logits_, advance tok / pos, id ring (step_tail_kernel)
   int run_step_graph(int B);
   bool ensure_graph(int B);
   void precapture_graphs();                       // graph launch (or eager enqueue)
@@ -208,14 +236,14 @@ class Engine {
   bool sched_multi_prefill_ = false;       // group admission through prefill_multi (CL_SCHED_MULTI_PREFILL)
   int page_size_ = 32, max_batch_ = 8, max_seqs_ = 8, n_pages_ = 0, max_pages_per_seq_ = 0;
   int gemv_variant_ = 1, nsplit_ = 16;
-  bool use_graph_ = true, use_pdl_ = true, skip_attn_ = false;
+  bool use_graph_ = true, use_pdl_ = true;
   int pdl_early_ = 1;
-  bool use_flags_ = false, want_timeline_ = false, use_mega_ = false;
+  bool want_timeline_ = false, use_mega_ = false;
   MegaLayer* d_mega_layers_ = nullptr;
   CUtensorMap kmap_{}, vmap_{};
   bool have_kv_maps_ = false;
   long long* d_timeline_ = nullptr;
-  unsigned* d_sync_ = nullptr;
+  unsigned* d_sync_ = nullptr;             // the persistent kernel's counters (MegaArgs: bars, tile_ctr, pf_ctr)
   int n_sync_ = 0;
   int qkv_dim_ = 0, q_dim_ = 0, kv_dim_ = 0;
 
@@ -259,12 +287,6 @@ class Engine {
   struct BatchWs { __nv_bfloat16* xn = nullptr; __nv_bfloat16* attn = nullptr; __nv_bfloat16* act = nullptr; float* part = nullptr; float* logits = nullptr; };
   std::unique_ptr<BatchWs> bws_;
   bool use_batch_gemm_ = false;
-  // persistent batched step (decode_mega_batch.cu)
-  bool use_batch_mega_ = false;
-  BatchMegaLayer* d_bm_layers_ = nullptr;
-  CUtensorMap* d_bm_wmaps_ = nullptr;
-  CUtensorMap bm_map_xn_{}, bm_map_attn_{}, bm_map_act_{};
-  int enqueue_step_batch_mega(int B);
   int batch_gemm_min_ = 2;
   int prefill_chunk_tokens_ = 4096;
 

@@ -89,7 +89,7 @@ struct StepTailArgs {                // argmax over logits, advance the sequence
   int* pos = nullptr;                // [slot] incremented
   int* ids_ring = nullptr;           // [ring_steps][max_batch] generated ids
   int* step_counter = nullptr;       // device scalar, incremented once per step
-  unsigned* sync_counters = nullptr; // zeroed at the end of every step (StepSync)
+  unsigned* sync_counters = nullptr; // zeroed at the end of every step (MegaArgs: bars, tile_ctr, pf_ctr)
   int n_sync_counters = 0;
   int ring_steps = 0, ring_stride = 0;
   float* part_val = nullptr;         // [slot][nblk]
@@ -162,44 +162,6 @@ bool make_tmap_2d_bf16(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_
 bool mega_supported(int d, int d_ff, int head_dim, int n_heads, int n_kv, int page_size, int nsplit);
 bool mega_prepare_device();   // per device: shared-memory opt-in + "one CTA per SM fits" (call with the device current)
 int launch_decode_mega(const MegaArgs& a, cudaStream_t st);
-
-// ---- persistent BATCHED decode step (decode_mega_batch.cu): B = 2..32 sequences, Llama-3-8B / Mistral-7B layer shape ----
-struct BatchMegaLayer { const float* attn_norm; const float* ffn_norm; __nv_bfloat16* kpool; __nv_bfloat16* vpool; };
-struct BatchMegaArgs {
-  const BatchMegaLayer* layers = nullptr;  // device array [n_layers]
-  const CUtensorMap* wmaps = nullptr;      // device array [n_layers * 4 + 1]: q|k|v, o, gate|up, down per layer, then the LM head
-  int n_layers = 0, B = 0, n_kv = 0, nsplit = 1, q_dim = 0, qkv_dim = 0, vocab = 0;
-  int s_qkv = 1, s_o = 1, s_gu = 1, s_dn = 1;   // k splits of the four projections (engine.cu pick_splits)
-  float eps = 0.f;
-  const float2* rope = nullptr;
-  const int* pos = nullptr;                // [slot]
-  const int* block_tables = nullptr;       // [slot][bt_stride]
-  int bt_stride = 0;
-  const int* slots = nullptr;              // [B]
-  float* h = nullptr;                      // [slot][d] residual stream
-  __nv_bfloat16* xn = nullptr;             // [32][d]    normalised rows (X of q|k|v, gate|up, LM head)
-  __nv_bfloat16* attn = nullptr;           // [32][q_dim] attention output (X of o)
-  __nv_bfloat16* act = nullptr;            // [32][d_ff] SwiGLU activation (X of down)
-  float* part = nullptr;                   // split-K partials [s][32][N]
-  float* att_part = nullptr;               // attention split partials [slot][n_kv][nsplit][4][130]
-  unsigned* att_cnt = nullptr;             // [slot][n_kv] self re-arming arrival counters
-  float* logits = nullptr;                 // [slot][vocab]
-  const float* final_norm = nullptr;
-  unsigned* bars = nullptr;                // [n_layers * 8 + 1] grid-barrier counters, zero at kernel start
-  long long kv_layer_rows = 0;
-  int max_flight = 4;                      // 16 KB bulk copies in flight per CTA (<= ring slots); 0 = no cap
-  int pause_in_barrier = 1;                // no new copy while this CTA's consumers sit in a grid barrier
-  long long* tl = nullptr;                 // debug (CL_TIMELINE=1): [n_layers][16] globaltimer stamps of CTA 0 at phase ends / barrier exits
-  alignas(64) CUtensorMap map_xn;          // [32][d] box {64, 32}
-  alignas(64) CUtensorMap map_attn;
-  alignas(64) CUtensorMap map_act;
-  alignas(64) CUtensorMap kmap;            // pool-wide K / V maps, box {64, 32}
-  alignas(64) CUtensorMap vmap;
-};
-bool batch_mega_supported(int d, int d_ff, int head_dim, int n_heads, int n_kv, int page_size, int vocab);
-bool batch_mega_prepare_device();
-bool make_wmap(CUtensorMap* map, const void* W, int N, int K);
-int launch_decode_mega_batch(const BatchMegaArgs& a, cudaStream_t st);
 
 bool gemv_variant_supported(int variant, int N, int K);
 int sm_count();

@@ -6,7 +6,6 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -26,48 +25,6 @@ bool Engine::prefill_path_ok() const {
 
 // split-K rule shared with the batched decode step (engine.cu)
 int pick_splits_public(int n_rows, int K);
-
-// CL_PREFILL_PROFILE=1: a CUDA event after every launch, per-kernel-class device time printed to stderr (in-pipeline
-// times incl. the gap before each kernel; the ncu launch list measures cold, serialised launches instead).
-struct PrefillProfiler {
-  bool on;
-  cudaStream_t st;
-  std::vector<cudaEvent_t> ev;
-  std::vector<const char*> name;
-  explicit PrefillProfiler(cudaStream_t s) : st(s) {
-    static const bool prof = getenv("CL_PREFILL_PROFILE") && atoi(getenv("CL_PREFILL_PROFILE")) != 0;
-    on = prof;
-  }
-  void mark(const char* n) {
-    if (!on) return;
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, st);
-    ev.push_back(e);
-    name.push_back(n);
-  }
-  void report(int n_tokens, const char* path) {
-    if (!on || ev.size() < 2) return;
-    cudaStreamSynchronize(st);
-    std::map<std::string, std::pair<double, int>> acc;
-    double total = 0.0;
-    for (size_t i = 1; i < ev.size(); ++i) {
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, ev[i - 1], ev[i]);
-      const std::string full(name[i]);
-      std::string key = full.substr(0, full.find('('));
-      if (key == "launch_gemm_bf16_epi") key += full.find("L.wqkv") != std::string::npos ? ":qkv+rope" : ":gate|up+silu";
-      if (key == "launch_gemm_bf16")     // split by projection: the weight argument names it
-        key += full.find("L.wqkv") != std::string::npos ? ":qkv" : full.find("L.wo") != std::string::npos ? ":o" : full.find("L.wgu") != std::string::npos ? ":gate|up" : ":down";
-      acc[key].first += ms; acc[key].second += 1;
-      total += ms;
-    }
-    fprintf(stderr, "[prefill profile] %s path, %d tokens, %zu launches, %.3f ms on the device\n", path, n_tokens, ev.size() - 1, total);
-    for (auto& kv : acc) fprintf(stderr, "[prefill profile]   %-32s n=%4d total %8.3f ms  mean %8.2f us\n", kv.first.c_str(), kv.second.second, kv.second.first, 1e3 * kv.second.first / kv.second.second);
-    for (auto e : ev) cudaEventDestroy(e);
-    ev.clear(); name.clear();
-  }
-};
 
 // Short prompts (prefill_min_tokens_ <= n <= 256, e.g. a 128-token chat): one token tile per W row tile means only
 // N/128 CTAs stream the weights of a projection (48 for q|k|v, 32 for o and down), far below the
@@ -105,14 +62,12 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   SmallPrefillWs& w = *sws_;
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
   const int* bt = d_bt_ + (size_t)s * max_pages_per_seq_;
-  int launches = 0, r;
-  PrefillProfiler pp(stream_);
-#define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } launches += r; pp.mark(#call); } while (0)
+  int launches = 0;
   // programmatic dependent launch between the GEMMs and the per-row glue kernels, as in the batched decode step (the two
   // prefill kernels in between are launched normally and order the stream)
   static const bool small_pdl = !getenv("CL_SMALL_PDL") || atoi(getenv("CL_SMALL_PDL")) != 0;
   const bool bp = small_pdl && use_pdl_;
-  pp.mark("start");
+  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
   CL_LAUNCH(launch_embed_rows(embed_, d, d_prompt_, w.h, T, stream_));
   const float* pending = nullptr;   // split-K partials of the previous residual projection, folded in by the next norm
   int pending_s = 0;
@@ -144,18 +99,9 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &last_pos, 4, cudaMemcpyHostToDevice, stream_));
   rc = set_single_slot(s);
   if (rc) return rc;
-  GemvArgs lm;
-  lm.slots = d_slots_; lm.batch = 1;
-  lm.W = lm_head_; lm.N = cfg.vocab_size; lm.K = d; lm.h = d_h_; lm.gain = final_norm_; lm.eps = cfg.rms_eps;
-  lm.y = d_logits_; lm.x_stride = d; lm.y_stride = cfg.vocab_size;
-  CL_LAUNCH(launch_gemv(gemv_variant_, EPI_STORE, true, lm, stream_, false));
-  StepTailArgs t;
-  t.logits = d_logits_; t.vocab = cfg.vocab_size; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
-  t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
-  t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = 1;
-  CL_LAUNCH(launch_step_tail(t, stream_));
-#undef CL_LAUNCH
-  pp.report(n, "short-prompt");
+  CL_LAUNCH(enqueue_lm_head(1, false));
+  CL_LAUNCH(enqueue_step_tail(1));
+  prof.report("prefill profile", 32, "short-prompt path, " + std::to_string(n) + " tokens");
   launches_ += launches;
   q.len += n;
   q.history.insert(q.history.end(), ids, ids + n);
@@ -201,10 +147,8 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
   const bool fused_silu = (prefill_fused_ & 1) != 0, fused_rope = (prefill_fused_ & 2) != 0;   // CL_PREFILL_FUSED bit mask
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
   const int* bt = d_bt_ + (size_t)s * max_pages_per_seq_;
-  int launches = 0, r;
-  PrefillProfiler pp(stream_);
-#define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } launches += r; pp.mark(#call); } while (0)
-  pp.mark("start");
+  int launches = 0;
+  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
   for (int c0 = 0; c0 < n; c0 += w.cap_tokens) {
     const int T = std::min(w.cap_tokens, n - c0);
     const int pos0 = q.len + c0;
@@ -251,18 +195,9 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
   CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &last_pos, 4, cudaMemcpyHostToDevice, stream_));
   rc = set_single_slot(s);
   if (rc) return rc;
-  GemvArgs lm;
-  lm.slots = d_slots_; lm.batch = 1;
-  lm.W = lm_head_; lm.N = cfg.vocab_size; lm.K = d; lm.h = d_h_; lm.gain = final_norm_; lm.eps = cfg.rms_eps;
-  lm.y = d_logits_; lm.x_stride = d; lm.y_stride = cfg.vocab_size;
-  CL_LAUNCH(launch_gemv(gemv_variant_, EPI_STORE, true, lm, stream_, false));
-  StepTailArgs t;
-  t.logits = d_logits_; t.vocab = cfg.vocab_size; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
-  t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
-  t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = 1;
-  CL_LAUNCH(launch_step_tail(t, stream_));
-#undef CL_LAUNCH
-  pp.report(n, "tile");
+  CL_LAUNCH(enqueue_lm_head(1, false));
+  CL_LAUNCH(enqueue_step_tail(1));
+  prof.report("prefill profile", 32, "tile path, " + std::to_string(n) + " tokens");
   launches_ += launches;
   q.len += n;
   q.history.insert(q.history.end(), ids, ids + n);
@@ -310,10 +245,8 @@ int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* 
     pos0[i] = seqs_[ss[i]].len;
   }
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, all.data(), (size_t)total * 4, cudaMemcpyHostToDevice, stream_));
-  int launches = 0, r;
-  PrefillProfiler pp(stream_);
-#define CL_LAUNCH(call) do { r = (call); if (r < 0) { set_last_error(std::string(#call) + ": " + cudaGetErrorString(cudaGetLastError())); return CL_ERR_CUDA; } launches += r; pp.mark(#call); } while (0)
-  pp.mark("start");
+  int launches = 0;
+  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
   const int T = total;
   CL_LAUNCH(launch_embed_rows(embed_, d, d_prompt_, w.h, T, stream_));
   for (int l = 0; l < cfg.n_layers; ++l) {
@@ -363,13 +296,8 @@ int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* 
   CL_LAUNCH(launch_batch_resid_norm(d_h_, d, nullptr, 0, n_seqs, final_norm_, cfg.rms_eps, bw.xn, d_slots_, stream_, false));
   CL_LAUNCH(launch_gemm_bf16(bw.xn, lm_head_, bw.logits, nullptr, n_seqs, V, d, stream_, 1, false));
   CL_LAUNCH(launch_batch_scatter_rows(bw.logits, V, d_logits_, V, d_slots_, n_seqs, stream_));
-  StepTailArgs t;
-  t.logits = d_logits_; t.vocab = V; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
-  t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
-  t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = n_seqs;
-  CL_LAUNCH(launch_step_tail(t, stream_));
-#undef CL_LAUNCH
-  pp.report(total, "multi-prompt tile");
+  CL_LAUNCH(enqueue_step_tail(n_seqs));
+  prof.report("prefill profile", 32, "multi-prompt tile path, " + std::to_string(total) + " tokens");
   launches_ += launches;
   for (int i = 0; i < n_seqs; ++i) {
     auto& q = seqs_[ss[i]];

@@ -205,18 +205,15 @@ def test_llama3_8b_full_batched_b8_long_context():
 
 # ---- 4 layers at full width: more batch shapes for the same oracle budget ----------------------------------------
 @pytest.mark.parametrize("B", [2, 3, 16])
-@pytest.mark.parametrize("persistent", ["0", "1"])
-def test_llama3_8b_layers_batched_long_context(persistent, B):
+def test_llama3_8b_layers_batched_long_context(B):
     """B = 2, 3 and 16 (tensor-core path: KV splits 9, 6 and 1 per sequence) at
-    Llama-3-8B layer shapes, contexts up to 8188 tokens, 1-token and page-boundary sequences.  persistent = 1: the
-    whole batched step as one persistent kernel (decode_mega_batch.cu, CL_BATCH_MEGA=1) on the same inputs."""
+    Llama-3-8B layer shapes, contexts up to 8188 tokens, 1-token and page-boundary sequences."""
     cfg = _cfg("llama3-8b", n_layers=4)
     m = _Cache.model("l3x4", cfg, 99)
-    e = _Cache.engine(f"l3x4-p{persistent}", cfg, 99, env={"CL_BATCH_MEGA": persistent}, max_batch=16, max_seqs=16)
+    e = _Cache.engine("l3x4", cfg, 99, max_batch=16, max_seqs=16)
     lens = [8188, 4096, 4095, 31, 32, 33, 0, 1000, 2047, 2048, 6000, 100, 64, 500, 3000, 7][:B]
-    _run_fake_filled(f"llama3-8b/4L/B{B}/{'persistent' if persistent == '1' else 'batched'}", e, m, lens, 4, batched=True,
-                     ref_key=("l3x4-ref", B))
-    if B == 16 and persistent == "1":
+    _run_fake_filled(f"llama3-8b/4L/B{B}/batched", e, m, lens, 4, batched=True, ref_key=("l3x4-ref", B))
+    if B == 16:
         _Cache.drop("l3x4")
 
 
