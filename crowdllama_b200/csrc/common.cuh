@@ -9,8 +9,6 @@
 
 namespace cl {
 
-constexpr int kWarp = 32;
-
 // ---- bf16 <-> fp32 (bit tricks; RNE rounding identical to oracle/llama_oracle.c) -------------
 __device__ __forceinline__ float bf16_lo(uint32_t packed) { return __uint_as_float(packed << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t packed) { return __uint_as_float(packed & 0xffff0000u); }
@@ -24,14 +22,7 @@ __device__ __forceinline__ float bf16_round(float f) {
   return __uint_as_float((uint32_t)f32_to_bf16_bits(f) << 16);
 }
 
-// ---- streaming 128-bit global load (weights / KV are read once: keep them out of L1) ---------
-__device__ __forceinline__ uint4 ldg_stream(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-// 32 bytes per lane as two 128-bit streaming loads (Hopper has no 256-bit load)
+// ---- streaming weight load: 32 bytes per lane as two 128-bit loads that skip L1 (Hopper has no 256-bit load)
 struct u32x8 { uint32_t v[8]; };
 __device__ __forceinline__ u32x8 ldg_stream256(const void* p) {
   u32x8 r;
@@ -51,21 +42,6 @@ __device__ __forceinline__ float dot16(const u32x8& w, const float4* x4, float a
   }
   return acc;
 }
-__device__ __forceinline__ uint4 ldg_stream_keep(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-
-// dot of 8 bf16 (one uint4) with 8 fp32, fp32 FMA chain
-__device__ __forceinline__ float dot8(const uint4& w, const float4& xa, const float4& xb, float acc) {
-  acc = fmaf(bf16_lo(w.x), xa.x, acc); acc = fmaf(bf16_hi(w.x), xa.y, acc);
-  acc = fmaf(bf16_lo(w.y), xa.z, acc); acc = fmaf(bf16_hi(w.y), xa.w, acc);
-  acc = fmaf(bf16_lo(w.z), xb.x, acc); acc = fmaf(bf16_hi(w.z), xb.y, acc);
-  acc = fmaf(bf16_lo(w.w), xb.z, acc); acc = fmaf(bf16_hi(w.w), xb.w, acc);
-  return acc;
-}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -82,33 +58,10 @@ __device__ __forceinline__ float warp_max(float v) {
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// ---- flag-based dependencies between the kernels of one token step -----------------------------
-// griddepcontrol.wait releases a dependent grid only after the primary grid has fully completed and
-// flushed (~2-3 us).  Inside the token step every kernel instead publishes "my outputs are visible"
-// by a release-increment of a per-node counter, and its consumer (already resident thanks to the early
-// PDL trigger) acquires it by polling: the dependent starts ~0.5 us after the last producer CTA.
-// The counters are zeroed by step_bump_kernel at the end of every step (full stream dependency).
-typedef unsigned long long u64;
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
-}
-// lane 0 of the calling warp polls; the warp continues when the counter has reached `expect`
-__device__ __forceinline__ void wait_counter_warp(const unsigned* cnt, unsigned expect) {
-  if ((threadIdx.x & 31) == 0) {
-    const long long t0 = clock64();
-    while (ld_acquire_u32(cnt) < expect) {
-      __nanosleep(40);
-      if (clock64() - t0 > (1ll << 31)) __trap();   // ~1 s: protocol bug -> kernel error, never a hung box
-    }
-  }
-  __syncwarp();
-}
-// call after a CTA-wide barrier that follows the last global write of the CTA
-__device__ __forceinline__ void signal_counter(unsigned* cnt) {
-  __threadfence();
-  atomicAdd(cnt, 1u);
 }
 __device__ __forceinline__ long long gtime_ns() {
   long long t;
@@ -136,16 +89,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  return ok != 0;
-}
-// non-blocking probe (try_wait may suspend the thread for a system-dependent time)
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
       "selp.u32 %0, 1, 0, p;\n\t}"
       : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
   return ok != 0;
@@ -188,11 +131,6 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ uint64_t policy_evict_last() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
 __device__ __forceinline__ bool elect_one() {

@@ -116,7 +116,7 @@ __global__ void __launch_bounds__(256, 2) gemv_ldg_kernel(const GemvArgs a) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.y;
   if (a.pdl_early) pdl_launch_dependents();
-  if (a.sync.wait) wait_counter_warp(a.sync.wait, a.sync.n_wait); else pdl_wait();
+  pdl_wait();
   const int slot = a.slots ? a.slots[b] : b;
   const int K = a.K;
 
@@ -179,10 +179,6 @@ __global__ void __launch_bounds__(256, 2) gemv_ldg_kernel(const GemvArgs a) {
     if (lane == 0) gemv_epilogue<EPI>(a, slot, 2 * p, acc0, acc1);
     if (!a.pdl_early && p == p1 - 2) pdl_launch_dependents();   // about to start the last row pair
   }
-  if (a.sync.signal) {
-    __syncthreads();
-    if (tid == 0) signal_counter(a.sync.signal);
-  }
 }
 
 // ================================================================================================
@@ -243,43 +239,9 @@ __global__ void __launch_bounds__(288, 1) gemv_ring_kernel(const GemvArgs a) {
     // ---------------- consumers
     const int r = warp / S, s = warp % S;
     const int kbase = s * (K / S);
-    if (a.sync.wait) wait_counter_warp(a.sync.wait, a.sync.n_wait); else pdl_wait();
+    pdl_wait();
     if (stamp) a.tl[1] = gtime_ns();
     const int slot = a.slots ? a.slots[b] : b;
-    if (EPI == EPI_RESID && a.comb.part != nullptr) {
-      // ---- o-projection prologue: this CTA combines its slice of the attention outputs across the KV
-      // splits (softmax-weighted), publishes it, and waits until every CTA of this kernel has done so.
-      const AttnCombine& cb = a.comb;
-      const int HD = cb.head_dim, PS = HD + 2;
-      const int o0 = (int)(((long long)K * blockIdx.x) / gridDim.x), o1 = (int)(((long long)K * (blockIdx.x + 1)) / gridDim.x);
-      const float* pbase = cb.part + (size_t)slot * cb.n_kv * cb.nsplit * cb.rep * PS;
-      float* xo = cb.x_out + (size_t)slot * a.x_stride;
-      constexpr int MAXR = 8;   // rounds of 8 outputs (one per warp): covers K / gridDim.x <= 64
-      float mv[MAXR], lv[MAXR], av[MAXR];
-#pragma unroll
-      for (int q = 0; q < MAXR; ++q) {
-        const int o = o0 + q * 8 + warp;
-        mv[q] = -INFINITY; lv[q] = 0.f; av[q] = 0.f;
-        if (o < o1 && lane < cb.nsplit) {
-          const int hg = o / HD, i = o - hg * HD;
-          const float* p = pbase + (((size_t)(hg / cb.rep) * cb.nsplit + lane) * cb.rep + (hg % cb.rep)) * PS;
-          mv[q] = __ldcg(p); lv[q] = __ldcg(p + 1); av[q] = __ldcg(p + 2 + i);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < MAXR; ++q) {
-        const int o = o0 + q * 8 + warp;
-        if (o < o1) {   // warp-uniform
-          const float M = warp_max(mv[q]);
-          const float w = (mv[q] == -INFINITY) ? 0.f : exp2f(mv[q] - M);
-          const float L = warp_sum(lv[q] * w), A = warp_sum(av[q] * w);
-          if (lane == 0) xo[o] = bf16_round(A / L);
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid == 0) signal_counter(cb.phase + b);          // one barrier per batch entry
-      wait_counter_warp(cb.phase + b, gridDim.x);
-    }
     float xr[CPL][8];
     if (NORM) {
       const float* h = a.h + (size_t)slot * a.x_stride;
@@ -312,7 +274,7 @@ __global__ void __launch_bounds__(288, 1) gemv_ring_kernel(const GemvArgs a) {
         xr[c][6] = bf16_round(xr[c][6] * inv * g1.z); xr[c][7] = bf16_round(xr[c][7] * inv * g1.w);
       }
     } else {
-      const float* x = ((EPI == EPI_RESID && a.comb.part != nullptr) ? a.comb.x_out : a.x) + (size_t)slot * a.x_stride;
+      const float* x = a.x + (size_t)slot * a.x_stride;
 #pragma unroll
       for (int c = 0; c < CPL; ++c) {
         const int k = kbase + (c * 32 + lane) * 8;
@@ -333,6 +295,9 @@ __global__ void __launch_bounds__(288, 1) gemv_ring_kernel(const GemvArgs a) {
       uint4 w[CPL];
 #pragma unroll
       for (int c = 0; c < CPL; ++c) w[c] = *reinterpret_cast<const uint4*>(base + c * 512);
+      // The stage's next bulk copy writes through the async proxy, which the arrive's release does not order
+      // against these generic reads: without the fence the reads may still be in flight when the copy lands.
+      fence_proxy_async();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[st]);
       float acc = 0.f;
@@ -355,10 +320,6 @@ __global__ void __launch_bounds__(288, 1) gemv_ring_kernel(const GemvArgs a) {
 #pragma unroll
       for (int i = 0; i < S; ++i) { v0 += part[(2 * p) * S + i]; v1 += part[(2 * p + 1) * S + i]; }
       gemv_epilogue<EPI>(a, slot, row_base + 2 * p, v0, v1);
-    }
-    if (a.sync.signal) {
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid == 0) signal_counter(a.sync.signal);
     }
     if (stamp) a.tl[3] = gtime_ns();
   }
@@ -403,7 +364,6 @@ static cudaError_t launch_ring_inst(const GemvArgs& a, cudaStream_t st, bool pdl
     attr_set.mark();
   }
   if (smem > 160 * 1024) return cudaErrorInvalidValue;
-  if (a.comb.part && (a.comb.nsplit > 32 || (a.K + G - 1) / G > 64)) return cudaErrorInvalidValue;
   g_last_gemv_ctas = G * a.batch;
   return launch_ex(kern, dim3(G, a.batch), dim3(288), smem, st, pdl, a);
 }
@@ -436,7 +396,6 @@ static cudaError_t launch_ldg(const GemvArgs& a, cudaStream_t st, bool pdl) {
   int G = sm_count() * 2;
   int npairs = a.N / 2;
   if (G * 8 > npairs) G = (npairs + 7) / 8;
-  if (a.comb.part) return cudaErrorInvalidValue;   // the distributed combine lives in the ring kernel only
   g_last_gemv_ctas = G * a.batch;
   return launch_ex(kern, dim3(G, a.batch), dim3(256), smem, st, pdl, a);
 }
@@ -522,14 +481,7 @@ __global__ void __launch_bounds__(288) attn_decode_kernel(const AttnDecodeArgs a
         const int st = it % nstg;
         const uint32_t par = (uint32_t)(it / nstg) & 1u;
         mbar_wait(&empty[st], par ^ 1u);
-        if (pg0 + it == cur_page) {
-          if (a.sync.wait) {   // single thread: poll directly
-            const long long t0 = clock64();
-            while (ld_acquire_u32(a.sync.wait) < a.sync.n_wait) { __nanosleep(40); if (clock64() - t0 > (1ll << 31)) __trap(); }
-          } else {
-            pdl_wait();
-          }
-        }
+        if (pg0 + it == cur_page) pdl_wait();
         const int page = bt[pg0 + it];
         const size_t src = ((size_t)page * a.n_kv + g) * P * HD;
         uint8_t* dst = ring + (size_t)st * slot_bytes;
@@ -542,7 +494,7 @@ __global__ void __launch_bounds__(288) attn_decode_kernel(const AttnDecodeArgs a
   }
 
   // ---------------- consumers (warps 0..7)
-  if (a.sync.wait) wait_counter_warp(a.sync.wait, a.sync.n_wait); else pdl_wait();
+  pdl_wait();
   if (stamp) a.tl[1] = gtime_ns();
   const int sub = lane / LPT, j = lane % LPT;
   const float scale2 = rsqrtf((float)HD) * LOG2E;
@@ -607,6 +559,7 @@ __global__ void __launch_bounds__(288) attn_decode_kernel(const AttnDecodeArgs a
         }
       }
     }
+    fence_proxy_async();   // order the reads of this stage before the producer's next bulk copy into it
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[st]);
   }
@@ -660,11 +613,6 @@ __global__ void __launch_bounds__(288) attn_decode_kernel(const AttnDecodeArgs a
     ph[2 + i] = A;
   }
   if (stamp) a.tl[3] = gtime_ns();   // partial written (CTA 0 is rarely the combining CTA)
-  if (a.sync.signal) {   // deferred combine: the o-projection's prologue merges the splits
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (tid == 0) signal_counter(a.sync.signal);
-    return;
-  }
   __threadfence();
   asm volatile("bar.sync 1, 256;" ::: "memory");
   if (tid == 0) {
@@ -853,14 +801,7 @@ __global__ void step_bump_kernel(int* step_counter, unsigned* sync_counters, int
   pdl_launch_dependents();
   pdl_wait();
   if (threadIdx.x == 0) *step_counter += 1;
-  for (int i = threadIdx.x; i < n_sync; i += blockDim.x) sync_counters[i] = 0u;   // re-arm the StepSync counters
-}
-__global__ void zero_u32_kernel(unsigned* p, int n) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = 0u;
-}
-int launch_zero_u32(unsigned* p, int n, cudaStream_t st) {
-  zero_u32_kernel<<<1, 256, 0, st>>>(p, n);
-  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+  for (int i = threadIdx.x; i < n_sync; i += blockDim.x) sync_counters[i] = 0u;   // re-arm the persistent kernel's counters
 }
 
 int launch_step_tail(const StepTailArgs& a, cudaStream_t st) {

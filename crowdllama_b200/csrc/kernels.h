@@ -7,21 +7,6 @@
 
 namespace cl {
 
-// Dependencies inside the token step (common.cuh: wait_counter_warp / signal_counter).
-struct StepSync {
-  const unsigned* wait = nullptr;   // producer node's counter (nullptr => griddepcontrol.wait)
-  unsigned n_wait = 0;              // CTAs of the producer node
-  unsigned* signal = nullptr;       // this node's counter (nullptr => none)
-};
-// o-projection prologue: the cross-split softmax combine of the attention partials, distributed over the
-// o-projection's CTAs (each combines a slice of the H*D outputs), then a grid-wide counter barrier.
-struct AttnCombine {
-  const float* part = nullptr;      // [slot][n_kv][nsplit][rep][head_dim + 2]  (nullptr => x is read as is)
-  int nsplit = 0, n_kv = 0, rep = 0, head_dim = 0;
-  float* x_out = nullptr;           // [slot][x_stride] combined, bf16-rounded attention output
-  unsigned* phase = nullptr;        // counter: CTAs of THIS kernel that have written their slice
-};
-
 enum GemvEpi { EPI_STORE = 0, EPI_RESID = 1, EPI_GATEUP = 2, EPI_QKV = 3 };
 
 // EPI_QKV: the q|k|v projection's rows are stored ROPE-PAIR-INTERLEAVED (within each head, row 2j holds
@@ -54,8 +39,6 @@ struct GemvArgs {
   int batch = 1;
   int pdl_early = 1;                 // 1: trigger dependents at kernel start; 0: when this CTA has issued its last load
   QkvEpi qkv;                        // EPI_QKV only
-  StepSync sync;
-  AttnCombine comb;                  // EPI_RESID o-projection only
   long long* tl = nullptr;           // debug timeline (CL_TIMELINE=1): 4 globaltimer stamps written by CTA 0
 };
 
@@ -76,7 +59,6 @@ struct AttnDecodeArgs {
   int batch = 1;
   int n_heads = 0, n_kv = 0, head_dim = 0, page_size = 0, nsplit = 0;
   int pdl_early = 1;
-  StepSync sync;                     // sync.signal != nullptr: publish partials only, the consumer combines
   long long* tl = nullptr;
   int ring_bytes = 0;                // filled by the launcher
   int tc_small = 0;                  // attn_decode_tc: 4-warp CTAs, two per SM (attn_decode_tc_plan)
@@ -111,8 +93,6 @@ int launch_attn_decode_tc(const AttnDecodeArgs& a, const CUtensorMap& kmap, cons
 int launch_embed(const __nv_bfloat16* table, int d, const int* tok, float* h, int h_stride, const int* slots,
                  int batch, cudaStream_t st);
 int launch_step_tail(const StepTailArgs& a, cudaStream_t st);
-// zero the step counters (run once at init; the per-step reset is part of step_bump_kernel)
-int launch_zero_u32(unsigned* p, int n, cudaStream_t st);
 // rope_hd > 0: rows are written rope-pair-interleaved per head of rope_hd rows (see QkvEpi)
 int launch_synth_bf16(__nv_bfloat16* out, int64_t n_logical, int k_cols, int row_mult, int row_off, uint64_t seed,
                       int key, float scale, cudaStream_t st, int rope_hd = 0);
