@@ -737,8 +737,186 @@ int launch_embed(const __nv_bfloat16* table, int d, const int* tok, float* h, in
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
-constexpr int kTailBlocks = 64;
-__global__ void __launch_bounds__(256) step_tail_kernel(const StepTailArgs a) {
+// ---- device sampler of the step tail: the host sampler (host_util.cpp sample_token) step for step ------------------
+// A candidate is the 64-bit key (orderable(v) << 32) | (0xFFFFFFFF - id): keys are distinct, and "largest k keys" is
+// exactly the host's top-k order (value descending, id ascending).  -0 is keyed as +0 because the host compares them equal.
+__device__ __forceinline__ unsigned long long sample_key(float v, int id) {
+  uint32_t u = __float_as_uint(v);
+  if ((u << 1) == 0u) u = 0u;
+  u ^= (u >> 31) ? 0xFFFFFFFFu : 0x80000000u;
+  return ((unsigned long long)u << 32) | (unsigned long long)(0xFFFFFFFFu - (uint32_t)id);
+}
+__device__ __forceinline__ float sample_key_value(unsigned long long k) {
+  const uint32_t o = (uint32_t)(k >> 32);
+  return __uint_as_float((o & 0x80000000u) ? (o ^ 0x80000000u) : ~o);
+}
+__device__ __forceinline__ int sample_key_id(unsigned long long k) { return (int)(0xFFFFFFFFu - (uint32_t)k); }
+
+// Smallest T such that exactly k of the nonzero keys get(0..n-1) are >= T (8-bit radix select, most significant digit
+// first; stops at the first digit whose whole bucket is taken).  Needs at least k nonzero keys.  All 256 threads call it.
+template <class Get>
+__device__ unsigned long long block_topk_threshold(const Get& get, int n, int k) {
+  __shared__ unsigned hist[256];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_need, s_done;
+  const int tid = threadIdx.x, lane = tid & 31;
+  unsigned long long prefix = 0ull, mask = 0ull;
+  int need = k;
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    hist[tid] = 0u;
+    __syncthreads();
+    for (int i = tid; i < n; i += 256) {
+      const unsigned long long key = get(i);
+      if (key != 0ull && (key & mask) == prefix) atomicAdd(&hist[(unsigned)(key >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (tid < 32) {   // lane l owns buckets 255 - 8l down to 248 - 8l
+      unsigned c[8], s = 0u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { c[j] = hist[255 - 8 * lane - j]; s += c[j]; }
+      unsigned incl = s;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      const unsigned hit = __ballot_sync(0xffffffffu, incl >= (unsigned)need);
+      if (lane == __ffs(hit) - 1) {
+        unsigned acc = incl - s, cnt = 0u;
+        int d = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (cnt == 0u && acc + c[j] >= (unsigned)need) { d = 255 - 8 * lane - j; cnt = c[j]; }
+          else if (cnt == 0u) acc += c[j];
+        s_prefix = prefix | ((unsigned long long)d << shift);
+        s_need = need - (int)acc;
+        s_done = cnt == (unsigned)(need - (int)acc);
+      }
+    }
+    __syncthreads();
+    prefix = s_prefix; need = s_need;
+    const int done = s_done;
+    mask |= 0xFFull << shift;
+    __syncthreads();
+    if (done) break;
+  }
+  return prefix;
+}
+
+__device__ __forceinline__ double sample_uniform01(unsigned long long seed, unsigned long long step) {   // host_util.cpp uniform01
+  const unsigned long long x = mix64(seed * 0x9E3779B97F4A7C15ull + step + 0x632BE59BD9B4E019ull);
+  return __dmul_rn((double)(x >> 11), 1.0 / 9007199254740992.0);
+}
+
+// One block of a sampled slot: the top-k keys of its vocabulary slice (repeat penalty applied) -> a.sample.cand; the
+// last block to finish merges them, draws, and advances the slot.
+__device__ __forceinline__ void step_tail_sample(const StepTailArgs& a, int b, int slot) {
+  __shared__ unsigned long long keys[kSampleSliceMax];
+  __shared__ unsigned pen[kSampleSliceMax / 32];
+  __shared__ unsigned long long top[kSampleTopKMax], sorted[kSampleTopKMax];
+  __shared__ double p[kSampleTopKMax];
+  __shared__ int n_out, is_last_s;
+  __shared__ double s_den;
+  const int tid = threadIdx.x;
+  const SampleState& S = a.sample;
+  const SampleParams sp = S.par[slot];
+  const int V = a.vocab, K = sp.top_k;
+  const int input = a.tok[slot];
+  const int hlen = S.hist_len[slot];
+  const int* ring = S.hist + (size_t)slot * kSampleHistMax;
+  const int slice = (V + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int lo = blockIdx.x * slice, n = max(0, min(slice, V - lo));
+  const float* lg = a.logits + (size_t)slot * V + lo;
+
+  for (int i = tid; i < kSampleSliceMax / 32; i += 256) pen[i] = 0u;
+  if (tid == 0) n_out = 0;
+  __syncthreads();
+  if (sp.repeat_penalty != 1.0f && sp.repeat_last_n != 0) {   // the distinct in-range ids of the last repeat_last_n
+    const int total = hlen + (S.push_input ? 1 : 0);
+    const int w = sp.repeat_last_n > 0 && total > sp.repeat_last_n ? sp.repeat_last_n : total;
+    for (int j = tid; j < w; j += 256) {
+      const int idx = total - w + j;
+      const int id = (S.push_input && idx == hlen) ? input : ring[idx % kSampleHistMax];
+      if (id >= lo && id < lo + n) atomicOr(&pen[(id - lo) >> 5], 1u << ((id - lo) & 31));
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < n; i += 256) {
+    float v = lg[i];
+    if (pen[i >> 5] & (1u << (i & 31))) v = v > 0.f ? __fdiv_rn(v, sp.repeat_penalty) : __fmul_rn(v, sp.repeat_penalty);
+    keys[i] = sample_key(v, lo + i);
+  }
+  __syncthreads();
+  const unsigned long long t1 = n > K ? block_topk_threshold([&](int i) { return keys[i]; }, n, K) : 1ull;
+  unsigned long long* cand = S.cand + ((size_t)slot * gridDim.x + blockIdx.x) * kSampleTopKMax;
+  for (int i = tid; i < n; i += 256)
+    if (keys[i] >= t1) cand[atomicAdd(&n_out, 1)] = keys[i];
+  __syncthreads();
+  for (int j = n_out + tid; j < K; j += 256) cand[j] = 0ull;   // short slice: empty entries
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned old = atomicAdd(a.counters + slot, 1u);
+    is_last_s = (old == gridDim.x - 1);
+    if (is_last_s) a.counters[slot] = 0u;
+    n_out = 0;
+  }
+  __syncthreads();
+  if (!is_last_s) return;
+  __threadfence();
+
+  // merge: the k largest of the kTailBlocks * k candidates, sorted descending
+  const unsigned long long* cs = S.cand + (size_t)slot * gridDim.x * kSampleTopKMax;
+  auto cget = [&](int i) { return __ldcg(cs + (size_t)(i / K) * kSampleTopKMax + (i % K)); };
+  const int nc = (int)gridDim.x * K;
+  const unsigned long long t2 = block_topk_threshold(cget, nc, K);
+  for (int i = tid; i < nc; i += 256) {
+    const unsigned long long key = cget(i);
+    if (key != 0ull && key >= t2) top[atomicAdd(&n_out, 1)] = key;
+  }
+  __syncthreads();
+  if (tid < K) {
+    const unsigned long long mine = top[tid];
+    int rank = 0;
+    for (int j = 0; j < K; ++j) rank += top[j] > mine;
+    sorted[rank] = mine;
+  }
+  __syncthreads();
+  // p_i = exp((double)(v_i - max) / T); the sums run sequentially in rank order, as on the host
+  const float mx = sample_key_value(sorted[0]);
+  if (tid < K) p[tid] = exp(__ddiv_rn((double)__fsub_rn(sample_key_value(sorted[tid]), mx), (double)sp.temperature));
+  __syncthreads();
+  if (tid == 0) {
+    double den = 0.0;
+    for (int i = 0; i < K; ++i) den = __dadd_rn(den, p[i]);
+    s_den = den;
+  }
+  __syncthreads();
+  __shared__ double q[kSampleTopKMax];
+  if (tid < K) q[tid] = __ddiv_rn(p[tid], s_den);
+  __syncthreads();
+  if (tid != 0) return;
+  int keep = K;
+  if (sp.top_p > 0.f && sp.top_p < 1.f) {
+    double cum = 0.0;
+    for (int i = 0; i < K; ++i) { cum = __dadd_rn(cum, q[i]); if (cum >= (double)sp.top_p) { keep = i + 1; break; } }
+  }
+  double tot = 0.0;
+  for (int i = 0; i < keep; ++i) tot = __dadd_rn(tot, p[i]);
+  const unsigned long long step = S.step[slot];
+  const double u = __dmul_rn(sample_uniform01(sp.seed, step), tot);
+  double cum = 0.0;
+  int pick = sample_key_id(sorted[keep - 1]);
+  for (int i = 0; i < keep; ++i) { cum = __dadd_rn(cum, p[i]); if (u < cum) { pick = sample_key_id(sorted[i]); break; } }
+  if (S.push_input) { S.hist[(size_t)slot * kSampleHistMax + hlen % kSampleHistMax] = input; S.hist_len[slot] = hlen + 1; }
+  S.step[slot] = step + 1;
+  a.tok[slot] = pick;
+  a.pos[slot] += 1;
+  const int sc = *a.step_counter;
+  a.ids_ring[(size_t)(sc % a.ring_steps) * a.ring_stride + b] = pick;
+}
+
+__global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a) {
   __shared__ float sv[8];
   __shared__ int si[8];
   __shared__ int is_last_s;
@@ -746,6 +924,7 @@ __global__ void __launch_bounds__(256) step_tail_kernel(const StepTailArgs a) {
   pdl_wait();
   const int b = blockIdx.y;
   const int slot = a.slots ? a.slots[b] : b;
+  if (a.sample.mode && a.sample.mode[slot]) { step_tail_sample(a, b, slot); return; }
   const float* lg = a.logits + (size_t)slot * a.vocab;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float best = -INFINITY;

@@ -185,6 +185,7 @@ int Engine::init(const cl_engine_config& c) {
   if (sched_prefill_chunk_ > 0 && sched_prefill_chunk_ < 16) sched_prefill_chunk_ = 16;
   prefill_small_max_ = std::min(256, env_int("CL_PREFILL_SMALL_MAX", kDefaultPrefillSmallMax));
   prefill_fused_ = env_int("CL_PREFILL_FUSED", kDefaultPrefillFused);
+  device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
   if (c.start_scheduler) start_scheduler();
   return CL_OK;
 }
@@ -316,9 +317,17 @@ int Engine::alloc_state() {
   const int rep = cfg.n_heads / cfg.n_kv_heads;
   DMALLOC(d_attn_part_, S * cfg.n_kv_heads * nsplit_ * rep * (cfg.head_dim + 2) * 4);
   DMALLOC(d_attn_cnt_, S * cfg.n_kv_heads * 4);
-  DMALLOC(d_tail_val_, S * 64 * 4);
-  DMALLOC(d_tail_idx_, S * 64 * 4);
+  DMALLOC(d_tail_val_, S * kTailBlocks * 4);
+  DMALLOC(d_tail_idx_, S * kTailBlocks * 4);
   DMALLOC(d_tail_cnt_, S * 4);
+  DMALLOC(d_samp_mode_, S * 4);
+  DMALLOC(d_samp_par_, S * sizeof(SampleParams));
+  DMALLOC(d_samp_step_, S * 8);
+  DMALLOC(d_samp_hist_, S * kSampleHistMax * 4);
+  DMALLOC(d_samp_hlen_, S * 4);
+  DMALLOC(d_samp_cand_, S * kTailBlocks * kSampleTopKMax * 8);
+  CL_CUDA_OK(cudaMemsetAsync(d_samp_mode_, 0, S * 4, stream_));
+  samp_hlen_.assign(S, -1);
   DMALLOC(d_ids_ring_, (size_t)ring_steps_ * max_batch_ * 4);
   DMALLOC(d_step_counter_, 4);
   n_sync_ = cfg.n_layers * 10 + 1;   // persistent kernel: 6 grid barriers + 4 tile counters per layer + the lookahead frontier
@@ -371,7 +380,7 @@ int Engine::seq_create(cl_seq_t* out) {
       seqs_[i] = SeqState();
       seqs_[i].live = true;
       *out = i;
-      return CL_OK;
+      return disarm_sampling(i);
     }
   set_last_error("no free sequence slot (max_seqs)");
   return CL_ERR_OOM;
@@ -380,6 +389,39 @@ int Engine::seq_free(cl_seq_t s) {
   if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
   pool_->release(s);
   seqs_[s] = SeqState();
+  return disarm_sampling(s);
+}
+
+int Engine::arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist) {
+  if (!device_sampling_ok(sp, cfg.vocab_size)) { set_last_error("sampling settings need the host sampler"); return CL_ERR_INVALID_ARG; }
+  SampleParams par;
+  par.temperature = sp.temperature; par.top_p = sp.top_p; par.repeat_penalty = sp.repeat_penalty;
+  par.top_k = sp.top_k; par.repeat_last_n = sp.repeat_last_n; par.seed = sp.seed;
+  std::vector<int> ring(kSampleHistMax, 0);
+  for (int i = std::max(0, n_hist - kSampleHistMax); i < n_hist; ++i) ring[i % kSampleHistMax] = hist[i];
+  const int mode = 1;
+  const unsigned long long st = step0;
+  CL_CUDA_OK(cudaMemcpyAsync(d_samp_par_ + s, &par, sizeof par, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaMemcpyAsync(d_samp_step_ + s, &st, 8, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaMemcpyAsync(d_samp_hist_ + (size_t)s * kSampleHistMax, ring.data(), kSampleHistMax * 4, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaMemcpyAsync(d_samp_hlen_ + s, &n_hist, 4, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaMemcpyAsync(d_samp_mode_ + s, &mode, 4, cudaMemcpyHostToDevice, stream_));
+  samp_hlen_[s] = n_hist;
+  return CL_OK;
+}
+
+int Engine::disarm_sampling(cl_seq_t s) {
+  if (samp_hlen_[s] < 0) return CL_OK;
+  const int mode = 0;
+  CL_CUDA_OK(cudaMemcpyAsync(d_samp_mode_ + s, &mode, 4, cudaMemcpyHostToDevice, stream_));
+  samp_hlen_[s] = -1;
+  return CL_OK;
+}
+
+int Engine::read_next_token(cl_seq_t s, int32_t* out) {
+  CL_CUDA_OK(cudaMemcpyAsync(h_ids_pinned_, d_tok_ + s, 4, cudaMemcpyDeviceToHost, stream_));
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  *out = h_ids_pinned_[0];
   return CL_OK;
 }
 
@@ -496,7 +538,7 @@ int Engine::enqueue_step(int B) {
   }
   if (probe_ev_) cudaEventRecord(probe_ev_[probe_idx_ + 1], stream_);
   CL_LAUNCH(enqueue_lm_head(B, use_pdl_ && !mega));
-  CL_LAUNCH(enqueue_step_tail(B));
+  CL_LAUNCH(enqueue_step_tail(B, true));
   return launches;
 }
 
@@ -510,15 +552,18 @@ int Engine::enqueue_lm_head(int B, bool pdl) {
   return launch_gemv(gemv_variant_, EPI_STORE, true, lm, stream_, pdl);
 }
 
-// The tail of every decode step and prefill: greedy id of d_logits_ for d_slots_[0..B) into d_tok_ and the id ring,
-// d_pos_ += 1.  It also zeroes the persistent kernel's counters.  They are zero whenever no step is running, so the
+// The tail of every decode step and prefill: greedy id (or, on slots armed by arm_sampling, a draw) of d_logits_ for
+// d_slots_[0..B) into d_tok_ and the id ring, d_pos_ += 1.  It also zeroes the persistent kernel's counters.  They are zero whenever no step is running, so the
 // zeroing is needed only behind the persistent kernel and harmless everywhere else.
-int Engine::enqueue_step_tail(int B) {
+int Engine::enqueue_step_tail(int B, bool push_input) {
   StepTailArgs t;
   t.logits = d_logits_; t.vocab = cfg.vocab_size; t.tok = d_tok_; t.pos = d_pos_; t.ids_ring = d_ids_ring_;
   t.step_counter = d_step_counter_; t.ring_steps = ring_steps_; t.ring_stride = max_batch_;
   t.part_val = d_tail_val_; t.part_idx = d_tail_idx_; t.counters = d_tail_cnt_; t.slots = d_slots_; t.batch = B;
   t.sync_counters = d_sync_; t.n_sync_counters = n_sync_;
+  SampleState& smp = t.sample;
+  smp.mode = d_samp_mode_; smp.par = d_samp_par_; smp.step = d_samp_step_; smp.hist = d_samp_hist_; smp.hist_len = d_samp_hlen_;
+  smp.cand = d_samp_cand_; smp.push_input = push_input ? 1 : 0;
   return launch_step_tail(t, stream_);
 }
 
@@ -588,7 +633,7 @@ int Engine::enqueue_step_batched(int B) {
   CL_LAUNCH(launch_batch_resid_norm(d_h_, d, pending, pending_s, B, final_norm_, cfg.rms_eps, w.xn, d_slots_, stream_, bp));
   CL_LAUNCH(launch_gemm_bf16(w.xn, lm_head_, w.logits, nullptr, B, V, d, stream_, 1, bp));
   CL_LAUNCH(launch_batch_scatter_rows(w.logits, V, d_logits_, V, d_slots_, B, stream_));
-  CL_LAUNCH(enqueue_step_tail(B));
+  CL_LAUNCH(enqueue_step_tail(B, true));
   prof.report("step profile", 34, "B=" + std::to_string(B));
   return launches;
 }
@@ -702,8 +747,17 @@ int Engine::prefill_tokenwise(cl_seq_t s, const int32_t* ids, int n, float* logi
   CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &q.len, 4, cudaMemcpyHostToDevice, stream_));
   rc = set_single_slot(s);
   if (rc) return rc;
+  // An armed slot draws once, at the last prompt token.  The step graph's tail pushes its input, so the history length is
+  // taken back by one first: the push then rewrites the ring entry that already holds that token.
+  const int armed_hlen = samp_hlen_[s];
+  const int off = 0, on = 1, hlen_before_last = std::max(0, armed_hlen - 1);
+  if (armed_hlen >= 0 && n > 1) CL_CUDA_OK(cudaMemcpyAsync(d_samp_mode_ + s, &off, 4, cudaMemcpyHostToDevice, stream_));
   for (int i = 0; i < n; ++i) {
     CL_CUDA_OK(cudaMemcpyAsync(d_tok_ + s, d_prompt_ + i, 4, cudaMemcpyDeviceToDevice, stream_));
+    if (armed_hlen >= 0 && i == n - 1) {
+      CL_CUDA_OK(cudaMemcpyAsync(d_samp_mode_ + s, &on, 4, cudaMemcpyHostToDevice, stream_));
+      CL_CUDA_OK(cudaMemcpyAsync(d_samp_hlen_ + s, &hlen_before_last, 4, cudaMemcpyHostToDevice, stream_));
+    }
     rc = run_step_graph(1);
     if (rc) return rc;
   }
@@ -778,6 +832,30 @@ int Engine::decode_greedy(const cl_seq_t* ss, int B, const int32_t* first_ids, i
   }
   if (device_ms) *device_ms = total_ms;
   return CL_OK;
+}
+
+int Engine::decode_sample(const cl_seq_t* ss, int B, const int32_t* first_ids, const cl_sampling* sp, const uint64_t* step0,
+                          int n_steps, int32_t* ids_out, float* device_ms) {
+  if (B <= 0 || B > max_batch_) { set_last_error("bad batch / steps"); return CL_ERR_INVALID_ARG; }
+  for (int b = 0; b < B; ++b) {
+    if (ss[b] < 0 || ss[b] >= max_seqs_ || !seqs_[ss[b]].live) return CL_ERR_BAD_SEQ;
+    if (sp[b].temperature > 0.f && !device_sampling_ok(sp[b], cfg.vocab_size)) {
+      set_last_error("sampling settings of sequence " + std::to_string(b) + " need the host sampler");
+      return CL_ERR_INVALID_ARG;
+    }
+  }
+  int rc = CL_OK;
+  for (int b = 0; b < B && rc == CL_OK; ++b)
+    if (sp[b].temperature > 0.f) {
+      const auto& h = seqs_[ss[b]].history;
+      rc = arm_sampling(ss[b], sp[b], step0 ? step0[b] : 0, h.data(), (int)h.size());
+    }
+  if (rc == CL_OK) rc = decode_greedy(ss, B, first_ids, n_steps, ids_out, device_ms);
+  for (int b = 0; b < B; ++b) {
+    const int r2 = disarm_sampling(ss[b]);
+    if (rc == CL_OK) rc = r2;
+  }
+  return rc;
 }
 
 // ---- parity / benchmark aids ------------------------------------------------------------------------

@@ -129,6 +129,15 @@ int model_config_from_dir(const std::string& dir, cl_model_config* out);
 double rope_inv_freq(const cl_model_config& c, int i);
 int32_t sample_token(const float* logits, int32_t vocab, const cl_sampling& sp, const int32_t* history, int32_t n_history,
                      uint64_t step);
+// True when the step tail's device sampler draws exactly what sample_token draws for these settings: temperature > 0,
+// 1 <= top_k <= kSampleTopKMax with top_k < vocab, vocab <= kTailBlocks * kSampleSliceMax, and the repeat penalty off or
+// over a window of 1..kSampleHistMax ids.  Everything else (top_k 0, repeat_last_n -1, ...) stays on the host sampler.
+inline bool device_sampling_ok(const cl_sampling& sp, int vocab) {
+  if (!(sp.temperature > 0.f)) return false;
+  if (sp.top_k < 1 || sp.top_k > kSampleTopKMax || sp.top_k >= vocab || vocab > kTailBlocks * kSampleSliceMax) return false;
+  const bool penalty = sp.repeat_penalty != 1.0f && sp.repeat_last_n != 0;
+  return !penalty || (sp.repeat_last_n > 0 && sp.repeat_last_n <= kSampleHistMax);
+}
 
 // ---- minimal protobuf codec for llama.v1.BaseMessage (pbmsg.cpp) -------------------------------
 // GenerateOptions: the proto extension SURVEY.md §8f row 3 asks for (seed / temperature / num_predict ... are
@@ -183,6 +192,16 @@ class Engine {
   int decode_step(cl_seq_t s, int32_t id, float* logits_out, int32_t* argmax_out);
   int decode_greedy(const cl_seq_t* seqs, int n_seqs, const int32_t* first_ids, int n_steps, int32_t* ids_out,
                     float* device_ms);
+  // decode_greedy with the device sampler on the slots whose sp[b].temperature > 0 (every one must pass
+  // device_sampling_ok); draw i of sequence b uses RNG step step0[b] + i (step0 may be nullptr: 0)
+  int decode_sample(const cl_seq_t* seqs, int n_seqs, const int32_t* first_ids, const cl_sampling* sp, const uint64_t* step0,
+                    int n_steps, int32_t* ids_out, float* device_ms);
+  // Device sampler of one slot: every later step tail of `s` draws with `sp`, the first draw at RNG step `step0`, with the
+  // last kSampleHistMax ids of hist[0..n_hist) as its history.  seq_create / seq_free disarm.
+  int arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist);
+  int disarm_sampling(cl_seq_t s);
+  int read_next_token(cl_seq_t s, int32_t* out);   // d_tok_[s]: what the last step tail of `s` chose
+  bool device_sample() const { return device_sample_; }
   int set_tensor(int layer, int kind, const uint16_t* data, int64_t n);
   int load_safetensors(const std::string& path);   // HF llama-layout checkpoint (file or directory) -> set_tensor (weights_io.cpp)
   // parity / benchmark aids (token level)
@@ -215,7 +234,9 @@ class Engine {
   int enqueue_step(int B);                         // kernels of one token step for d_slots_[0..B)
   int enqueue_step_batched(int B);                 // B >= 2: wgmma projections + per-sequence glue kernels
   int enqueue_lm_head(int B, bool pdl);            // final norm + LM-head GEMV of d_h_ -> d_logits_ for d_slots_[0..B)
-  int enqueue_step_tail(int B);                    // argmax of d_logits_, advance tok / pos, id ring (step_tail_kernel)
+  // argmax (or, on armed slots, a draw) of d_logits_, advance tok / pos, id ring (step_tail_kernel); push_input: decode
+  // steps, whose input token joins an armed slot's history.  Prefill tails do not push: the armed history holds the prompt.
+  int enqueue_step_tail(int B, bool push_input);
   int run_step_graph(int B);
   bool ensure_graph(int B);
   void precapture_graphs();                       // graph launch (or eager enqueue)
@@ -266,6 +287,11 @@ class Engine {
   int* d_ids_ring_ = nullptr; int* d_step_counter_ = nullptr; int* d_prompt_ = nullptr;
   int ring_steps_ = 1024, prompt_cap_ = 0;
   float* h_logits_pinned_ = nullptr; int* h_ids_pinned_ = nullptr;
+  // device sampler (kernels.h SampleState), indexed by sequence handle
+  int* d_samp_mode_ = nullptr; SampleParams* d_samp_par_ = nullptr; unsigned long long* d_samp_step_ = nullptr;
+  int* d_samp_hist_ = nullptr; int* d_samp_hlen_ = nullptr; unsigned long long* d_samp_cand_ = nullptr;
+  std::vector<int> samp_hlen_;        // host: history length uploaded by arm_sampling, -1 = disarmed
+  bool device_sample_ = true;         // CL_DEVICE_SAMPLE: the scheduler and the synchronous path draw on the device where they can
 
   // prefill workspace (allocated lazily)
   struct PrefillWs {

@@ -64,7 +64,30 @@ struct AttnDecodeArgs {
   int tc_small = 0;                  // attn_decode_tc: 4-warp CTAs, two per SM (attn_decode_tc_plan)
 };
 
-struct StepTailArgs {                // argmax over logits, advance the sequence
+// ---- step tail: argmax or a seeded draw, then advance the sequence ----------------------------------
+constexpr int kTailBlocks = 64;          // blocks per slot; each owns a contiguous slice of the vocabulary
+constexpr int kSampleTopKMax = 128;      // device draws cover 1 <= top_k <= this
+constexpr int kSampleHistMax = 256;      // ... and a repeat-penalty window of at most this many ids
+constexpr int kSampleSliceMax = 2560;    // ... and vocab <= kTailBlocks * kSampleSliceMax (one slice's keys sit in shared memory)
+
+struct SampleParams {                    // cl_sampling fields the draw reads
+  float temperature = 0.f, top_p = 1.f, repeat_penalty = 1.f;
+  int top_k = 0, repeat_last_n = 0;
+  unsigned long long seed = 0;
+};
+// Per-slot sampler state of the step tail.  A slot whose mode is 1 draws exactly as the host sampler (host_util.cpp
+// sample_token) would with history = its ring (+ the step's input token when push_input) and step = its draw counter.
+struct SampleState {
+  const int* mode = nullptr;             // [slot] 0: argmax, 1: draw (nullptr: argmax everywhere)
+  const SampleParams* par = nullptr;     // [slot]
+  unsigned long long* step = nullptr;    // [slot] RNG step of the next draw (+1 per draw)
+  int* hist = nullptr;                   // [slot][kSampleHistMax] ring: id i of the history at i % kSampleHistMax
+  int* hist_len = nullptr;               // [slot] ids in the history so far
+  unsigned long long* cand = nullptr;    // [slot][kTailBlocks][kSampleTopKMax] per-block top-k keys
+  int push_input = 0;                    // 1 (decode steps): tok[slot], the step's input, joins the history before the draw
+};
+
+struct StepTailArgs {                // argmax (or a draw) over logits, advance the sequence
   const float* logits = nullptr;     // [slot][vocab]
   int vocab = 0;
   int* tok = nullptr;                // [slot] next input token (written)
@@ -79,6 +102,7 @@ struct StepTailArgs {                // argmax over logits, advance the sequence
   unsigned* counters = nullptr;      // [slot]
   const int* slots = nullptr;
   int batch = 1;
+  SampleState sample;
 };
 
 // every launcher returns the number of kernels it enqueued (for cl_stats.kernel_launches)

@@ -216,6 +216,55 @@ int cl_op_qkv_rope_append(int device, int variant, const uint16_t* w_qkv, const 
   return CL_OK;
 }
 
+int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
+                 const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out) {
+  if (!logits || n_rows <= 0 || vocab <= 1 || !sp || !n_history || !step || !ids_out) return CL_ERR_INVALID_ARG;
+  const size_t R = (size_t)n_rows;
+  std::vector<SampleParams> par(R);
+  std::vector<int> ring(R * kSampleHistMax, 0), hlen(R), mode(R, 1);
+  for (size_t r = 0; r < R; ++r) {
+    if (!device_sampling_ok(sp[r], vocab)) { set_last_error("cl_op_sample: settings the device sampler does not cover"); return CL_ERR_INVALID_ARG; }
+    const int n = n_history[r];
+    if (n < 0 || (n > 0 && (!history || n > hist_stride))) return CL_ERR_INVALID_ARG;
+    par[r].temperature = sp[r].temperature; par[r].top_p = sp[r].top_p; par[r].repeat_penalty = sp[r].repeat_penalty;
+    par[r].top_k = sp[r].top_k; par[r].repeat_last_n = sp[r].repeat_last_n; par[r].seed = sp[r].seed;
+    for (int i = std::max(0, n - kSampleHistMax); i < n; ++i) ring[r * kSampleHistMax + i % kSampleHistMax] = history[r * hist_stride + i];
+    hlen[r] = n;
+  }
+  int rc = check_device(device);
+  if (rc) return rc;
+  DevBuf dl, dpar, dstep, dhist, dhlen, dmode, dcand, dtok, dpos, dring, dsc, dval, didx, dcnt;
+  CL_CUDA_OK(dl.upload(logits, R * vocab * 4));
+  CL_CUDA_OK(dpar.upload(par.data(), R * sizeof(SampleParams)));
+  CL_CUDA_OK(dstep.upload(step, R * 8));
+  CL_CUDA_OK(dhist.upload(ring.data(), ring.size() * 4));
+  CL_CUDA_OK(dhlen.upload(hlen.data(), R * 4));
+  CL_CUDA_OK(dmode.upload(mode.data(), R * 4));
+  CL_CUDA_OK(dcand.alloc(R * kTailBlocks * kSampleTopKMax * 8));
+  CL_CUDA_OK(dtok.alloc(R * 4));
+  CL_CUDA_OK(dpos.alloc(R * 4));
+  CL_CUDA_OK(dring.alloc(R * 4));
+  CL_CUDA_OK(dsc.alloc(4));
+  CL_CUDA_OK(dval.alloc(R * kTailBlocks * 4));
+  CL_CUDA_OK(didx.alloc(R * kTailBlocks * 4));
+  CL_CUDA_OK(dcnt.alloc(R * 4));
+  CL_CUDA_OK(cudaMemset(dtok.p, 0, R * 4));
+  CL_CUDA_OK(cudaMemset(dpos.p, 0, R * 4));
+  CL_CUDA_OK(cudaMemset(dsc.p, 0, 4));
+  CL_CUDA_OK(cudaMemset(dcnt.p, 0, R * 4));
+  StepTailArgs t;
+  t.logits = dl.as<float>(); t.vocab = vocab; t.tok = dtok.as<int>(); t.pos = dpos.as<int>(); t.ids_ring = dring.as<int>();
+  t.step_counter = dsc.as<int>(); t.ring_steps = 1; t.ring_stride = n_rows;
+  t.part_val = dval.as<float>(); t.part_idx = didx.as<int>(); t.counters = dcnt.as<unsigned>(); t.batch = n_rows;
+  t.sample.mode = dmode.as<int>(); t.sample.par = dpar.as<SampleParams>(); t.sample.step = dstep.as<unsigned long long>();
+  t.sample.hist = dhist.as<int>(); t.sample.hist_len = dhlen.as<int>(); t.sample.cand = dcand.as<unsigned long long>();
+  t.sample.push_input = 0;
+  if (launch_step_tail(t, nullptr) < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("launch_step_tail failed"); return CL_ERR_CUDA; }
+  CL_CUDA_OK(cudaDeviceSynchronize());
+  CL_CUDA_OK(cudaMemcpy(ids_out, dtok.p, R * 4, cudaMemcpyDeviceToHost));
+  return CL_OK;
+}
+
 int cl_op_synth_weights(int device, uint64_t seed, int32_t tensor_key, int64_t n, float scale, uint16_t* out_bf16) {
   if (!out_bf16 || n <= 0) return CL_ERR_INVALID_ARG;
   int rc = check_device(device);

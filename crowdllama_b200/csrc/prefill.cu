@@ -100,7 +100,7 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   rc = set_single_slot(s);
   if (rc) return rc;
   CL_LAUNCH(enqueue_lm_head(1, false));
-  CL_LAUNCH(enqueue_step_tail(1));
+  CL_LAUNCH(enqueue_step_tail(1, false));
   prof.report("prefill profile", 32, "short-prompt path, " + std::to_string(n) + " tokens");
   launches_ += launches;
   q.len += n;
@@ -196,7 +196,7 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
   rc = set_single_slot(s);
   if (rc) return rc;
   CL_LAUNCH(enqueue_lm_head(1, false));
-  CL_LAUNCH(enqueue_step_tail(1));
+  CL_LAUNCH(enqueue_step_tail(1, false));
   prof.report("prefill profile", 32, "tile path, " + std::to_string(n) + " tokens");
   launches_ += launches;
   q.len += n;
@@ -296,7 +296,7 @@ int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* 
   CL_LAUNCH(launch_batch_resid_norm(d_h_, d, nullptr, 0, n_seqs, final_norm_, cfg.rms_eps, bw.xn, d_slots_, stream_, false));
   CL_LAUNCH(launch_gemm_bf16(bw.xn, lm_head_, bw.logits, nullptr, n_seqs, V, d, stream_, 1, false));
   CL_LAUNCH(launch_batch_scatter_rows(bw.logits, V, d_logits_, V, d_slots_, n_seqs, stream_));
-  CL_LAUNCH(enqueue_step_tail(n_seqs));
+  CL_LAUNCH(enqueue_step_tail(n_seqs, false));
   prof.report("prefill profile", 32, "multi-prompt tile path, " + std::to_string(total) + " tokens");
   launches_ += launches;
   for (int i = 0; i < n_seqs; ++i) {

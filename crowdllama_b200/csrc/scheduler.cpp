@@ -39,7 +39,9 @@ struct Request {
   uint64_t arrival = 0;
   std::vector<int32_t> full;        // prompt + tokens generated before a preemption: what the (re-)prefill has to process
   size_t prefilled = 0;             // tokens of `full` already in the cache (chunked admission)
+  bool dev_sample = false;          // sampled, and the step tail draws its tokens (device_sampling_ok, CL_DEVICE_SAMPLE)
   bool greedy() const { return sp.temperature <= 0.f; }
+  bool device_next() const { return greedy() || dev_sample; }   // the next id is d_tok_ after the step: no host sampler
 };
 
 static void fill_result(const Request& r, cl_result* out, const Tokenizer* tok) {
@@ -88,16 +90,21 @@ static int generate_sync(Engine& e, Request& r, const Engine::TokenSink* sink) {
   if (rc) return rc;
   std::vector<float> logits(V);
   int64_t t0 = now_ns();
-  rc = e.prefill(r.seq, r.prompt.data(), (int)r.prompt.size(), logits.data());
+  // a device-sampled request is armed before the prefill, whose tail then draws the first token
+  if (r.dev_sample) rc = e.arm_sampling(r.seq, r.sp, 0, r.prompt.data(), (int)r.prompt.size());
+  if (rc == CL_OK) rc = e.prefill(r.seq, r.prompt.data(), (int)r.prompt.size(), r.dev_sample ? nullptr : logits.data());
   r.prefill_ns = now_ns() - t0;
   if (rc) { e.seq_free(r.seq); return rc; }
   t0 = now_ns();
   std::vector<int32_t> hist(r.prompt);
-  int32_t next = sample_token(logits.data(), V, r.sp, hist.data(), (int)hist.size(), 0);
+  int32_t next = 0;
+  if (r.dev_sample) rc = e.read_next_token(r.seq, &next);
+  else next = sample_token(logits.data(), V, r.sp, hist.data(), (int)hist.size(), 0);
+  if (rc) { e.seq_free(r.seq); return rc; }
   r.out.push_back(next);
   emit();
   while (!finished(r, *e.tok, e.cfg.max_seq_len)) {
-    if (r.greedy()) {
+    if (r.device_next()) {   // greedy or device-sampled: the token loop stays on the device
       int room = std::min(r.max_new - (int)r.out.size(), e.cfg.max_seq_len - (int)(r.prompt.size() + r.out.size()));
       int chunk = std::min(room, sink ? 8 : 32);
       std::vector<int32_t> ids(chunk);
@@ -135,6 +142,7 @@ int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling&
   r->max_new = std::min(r->max_new, cfg.max_seq_len - n_prompt);
   r->t_arrive = now_ns();
   r->streaming = sink && sink->fn;
+  r->dev_sample = device_sample_ && device_sampling_ok(sp, cfg.vocab_size);
   if (!sched_started_) {
     r->status = generate_sync(*this, *r, sink);
     if (r->status == CL_OK) { requests_completed_++; tokens_generated_ += (int64_t)r->out.size(); }
@@ -279,6 +287,8 @@ void Engine::scheduler_main() {
           r->full.insert(r->full.end(), r->out.begin(), r->out.end());
           rc = seq_create(&r->seq);
           if (rc == CL_OK) rc = ensure_capacity(r->seq, (int)r->full.size() + 1);
+          // the pass's tail draws the next token of a device-sampled request (step = tokens generated before a preemption)
+          if (rc == CL_OK && r->dev_sample) rc = arm_sampling(r->seq, r->sp, r->out.size(), r->full.data(), (int)r->full.size());
           if (rc) break;
           ss.push_back(r->seq); ptrs.push_back(r->full.data()); lens.push_back((int)r->full.size());
           total += (int)r->full.size();
@@ -298,8 +308,8 @@ void Engine::scheduler_main() {
           for (auto& r : group) {
             r->prefill_ns += pdt;
             r->prefilled = r->full.size();
-            int32_t next = toks[r->seq];                       // greedy: the device argmax of the pass
-            if (!r->greedy()) {
+            int32_t next = toks[r->seq];                       // greedy / device-sampled: the pass's tail chose it
+            if (!r->device_next()) {
               read_logits(r->seq, logits.data());
               next = sample_token(logits.data(), V, r->sp, r->full.data(), (int)r->full.size(), (uint64_t)r->out.size());
               cudaMemcpyAsync(d_tok_ + r->seq, &next, 4, cudaMemcpyHostToDevice, stream_);
@@ -361,7 +371,11 @@ void Engine::scheduler_main() {
       const size_t chunk = active_.empty() ? left : std::min(left, (size_t)budget);   // nobody to stall: the whole prompt at once
       const bool last = chunk == left;
       const int64_t t0 = now_ns();
-      const int rc = prefill(r->seq, r->full.data() + r->prefilled, (int)chunk, last ? logits.data() : nullptr);
+      // only the last chunk's tail draws: earlier chunks run with the slot disarmed
+      int rc = last && r->dev_sample ? arm_sampling(r->seq, r->sp, r->out.size(), r->full.data(), (int)r->full.size()) : CL_OK;
+      if (rc == CL_OK) rc = prefill(r->seq, r->full.data() + r->prefilled, (int)chunk, last && !r->dev_sample ? logits.data() : nullptr);
+      int32_t next = 0;
+      if (rc == CL_OK && last && r->dev_sample) rc = read_next_token(r->seq, &next);
       const int64_t pdt = now_ns() - t0;
       r->prefill_ns += pdt;
       sched_prefill_calls_++; sched_prefill_tokens_ += (int64_t)chunk; sched_prefill_ns_ += pdt;
@@ -371,10 +385,10 @@ void Engine::scheduler_main() {
       r->prefilled += chunk;
       if (!last) break;                   // budget used up in the middle of a prompt
       prefilling_.reset();
-      const int32_t next = sample_token(logits.data(), V, r->sp, r->full.data(), (int)r->full.size(), (uint64_t)r->out.size());
+      if (!r->dev_sample) next = sample_token(logits.data(), V, r->sp, r->full.data(), (int)r->full.size(), (uint64_t)r->out.size());
       r->out.push_back(next);
       publish(*r, next);
-      if (!r->greedy()) cudaMemcpyAsync(d_tok_ + r->seq, &r->out.back(), 4, cudaMemcpyHostToDevice, stream_);
+      if (!r->device_next()) cudaMemcpyAsync(d_tok_ + r->seq, &r->out.back(), 4, cudaMemcpyHostToDevice, stream_);
       if (finished(*r, *tok, cfg.max_seq_len)) {
         seq_free(r->seq);
         requests_completed_++;
@@ -459,7 +473,7 @@ void Engine::scheduler_main() {
       st.history.push_back(r->out.back());
       st.len += 1;
       int32_t next = toks[r->seq];
-      if (!r->greedy()) {
+      if (!r->device_next()) {
         read_logits(r->seq, logits.data());
         next = sample_token(logits.data(), V, r->sp, st.history.data(), (int)st.history.size(), (uint64_t)r->out.size());
         cudaMemcpyAsync(d_tok_ + r->seq, &next, 4, cudaMemcpyHostToDevice, stream_);

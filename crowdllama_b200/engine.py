@@ -68,10 +68,10 @@ EXPORTS = [
     "cl_greedy_sampling", "cl_sample_token", "cl_model_preset", "cl_engine_create", "cl_engine_destroy", "cl_engine_model_config",
     "cl_engine_stats", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
-    "cl_seq_len", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
+    "cl_seq_len", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
     "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
-    "cl_op_gemm_bf16", "cl_op_attn_prefill", "cl_op_attn_prefill_variant", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
+    "cl_op_gemm_bf16", "cl_op_attn_prefill", "cl_op_attn_prefill_variant", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_tokenizer_load", "cl_tokenizer_free", "cl_tokenizer_encode", "cl_tokenizer_decode", "cl_tokenizer_info", "cl_engine_load_tokenizer",
 ]
@@ -126,6 +126,7 @@ def lib():
         "cl_decode_step": (C.c_int, [vp, i32, i32, vp, P(i32)]),
         "cl_decode_greedy": (C.c_int, [vp, i32, i32, i32, vp, P(f32)]),
         "cl_decode_greedy_batch": (C.c_int, [vp, vp, i32, vp, i32, vp, P(f32)]),
+        "cl_decode_sample_batch": (C.c_int, [vp, vp, i32, vp, P(Sampling), vp, i32, vp, P(f32)]),
         "cl_decode_step_batch": (C.c_int, [vp, vp, i32, vp, vp, vp]),
         "cl_seq_fake_fill": (C.c_int, [vp, i32, i32]),
         "cl_time_dominant_kernel": (C.c_int, [vp, i32, i32, i32, P(f32), P(f32)]),
@@ -141,6 +142,7 @@ def lib():
         "cl_op_gemm_bf16": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, P(f32)]),
         "cl_op_attn_prefill": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, vp]),
         "cl_op_attn_prefill_variant": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, vp, i32, P(f32)]),
+        "cl_op_sample": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), vp, vp, i32, vp, vp]),
         "cl_op_synth_weights": (C.c_int, [C.c_int, u64, i32, i64, f32, vp]),
         "cl_tokenizer_load": (C.c_int, [C.c_char_p, C.c_char_p, P(vp)]),
         "cl_tokenizer_free": (None, [vp]),
@@ -350,6 +352,19 @@ class Engine:
         ms = C.c_float(0)
         _check(lib().cl_decode_greedy_batch(self._h, _ptr(seqs), len(seqs), _ptr(first), n_steps, _ptr(ids),
                                             C.byref(ms)), "cl_decode_greedy_batch")
+        return ids, ms.value
+
+    def decode_sample_batch(self, seqs, first_ids, samplings, n_steps: int, step0=None):
+        """cl_decode_sample_batch: like decode_greedy_batch, sequence b drawing with samplings[b] on the device (greedy where
+        its temperature is 0); draw i of sequence b uses RNG step step0[b] + i.  Returns (ids [n_steps][B], device ms)."""
+        seqs = np.ascontiguousarray(seqs, dtype=np.int32)
+        first = np.ascontiguousarray(first_ids, dtype=np.int32)
+        sp = (Sampling * len(seqs))(*samplings)
+        st = np.ascontiguousarray(step0 if step0 is not None else np.zeros(len(seqs)), dtype=np.uint64)
+        ids = np.empty((n_steps, len(seqs)), np.int32)
+        ms = C.c_float(0)
+        _check(lib().cl_decode_sample_batch(self._h, _ptr(seqs), len(seqs), _ptr(first), sp, _ptr(st), n_steps, _ptr(ids),
+                                            C.byref(ms)), "cl_decode_sample_batch")
         return ids, ms.value
 
     def decode_step_batch(self, seqs, toks, want_logits: bool = True):
@@ -583,6 +598,24 @@ def op_attn_prefill_variant(q_bf16, k_bf16, v_bf16, n_heads, n_kv, head_dim, var
     _check(lib().cl_op_attn_prefill_variant(device, variant, _ptr(q), _ptr(k), _ptr(v), t, n_heads, n_kv, head_dim, _ptr(out), iters,
                                             C.byref(ms)), "cl_op_attn_prefill_variant")
     return out, (ms.value if iters > 0 else None)
+
+
+def op_sample(logits, samplings, histories, steps, device=0):
+    """cl_op_sample: the step tail's device sampler on host logits [n_rows][vocab]; row r draws with samplings[r], history
+    histories[r] (a sequence of ids) at RNG step steps[r].  Returns the ids [n_rows]."""
+    lg = np.ascontiguousarray(np.atleast_2d(logits), dtype=np.float32)
+    rows = lg.shape[0]
+    stride = max(1, max(len(h) for h in histories))
+    hist = np.zeros((rows, stride), np.int32)
+    for r, h in enumerate(histories):
+        hist[r, :len(h)] = np.asarray(h, np.int32)
+    nh = np.ascontiguousarray([len(h) for h in histories], dtype=np.int32)
+    st = np.ascontiguousarray(steps, dtype=np.uint64)
+    sp = (Sampling * rows)(*samplings)
+    out = np.empty(rows, np.int32)
+    _check(lib().cl_op_sample(device, _ptr(lg), rows, lg.shape[1], sp, _ptr(hist), _ptr(nh), stride, _ptr(st), _ptr(out)),
+           "cl_op_sample")
+    return out
 
 
 def op_synth_weights(seed, key, n, scale, device=0):

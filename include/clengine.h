@@ -97,7 +97,12 @@ typedef struct cl_engine_config {
 
 /* Sampler.  The reference sends no options (api.go:109-118), so Ollama defaults apply upstream:
  * temperature 0.8, top_k 40, top_p 0.9, repeat_penalty 1.1 over the last 64 tokens, random seed.
- * temperature <= 0 selects greedy argmax with lowest-index tie-break (the parity mode). */
+ * temperature <= 0 selects greedy argmax with lowest-index tie-break (the parity mode).
+ * Where the draw runs: with temperature > 0, 1 <= top_k <= 128, top_k < vocab_size, vocab_size <= 163840, and the repeat
+ * penalty off (repeat_penalty 1 or repeat_last_n 0) or over 1..256 ids, the decode step's last kernel draws the token on
+ * the GPU, so the token loop never waits for the host (Ollama's defaults qualify).  Other settings (top_k 0,
+ * repeat_last_n -1, ...) run the host sampler on the step's logits.  Both draw the same id for the same logits, history,
+ * seed and step (cl_sample_token is the host one; env CL_DEVICE_SAMPLE=0 sends every request to it). */
 typedef struct cl_sampling {
   float temperature;
   int32_t top_k;
@@ -244,6 +249,14 @@ int cl_decode_greedy(cl_engine* e, cl_seq_t seq, int32_t first_id, int32_t n_ste
 int cl_decode_greedy_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs,
                            const int32_t* first_ids, int32_t n_steps, int32_t* ids_out,
                            float* device_ms);
+/* cl_decode_greedy_batch with the device sampler: sequence b draws with sp[b] (temperature <= 0: greedy argmax, so greedy
+ * and sampled sequences may share the batch); draw i of sequence b uses RNG step step0[b] + i (step0 may be NULL: 0)
+ * and the repeat-penalty window of the sequence's history plus the tokens fed.  The ids are the ones cl_sample_token
+ * draws on the logits of cl_decode_step_batch fed the same tokens.  CL_ERR_INVALID_ARG if some sp[b] needs the host
+ * sampler (see cl_sampling).  Kernel launches per step are those of cl_decode_greedy_batch. */
+int cl_decode_sample_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* first_ids,
+                           const cl_sampling* sp, const uint64_t* step0, int32_t n_steps, int32_t* ids_out,
+                           float* device_ms);
 /* One batched decode step with caller-chosen input tokens (teacher forcing for the parity tests of the batched
  * path): ids[n_seqs]; logits_out (host, may be NULL) receives [n_seqs][vocab_size] fp32; argmax_out (may be NULL)
  * the greedy next ids. */
@@ -308,6 +321,11 @@ int cl_op_attn_prefill(int device, const uint16_t* q, const uint16_t* k, const u
  * 1: wgmma kernel (attn_prefill_tc.cu, head_dim 128), -1: what the engine would pick — and an optional timing loop */
 int cl_op_attn_prefill_variant(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t,
                                int32_t n_heads, int32_t n_kv, int32_t head_dim, float* out, int32_t iters, float* ms);
+/* the decode step's device sampler (the step tail kernel) on host logits [n_rows][vocab]: row r draws with sp[r] at RNG
+ * step step[r], with history row r = history + r * hist_stride, n_history[r] ids (history may be NULL when every
+ * n_history[r] is 0).  ids_out[n_rows].  CL_ERR_INVALID_ARG for settings the device sampler does not cover. */
+int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
+                 const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out);
 /* synthetic weight generator (device kernel) -> host copy, for known-answer tests */
 int cl_op_synth_weights(int device, uint64_t seed, int32_t tensor_key, int64_t n, float scale,
                         uint16_t* out_bf16);
