@@ -119,6 +119,11 @@ int cl_engine_stats(cl_engine* e, cl_stats* out) {
   return e->impl.stats(out);
 }
 
+int cl_engine_prefix_stats(cl_engine* e, cl_prefix_stats* out) {
+  if (!e || !out) return CL_ERR_INVALID_ARG;
+  return e->impl.prefix_stats(out);   // like cl_engine_stats: no engine lock, so it never waits behind a scheduler iteration
+}
+
 int cl_engine_set_tensor(cl_engine* e, int32_t layer, int32_t kind, const uint16_t* data, int64_t n) {
   if (!e || !data) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
@@ -398,6 +403,15 @@ int cl_seq_len(cl_engine* e, cl_seq_t s, int32_t* len_out) {
   std::lock_guard<std::mutex> lk(e->impl.mu_);
   return e->impl.seq_len(s, len_out);
 }
+int cl_seq_attach_prefix(cl_engine* e, cl_seq_t s, const int32_t* ids, int32_t n, int32_t* n_reused) {
+  if (!e || !n_reused || n < 0 || (n > 0 && !ids)) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  int reused = 0;
+  int rc;
+  CL_GUARD(rc = e->impl.attach_prefix(s, ids, n, &reused);)
+  *n_reused = reused;
+  return rc;
+}
 int cl_prefill(cl_engine* e, cl_seq_t s, const int32_t* ids, int32_t n, float* logits_out) {
   if (!e || !ids) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
@@ -505,6 +519,24 @@ int cl_kvpool_used_pages(cl_kvpool* p) {
   if (!p) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(p->mu);
   return p->pool.used_pages();
+}
+int cl_kvpool_attach(cl_kvpool* p, int32_t owner, const int32_t* ids, int32_t n, int32_t* n_reused) {
+  if (!p || !n_reused || n < 0 || (n > 0 && !ids)) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(p->mu);
+  const int r = p->pool.attach(owner, ids, n);
+  if (r < 0) return r;
+  *n_reused = r;
+  return CL_OK;
+}
+int cl_kvpool_publish(cl_kvpool* p, int32_t owner, const int32_t* ids, int32_t n_known) {
+  if (!p || n_known < 0 || (n_known > 0 && !ids)) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(p->mu);
+  return p->pool.publish(owner, ids, n_known);
+}
+int cl_kvpool_cached_pages(cl_kvpool* p) {
+  if (!p) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(p->mu);
+  return p->pool.cached_pages();
 }
 
 }  // extern "C"

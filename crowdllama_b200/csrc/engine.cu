@@ -186,6 +186,7 @@ int Engine::init(const cl_engine_config& c) {
   prefill_small_max_ = std::min(256, env_int("CL_PREFILL_SMALL_MAX", kDefaultPrefillSmallMax));
   prefill_fused_ = env_int("CL_PREFILL_FUSED", kDefaultPrefillFused);
   device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
+  prefix_cache_ = env_int("CL_PREFIX_CACHE", c.prefix_cache) != 0;
   if (c.start_scheduler) start_scheduler();
   return CL_OK;
 }
@@ -434,6 +435,46 @@ int Engine::ensure_capacity(cl_seq_t s, int n_tokens) {
   if (pages.size() != before)
     CL_CUDA_OK(cudaMemcpyAsync(d_bt_ + (size_t)s * max_pages_per_seq_ + before, pages.data() + before,
                                (pages.size() - before) * 4, cudaMemcpyHostToDevice, stream_));
+  return CL_OK;
+}
+
+void Engine::seq_advance(cl_seq_t s, const int32_t* ids, int n, int n_known) {
+  auto& q = seqs_[s];
+  if (q.known == (int)q.history.size()) q.known += n_known;
+  q.len += n;
+  q.history.insert(q.history.end(), ids, ids + n);
+  if (prefix_cache_ && q.known >= page_size_) pool_->publish(s, q.history.data(), q.known);
+}
+
+// ---- prefix cache ---------------------------------------------------------------------------------
+int Engine::attach_prefix(cl_seq_t s, const int32_t* ids, int n, int* reused) {
+  *reused = 0;
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  if (!prefix_cache_) return CL_OK;
+  auto& q = seqs_[s];
+  if (q.len != 0 || !pool_->pages_of(s).empty()) { set_last_error("attach_prefix needs a new sequence (no tokens, no pages)"); return CL_ERR_INVALID_ARG; }
+  const int r = pool_->attach(s, ids, std::min(n, cfg.max_seq_len));   // >= 0: the owner has no pages
+  prefix_lookups_++;
+  prefix_tokens_looked_up_ += n;
+  prefix_tokens_reused_ += r;
+  if (r == 0) return CL_OK;
+  const auto& pages = pool_->pages_of(s);
+  CL_CUDA_OK(cudaMemcpyAsync(d_bt_ + (size_t)s * max_pages_per_seq_, pages.data(), pages.size() * 4, cudaMemcpyHostToDevice, stream_));
+  q.len = r;
+  q.known = r;
+  q.history.assign(ids, ids + r);
+  *reused = r;
+  return CL_OK;
+}
+
+int Engine::prefix_stats(cl_prefix_stats* out) {
+  memset(out, 0, sizeof *out);
+  out->enabled = prefix_cache_ ? 1 : 0;
+  out->cached_pages = pool_ ? pool_->cached_pages() : 0;
+  out->lookups = prefix_lookups_;
+  out->tokens_looked_up = prefix_tokens_looked_up_;
+  out->tokens_reused = prefix_tokens_reused_;
+  out->pages_evicted = pool_ ? pool_->evicted_pages() : 0;
   return CL_OK;
 }
 
@@ -726,8 +767,7 @@ int Engine::decode_step(cl_seq_t s, int32_t id, float* logits_out, int32_t* argm
   if (rc) return rc;
   rc = run_step_graph(1);
   if (rc) return rc;
-  q.len += 1;
-  q.history.push_back(id);
+  seq_advance(s, &id, 1, 1);
   if (logits_out) { rc = read_logits(s, logits_out); if (rc) return rc; }
   if (argmax_out) {
     CL_CUDA_OK(cudaMemcpyAsync(h_ids_pinned_, d_tok_ + s, 4, cudaMemcpyDeviceToHost, stream_));
@@ -761,8 +801,7 @@ int Engine::prefill_tokenwise(cl_seq_t s, const int32_t* ids, int n, float* logi
     rc = run_step_graph(1);
     if (rc) return rc;
   }
-  q.len += n;
-  q.history.insert(q.history.end(), ids, ids + n);
+  seq_advance(s, ids, n, n);
   if (logits_out) return read_logits(s, logits_out);
   CL_CUDA_OK(cudaStreamSynchronize(stream_));
   return CL_OK;
@@ -819,11 +858,11 @@ int Engine::decode_greedy(const cl_seq_t* ss, int B, const int32_t* first_ids, i
       for (int b = 0; b < B; ++b) ids_out[(size_t)(done + i) * B + b] = h_ids_pinned_[(size_t)i * max_batch_ + b];
     done += chunk;
   }
-  for (int b = 0; b < B; ++b) {
-    auto& q = seqs_[ss[b]];
-    q.history.push_back(first_ids[b]);
-    for (int i = 0; i + 1 < n_steps; ++i) q.history.push_back(ids_out[(size_t)i * B + b]);
-    q.len += n_steps;
+  std::vector<int32_t> fed((size_t)n_steps);
+  for (int b = 0; b < B; ++b) {   // step i was fed first_ids[b], then the id of step i - 1: all read back, all known
+    fed[0] = first_ids[b];
+    for (int i = 0; i + 1 < n_steps; ++i) fed[(size_t)i + 1] = ids_out[(size_t)i * B + b];
+    seq_advance(ss[b], fed.data(), n_steps, n_steps);
   }
   tokens_generated_ += (int64_t)n_steps * B;
   if (total_ms > 0.f) {
@@ -870,7 +909,8 @@ int Engine::seq_fake_fill(cl_seq_t s, int n_tokens) {
   launches_ += n;
   CL_CUDA_OK(cudaStreamSynchronize(stream_));
   seqs_[s].len = n_tokens;
-  seqs_[s].history.assign((size_t)n_tokens, 0);
+  seqs_[s].history.assign((size_t)n_tokens, 0);   // placeholders under a synthetic cache: never published
+  seqs_[s].known = 0;
   return CL_OK;
 }
 
@@ -913,9 +953,7 @@ int Engine::decode_step_batch(const cl_seq_t* ss, int B, const int32_t* ids, flo
   const int rc = run_step_graph(B);
   if (rc) return rc;
   for (int b = 0; b < B; ++b) {
-    auto& q = seqs_[ss[b]];
-    q.len += 1;
-    q.history.push_back(ids[b]);
+    seq_advance(ss[b], &ids[b], 1, 1);
     if (logits_out) { const int r2 = read_logits(ss[b], logits_out + (size_t)b * cfg.vocab_size); if (r2) return r2; }
   }
   if (argmax_out) {
@@ -963,10 +1001,12 @@ int Engine::time_dominant_kernel(cl_seq_t s, int32_t first_id, int n_steps, floa
     if (step_ms) *step_ms = ms / n_steps;
     // the device advanced tok/pos itself; mirror it on the host
     CL_CUDA_OK(cudaMemcpy(h_ids_pinned_, d_ids_ring_, (size_t)std::min(n_steps, ring_steps_) * max_batch_ * 4, cudaMemcpyDeviceToHost));
-    auto& q = seqs_[s];
-    q.history.push_back(first_id);
-    for (int i = 0; i + 1 < n_steps; ++i) q.history.push_back(i < ring_steps_ ? h_ids_pinned_[(size_t)i * max_batch_] : 0);
-    q.len += n_steps;
+    // The id ring holds the last ring_steps_ ids: with more steps, step i's id was overwritten by step i + ring_steps_'s
+    // and the ids after the ring are zeros.  Only first_id is known then, and nothing after it is ever published.
+    std::vector<int32_t> fed((size_t)n_steps, 0);
+    fed[0] = first_id;
+    for (int i = 0; i + 1 < n_steps && i < ring_steps_; ++i) fed[(size_t)i + 1] = h_ids_pinned_[(size_t)i * max_batch_];
+    seq_advance(s, fed.data(), n_steps, n_steps <= ring_steps_ ? n_steps : 1);
     tokens_generated_ += n_steps;
   }
   for (auto& e : ev) cudaEventDestroy(e);

@@ -6,6 +6,7 @@
 #include <atomic>
 #include <condition_variable>
 #include <deque>
+#include <list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -66,22 +67,56 @@ class LaunchProfiler {
   } while (0)
 
 // ---- paged-KV allocator: host-side free list + per-owner page lists (no GPU needed) -----------
+// Prefix sharing: a full page whose P tokens are known can be published into an index keyed by (entry uid of the previous
+// page of the chain, the page's P token ids), compared exactly.  Chains start at kRootUid.  A page is then free, referenced
+// by one or more owners (refcount), or cached: refcount 0 but still indexed, on an LRU list that reserve() evicts from
+// once the free list is empty.  Attached pages are read-only for their owners: every kernel writes K/V only at positions
+// >= the sequence's length, and attach() leaves at least one token of the prompt to compute.  Without attach / publish
+// the allocator hands out exactly the pages it always did.
 class KvPool {
  public:
+  static constexpr uint64_t kRootUid = 0;
   KvPool(int n_pages, int page_size);
-  int reserve(int owner, int n_tokens);  // CL_OK / CL_ERR_OOM (atomic: nothing taken on failure)
-  int release(int owner);
+  int reserve(int owner, int n_tokens);  // CL_OK / CL_ERR_OOM (atomic: nothing taken on failure); evicts cached pages last
+  int release(int owner);                // published pages whose refcount drops to 0 become cached, the rest free
+  // Only on an owner without pages: takes the longest indexed chain matching ids[0..n), at most P * floor((n - 1) / P)
+  // tokens.  Returns the tokens reused (>= 0) or CL_ERR_INVALID_ARG.
+  int attach(int owner, const int32_t* ids, int n);
+  // Tokens attach() would reuse, without taking anything; *cached_pages (may be nullptr): how many of the matching pages
+  // are cached (attaching them takes them out of free_pages()).
+  int lookup(const int32_t* ids, int n, int* cached_pages) const;
+  // Index the owner's full pages covering ids[0..n_known) not published yet.  A page whose key is already indexed stays private.
+  int publish(int owner, const int32_t* ids, int n_known);
   const std::vector<int>& pages_of(int owner);
-  int free_pages() const { return (int)free_.size(); }
-  int used_pages() const { return n_pages_ - (int)free_.size(); }
+  int free_pages() const { return (int)free_.size() + (int)lru_.size(); }   // allocatable: free + cached
+  int used_pages() const { return n_pages_ - free_pages(); }                // referenced by some owner
+  int cached_pages() const { return (int)lru_.size(); }
+  int64_t evicted_pages() const { return evicted_; }
   int n_pages() const { return n_pages_; }
   int page_size() const { return page_size_; }
 
  private:
+  struct Key {
+    uint64_t parent;
+    std::vector<int32_t> ids;
+    bool operator<(const Key& o) const { return parent != o.parent ? parent < o.parent : ids < o.ids; }
+  };
+  struct Chain { int published = 0; uint64_t tail = kRootUid; };   // leading pages indexed (or matched), uid of the last
+  int walk(const int32_t* ids, int n, std::vector<int>* pages) const;
   int n_pages_, page_size_;
   std::vector<int> free_;  // stack; low page ids are handed out first
   std::map<int, std::vector<int>> owned_;
   std::vector<int> empty_;
+  // prefix sharing
+  std::map<Key, int> index_;                       // -> page
+  std::vector<std::map<Key, int>::iterator> entry_;   // page -> its index entry (index_.end(): not published)
+  std::vector<uint64_t> uid_;                      // page -> uid of its entry
+  std::vector<int> ref_;                           // page -> owners holding it
+  std::list<int> lru_;                             // cached pages, evicted from the front
+  std::vector<std::list<int>::iterator> lru_pos_;
+  std::map<int, Chain> chain_;
+  uint64_t next_uid_ = kRootUid + 1;
+  int64_t evicted_ = 0;
 };
 
 // ---- tokenizers ---------------------------------------------------------------------------------
@@ -171,6 +206,7 @@ struct LayerWeights {
 struct SeqState {
   bool live = false;
   int len = 0;            // tokens whose K/V are in the cache
+  int known = 0;          // leading history ids that are the real tokens of the cached K/V (seq_fake_fill's are not)
   std::vector<int32_t> history;
 };
 
@@ -186,6 +222,11 @@ class Engine {
   int seq_create(cl_seq_t* out);
   int seq_free(cl_seq_t s);
   int seq_len(cl_seq_t s, int32_t* out) { if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ; *out = seqs_[s].len; return CL_OK; }
+  // Prefix cache (CL_PREFIX_CACHE / cl_engine_config.prefix_cache): a live sequence with len 0 takes the cached pages of
+  // the longest page-aligned prefix of ids[0..n), at most n - 1 tokens; len = *reused.  A no-op (0) with the cache off.
+  int attach_prefix(cl_seq_t s, const int32_t* ids, int n, int* reused);
+  bool prefix_cache() const { return prefix_cache_; }
+  int prefix_stats(cl_prefix_stats* out);
   int prefill(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
   // several prompts in one pass of the tile path (prefill.cu); logits_out: [n_seqs][vocab] or nullptr
   int prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* ids, const int* lens, float* logits_out);
@@ -231,6 +272,10 @@ class Engine {
   int fill_synthetic(uint64_t seed);
   int alloc_state();
   int ensure_capacity(cl_seq_t s, int n_tokens);  // reserve pages + upload block table row
+  // Every call that appends K/V to sequence s ends here: len += n, ids join the history, and with the prefix cache on the
+  // full pages whose tokens are all known are published.  The first n_known ids are real tokens; a placeholder stops
+  // publishing for the rest of the sequence.  The work that wrote the pages is already on stream_, ahead of any reader.
+  void seq_advance(cl_seq_t s, const int32_t* ids, int n, int n_known);
   int enqueue_step(int B);                         // kernels of one token step for d_slots_[0..B)
   int enqueue_step_batched(int B);                 // B >= 2: wgmma projections + per-sequence glue kernels
   int enqueue_lm_head(int B, bool pdl);            // final norm + LM-head GEMV of d_h_ -> d_logits_ for d_slots_[0..B)
@@ -318,6 +363,8 @@ class Engine {
 
   std::unique_ptr<KvPool> pool_;
   std::vector<SeqState> seqs_;
+  bool prefix_cache_ = false;         // share full KV pages across sequences with the same prefix (CL_PREFIX_CACHE)
+  std::atomic<int64_t> prefix_lookups_{0}, prefix_tokens_looked_up_{0}, prefix_tokens_reused_{0};
   std::map<int, cudaGraphExec_t> graphs_;
   std::map<int, int> graph_nodes_;
   int prefill_min_tokens_ = 16;

@@ -18,24 +18,97 @@ const char* get_last_error() { return g_last_error.c_str(); }
 KvPool::KvPool(int n_pages, int page_size) : n_pages_(n_pages), page_size_(page_size) {
   free_.reserve(n_pages);
   for (int i = n_pages - 1; i >= 0; --i) free_.push_back(i);
+  entry_.assign(n_pages, index_.end());
+  uid_.assign(n_pages, kRootUid);
+  ref_.assign(n_pages, 0);
+  lru_pos_.assign(n_pages, lru_.end());
 }
 int KvPool::reserve(int owner, int n_tokens) {
   auto& v = owned_[owner];
   const int need = (n_tokens + page_size_ - 1) / page_size_;
   const int extra = need - (int)v.size();
   if (extra <= 0) return CL_OK;
-  if (extra > (int)free_.size()) return CL_ERR_OOM;
+  if (extra > free_pages()) return CL_ERR_OOM;
   for (int i = 0; i < extra; ++i) {
-    v.push_back(free_.back());
-    free_.pop_back();
+    int p;
+    if (!free_.empty()) {
+      p = free_.back();
+      free_.pop_back();
+    } else {   // evict the least recently released cached page; its index entry goes with it
+      p = lru_.front();
+      lru_.pop_front();
+      lru_pos_[p] = lru_.end();
+      index_.erase(entry_[p]);
+      entry_[p] = index_.end();
+      ++evicted_;
+    }
+    ref_[p] = 1;
+    v.push_back(p);
   }
   return CL_OK;
 }
 int KvPool::release(int owner) {
+  chain_.erase(owner);
   auto it = owned_.find(owner);
   if (it == owned_.end()) return CL_OK;
-  for (auto rit = it->second.rbegin(); rit != it->second.rend(); ++rit) free_.push_back(*rit);
+  // deepest page first: a chain is reachable only from its root, so the LRU must evict its leaves before its root
+  for (auto rit = it->second.rbegin(); rit != it->second.rend(); ++rit) {
+    const int p = *rit;
+    if (--ref_[p] > 0) continue;
+    if (entry_[p] != index_.end()) lru_pos_[p] = lru_.insert(lru_.end(), p);
+    else free_.push_back(p);
+  }
   owned_.erase(it);
+  return CL_OK;
+}
+int KvPool::walk(const int32_t* ids, int n, std::vector<int>* pages) const {
+  const int max_pages = n > 1 ? (n - 1) / page_size_ : 0;   // at least one token is left to compute
+  Key key{kRootUid, {}};
+  for (int k = 0; k < max_pages; ++k) {
+    key.ids.assign(ids + (size_t)k * page_size_, ids + (size_t)(k + 1) * page_size_);
+    auto it = index_.find(key);
+    if (it == index_.end()) break;
+    pages->push_back(it->second);
+    key.parent = uid_[it->second];
+  }
+  return (int)pages->size() * page_size_;
+}
+int KvPool::lookup(const int32_t* ids, int n, int* cached_pages) const {
+  std::vector<int> pages;
+  const int tokens = walk(ids, n, &pages);
+  if (cached_pages) *cached_pages = (int)std::count_if(pages.begin(), pages.end(), [&](int p) { return ref_[p] == 0; });
+  return tokens;
+}
+int KvPool::attach(int owner, const int32_t* ids, int n) {
+  auto& v = owned_[owner];
+  if (!v.empty()) return CL_ERR_INVALID_ARG;
+  const int tokens = walk(ids, n, &v);
+  for (int p : v)
+    if (ref_[p]++ == 0) {   // cached -> referenced
+      lru_.erase(lru_pos_[p]);
+      lru_pos_[p] = lru_.end();
+    }
+  chain_[owner] = Chain{(int)v.size(), v.empty() ? kRootUid : uid_[v.back()]};
+  return tokens;
+}
+int KvPool::publish(int owner, const int32_t* ids, int n_known) {
+  auto it = owned_.find(owner);
+  if (it == owned_.end()) return CL_OK;
+  const std::vector<int>& v = it->second;
+  Chain& c = chain_[owner];
+  for (int k = c.published; k < (int)v.size() && (int64_t)(k + 1) * page_size_ <= n_known; ++k) {
+    Key key{c.tail, std::vector<int32_t>(ids + (size_t)k * page_size_, ids + (size_t)(k + 1) * page_size_)};
+    auto f = index_.find(key);
+    if (f != index_.end()) {   // the same tokens are indexed on another page: this one stays private, the chain goes on there
+      c.tail = uid_[f->second];
+    } else {
+      const int p = v[k];
+      entry_[p] = index_.emplace(std::move(key), p).first;
+      uid_[p] = next_uid_++;
+      c.tail = uid_[p];
+    }
+    c.published = k + 1;
+  }
   return CL_OK;
 }
 const std::vector<int>& KvPool::pages_of(int owner) {

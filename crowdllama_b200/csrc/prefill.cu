@@ -103,8 +103,7 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   CL_LAUNCH(enqueue_step_tail(1, false));
   prof.report("prefill profile", 32, "short-prompt path, " + std::to_string(n) + " tokens");
   launches_ += launches;
-  q.len += n;
-  q.history.insert(q.history.end(), ids, ids + n);
+  seq_advance(s, ids, n, n);
   if (logits_out) return read_logits(s, logits_out);
   CL_CUDA_OK(cudaStreamSynchronize(stream_));
   return CL_OK;
@@ -199,8 +198,7 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
   CL_LAUNCH(enqueue_step_tail(1, false));
   prof.report("prefill profile", 32, "tile path, " + std::to_string(n) + " tokens");
   launches_ += launches;
-  q.len += n;
-  q.history.insert(q.history.end(), ids, ids + n);
+  seq_advance(s, ids, n, n);
   if (logits_out) return read_logits(s, logits_out);
   CL_CUDA_OK(cudaStreamSynchronize(stream_));
   return CL_OK;
@@ -299,11 +297,7 @@ int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* 
   CL_LAUNCH(enqueue_step_tail(n_seqs, false));
   prof.report("prefill profile", 32, "multi-prompt tile path, " + std::to_string(total) + " tokens");
   launches_ += launches;
-  for (int i = 0; i < n_seqs; ++i) {
-    auto& q = seqs_[ss[i]];
-    q.len += lens[i];
-    q.history.insert(q.history.end(), ids[i], ids[i] + lens[i]);
-  }
+  for (int i = 0; i < n_seqs; ++i) seq_advance(ss[i], ids[i], lens[i], lens[i]);
   if (logits_out) {
     for (int i = 0; i < n_seqs; ++i)
       if ((rc = read_logits(ss[i], logits_out + (size_t)i * V))) return rc;

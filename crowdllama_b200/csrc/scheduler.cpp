@@ -90,9 +90,12 @@ static int generate_sync(Engine& e, Request& r, const Engine::TokenSink* sink) {
   if (rc) return rc;
   std::vector<float> logits(V);
   int64_t t0 = now_ns();
+  // prefix cache: the prompt's cached pages are taken over, only the rest is prefilled (reused = 0 with the cache off)
+  int reused = 0;
+  rc = e.attach_prefix(r.seq, r.prompt.data(), (int)r.prompt.size(), &reused);
   // a device-sampled request is armed before the prefill, whose tail then draws the first token
-  if (r.dev_sample) rc = e.arm_sampling(r.seq, r.sp, 0, r.prompt.data(), (int)r.prompt.size());
-  if (rc == CL_OK) rc = e.prefill(r.seq, r.prompt.data(), (int)r.prompt.size(), r.dev_sample ? nullptr : logits.data());
+  if (rc == CL_OK && r.dev_sample) rc = e.arm_sampling(r.seq, r.sp, 0, r.prompt.data(), (int)r.prompt.size());
+  if (rc == CL_OK) rc = e.prefill(r.seq, r.prompt.data() + reused, (int)r.prompt.size() - reused, r.dev_sample ? nullptr : logits.data());
   r.prefill_ns = now_ns() - t0;
   if (rc) { e.seq_free(r.seq); return rc; }
   t0 = now_ns();
@@ -269,10 +272,20 @@ void Engine::scheduler_main() {
         for (auto& r : queue_) {
           if ((int)(active_.size() + group.size()) >= max_batch_) break;
           const int n = (int)(r->prompt.size() + r->out.size());
-          const int need = (n + 1 + page_size_ - 1) / page_size_;
-          if (r->cancel.load(std::memory_order_relaxed) || tokens + n > cap_tokens || pages + need > pool_->free_pages()) break;
+          int need = (n + 1 + page_size_ - 1) / page_size_;
+          int hit = 0;   // prefix cache: tokens the member will attach instead of computing
+          if (prefix_cache_) {
+            // Attaching a cached page takes it out of free_pages(): count those pages as needed too (an upper bound
+            // when members share pages), so that every member's reserve succeeds after all of them have attached.
+            r->full.assign(r->prompt.begin(), r->prompt.end());
+            r->full.insert(r->full.end(), r->out.begin(), r->out.end());
+            int cached = 0;
+            hit = pool_->lookup(r->full.data(), n, &cached);
+            need += cached - hit / page_size_;
+          }
+          if (r->cancel.load(std::memory_order_relaxed) || tokens + n - hit > cap_tokens || pages + need > pool_->free_pages()) break;
           group.push_back(r);
-          tokens += n;
+          tokens += n - hit;
           pages += need;
         }
         if (group.size() >= 2) queue_.erase(queue_.begin(), queue_.begin() + (long)group.size());
@@ -282,16 +295,24 @@ void Engine::scheduler_main() {
         std::vector<const int32_t*> ptrs;
         std::vector<int> lens;
         int rc = CL_OK, total = 0;
+        // every member attaches its cached prefix before any of them reserves: a reserve may evict cached pages
         for (auto& r : group) {
           r->full.assign(r->prompt.begin(), r->prompt.end());
           r->full.insert(r->full.end(), r->out.begin(), r->out.end());
           rc = seq_create(&r->seq);
-          if (rc == CL_OK) rc = ensure_capacity(r->seq, (int)r->full.size() + 1);
+          int reused = 0;
+          if (rc == CL_OK) rc = attach_prefix(r->seq, r->full.data(), (int)r->full.size(), &reused);
+          if (rc) break;
+          r->prefilled = reused;
+        }
+        for (size_t i = 0; rc == CL_OK && i < group.size(); ++i) {
+          auto& r = group[i];
+          rc = ensure_capacity(r->seq, (int)r->full.size() + 1);
           // the pass's tail draws the next token of a device-sampled request (step = tokens generated before a preemption)
           if (rc == CL_OK && r->dev_sample) rc = arm_sampling(r->seq, r->sp, r->out.size(), r->full.data(), (int)r->full.size());
           if (rc) break;
-          ss.push_back(r->seq); ptrs.push_back(r->full.data()); lens.push_back((int)r->full.size());
-          total += (int)r->full.size();
+          ss.push_back(r->seq); ptrs.push_back(r->full.data() + r->prefilled); lens.push_back((int)(r->full.size() - r->prefilled));
+          total += lens.back();
         }
         const int64_t t0 = now_ns();
         if (rc == CL_OK) rc = prefill_multi((int)ss.size(), ss.data(), ptrs.data(), lens.data(), nullptr);
@@ -341,7 +362,12 @@ void Engine::scheduler_main() {
         if (r) {
           r->full.assign(r->prompt.begin(), r->prompt.end());
           r->full.insert(r->full.end(), r->out.begin(), r->out.end());
-          const int need_pages = ((int)r->full.size() + 1 + page_size_ - 1) / page_size_;
+          // prefix cache: only the pages the prompt does not find cached count against the pool.  Attaching takes the
+          // cached ones out of free_pages(), so they are counted as needed too: the check equals attaching first and
+          // then comparing the missing pages with what is left, without attaching while the request has to wait.
+          int hit = 0, cached = 0;
+          if (prefix_cache_) hit = pool_->lookup(r->full.data(), (int)r->full.size(), &cached);
+          const int need_pages = ((int)r->full.size() + 1 + page_size_ - 1) / page_size_ - hit / page_size_ + cached;
           if (need_pages > pool_->free_pages()) {
             if (active_.empty()) {
               { std::lock_guard<std::mutex> lk(q_mu_); queue_.pop_front(); }
@@ -351,10 +377,12 @@ void Engine::scheduler_main() {
             // else: wait for running requests to release pages
           } else {
             { std::lock_guard<std::mutex> lk(q_mu_); queue_.pop_front(); }
+            int reused = 0;
             int rc = seq_create(&r->seq);
+            if (rc == CL_OK) rc = attach_prefix(r->seq, r->full.data(), (int)r->full.size(), &reused);   // takes `hit` tokens
             if (rc == CL_OK) rc = ensure_capacity(r->seq, (int)r->full.size() + 1);   // all pages up front: a later chunk cannot run dry
             if (rc) { if (r->seq >= 0) seq_free(r->seq); r->seq = -1; complete(r, rc, get_last_error()); continue; }
-            r->prefilled = 0;
+            r->prefilled = reused;
             prefilling_ = r;
           }
         }
@@ -470,8 +498,7 @@ void Engine::scheduler_main() {
     for (int b = 0; b < B; ++b) {
       auto& r = active_[b];
       auto& st = seqs_[r->seq];
-      st.history.push_back(r->out.back());
-      st.len += 1;
+      seq_advance(r->seq, &r->out.back(), 1, 1);
       int32_t next = toks[r->seq];
       if (!r->device_next()) {
         read_logits(r->seq, logits.data());

@@ -37,7 +37,7 @@ class EngineConfig(C.Structure):
                 ("model", ModelConfig), ("weights_path", C.c_char_p), ("weights_seed", C.c_uint64),
                 ("kv_pool_bytes", C.c_int64), ("page_size", C.c_int32), ("max_batch", C.c_int32),
                 ("max_seqs", C.c_int32), ("use_cuda_graph", C.c_int32), ("decode_path", C.c_int32),
-                ("start_scheduler", C.c_int32), ("reserved", C.c_int32 * 8)]
+                ("start_scheduler", C.c_int32), ("prefix_cache", C.c_int32), ("reserved", C.c_int32 * 7)]
 
 
 class Sampling(C.Structure):
@@ -62,17 +62,23 @@ class Stats(C.Structure):
                 ("sched_prefill_calls", C.c_int64), ("sched_prefill_tokens", C.c_int64), ("sched_prefill_ns", C.c_int64)]
 
 
+class PrefixStats(C.Structure):
+    _fields_ = [("enabled", C.c_int32), ("cached_pages", C.c_int32), ("lookups", C.c_int64), ("tokens_looked_up", C.c_int64),
+                ("tokens_reused", C.c_int64), ("pages_evicted", C.c_int64), ("reserved", C.c_int64 * 4)]
+
+
 # every symbol include/clengine.h declares (tests check the library exports all of them)
 EXPORTS = [
     "cl_abi_version", "cl_strerror", "cl_last_error", "cl_default_engine_config", "cl_default_sampling",
     "cl_greedy_sampling", "cl_sample_token", "cl_model_preset", "cl_engine_create", "cl_engine_destroy", "cl_engine_model_config",
-    "cl_engine_stats", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
+    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
-    "cl_seq_len", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
+    "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
     "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
     "cl_op_gemm_bf16", "cl_op_attn_prefill", "cl_op_attn_prefill_variant", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
+    "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages",
     "cl_tokenizer_load", "cl_tokenizer_free", "cl_tokenizer_encode", "cl_tokenizer_decode", "cl_tokenizer_info", "cl_engine_load_tokenizer",
 ]
 
@@ -106,6 +112,7 @@ def lib():
         "cl_engine_destroy": (None, [vp]),
         "cl_engine_model_config": (C.c_int, [vp, P(ModelConfig)]),
         "cl_engine_stats": (C.c_int, [vp, P(Stats)]),
+        "cl_engine_prefix_stats": (C.c_int, [vp, P(PrefixStats)]),
         "cl_engine_set_tensor": (C.c_int, [vp, i32, i32, vp, i64]),
         "cl_checkpoint_info": (C.c_int, [C.c_char_p, P(ModelConfig), P(i32), P(i64)]),
         "cl_generate": (C.c_int, [vp, C.c_char_p, C.c_char_p, sz, P(Sampling), P(Result)]),
@@ -121,6 +128,7 @@ def lib():
         "cl_sample_token": (C.c_int, [vp, i32, vp, vp, i32, C.c_uint64, P(i32)]),
         "cl_seq_free": (C.c_int, [vp, i32]),
         "cl_seq_len": (C.c_int, [vp, i32, P(i32)]),
+        "cl_seq_attach_prefix": (C.c_int, [vp, i32, vp, i32, P(i32)]),
         "cl_prefill": (C.c_int, [vp, i32, vp, i32, vp]),
         "cl_prefill_batch": (C.c_int, [vp, vp, i32, vp, vp, vp]),
         "cl_decode_step": (C.c_int, [vp, i32, i32, vp, P(i32)]),
@@ -157,6 +165,9 @@ def lib():
         "cl_kvpool_pages_of": (C.c_int, [vp, i32, vp, i32, P(i32)]),
         "cl_kvpool_free_pages": (C.c_int, [vp]),
         "cl_kvpool_used_pages": (C.c_int, [vp]),
+        "cl_kvpool_attach": (C.c_int, [vp, i32, vp, i32, P(i32)]),
+        "cl_kvpool_publish": (C.c_int, [vp, i32, vp, i32]),
+        "cl_kvpool_cached_pages": (C.c_int, [vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -251,7 +262,7 @@ class Engine:
     def __init__(self, preset: str | None = None, model: dict | None = None, model_name: str | None = None,
                  device: int = 0, seed: int = 1234, max_batch: int = 8, max_seqs: int | None = None,
                  page_size: int = 32, kv_pool_bytes: int = 0, use_cuda_graph: bool = True, decode_path: int = 0,
-                 start_scheduler: bool = False, weights_path: str | None = None):
+                 start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -273,6 +284,7 @@ class Engine:
         cfg.use_cuda_graph = 1 if use_cuda_graph else -1
         cfg.decode_path = decode_path
         cfg.start_scheduler = 1 if start_scheduler else 0
+        cfg.prefix_cache = 1 if prefix_cache else 0     # env CL_PREFIX_CACHE=0|1 overrides
         h = C.c_void_p()
         _check(L.cl_engine_create(C.byref(cfg), C.byref(h)), "cl_engine_create")
         self._h = h
@@ -315,6 +327,14 @@ class Engine:
     def seq_len(self, s: int) -> int:
         n = C.c_int32()
         _check(lib().cl_seq_len(self._h, s, C.byref(n)), "cl_seq_len")
+        return n.value
+
+    def attach_prefix(self, s: int, ids) -> int:
+        """cl_seq_attach_prefix: a new sequence takes the cached K/V of the longest page-aligned prefix of ids (at most
+        len(ids) - 1 tokens); returns the tokens reused, after which the caller prefills ids[reused:].  0 with the cache off."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        n = C.c_int32(0)
+        _check(lib().cl_seq_attach_prefix(self._h, s, _ptr(ids), len(ids), C.byref(n)), "cl_seq_attach_prefix")
         return n.value
 
     def prefill(self, s: int, ids, want_logits: bool = True):
@@ -501,6 +521,12 @@ class Engine:
         d = {n: getattr(st, n) for n, _ in st._fields_}
         d["gpu_model"] = st.gpu_model.decode(errors="replace")
         return d
+
+    def prefix_stats(self) -> dict:
+        """cl_engine_prefix_stats: enabled, cached_pages, lookups, tokens_looked_up, tokens_reused, pages_evicted."""
+        st = PrefixStats()
+        _check(lib().cl_engine_prefix_stats(self._h, C.byref(st)), "cl_engine_prefix_stats")
+        return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved"}
 
 
 # ---- single-op wrappers (host numpy in / out) -----------------------------------------------------
@@ -703,3 +729,19 @@ class KvPool:
     @property
     def used_pages(self) -> int:
         return lib().cl_kvpool_used_pages(self._h)
+
+    def attach(self, owner: int, ids) -> int:
+        """Take the longest published page chain matching ids (owner must hold no pages); returns the tokens reused."""
+        a = np.ascontiguousarray(ids, dtype=np.int32)
+        n = C.c_int32(0)
+        _check(lib().cl_kvpool_attach(self._h, owner, _ptr(a), len(a), C.byref(n)), "cl_kvpool_attach")
+        return n.value
+
+    def publish(self, owner: int, ids, n_known: int | None = None) -> int:
+        """Index the owner's full pages covering ids[:n_known] (default: all of ids)."""
+        a = np.ascontiguousarray(ids, dtype=np.int32)
+        return lib().cl_kvpool_publish(self._h, owner, _ptr(a), len(a) if n_known is None else min(n_known, len(a)))
+
+    @property
+    def cached_pages(self) -> int:
+        return lib().cl_kvpool_cached_pages(self._h)

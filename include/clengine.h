@@ -92,7 +92,12 @@ typedef struct cl_engine_config {
   int32_t use_cuda_graph;  /* 1 => capture the token step in a CUDA graph (default 1; -1 => 0) */
   int32_t decode_path;     /* 0 auto, 1 = generic LDG GEMV kernels, 2 = TMA-ring streaming GEMV */
   int32_t start_scheduler; /* 1 => start the continuous-batching thread behind cl_generate */
-  int32_t reserved[8];
+  int32_t prefix_cache;    /* 1 => reuse the cached KV pages of earlier requests that share a prompt prefix (default 0;
+                              env CL_PREFIX_CACHE=0|1 overrides).  Full pages of known tokens stay indexed after their
+                              sequence is freed and are evicted least recently used first when the pool runs dry, so a
+                              request whose prompt starts with an earlier prompt (or a preempted request coming back)
+                              prefills only the rest.  See cl_seq_attach_prefix / cl_engine_prefix_stats. */
+  int32_t reserved[7];
 } cl_engine_config;
 
 /* Sampler.  The reference sends no options (api.go:109-118), so Ollama defaults apply upstream:
@@ -149,6 +154,17 @@ typedef struct cl_stats {
   int64_t sched_prefill_calls, sched_prefill_tokens, sched_prefill_ns;
 } cl_stats;
 
+/* Prefix cache accounting since engine creation (all zero with the cache off). */
+typedef struct cl_prefix_stats {
+  int32_t enabled;
+  int32_t cached_pages;      /* now: pages no sequence holds that are kept for reuse (counted as free in cl_stats) */
+  int64_t lookups;           /* sequences that looked their prompt up (cl_seq_attach_prefix, every request admission) */
+  int64_t tokens_looked_up;  /* prompt tokens of those lookups */
+  int64_t tokens_reused;     /* of which found in the cache: their prefill was skipped */
+  int64_t pages_evicted;     /* cached pages handed out again because the pool ran dry */
+  int64_t reserved[4];
+} cl_prefix_stats;
+
 typedef struct cl_engine cl_engine;
 typedef int32_t cl_seq_t;
 
@@ -173,6 +189,7 @@ int cl_engine_create(const cl_engine_config* cfg, cl_engine** out);
 void cl_engine_destroy(cl_engine* e);
 int cl_engine_model_config(const cl_engine* e, cl_model_config* out);
 int cl_engine_stats(cl_engine* e, cl_stats* out);
+int cl_engine_prefix_stats(cl_engine* e, cl_prefix_stats* out);
 /* Overwrite one weight tensor from host memory (bf16 bits, logical [out][in] row-major; norm
  * gains as bf16 too).  kind: 0 embed, 1 lm_head, 2 final_norm, 3 attn_norm, 4 wq, 5 wk, 6 wv,
  * 7 wo, 8 ffn_norm, 9 w_gate, 10 w_up, 11 w_down (same numbering as the synthetic generator).
@@ -228,6 +245,12 @@ int cl_detokenize(cl_engine* e, const int32_t* ids, int32_t n, char* buf, size_t
 int cl_seq_create(cl_engine* e, cl_seq_t* out);
 int cl_seq_free(cl_engine* e, cl_seq_t seq);
 int cl_seq_len(cl_engine* e, cl_seq_t seq, int32_t* len_out);
+/* Prefix cache, token level: on a new sequence (length 0), take the cached K/V of the longest page-aligned prefix of
+ * ids[0..n) that an earlier sequence computed, at most n - 1 tokens (the last position is always computed, so the
+ * caller gets its logits).  *n_reused = the sequence's length afterwards; the caller then cl_prefills ids[n_reused..n).
+ * Shared pages are read-only: every later write lands at positions >= the sequence's length, on pages of its own.
+ * With the cache off *n_reused = 0 and nothing changes. */
+int cl_seq_attach_prefix(cl_engine* e, cl_seq_t seq, const int32_t* ids, int32_t n, int32_t* n_reused);
 /* Append n prompt tokens to the sequence.  logits_out (host, may be NULL) receives the
  * vocab_size fp32 logits of the LAST position. */
 int cl_prefill(cl_engine* e, cl_seq_t seq, const int32_t* ids, int32_t n, float* logits_out);
@@ -356,8 +379,16 @@ void cl_kvpool_destroy(cl_kvpool* p);
 int cl_kvpool_reserve(cl_kvpool* p, int32_t owner, int32_t n_tokens);
 int cl_kvpool_release(cl_kvpool* p, int32_t owner);
 int cl_kvpool_pages_of(cl_kvpool* p, int32_t owner, int32_t* pages, int32_t cap, int32_t* n_out);
-int cl_kvpool_free_pages(cl_kvpool* p);
-int cl_kvpool_used_pages(cl_kvpool* p);
+int cl_kvpool_free_pages(cl_kvpool* p);   /* allocatable: free + cached */
+int cl_kvpool_used_pages(cl_kvpool* p);   /* held by some owner */
+/* Prefix sharing (what the engine's prefix cache runs on).  attach: only on an owner without pages; takes the longest
+ * published page chain matching ids[0..n), at most page_size * floor((n - 1) / page_size) tokens, into the owner's page
+ * list (*n_reused tokens).  publish: index the owner's full pages covering ids[0..n_known) (incremental; a page whose
+ * tokens and prefix are already indexed stays private).  Published pages outlive their owners as cached pages, which
+ * reserve hands out (least recently released first, deepest page of a chain first) once no free page is left. */
+int cl_kvpool_attach(cl_kvpool* p, int32_t owner, const int32_t* ids, int32_t n, int32_t* n_reused);
+int cl_kvpool_publish(cl_kvpool* p, int32_t owner, const int32_t* ids, int32_t n_known);
+int cl_kvpool_cached_pages(cl_kvpool* p);
 
 #ifdef __cplusplus
 }

@@ -49,7 +49,7 @@ def main():
     done, lock, stop = [], threading.Lock(), threading.Event()
     with eng.Engine(preset=a.preset, seed=1234, max_batch=a.max_batch, kv_pool_bytes=pool_bytes, start_scheduler=True) as e:
         sp = eng.greedy(a.gen, ignore_eos=True)
-        st0 = e.stats()
+        st0, ps0 = e.stats(), e.prefix_stats()
 
         def client(cid):
             r = np.random.default_rng(1000 + cid)
@@ -76,7 +76,7 @@ def main():
         t_window = time.time()
         for t in threads:
             t.join(timeout=120)
-        st1 = e.stats()
+        st1, ps1 = e.stats(), e.prefix_stats()
         with lock:
             ok = [d for d in done if "error" not in d]
             errs = [d for d in done if "error" in d]
@@ -120,7 +120,14 @@ def main():
                    check=dict(method="teacher-forced replay: top logit minus the logit of every produced token", tolerance=round(tol, 4),
                               evicted_checked=len(ev_s), evicted_tokens_over_tolerance=ev_over, evicted_worst_gap=ev_worst,
                               clean_checked=len(cl_s), clean_tokens_over_tolerance=cl_over, clean_worst_gap=cl_worst),
-                   kv_pages=dict(total=st1.get("kv_pages_total"), used_at_end=st1.get("kv_pages_used")))
+                   kv_pages=dict(total=st1.get("kv_pages_total"), used_at_end=st1.get("kv_pages_used")),
+                   # prompt tokens prefilled by the scheduler (first admissions and recomputes after a preemption), and the
+                   # prefix cache (CL_PREFIX_CACHE=1): tokens found cached instead of recomputed
+                   prefill_tokens=int(st1["sched_prefill_tokens"] - st0["sched_prefill_tokens"]),
+                   prefix_cache=dict(enabled=ps1["enabled"], lookups=ps1["lookups"] - ps0["lookups"],
+                                     tokens_looked_up=ps1["tokens_looked_up"] - ps0["tokens_looked_up"],
+                                     tokens_reused=ps1["tokens_reused"] - ps0["tokens_reused"],
+                                     pages_evicted=ps1["pages_evicted"] - ps0["pages_evicted"], cached_pages_at_end=ps1["cached_pages"]))
         print(json.dumps(out))
 
 
