@@ -17,8 +17,6 @@
 // (the documented deviation of the prefill path); output rounded to bf16 = the o-projection's GEMM operand.
 #include <cuda.h>
 
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.h"
 #include "wgmma.cuh"
@@ -241,9 +239,7 @@ constexpr size_t kSmem = (size_t)Q_BYTES + (size_t)NRING * SLOT + (2 + 2 * NRING
 }  // namespace
 
 bool attn_prefill_tc_supported(int n_heads, int n_kv, int head_dim, int page_size, int pos0, int T) {
-  const char* ev = getenv("CL_PREFILL_ATTN_TC");     // 0: keep the mma.sync kernel (prefill_kernels.cu)
-  const bool off = ev && atoi(ev) == 0;
-  return !off && head_dim == HD && page_size == PAGE && n_kv > 0 && n_heads % n_kv == 0 && T > 0 &&
+  return head_dim == HD && page_size == PAGE && n_kv > 0 && n_heads % n_kv == 0 && T > 0 &&
          (pos0 + T + PAGE - 1) / PAGE <= MAX_BT;
 }
 

@@ -75,54 +75,6 @@ int launch_batch_resid_norm(float* h, int d, const float* ypart, int n_split, in
   return launch_k(batch_resid_norm_kernel, dim3(B), dim3(1024), st, pdl, h, d, ypart, n_split, B, gain, eps, xn, slots);
 }
 
-// xn[b] = bf16(rmsnorm(h[slots[b]]) * gain): one CTA of 1024 threads per sequence, one float4 per thread and pass
-__global__ void __launch_bounds__(1024) batch_norm_kernel(const float* __restrict__ h, int d, const float* __restrict__ gain, float eps,
-                                                          __nv_bfloat16* __restrict__ xn, const int* __restrict__ slots) {
-  __shared__ float red[32];
-  pdl_launch_dependents();
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  float4 g[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) { const int i = (tid + r * 1024) * 4; g[r] = i < d ? *reinterpret_cast<const float4*>(gain + i) : make_float4(0.f, 0.f, 0.f, 0.f); }
-  pdl_wait();
-  const float* hr = h + (size_t)slots[b] * d;
-  float4 v[2];
-  float ss = 0.f;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int i = (tid + r * 1024) * 4;
-    v[r] = i < d ? ldcg4(hr + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-    ss = fmaf(v[r].x, v[r].x, ss); ss = fmaf(v[r].y, v[r].y, ss); ss = fmaf(v[r].z, v[r].z, ss); ss = fmaf(v[r].w, v[r].w, ss);
-  }
-  ss = warp_sum(ss);
-  if (lane == 0) red[warp] = ss;
-  __syncthreads();
-  float tot = 0.f;
-#pragma unroll
-  for (int w = 0; w < 32; ++w) tot += red[w];
-  const float inv = 1.0f / sqrtf(tot / (float)d + eps);
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int i = (tid + r * 1024) * 4;
-    if (i < d) {
-      uint2 pk;
-      pk.x = pack_bf16(v[r].x * inv * g[r].x, v[r].y * inv * g[r].y);
-      pk.y = pack_bf16(v[r].z * inv * g[r].z, v[r].w * inv * g[r].w);
-      *reinterpret_cast<uint2*>(xn + (size_t)b * d + i) = pk;
-    }
-  }
-}
-int launch_batch_norm(const float* h, int d, int B, const float* gain, float eps, __nv_bfloat16* xn, const int* slots, cudaStream_t st, bool pdl) {
-  if (d > 8192 || d % 4) return -1;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(B); cfg.blockDim = dim3(1024); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, batch_norm_kernel, h, d, gain, eps, xn, slots) == cudaSuccess ? 1 : -1;
-}
-
 // q|k|v partials (rope-pair-interleaved columns) -> RoPE at pos[slot] -> q (fp32, bf16-rounded) and the paged cache
 __global__ void __launch_bounds__(256) batch_rope_append_kernel(const float* __restrict__ ypart, int n_split, int B, QkvEpi e,
                                                                 float* __restrict__ q_out, int q_stride, const int* __restrict__ slots) {
@@ -162,24 +114,6 @@ int launch_batch_rope_append(const float* ypart, int n_split, int B, const QkvEp
                              cudaStream_t st, bool pdl) {
   const int pairs = (e.n_heads + 2 * e.n_kv) * e.head_dim / 2;
   return launch_k(batch_rope_append_kernel, dim3((pairs + 255) / 256, B), dim3(256), st, pdl, ypart, n_split, B, e, q_out, q_stride, slots);
-}
-
-// x[slot][n] (fp32, already bf16-rounded) -> xb[b][n] bf16
-__global__ void batch_gather_bf16_kernel(const float* __restrict__ x, int n, int x_stride, __nv_bfloat16* __restrict__ xb,
-                                         const int* __restrict__ slots) {
-  const int b = blockIdx.y;
-  const float* src = x + (size_t)slots[b] * x_stride;
-  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) * 4; i < n; i += gridDim.x * blockDim.x * 4) {
-    const float4 v = *reinterpret_cast<const float4*>(src + i);
-    uint2 pk;
-    pk.x = pack_bf16(v.x, v.y);
-    pk.y = pack_bf16(v.z, v.w);
-    *reinterpret_cast<uint2*>(xb + (size_t)b * n + i) = pk;
-  }
-}
-int launch_batch_gather_bf16(const float* x, int n, int x_stride, __nv_bfloat16* xb, const int* slots, int B, cudaStream_t st) {
-  batch_gather_bf16_kernel<<<dim3((n / 4 + 255) / 256, B), 256, 0, st>>>(x, n, x_stride, xb, slots);
-  return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
 // gate|up partials (interleaved pairs) -> act[b][i] = bf16(silu(g) * u)

@@ -1033,16 +1033,6 @@ int launch_bf16_to_f32(const __nv_bfloat16* in, float* out, int64_t n, cudaStrea
   bf16_to_f32_kernel<<<blocks, 256, 0, st>>>(in, out, n);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
-__global__ void fill_u16_kernel(uint16_t* p, int64_t n, uint16_t v) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
-}
-int launch_fill_u16(uint16_t* p, int64_t n, uint16_t v, cudaStream_t st) {
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 1184) blocks = 1184;
-  if (blocks < 1) blocks = 1;
-  fill_u16_kernel<<<blocks, 256, 0, st>>>(p, n, v);
-  return cudaGetLastError() == cudaSuccess ? 1 : -1;
-}
 
 // ---- parity aid: fill a sequence's paged K/V with the oracle's cheap pattern (oracle/llama_oracle.c oc_seq_fake_fill:
 // every value is n/128 with n in [-128, 127], exact in bf16), the same in every layer.  i = token * kv_dim + head * hd + dim.

@@ -184,7 +184,6 @@ int Engine::init(const cl_engine_config& c) {
   sched_prefill_chunk_ = env_int("CL_SCHED_PREFILL_CHUNK", kDefaultSchedPrefillChunk);
   if (sched_prefill_chunk_ > 0 && sched_prefill_chunk_ < 16) sched_prefill_chunk_ = 16;
   prefill_small_max_ = std::min(256, env_int("CL_PREFILL_SMALL_MAX", kDefaultPrefillSmallMax));
-  prefill_fused_ = env_int("CL_PREFILL_FUSED", kDefaultPrefillFused);
   device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
   prefix_cache_ = env_int("CL_PREFIX_CACHE", c.prefix_cache) != 0;
   if (c.start_scheduler) start_scheduler();
@@ -506,7 +505,6 @@ void LaunchProfiler::report(const char* tag, int key_width, const std::string& h
     const std::string full(name_[i]);
     std::string key = full.substr(0, full.find('('));
     auto has = [&](const char* arg) { return full.find(arg) != std::string::npos; };
-    if (key == "launch_gemm_bf16_epi") key += has("L.wqkv") ? ":qkv+rope" : ":gate|up+silu";
     if (key == "launch_gemm_bf16")     // split by projection: the weight argument names it
       key += has("L.wqkv") ? ":qkv" : has("L.wo") ? ":o" : has("L.wgu") ? ":gate|up" : has("lm_head_") ? ":lm_head" : ":down";
     acc[key].first += ms; acc[key].second += 1;

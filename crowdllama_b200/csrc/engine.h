@@ -23,7 +23,6 @@ namespace cl {
 // of the parity tests and the benchmark with it.
 constexpr int kDefaultSchedPrefillChunk = 1024; // CL_SCHED_PREFILL_CHUNK: admission token budget per scheduler iteration (0 = whole prompts); validated r2e
 constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts up to this many tokens take the split-K path (0 = off)
-constexpr int kDefaultPrefillFused = 1;         // CL_PREFILL_FUSED bit mask: 1 = SiLU*mul, 2 = RoPE + cache scatter (correct, measured slower) fused into the prefill GEMM epilogues
 constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi)
 constexpr int kDefaultSchedLingerUs = 1000;     // CL_SCHED_LINGER_US: with an empty batch, keep collecting while requests arrive within this gap (max 8x in total)
 
@@ -289,6 +288,10 @@ class Engine {
   int prefill_tokenwise(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
   int prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
   int ensure_prefill_ws(int tokens);  // tensor-core path (prefill.cu)
+  struct PrefillSegment { int seq, row0, n, pos0; };   // rows row0 .. row0 + n - 1 of a pass: sequence seq from position pos0
+  // one tile-path pass of T rows made of n_segs segments; leaves the final residual rows in pws_->h
+  int prefill_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, int& launches, LaunchProfiler& prof);
+  int attn_prefill(const AttnPrefillArgs& a, int layer, int& launches, LaunchProfiler& prof);   // the one choice of prefill attention kernel
   int prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_out);    // short prompts: split-K projections (prefill.cu)
   bool prefill_path_ok() const;
   int set_single_slot(cl_seq_t s);
@@ -346,14 +349,12 @@ class Engine {
     __nv_bfloat16* q = nullptr;     // [T][q_dim]
     __nv_bfloat16* attn = nullptr;  // [T][q_dim]
     float* h = nullptr;             // [T][d]
-    float* gu = nullptr;            // [T][2F]
     __nv_bfloat16* act = nullptr;   // [T][F]
   };
   std::unique_ptr<PrefillWs> pws_;
   struct SmallPrefillWs { float* part = nullptr; __nv_bfloat16* xn = nullptr; __nv_bfloat16* q = nullptr; __nv_bfloat16* attn = nullptr;
                           float* h = nullptr; __nv_bfloat16* act = nullptr; int* iota = nullptr; };
   std::unique_ptr<SmallPrefillWs> sws_;
-  int prefill_fused_ = 0;             // bit 0: SiLU*mul, bit 1: RoPE + cache scatter in the prefill GEMM epilogues (CL_PREFILL_FUSED)
   int prefill_small_max_ = 0;         // prompts up to this many tokens take the split-K path (CL_PREFILL_SMALL_MAX, 0 = off)
   struct BatchWs { __nv_bfloat16* xn = nullptr; __nv_bfloat16* attn = nullptr; __nv_bfloat16* act = nullptr; float* part = nullptr; float* logits = nullptr; };
   std::unique_ptr<BatchWs> bws_;

@@ -34,13 +34,16 @@ struct GemmParams {
   int accumulate_into_y;  // 1: Y += result (residual add in place)
   int k_splits;           // > 1: split-K; split s writes its partial to Y + s * T * ldy (the consumer sums in fixed order)
   int pre_stages;         // PDL launches only: W tiles of the first stages requested before griddepcontrol.wait (0 = none)
-  GemmEpi epi;            // fused prefill epilogues (EPI template parameter != 0): see kernels.h
+  __nv_bfloat16* act;     // EPI_SILU: act[t][i] = bf16(silu(gate_i) * up_i), row stride ld_act
+  int ld_act;
 };
-enum { EPI_F32 = 0, EPI_SILU = 1, EPI_ROPE = 2 };
+enum { EPI_F32 = 0, EPI_SILU = 1 };
 
+// p is __grid_constant__ so that its fields are read from the parameter bank where they are used: as a plain by-value
+// struct the compiler loads them all into registers at kernel entry (+2 to +10 registers per instantiation).
 template <int BT, int NST, int EPI>
 __global__ void __launch_bounds__(384, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr uint32_t A_BYTES = BM * BK * 2;         // 16 KB
   constexpr uint32_t B_BYTES = BT * BK * 2;
@@ -176,7 +179,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_consta
                 }
             }
           }
-        } else if constexpr (EPI == EPI_SILU) {
+        } else {
           // rows are interleaved (2i = gate_i, 2i+1 = up_i): lanes l and l ^ 4 hold rows n and n ^ 1 of the same tokens.
           // Per token pair (c, c + 1) the even-row lane finishes token c (owns g, receives u), the odd-row lane token c + 1
           // (owns u, receives g): one shuffle, one SiLU, one store per lane.
@@ -188,38 +191,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_consta
             const float gt = odd ? recv : a0, up = odd ? a1 : recv;
             const int t = t0 + i * 8 + 2 * cq + odd;
             if (n < p.N && t < p.T)
-              p.epi.act[(size_t)t * p.epi.ld_act + i2] = __float2bfloat16_rn(__fdividef(gt, 1.0f + __expf(-gt)) * up);
+              p.act[(size_t)t * p.ld_act + i2] = __float2bfloat16_rn(__fdividef(gt, 1.0f + __expf(-gt)) * up);
           }
-        } else {
-          // q|k|v rows are rope-pair-interleaved per head (row 2j = dim j, row 2j+1 = dim j + 64; BM = head_dim = 128, so
-          // a tile is exactly one head): lanes l and l ^ 4 hold one rotation pair per token.  Rotate at the token's
-          // position, round to bf16, write q to q_out[t][head][dim] and k / v straight into the paged cache.
-          const GemmEpi& e = p.epi;
-          const int head = n0 >> 7, w = n & 127, j = w >> 1, odd = rq & 1;
-          const int dim = odd ? j + 64 : j;
-          const bool rot = head < e.n_heads + e.n_kv, isq = head < e.n_heads;
-          const int g = rot ? head - e.n_heads : head - e.n_heads - e.n_kv;
-          __nv_bfloat16* pool = rot ? e.kpool : e.vpool;
-#pragma unroll
-          for (int i = 0; i < NI; ++i)
-#pragma unroll
-            for (int ee = 0; ee < 2; ++ee) {
-              const int t = t0 + i * 8 + 2 * cq + ee, pos = e.pos0 + (t < p.T ? t : 0);
-              const float2 cs = rot ? __ldg(e.rope + (size_t)pos * 64 + j) : make_float2(1.f, 0.f);
-              const float mine = acc[4 * i + 2 * h + ee];
-              const float other = __shfl_xor_sync(0xffffffffu, mine, 4);
-              // even row: v0 = mine (dim j), v1 = other -> v0 cos - v1 sin; odd row: v1 = mine (dim j + 64) -> v1 cos + v0 sin
-              const float val = odd ? mine * cs.x + other * cs.y : mine * cs.x - other * cs.y;
-              if (t < p.T && n < p.N) {
-                if (isq) {
-                  e.q_out[(size_t)t * e.q_dim + head * 128 + dim] = __float2bfloat16_rn(val);
-                } else {
-                  const int pg = __ldg(e.block_table + pos / e.page_size);
-                  const int off = pos % e.page_size;
-                  pool[(((size_t)pg * e.n_kv + g) * e.page_size + off) * 128 + dim] = __float2bfloat16_rn(val);
-                }
-              }
-            }
         }
       }
     }
@@ -310,7 +283,7 @@ int launch_gemm_bf16(const __nv_bfloat16* X, const __nv_bfloat16* W, float* Y, c
   if (k_splits > 1 && ((K + BK - 1) / BK + k_splits - 1) / k_splits * (k_splits - 1) >= (K + BK - 1) / BK) return -1;
   // PDL launches request the W tiles of the whole ring before waiting for the kernel in front (CL_GEMM_PRE stages)
   static const int pre_env = getenv("CL_GEMM_PRE") ? atoi(getenv("CL_GEMM_PRE")) : 8;
-  GemmParams p{Y, T, N, K, N, resid ? 1 : 0, k_splits, pdl ? pre_env : 0, GemmEpi()};
+  GemmParams p{Y, T, N, K, N, resid ? 1 : 0, k_splits, pdl ? pre_env : 0, nullptr, 0};
   cudaError_t e;
   switch (BT) {
     case 128: e = launch_inst<128, 6>(mw, mx, p, st, pdl); break;
@@ -320,28 +293,18 @@ int launch_gemm_bf16(const __nv_bfloat16* X, const __nv_bfloat16* W, float* Y, c
   return e == cudaSuccess ? 1 : -1;
 }
 
-// Prefill projections with a fused epilogue (no fp32 round trip through HBM): kind 1 = gate|up -> bf16(SiLU(g) * u),
-// kind 2 = q|k|v -> RoPE + bf16 + q buffer / paged KV cache.  One CTA per 128 x BT tile (no split-K).
-int launch_gemm_bf16_epi(const __nv_bfloat16* X, const __nv_bfloat16* W, int T, int N, int K, const GemmEpi& epi, cudaStream_t st) {
-  if (!gemm_tc_supported(T, N, K) || (epi.kind != 1 && epi.kind != 2) || (N & 1)) return -1;
-  if (epi.kind == 2 && (N % 128 || N != (epi.n_heads + 2 * epi.n_kv) * 128)) return -1;   // head_dim 128 = one tile per head
+// Prefill gate|up projection with the SiLU epilogue (no fp32 round trip through HBM).  One CTA per 128 x BT tile (no split-K).
+int launch_gemm_bf16_silu(const __nv_bfloat16* X, const __nv_bfloat16* W, int T, int N, int K, __nv_bfloat16* act, int ld_act, cudaStream_t st) {
+  if (!gemm_tc_supported(T, N, K) || (N & 1)) return -1;
   const int BT = token_tile(T);
   CUtensorMap mw, mx;
   if (!make_map(&mw, W, N, K, BM) || !make_map(&mx, X, T, K, BT)) return -1;
-  GemmParams p{nullptr, T, N, K, N, 0, 1, 0, epi};
+  GemmParams p{nullptr, T, N, K, N, 0, 1, 0, act, ld_act};
   cudaError_t e;
-  if (epi.kind == 1) {
-    switch (BT) {
-      case 128: e = launch_inst<128, 6, EPI_SILU>(mw, mx, p, st, false); break;
-      case 64: e = launch_inst<64, 8, EPI_SILU>(mw, mx, p, st, false); break;
-      default: e = launch_inst<32, 8, EPI_SILU>(mw, mx, p, st, false); break;
-    }
-  } else {
-    switch (BT) {
-      case 128: e = launch_inst<128, 6, EPI_ROPE>(mw, mx, p, st, false); break;
-      case 64: e = launch_inst<64, 8, EPI_ROPE>(mw, mx, p, st, false); break;
-      default: e = launch_inst<32, 8, EPI_ROPE>(mw, mx, p, st, false); break;
-    }
+  switch (BT) {
+    case 128: e = launch_inst<128, 6, EPI_SILU>(mw, mx, p, st, false); break;
+    case 64: e = launch_inst<64, 8, EPI_SILU>(mw, mx, p, st, false); break;
+    default: e = launch_inst<32, 8, EPI_SILU>(mw, mx, p, st, false); break;
   }
   return e == cudaSuccess ? 1 : -1;
 }

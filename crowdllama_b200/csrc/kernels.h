@@ -122,7 +122,6 @@ int launch_synth_bf16(__nv_bfloat16* out, int64_t n_logical, int k_cols, int row
                       int key, float scale, cudaStream_t st, int rope_hd = 0);
 int launch_synth_gain(float* out, int n, uint64_t seed, int key, float scale, cudaStream_t st);
 int launch_bf16_to_f32(const __nv_bfloat16* in, float* out, int64_t n, cudaStream_t st);
-int launch_fill_u16(uint16_t* p, int64_t n, uint16_t v, cudaStream_t st);
 // parity aid: the oracle's oc_seq_fake_fill pattern into tokens 0..n_tokens-1 of one sequence, all layers
 int launch_fake_fill_kv(__nv_bfloat16* kpool, __nv_bfloat16* vpool, size_t layer_elems, int n_layers, const int* block_table,
                         int page_size, int n_kv, int head_dim, int n_tokens, cudaStream_t st);
@@ -184,17 +183,9 @@ struct PerDeviceOnce {
 int launch_gemm_bf16(const __nv_bfloat16* X, const __nv_bfloat16* W, float* Y, const float* resid, int T, int N, int K,
                      cudaStream_t st, int k_splits = 1, bool pdl = false);
 bool gemm_tc_supported(int T, int N, int K);
-// fused prefill epilogues of the wgmma GEMM (gemm_wgmma.cu): the fp32 result never leaves the SM
-struct GemmEpi {
-  int kind = 0;                              // 1: gate|up rows interleaved (2i gate, 2i+1 up) -> act[t][i] = bf16(silu(g) * u)
-                                             // 2: q|k|v rows rope-pair-interleaved, head_dim 128 -> RoPE at pos0 + t, bf16, q_out / paged cache
-  __nv_bfloat16* act = nullptr; int ld_act = 0;
-  const float2* rope = nullptr; int pos0 = 0;
-  __nv_bfloat16* q_out = nullptr; int q_dim = 0;
-  __nv_bfloat16* kpool = nullptr; __nv_bfloat16* vpool = nullptr;   // this layer
-  const int* block_table = nullptr; int page_size = 0, n_heads = 0, n_kv = 0;
-};
-int launch_gemm_bf16_epi(const __nv_bfloat16* X, const __nv_bfloat16* W, int T, int N, int K, const GemmEpi& epi, cudaStream_t st);
+// gate|up projection with the SiLU epilogue (gemm_wgmma.cu): W rows interleaved (2i gate, 2i+1 up) -> act[t][i] =
+// bf16(silu(g) * u), act row stride ld_act; the fp32 result never leaves the SM
+int launch_gemm_bf16_silu(const __nv_bfloat16* X, const __nv_bfloat16* W, int T, int N, int K, __nv_bfloat16* act, int ld_act, cudaStream_t st);
 // xn[t] = bf16(rmsnorm(h[t]) * gain)
 int launch_rmsnorm_bf16(const float* h, const float* gain, float eps, __nv_bfloat16* out, int T, int d, cudaStream_t st);
 // rope q,k of T tokens starting at pos0; q -> bf16 [T][H][D]; k,v -> paged cache (bf16) and optional dense copies
@@ -218,16 +209,11 @@ int launch_attn_prefill(const AttnPrefillArgs& a, cudaStream_t st);
 // wgmma variant (attn_prefill_tc.cu): head_dim 128, page 32; kmap / vmap = pool-wide 2-D tensor maps (box {64, 32})
 bool attn_prefill_tc_supported(int n_heads, int n_kv, int head_dim, int page_size, int pos0, int T);
 int launch_attn_prefill_tc(const AttnPrefillArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st);
-// act = bf16(silu(gu[:, 2i]) * gu[:, 2i+1])
-int launch_silu_mul_bf16(const float* gu, __nv_bfloat16* act, int T, int d_ff, cudaStream_t st);
 // ---- batched decode glue (batch_kernels.cu) ------------------------------------------------------
 int launch_batch_resid_norm(float* h, int d, const float* ypart, int n_split, int B, const float* gain, float eps, __nv_bfloat16* xn,
                             const int* slots, cudaStream_t st, bool pdl = false);
-// xn[b] = bf16(rmsnorm(h[slots[b]]) * gain)   (PDL-aware)
-int launch_batch_norm(const float* h, int d, int B, const float* gain, float eps, __nv_bfloat16* xn, const int* slots, cudaStream_t st, bool pdl);
 int launch_batch_rope_append(const float* ypart, int n_split, int B, const QkvEpi& e, float* q_out, int q_stride, const int* slots,
                              cudaStream_t st, bool pdl = false);
-int launch_batch_gather_bf16(const float* x, int n, int x_stride, __nv_bfloat16* xb, const int* slots, int B, cudaStream_t st);
 int launch_batch_silu(const float* ypart, int n_split, int B, int d_ff, __nv_bfloat16* act, cudaStream_t st, bool pdl = false);
 int launch_batch_scatter_rows(const float* y, int n, float* out, int out_stride, const int* slots, int B, cudaStream_t st);
 int launch_embed_rows(const __nv_bfloat16* table, int d, const int* ids_dev, float* h, int T, cudaStream_t st);

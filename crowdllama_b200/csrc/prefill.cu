@@ -1,10 +1,11 @@
-// prefill.cu — prompt (prefill) path of the engine: chunks of up to prefill_chunk_tokens_ tokens go
-// through wgmma GEMMs (gemm_wgmma.cu) and the causal paged attention kernel
-// (prefill_kernels.cu); the last position's logits come from the decode LM-head GEMV so that
-// prefill and decode share one logits/argmax tail.  Also: cl_op_gemm_bf16 / cl_op_attn_prefill.
+// prefill.cu — prompt (prefill) path of the engine.  Prompts of up to 256 tokens take the short-prompt path (split-K
+// projections, prefill_small); longer ones go through the tile path: prefill_pass runs T rows through wgmma GEMMs
+// (gemm_wgmma.cu) and the causal paged attention (prefill_kernels.cu / attn_prefill_tc.cu), once per chunk of up to
+// prefill_chunk_tokens_ tokens (prefill_chunked) or once for several prompts (prefill_multi).  The last position's logits
+// come from the decode LM head, so that prefill and decode share one logits/argmax tail.  Also: cl_op_gemm_bf16 /
+// cl_op_attn_prefill.
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -14,17 +15,31 @@
 
 namespace cl {
 
-bool Engine::prefill_path_ok() const {
-  static int disabled = -1;
-  if (disabled < 0) {
-    const char* v = getenv("CL_PREFILL_TCGEN05");
-    disabled = (v && *v == '0') ? 1 : 0;
-  }
-  return !disabled && gemm_tc_supported(16, cfg.d_model, cfg.d_model);
-}
+bool Engine::prefill_path_ok() const { return gemm_tc_supported(16, cfg.d_model, cfg.d_model); }
 
 // split-K rule shared with the batched decode step (engine.cu)
 int pick_splits_public(int n_rows, int K);
+
+// A prefill workspace buffer: lives until the engine dies (allocs_).  Out of memory is reported, and the CUDA error state
+// cleared, so that later launches do not see it.
+template <typename T>
+static int ws_alloc(std::vector<void*>& allocs, T*& p, size_t bytes) {
+  void* v = nullptr;
+  if (cudaMalloc(&v, bytes) != cudaSuccess) { cudaGetLastError(); set_last_error("prefill workspace: out of memory"); return CL_ERR_OOM; }
+  allocs.push_back(v);
+  p = reinterpret_cast<T*>(v);
+  return CL_OK;
+}
+
+// Causal attention of one prefill segment in layer l: the wgmma kernel where it applies (head_dim 128, page 32, the pool's
+// tensor maps), the mma.sync kernel otherwise.
+int Engine::attn_prefill(const AttnPrefillArgs& a, int l, int& launches, LaunchProfiler& prof) {
+  if (have_kv_maps_ && attn_prefill_tc_supported(a.n_heads, a.n_kv, a.head_dim, a.page_size, a.pos0, a.T))
+    CL_LAUNCH(launch_attn_prefill_tc(a, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_));
+  else
+    CL_LAUNCH(launch_attn_prefill(a, stream_));
+  return CL_OK;
+}
 
 // Short prompts (prefill_min_tokens_ <= n <= 256, e.g. a 128-token chat): one token tile per W row tile means only
 // N/128 CTAs stream the weights of a projection (48 for q|k|v, 32 for o and down), far below the
@@ -45,16 +60,10 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
     part = std::max(part, (size_t)s_o * Tm * d);
     part = std::max(part, (size_t)s_gu * Tm * 2 * F);
     part = std::max(part, (size_t)s_dn * Tm * d);
-    auto alloc = [&](auto*& p, size_t bytes) -> int {
-      void* v = nullptr;
-      if (cudaMalloc(&v, bytes) != cudaSuccess) { cudaGetLastError(); set_last_error("short-prompt prefill workspace: out of memory"); return CL_ERR_OOM; }
-      allocs_.push_back(v);
-      p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(v);
-      return CL_OK;
-    };
-    if ((rc = alloc(sws_->part, part * 4)) || (rc = alloc(sws_->xn, Tm * d * 2)) || (rc = alloc(sws_->q, Tm * q_dim_ * 2)) ||
-        (rc = alloc(sws_->attn, Tm * q_dim_ * 2)) || (rc = alloc(sws_->h, Tm * d * 4)) || (rc = alloc(sws_->act, Tm * F * 2)) ||
-        (rc = alloc(sws_->iota, Tm * 4))) { sws_.reset(); return rc; }
+    if ((rc = ws_alloc(allocs_, sws_->part, part * 4)) || (rc = ws_alloc(allocs_, sws_->xn, Tm * d * 2)) ||
+        (rc = ws_alloc(allocs_, sws_->q, Tm * q_dim_ * 2)) || (rc = ws_alloc(allocs_, sws_->attn, Tm * q_dim_ * 2)) ||
+        (rc = ws_alloc(allocs_, sws_->h, Tm * d * 4)) || (rc = ws_alloc(allocs_, sws_->act, Tm * F * 2)) ||
+        (rc = ws_alloc(allocs_, sws_->iota, Tm * 4))) { sws_.reset(); return rc; }
     std::vector<int> io(Tm);
     for (size_t i = 0; i < Tm; ++i) io[i] = (int)i;
     CL_CUDA_OK(cudaMemcpy(sws_->iota, io.data(), Tm * 4, cudaMemcpyHostToDevice));
@@ -65,8 +74,7 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   int launches = 0;
   // programmatic dependent launch between the GEMMs and the per-row glue kernels, as in the batched decode step (the two
   // prefill kernels in between are launched normally and order the stream)
-  static const bool small_pdl = !getenv("CL_SMALL_PDL") || atoi(getenv("CL_SMALL_PDL")) != 0;
-  const bool bp = small_pdl && use_pdl_;
+  const bool bp = use_pdl_;
   LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
   CL_LAUNCH(launch_embed_rows(embed_, d, d_prompt_, w.h, T, stream_));
   const float* pending = nullptr;   // split-K partials of the previous residual projection, folded in by the next norm
@@ -81,10 +89,7 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
     CL_LAUNCH(launch_rope_scatter(ra, stream_));
     AttnPrefillArgs aa{w.q, kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_, bt, page_size_,
                        pos0, T, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, w.attn};
-    if (have_kv_maps_ && attn_prefill_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, pos0, T))
-      CL_LAUNCH(launch_attn_prefill_tc(aa, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_));
-    else
-      CL_LAUNCH(launch_attn_prefill(aa, stream_));
+    if ((rc = attn_prefill(aa, l, launches, prof))) return rc;
     CL_LAUNCH(launch_gemm_bf16(w.attn, L.wo, w.part, nullptr, T, d, q_dim_, stream_, s_o, bp));
     CL_LAUNCH(launch_batch_resid_norm(w.h, d, w.part, s_o, T, L.ffn_norm, cfg.rms_eps, w.xn, w.iota, stream_, bp));
     CL_LAUNCH(launch_gemm_bf16(w.xn, L.wgu, w.part, nullptr, T, 2 * F, d, stream_, s_gu, bp));
@@ -109,7 +114,7 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   return CL_OK;
 }
 
-// (Re)allocate the tile-path workspace for chunks of up to `tokens` rows; old buffers stay in allocs_ until the engine dies
+// (Re)allocate the tile-path workspace for passes of up to `tokens` rows; old buffers stay in allocs_ until the engine dies
 // (grows at most once or twice).
 int Engine::ensure_prefill_ws(int tokens) {
   const int d = cfg.d_model, F = cfg.d_ff;
@@ -117,21 +122,45 @@ int Engine::ensure_prefill_ws(int tokens) {
   if (!pws_) pws_.reset(new PrefillWs());
   if (pws_->cap_tokens >= tokens) return CL_OK;
   const size_t T = (size_t)std::max(tokens, std::min(prefill_chunk_tokens_, cfg.max_seq_len));
-  auto alloc = [&](auto*& p, size_t bytes) -> int {
-    void* v = nullptr;
-    if (cudaMalloc(&v, bytes) != cudaSuccess) { cudaGetLastError(); set_last_error("prefill workspace: out of memory"); return CL_ERR_OOM; }
-    allocs_.push_back(v);
-    p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(v);
-    return CL_OK;
-  };
-  if ((rc = alloc(pws_->xn, T * d * 2))) return rc;
-  if ((rc = alloc(pws_->qkv, T * qkv_dim_ * 4))) return rc;
-  if ((rc = alloc(pws_->q, T * q_dim_ * 2))) return rc;
-  if ((rc = alloc(pws_->attn, T * q_dim_ * 2))) return rc;
-  if ((rc = alloc(pws_->h, T * d * 4))) return rc;
-  if ((rc = alloc(pws_->gu, T * 2 * F * 4))) return rc;
-  if ((rc = alloc(pws_->act, T * F * 2))) return rc;
+  if ((rc = ws_alloc(allocs_, pws_->xn, T * d * 2)) || (rc = ws_alloc(allocs_, pws_->qkv, T * qkv_dim_ * 4)) ||
+      (rc = ws_alloc(allocs_, pws_->q, T * q_dim_ * 2)) || (rc = ws_alloc(allocs_, pws_->attn, T * q_dim_ * 2)) ||
+      (rc = ws_alloc(allocs_, pws_->h, T * d * 4)) || (rc = ws_alloc(allocs_, pws_->act, T * F * 2))) return rc;
   pws_->cap_tokens = (int)T;
+  return CL_OK;
+}
+
+// One pass of the tile path over T rows whose token ids are at ids (device): embedding and every layer, leaving the final
+// residual rows in pws_->h.  The rows are the segments' tokens, back to back.  Everything row-wise (RMSNorm, the four
+// GEMMs, SiLU in the gate|up epilogue) runs once over all T rows; RoPE + cache scatter and the causal attention run per
+// segment, at its sequence's positions and into its pages.  A row's results therefore do not depend on the other rows.
+int Engine::prefill_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, int& launches, LaunchProfiler& prof) {
+  const int d = cfg.d_model, F = cfg.d_ff;
+  PrefillWs& w = *pws_;
+  int rc;
+  CL_LAUNCH(launch_embed_rows(embed_, d, ids, w.h, T, stream_));
+  for (int l = 0; l < cfg.n_layers; ++l) {
+    const auto& L = layers_[l];
+    __nv_bfloat16* kp = kpool_ + (size_t)l * kv_layer_elems_;
+    __nv_bfloat16* vp = vpool_ + (size_t)l * kv_layer_elems_;
+    CL_LAUNCH(launch_rmsnorm_bf16(w.h, L.attn_norm, cfg.rms_eps, w.xn, T, d, stream_));
+    CL_LAUNCH(launch_gemm_bf16(w.xn, L.wqkv, w.qkv, nullptr, T, qkv_dim_, d, stream_));
+    for (int i = 0; i < n_segs; ++i) {
+      const PrefillSegment& g = segs[i];
+      RopeScatterArgs ra{w.qkv + (size_t)g.row0 * qkv_dim_, qkv_dim_, rope_, g.pos0, g.n, w.q + (size_t)g.row0 * q_dim_, kp, vp,
+                         d_bt_ + (size_t)g.seq * max_pages_per_seq_, page_size_, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim};
+      CL_LAUNCH(launch_rope_scatter(ra, stream_));
+    }
+    for (int i = 0; i < n_segs; ++i) {
+      const PrefillSegment& g = segs[i];
+      AttnPrefillArgs aa{w.q + (size_t)g.row0 * q_dim_, kp, vp, d_bt_ + (size_t)g.seq * max_pages_per_seq_, page_size_, g.pos0, g.n,
+                         cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, w.attn + (size_t)g.row0 * q_dim_};
+      if ((rc = attn_prefill(aa, l, launches, prof))) return rc;
+    }
+    CL_LAUNCH(launch_gemm_bf16(w.attn, L.wo, w.h, w.h, T, d, q_dim_, stream_));
+    CL_LAUNCH(launch_rmsnorm_bf16(w.h, L.ffn_norm, cfg.rms_eps, w.xn, T, d, stream_));
+    CL_LAUNCH(launch_gemm_bf16_silu(w.xn, L.wgu, T, 2 * F, d, w.act, F, stream_));
+    CL_LAUNCH(launch_gemm_bf16(w.act, L.wdown, w.h, w.h, T, d, F, stream_));
+  }
   return CL_OK;
 }
 
@@ -139,57 +168,20 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
   auto& q = seqs_[s];
   int rc = ensure_capacity(s, q.len + n);
   if (rc) return rc;
-  const int d = cfg.d_model, F = cfg.d_ff;
-  const int CH = std::min(n, prefill_chunk_tokens_);
-  if ((rc = ensure_prefill_ws(CH))) return rc;
+  const int d = cfg.d_model;
+  if ((rc = ensure_prefill_ws(std::min(n, prefill_chunk_tokens_)))) return rc;
   PrefillWs& w = *pws_;
-  const bool fused_silu = (prefill_fused_ & 1) != 0, fused_rope = (prefill_fused_ & 2) != 0;   // CL_PREFILL_FUSED bit mask
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
-  const int* bt = d_bt_ + (size_t)s * max_pages_per_seq_;
   int launches = 0;
   LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
-  for (int c0 = 0; c0 < n; c0 += w.cap_tokens) {
-    const int T = std::min(w.cap_tokens, n - c0);
-    const int pos0 = q.len + c0;
-    CL_LAUNCH(launch_embed_rows(embed_, d, d_prompt_ + c0, w.h, T, stream_));
-    for (int l = 0; l < cfg.n_layers; ++l) {
-      const auto& L = layers_[l];
-      CL_LAUNCH(launch_rmsnorm_bf16(w.h, L.attn_norm, cfg.rms_eps, w.xn, T, d, stream_));
-      if (fused_rope && cfg.head_dim == 128) {   // RoPE + bf16 + q / paged-cache scatter in the GEMM epilogue
-        GemmEpi eq;
-        eq.kind = 2; eq.rope = rope_; eq.pos0 = pos0; eq.q_out = w.q; eq.q_dim = q_dim_;
-        eq.kpool = kpool_ + (size_t)l * kv_layer_elems_; eq.vpool = vpool_ + (size_t)l * kv_layer_elems_;
-        eq.block_table = bt; eq.page_size = page_size_; eq.n_heads = cfg.n_heads; eq.n_kv = cfg.n_kv_heads;
-        CL_LAUNCH(launch_gemm_bf16_epi(w.xn, L.wqkv, T, qkv_dim_, d, eq, stream_));
-      } else {
-        CL_LAUNCH(launch_gemm_bf16(w.xn, L.wqkv, w.qkv, nullptr, T, qkv_dim_, d, stream_));
-        RopeScatterArgs ra{w.qkv, qkv_dim_, rope_, pos0, T, w.q, kpool_ + (size_t)l * kv_layer_elems_,
-                           vpool_ + (size_t)l * kv_layer_elems_, bt, page_size_, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim};
-        CL_LAUNCH(launch_rope_scatter(ra, stream_));
-      }
-      AttnPrefillArgs aa{w.q, kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_, bt, page_size_,
-                         pos0, T, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, w.attn};
-      if (have_kv_maps_ && attn_prefill_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, pos0, T))
-        CL_LAUNCH(launch_attn_prefill_tc(aa, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_));
-      else
-        CL_LAUNCH(launch_attn_prefill(aa, stream_));
-      CL_LAUNCH(launch_gemm_bf16(w.attn, L.wo, w.h, w.h, T, d, q_dim_, stream_));
-      CL_LAUNCH(launch_rmsnorm_bf16(w.h, L.ffn_norm, cfg.rms_eps, w.xn, T, d, stream_));
-      if (fused_silu) {                     // SiLU(g) * u -> bf16 in the GEMM epilogue
-        GemmEpi eg;
-        eg.kind = 1; eg.act = w.act; eg.ld_act = F;
-        CL_LAUNCH(launch_gemm_bf16_epi(w.xn, L.wgu, T, 2 * F, d, eg, stream_));
-      } else {
-        CL_LAUNCH(launch_gemm_bf16(w.xn, L.wgu, w.gu, nullptr, T, 2 * F, d, stream_));
-        CL_LAUNCH(launch_silu_mul_bf16(w.gu, w.act, T, F, stream_));
-      }
-      CL_LAUNCH(launch_gemm_bf16(w.act, L.wdown, w.h, w.h, T, d, F, stream_));
-    }
-    if (c0 + T == n) {
-      // last position -> slot residual row, then the shared decode tail (final norm + LM head + argmax)
-      CL_CUDA_OK(cudaMemcpyAsync(d_h_ + (size_t)s * d, w.h + (size_t)(T - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, stream_));
-    }
+  int T = 0;
+  for (int c0 = 0; c0 < n; c0 += T) {
+    T = std::min(w.cap_tokens, n - c0);
+    const PrefillSegment seg{s, 0, T, q.len + c0};
+    if ((rc = prefill_pass(&seg, 1, d_prompt_ + c0, T, launches, prof))) return rc;
   }
+  // last position -> slot residual row, then the shared decode tail (final norm + LM head + argmax)
+  CL_CUDA_OK(cudaMemcpyAsync(d_h_ + (size_t)s * d, w.h + (size_t)(T - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, stream_));
   const int last_pos = q.len + n - 1;
   CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &last_pos, 4, cudaMemcpyHostToDevice, stream_));
   rc = set_single_slot(s);
@@ -205,18 +197,16 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
 }
 
 
-// Several prompts in ONE pass of the tile path (admission of a burst of short chats): the rows of all prompts are
-// concatenated, so every projection streams its weights once for all of them and runs on full tiles (the split-K
-// short-prompt path streams all weights once per prompt).  Everything row-wise (embedding, RMSNorm, the four GEMMs,
-// SiLU) is unchanged; RoPE + cache scatter and the causal attention run per sequence on its row range (pointer
-// offsets into the same workspace; each sequence has its own position offset and block table); the last row of every
-// sequence goes through the batched LM head of the decode step (final norm + wgmma GEMM + argmax), which leaves
-// d_tok_ / d_pos_ of every slot ready for the first decode step.  A row's results do not depend on the other rows of
-// the pass: logits and cache contents are bit-identical to prefill_chunked on each prompt alone (tests/test_gpu_prefill.py).
+// Several prompts in ONE pass of the tile path (admission of a burst of short chats): each prompt is a segment of the
+// pass, so every projection streams its weights once for all of them and runs on full tiles (the split-K short-prompt
+// path streams all weights once per prompt).  The last row of every sequence goes through the batched LM head of the
+// decode step (final norm + wgmma GEMM + argmax), which leaves d_tok_ / d_pos_ of every slot ready for the first decode
+// step.  Cache contents are bit-identical to prefill_chunked on each prompt alone; the logits differ from its GEMV head
+// by the summation order only (tests/test_gpu_prefill.py).
 int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* ids, const int* lens, float* logits_out) {
   if (n_seqs <= 0 || !ss || !ids || !lens) { set_last_error("prefill_multi: bad arguments"); return CL_ERR_INVALID_ARG; }
   if (!prefill_path_ok() || !bws_ || n_seqs > max_batch_) { set_last_error("prefill_multi: tensor-core paths unavailable or more sequences than max_batch"); return CL_ERR_INVALID_ARG; }
-  const int d = cfg.d_model, F = cfg.d_ff, V = cfg.vocab_size;
+  const int d = cfg.d_model, V = cfg.vocab_size;
   int total = 0, rc;
   for (int i = 0; i < n_seqs; ++i) {
     const int s = ss[i];
@@ -234,59 +224,24 @@ int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* 
   if ((rc = ensure_prefill_ws(total))) return rc;
   PrefillWs& w = *pws_;
   BatchWs& bw = *bws_;
-  const bool fused_silu = (prefill_fused_ & 1) != 0;
   std::vector<int32_t> all((size_t)total);
-  std::vector<int> row0(n_seqs), pos0(n_seqs);
+  std::vector<PrefillSegment> segs(n_seqs);
   for (int i = 0, r = 0; i < n_seqs; r += lens[i], ++i) {
     memcpy(all.data() + r, ids[i], (size_t)lens[i] * 4);
-    row0[i] = r;
-    pos0[i] = seqs_[ss[i]].len;
+    segs[i] = PrefillSegment{ss[i], r, lens[i], seqs_[ss[i]].len};
   }
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, all.data(), (size_t)total * 4, cudaMemcpyHostToDevice, stream_));
   int launches = 0;
   LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
-  const int T = total;
-  CL_LAUNCH(launch_embed_rows(embed_, d, d_prompt_, w.h, T, stream_));
-  for (int l = 0; l < cfg.n_layers; ++l) {
-    const auto& L = layers_[l];
-    __nv_bfloat16* kp = kpool_ + (size_t)l * kv_layer_elems_;
-    __nv_bfloat16* vp = vpool_ + (size_t)l * kv_layer_elems_;
-    CL_LAUNCH(launch_rmsnorm_bf16(w.h, L.attn_norm, cfg.rms_eps, w.xn, T, d, stream_));
-    CL_LAUNCH(launch_gemm_bf16(w.xn, L.wqkv, w.qkv, nullptr, T, qkv_dim_, d, stream_));
-    for (int i = 0; i < n_seqs; ++i) {                    // RoPE at the sequence's own positions, K/V into its own pages
-      const int* bt = d_bt_ + (size_t)ss[i] * max_pages_per_seq_;
-      RopeScatterArgs ra{w.qkv + (size_t)row0[i] * qkv_dim_, qkv_dim_, rope_, pos0[i], lens[i], w.q + (size_t)row0[i] * q_dim_, kp, vp, bt, page_size_,
-                         cfg.n_heads, cfg.n_kv_heads, cfg.head_dim};
-      CL_LAUNCH(launch_rope_scatter(ra, stream_));
-    }
-    for (int i = 0; i < n_seqs; ++i) {                    // causal attention inside each sequence
-      const int* bt = d_bt_ + (size_t)ss[i] * max_pages_per_seq_;
-      AttnPrefillArgs aa{w.q + (size_t)row0[i] * q_dim_, kp, vp, bt, page_size_, pos0[i], lens[i], cfg.n_heads, cfg.n_kv_heads, cfg.head_dim,
-                         w.attn + (size_t)row0[i] * q_dim_};
-      if (have_kv_maps_ && attn_prefill_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, pos0[i], lens[i]))
-        CL_LAUNCH(launch_attn_prefill_tc(aa, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_));
-      else
-        CL_LAUNCH(launch_attn_prefill(aa, stream_));
-    }
-    CL_LAUNCH(launch_gemm_bf16(w.attn, L.wo, w.h, w.h, T, d, q_dim_, stream_));
-    CL_LAUNCH(launch_rmsnorm_bf16(w.h, L.ffn_norm, cfg.rms_eps, w.xn, T, d, stream_));
-    if (fused_silu) {
-      GemmEpi eg;
-      eg.kind = 1; eg.act = w.act; eg.ld_act = F;
-      CL_LAUNCH(launch_gemm_bf16_epi(w.xn, L.wgu, T, 2 * F, d, eg, stream_));
-    } else {
-      CL_LAUNCH(launch_gemm_bf16(w.xn, L.wgu, w.gu, nullptr, T, 2 * F, d, stream_));
-      CL_LAUNCH(launch_silu_mul_bf16(w.gu, w.act, T, F, stream_));
-    }
-    CL_LAUNCH(launch_gemm_bf16(w.act, L.wdown, w.h, w.h, T, d, F, stream_));
-  }
+  if ((rc = prefill_pass(segs.data(), n_seqs, d_prompt_, total, launches, prof))) return rc;
   // last row of every sequence -> its slot's residual row and position, then the decode step's batched head
   std::vector<int> slots(n_seqs);
   for (int i = 0; i < n_seqs; ++i) {
-    const int s = ss[i], last_pos = pos0[i] + lens[i] - 1;
-    slots[i] = s;
-    CL_CUDA_OK(cudaMemcpyAsync(d_h_ + (size_t)s * d, w.h + (size_t)(row0[i] + lens[i] - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, stream_));
-    CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &last_pos, 4, cudaMemcpyHostToDevice, stream_));
+    const PrefillSegment& g = segs[i];
+    const int last_pos = g.pos0 + g.n - 1;
+    slots[i] = g.seq;
+    CL_CUDA_OK(cudaMemcpyAsync(d_h_ + (size_t)g.seq * d, w.h + (size_t)(g.row0 + g.n - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, stream_));
+    CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + g.seq, &last_pos, 4, cudaMemcpyHostToDevice, stream_));
   }
   CL_CUDA_OK(cudaMemcpyAsync(d_slots_, slots.data(), (size_t)n_seqs * 4, cudaMemcpyHostToDevice, stream_));
   slots_dirty_ = true;
@@ -374,7 +329,7 @@ int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, 
   return CL_OK;
 }
 
-// variant: -1 auto (wgmma kernel when the shape allows, CL_PREFILL_ATTN_TC=0 forces the other), 0 mma.sync kernel, 1 wgmma kernel
+// variant: -1 auto (wgmma kernel when the shape allows), 0 mma.sync kernel, 1 wgmma kernel
 static int attn_prefill_impl(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t, int32_t n_heads, int32_t n_kv,
                              int32_t head_dim, int variant, int iters, float* out, float* ms) {
   if (!q || !k || !v || !out || t <= 0) return CL_ERR_INVALID_ARG;
@@ -406,7 +361,6 @@ static int attn_prefill_impl(int device, const uint16_t* q, const uint16_t* k, c
                     dout.as<__nv_bfloat16>()};
   CUtensorMap km, vm;
   bool tc = variant != 0 && attn_prefill_tc_supported(n_heads, n_kv, HD, P, 0, t);
-  if (variant == 1 && !tc && head_dim == 128) tc = (t + P - 1) / P <= 320;          // explicit request overrides the env switch
   if (tc) tc = make_tmap_2d_bf16(&km, dk.p, (uint64_t)n_pages * n_kv * P, HD, 64, 32) && make_tmap_2d_bf16(&vm, dv.p, (uint64_t)n_pages * n_kv * P, HD, 64, 32);
   if (variant == 1 && !tc) { set_last_error("wgmma prefill attention does not support this shape"); return CL_ERR_INVALID_ARG; }
   auto run = [&]() { return tc ? launch_attn_prefill_tc(a, km, vm, 0, nullptr) : launch_attn_prefill(a, nullptr); };

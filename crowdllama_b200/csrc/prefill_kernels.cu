@@ -104,24 +104,6 @@ int launch_rope_scatter(const RopeScatterArgs& a, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------------------
-__global__ void silu_mul_bf16_kernel(const float* __restrict__ gu, __nv_bfloat16* __restrict__ act, int64_t total) {
-  // total = T * d_ff; gu holds interleaved (gate_i, up_i) pairs
-  for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 2; i < total; i += (int64_t)gridDim.x * blockDim.x * 2) {
-    const float4 v = *reinterpret_cast<const float4*>(gu + 2 * i);
-    const float a0 = v.x / (1.0f + __expf(-v.x)) * v.y;
-    const float a1 = v.z / (1.0f + __expf(-v.z)) * v.w;
-    *reinterpret_cast<__nv_bfloat162*>(act + i) = __floats2bfloat162_rn(a0, a1);
-  }
-}
-int launch_silu_mul_bf16(const float* gu, __nv_bfloat16* act, int T, int d_ff, cudaStream_t st) {
-  const int64_t total = (int64_t)T * d_ff;
-  int blocks = (int)std::min<int64_t>((total / 2 + 255) / 256, (int64_t)sm_count() * 16);
-  if (blocks < 1) blocks = 1;
-  silu_mul_bf16_kernel<<<blocks, 256, 0, st>>>(gu, act, total);
-  return cudaGetLastError() == cudaSuccess ? 1 : -1;
-}
-
-// ------------------------------------------------------------------------------------------------
 // causal GQA attention for T new tokens against the paged cache (which already holds them)
 // grid = (ceil(T/64), n_heads), block = 128 (4 warps x 16 query rows), KV blocks of 64 keys,
 // double-buffered cp.async, XOR-swizzled shared tiles, mma.sync.m16n8k16 bf16 -> fp32.

@@ -64,22 +64,24 @@ def _prompt(n, vocab, salt=0):
     return np.array([(i * 7919 + 13 + salt) % vocab for i in range(n)], np.int32)
 
 
-@pytest.mark.parametrize("path", ["small", "tiles-fused", "tiles"])
+@pytest.mark.parametrize("path", ["small", "tiles", "multi"])
 @pytest.mark.parametrize("n_prompt", [16, 40, 97, 200])
 def test_engine_chunked_prefill_matches_oracle(monkeypatch, n_prompt, path):
     """The tensor-core prefill paths against the oracle: "small" = short prompts (<= 256 tokens) on split-K projections
-    (prefill_small, CL_PREFILL_SMALL_MAX=256); "tiles-fused" = full tiles with the fused GEMM epilogues
-    (CL_PREFILL_FUSED=1; the tiny model has head_dim 64, so only the SiLU epilogue applies); "tiles" = separate kernels."""
+    (prefill_small, CL_PREFILL_SMALL_MAX=256); "tiles" = full tiles (the tiny model has head_dim 64: mma.sync attention);
+    "multi" = the same tile pass entered through cl_prefill_batch with one prompt (batched LM head, and the device state
+    it leaves behind must start decoding and a later prefill correctly)."""
     monkeypatch.setenv("CL_PREFILL_SMALL_MAX", "256" if path == "small" else "0")
-    monkeypatch.setenv("CL_PREFILL_FUSED", "3" if path == "tiles-fused" else "0")
     cfg = oc.PRESETS["tiny-test"]
     m = oc.Model(cfg, seed=1234)
     with eng.Engine(preset="tiny-test", seed=1234) as e:
+        def fill(s, ids):
+            return e.prefill_batch([s], [ids])[0] if path == "multi" else e.prefill(s, ids)
         p = _prompt(n_prompt, cfg["vocab_size"])
         so = m.new_seq()
         lo = so.forward(p)
         s = e.seq_create()
-        lg = e.prefill(s, p)                       # >= 16 tokens -> tensor-core path
+        lg = fill(s, p)                            # >= 16 tokens -> tensor-core path
         assert np.abs(lg - lo).max() < 0.125
         # decode continues from the prefix the prefill kernels wrote into the paged cache
         tok = int(lo.argmax())
@@ -91,22 +93,21 @@ def test_engine_chunked_prefill_matches_oracle(monkeypatch, n_prompt, path):
         # second prefill chunk appended to the same sequence (chunked prompt / multi-turn)
         p2 = _prompt(33, cfg["vocab_size"], salt=5)
         lo = so.forward(p2)
-        lg = e.prefill(s, p2)
+        lg = fill(s, p2)
         assert np.abs(lg - lo).max() < 0.125
         assert e.seq_len(s) == n_prompt + 8 + 33
 
 
-@pytest.mark.parametrize("fused", ["3", "0"])
-def test_prefill_paths_agree_on_llama_shapes(monkeypatch, fused):
-    """Token-wise (decode kernels), full-tile (wgmma; fused = RoPE / SiLU in the GEMM epilogues) and short-prompt
-    (split-K) prefill of the same prompts give the same logits within tolerance at Llama-3-8B layer shapes (2 layers);
-    the short-prompt path is also compared with the oracle directly."""
+@pytest.mark.parametrize("page", [32, 64])
+def test_prefill_paths_agree_on_llama_shapes(monkeypatch, page):
+    """Token-wise (decode kernels), full-tile (wgmma) and short-prompt (split-K) prefill of the same prompts give the same
+    logits within tolerance at Llama-3-8B layer shapes (2 layers); the short-prompt path is also compared with the oracle
+    directly.  Page 32 takes the wgmma prefill attention, page 64 the mma.sync kernel at head_dim 128."""
     monkeypatch.setenv("CL_PREFILL_SMALL_MAX", "256")
-    monkeypatch.setenv("CL_PREFILL_FUSED", fused)
     cfg = dict(oc.PRESETS["llama3-8b"])
     cfg["n_layers"] = 2
     cfg["max_seq_len"] = 512
-    with eng.Engine(model=cfg, seed=1234, max_batch=2) as e:
+    with eng.Engine(model=cfg, seed=1234, max_batch=2, page_size=page) as e:
         m = oc.Model(cfg, seed=1234)
         for n_small in (128, 250):
             ps = _prompt(n_small, cfg["vocab_size"], salt=3)
@@ -138,7 +139,6 @@ def test_prefill_continuation_at_an_unaligned_position_llama_shapes(monkeypatch,
     block (pos0 = 105) — the wgmma attention's diagonal then cuts through blocks, and keys come from pages written
     by an earlier prefill and by decode steps.  t2 = 150 takes the short-prompt path, 300 the full-tile path."""
     monkeypatch.setenv("CL_PREFILL_SMALL_MAX", "256")
-    monkeypatch.setenv("CL_PREFILL_FUSED", "3")
     cfg = dict(oc.PRESETS["llama3-8b"])
     cfg["n_layers"] = 2
     cfg["max_seq_len"] = 512
