@@ -29,6 +29,18 @@ constexpr int kDefaultSchedLingerUs = 1000;     // CL_SCHED_LINGER_US: with an e
 void set_last_error(const std::string& s);
 const char* get_last_error();
 
+// KV pool of the single-op entry points that take paged attention (cl_op_attn_decode_batch, cl_op_attn_prefill*): the token
+// rows of several sequences paged the way a long-running engine leaves them (ops_api.cu, op_build_kv_pool).
+struct OpKvPool {
+  std::vector<uint16_t> k, v;   // bf16 [2 layers][n_pages][n_kv][page][head_dim]; the tokens sit in layer 1
+  std::vector<int> bt;          // [sequence][bt_stride]
+  int n_pages = 0, bt_stride = 0;
+  int pad_page = 0;             // token-less page named by the block-table entries past a sequence's last page
+  size_t layer_elems = 0;       // n_pages * n_kv * page * head_dim
+};
+void op_build_kv_pool(const uint16_t* k, const uint16_t* v, const int* lens, int n_seqs, int n_kv, int head_dim, int page_size,
+                      OpKvPool* pool);
+
 #define CL_CUDA_OK(expr)                                                                          \
   do {                                                                                            \
     cudaError_t _e = (expr);                                                                      \

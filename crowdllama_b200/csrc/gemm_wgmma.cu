@@ -267,6 +267,12 @@ cudaError_t launch_inst(const CUtensorMap& mw, const CUtensorMap& mx, const Gemm
 
 }  // namespace
 
+// split s sums k-blocks [s * ceil(nkb / k_splits), ...): every split needs >= 1 k-block (k_splits <= 1: unsplit)
+bool gemm_splits_supported(int K, int k_splits) {
+  const int nkb = (K + BK - 1) / BK;
+  return k_splits <= 1 || (k_splits <= nkb && (nkb + k_splits - 1) / k_splits * (k_splits - 1) < nkb);
+}
+
 bool gemm_tc_supported(int T, int N, int K) { return T > 0 && N > 0 && K > 0 && K % 8 == 0 && get_encode() != nullptr; }
 
 // token tile: the smallest of 32 / 64 / 128 that holds T (prefill takes 128-token tiles)
@@ -279,8 +285,7 @@ int launch_gemm_bf16(const __nv_bfloat16* X, const __nv_bfloat16* W, float* Y, c
   const int BT = token_tile(T);
   CUtensorMap mw, mx;
   if (!make_map(&mw, W, N, K, BM) || !make_map(&mx, X, T, K, BT)) return -1;
-  if (k_splits > 1 && (resid || (K + BK - 1) / BK < k_splits)) return -1;   // every split needs >= 1 k-block
-  if (k_splits > 1 && ((K + BK - 1) / BK + k_splits - 1) / k_splits * (k_splits - 1) >= (K + BK - 1) / BK) return -1;
+  if (!gemm_splits_supported(K, k_splits) || (k_splits > 1 && resid)) return -1;
   // PDL launches request the W tiles of the whole ring before waiting for the kernel in front (CL_GEMM_PRE stages)
   static const int pre_env = getenv("CL_GEMM_PRE") ? atoi(getenv("CL_GEMM_PRE")) : 8;
   GemmParams p{Y, T, N, K, N, resid ? 1 : 0, k_splits, pdl ? pre_env : 0, nullptr, 0};

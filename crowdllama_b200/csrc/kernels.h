@@ -183,6 +183,7 @@ struct PerDeviceOnce {
 int launch_gemm_bf16(const __nv_bfloat16* X, const __nv_bfloat16* W, float* Y, const float* resid, int T, int N, int K,
                      cudaStream_t st, int k_splits = 1, bool pdl = false);
 bool gemm_tc_supported(int T, int N, int K);
+bool gemm_splits_supported(int K, int k_splits);   // the split-K counts launch_gemm_bf16 takes (no residual)
 // gate|up projection with the SiLU epilogue (gemm_wgmma.cu): W rows interleaved (2i gate, 2i+1 up) -> act[t][i] =
 // bf16(silu(g) * u), act row stride ld_act; the fp32 result never leaves the SM
 int launch_gemm_bf16_silu(const __nv_bfloat16* X, const __nv_bfloat16* W, int T, int N, int K, __nv_bfloat16* act, int ld_act, cudaStream_t st);

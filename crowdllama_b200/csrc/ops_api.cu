@@ -3,10 +3,59 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <numeric>
+#include <random>
 #include <vector>
 
 #include "common.cuh"
 #include "engine.h"
+
+namespace cl {
+
+// Pages of all sequences interleaved (page i of every sequence, then page i + 1) and scattered by a fixed pseudo-random
+// permutation; one filler page that block-table entries past a sequence's last page (and the rows of slots outside a batch)
+// name, and one page that nothing references.  Every pool element that holds no token (layer 0, the tails of last pages, the
+// two token-less pages) is set to the largest finite bf16: + for K, - for V.  Reading any of them puts an enormous term into
+// the output, while a masked probability of exactly 0 leaves it untouched (0 x finite = 0; a NaN filler would not, in the
+// tensor-core P.V).
+void op_build_kv_pool(const uint16_t* k, const uint16_t* v, const int* lens, int n_seqs, int n_kv, int head_dim, int page_size,
+                      OpKvPool* pool) {
+  const int P = page_size, HD = head_dim;
+  std::vector<int> npg(n_seqs);
+  int used = 0, maxp = 1;
+  for (int b = 0; b < n_seqs; ++b) {
+    npg[b] = (lens[b] + P - 1) / P;
+    used += npg[b];
+    maxp = std::max(maxp, npg[b]);
+  }
+  pool->n_pages = used + 2;                    // + the padding page (perm[used]) and the unreferenced one (perm[used + 1])
+  std::vector<int> perm(pool->n_pages);
+  std::iota(perm.begin(), perm.end(), 0);
+  std::shuffle(perm.begin(), perm.end(), std::mt19937(0x5eed));
+  pool->pad_page = perm[used];
+  pool->bt_stride = maxp;
+  pool->bt.assign((size_t)n_seqs * maxp, pool->pad_page);
+  for (int i = 0, r = 0; i < maxp; ++i)
+    for (int b = 0; b < n_seqs; ++b)
+      if (i < npg[b]) pool->bt[(size_t)b * maxp + i] = perm[r++];
+  pool->layer_elems = (size_t)pool->n_pages * n_kv * P * HD;
+  pool->k.assign(2 * pool->layer_elems, 0x7F7F);
+  pool->v.assign(2 * pool->layer_elems, 0xFF7F);
+  size_t row0 = 0;
+  for (int b = 0; b < n_seqs; ++b) {
+    const int* bt = pool->bt.data() + (size_t)b * maxp;
+    for (int t = 0; t < lens[b]; ++t)
+      for (int g = 0; g < n_kv; ++g) {
+        const size_t dst = pool->layer_elems + (((size_t)bt[t / P] * n_kv + g) * P + t % P) * HD;
+        const size_t src = ((row0 + t) * n_kv + g) * HD;
+        memcpy(&pool->k[dst], k + src, (size_t)HD * 2);
+        memcpy(&pool->v[dst], v + src, (size_t)HD * 2);
+      }
+    row0 += lens[b];
+  }
+}
+
+}  // namespace cl
 
 using namespace cl;
 
@@ -159,6 +208,97 @@ int cl_op_attn_decode(int device, const float* q, const uint16_t* k_cache, const
     if (launch_attn_decode(a, nullptr, false) < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("launch_attn_decode failed"); return CL_ERR_CUDA; }
   CL_CUDA_OK(cudaDeviceSynchronize());
   CL_CUDA_OK(cudaMemcpy(out, dout.p, (size_t)qd * 4, cudaMemcpyDeviceToHost));
+  return CL_OK;
+}
+
+int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_small, const float* q, const uint16_t* k_cache,
+                            const uint16_t* v_cache, const int32_t* ctx_lens, const int32_t* slots, int32_t batch, int32_t n_slots,
+                            int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, float* out, uint16_t* out_bf16,
+                            int32_t* nsplit_used, int32_t* tc_small_used) {
+  if (!q || !k_cache || !v_cache || !ctx_lens || !out || batch <= 0 || n_slots < batch || variant < -1 || variant > 1 || nsplit < 0 ||
+      tc_small < -1 || tc_small > 1)
+    return CL_ERR_INVALID_ARG;
+  int rc = check_device(device);
+  if (rc) return rc;
+  const int rep = n_kv > 0 ? n_heads / n_kv : 0;
+  if ((head_dim != 64 && head_dim != 128) || (rep != 1 && rep != 2 && rep != 4 && rep != 8) || n_heads % n_kv ||
+      (page_size != 16 && page_size != 32 && page_size != 64)) {
+    set_last_error("unsupported attention shape");
+    return CL_ERR_INVALID_ARG;
+  }
+  const int P = page_size, HD = head_dim;
+  const size_t qd = (size_t)n_heads * HD;
+  std::vector<int> slot(batch), taken(n_slots, 0);
+  for (int b = 0; b < batch; ++b) {
+    slot[b] = slots ? slots[b] : b;
+    if (ctx_lens[b] <= 0 || slot[b] < 0 || slot[b] >= n_slots || taken[slot[b]]++) {
+      set_last_error("cl_op_attn_decode_batch: every context needs >= 1 token and a distinct slot < n_slots");
+      return CL_ERR_INVALID_ARG;
+    }
+  }
+  // the batched step's plan (Engine::enqueue_step_batched); explicit choices override it
+  int ns = 0, small = 0;
+  attn_decode_tc_plan(n_kv, batch, std::max(1, std::min(64, sm_count() / n_kv)), sm_count(), &ns, &small);
+  if (nsplit > 0) ns = nsplit;
+  if (tc_small >= 0) small = tc_small;
+  OpKvPool pool;
+  op_build_kv_pool(k_cache, v_cache, ctx_lens, batch, n_kv, HD, P, &pool);
+  // q, pos, the block tables, out, the partials and the counters are indexed by slot, as in the engine; q rows of the slots
+  // outside the batch are NaN
+  std::vector<float> qs((size_t)n_slots * qd, NAN);
+  std::vector<int> pos(n_slots, 0), bts((size_t)n_slots * pool.bt_stride, pool.pad_page);
+  for (int b = 0; b < batch; ++b) {
+    memcpy(&qs[(size_t)slot[b] * qd], q + (size_t)b * qd, qd * 4);
+    pos[slot[b]] = ctx_lens[b] - 1;
+    memcpy(&bts[(size_t)slot[b] * pool.bt_stride], &pool.bt[(size_t)b * pool.bt_stride], (size_t)pool.bt_stride * 4);
+  }
+  DevBuf dq, dk, dv, dbt, dpos, dslots, dout, dob, dpart, dcnt;
+  CL_CUDA_OK(dq.upload(qs.data(), qs.size() * 4));
+  CL_CUDA_OK(dk.upload(pool.k.data(), pool.k.size() * 2));
+  CL_CUDA_OK(dv.upload(pool.v.data(), pool.v.size() * 2));
+  CL_CUDA_OK(dbt.upload(bts.data(), bts.size() * 4));
+  CL_CUDA_OK(dpos.upload(pos.data(), pos.size() * 4));
+  CL_CUDA_OK(dslots.upload(slot.data(), slot.size() * 4));
+  CL_CUDA_OK(dout.alloc((size_t)n_slots * qd * 4));
+  CL_CUDA_OK(dob.alloc((size_t)batch * qd * 2));
+  CL_CUDA_OK(dpart.alloc((size_t)n_slots * n_kv * ns * rep * (HD + 2) * 4));
+  CL_CUDA_OK(dcnt.alloc((size_t)n_slots * n_kv * 4));
+  CL_CUDA_OK(cudaMemset(dcnt.p, 0, (size_t)n_slots * n_kv * 4));
+  AttnDecodeArgs a;
+  a.q = dq.as<float>(); a.q_stride = (int)qd;
+  a.kpool = dk.as<__nv_bfloat16>() + pool.layer_elems; a.vpool = dv.as<__nv_bfloat16>() + pool.layer_elems;
+  a.block_tables = dbt.as<int>(); a.bt_stride = pool.bt_stride; a.pos = dpos.as<int>();
+  a.out = dout.as<float>(); a.out_stride = (int)qd; a.out_bf16 = out_bf16 ? dob.as<__nv_bfloat16>() : nullptr;
+  a.part = dpart.as<float>(); a.counters = dcnt.as<unsigned>(); a.slots = dslots.as<int>(); a.batch = batch;
+  a.n_heads = n_heads; a.n_kv = n_kv; a.head_dim = HD; a.page_size = P; a.nsplit = ns; a.pdl_early = 0; a.tc_small = small;
+  // variant -1: the tensor-core kernel where it takes the shape and the pool's tensor maps exist, as in the engine
+  const long long pool_rows = 2LL * pool.n_pages * n_kv * P;
+  CUtensorMap km, vm;
+  bool tc = variant != 0 && attn_decode_tc_supported(n_heads, n_kv, HD, P, ns);
+  if (tc) tc = make_tmap_2d_bf16(&km, dk.p, pool_rows, HD, 64, 32) && make_tmap_2d_bf16(&vm, dv.p, pool_rows, HD, 64, 32);
+  if ((variant == 1 && !tc) || (!tc && ns > 64)) {
+    set_last_error("the decode attention kernel does not take this shape or split count");
+    return CL_ERR_INVALID_ARG;
+  }
+  // two launches without re-arming the split counters in between must give the same bits
+  std::vector<float> out1((size_t)n_slots * qd);
+  std::vector<uint16_t> ob1((size_t)batch * qd), ob2(ob1.size());
+  for (int run = 0; run < 2; ++run) {
+    CL_CUDA_OK(cudaMemcpy(dout.p, out, (size_t)n_slots * qd * 4, cudaMemcpyHostToDevice));
+    CL_CUDA_OK(cudaMemset(dob.p, 0xff, (size_t)batch * qd * 2));   // NaN: every element must be written
+    const int r = tc ? launch_attn_decode_tc(a, km, vm, pool_rows / 2, nullptr, false) : launch_attn_decode(a, nullptr, false);
+    if (r < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("decode attention launch failed"); return CL_ERR_CUDA; }
+    CL_CUDA_OK(cudaDeviceSynchronize());
+    CL_CUDA_OK(cudaMemcpy(run ? out : out1.data(), dout.p, (size_t)n_slots * qd * 4, cudaMemcpyDeviceToHost));
+    CL_CUDA_OK(cudaMemcpy(run ? ob2.data() : ob1.data(), dob.p, ob1.size() * 2, cudaMemcpyDeviceToHost));
+  }
+  if (nsplit_used) *nsplit_used = ns;
+  if (tc_small_used) *tc_small_used = tc ? small : -1;
+  if (out_bf16) memcpy(out_bf16, ob2.data(), ob2.size() * 2);
+  if (memcmp(out, out1.data(), out1.size() * 4) || memcmp(ob1.data(), ob2.data(), ob1.size() * 2)) {
+    set_last_error("cl_op_attn_decode_batch: the second launch (split counters not reset) changed the output");
+    return CL_ERR_INTERNAL;
+  }
   return CL_OK;
 }
 

@@ -3,7 +3,7 @@
 // (gemm_wgmma.cu) and the causal paged attention (prefill_kernels.cu / attn_prefill_tc.cu), once per chunk of up to
 // prefill_chunk_tokens_ tokens (prefill_chunked) or once for several prompts (prefill_multi).  The last position's logits
 // come from the decode LM head, so that prefill and decode share one logits/argmax tail.  Also: cl_op_gemm_bf16 /
-// cl_op_attn_prefill.
+// cl_op_gemm_bf16_epi / cl_op_attn_prefill*.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -288,82 +288,114 @@ int check_device(int device) {
   CL_CUDA_OK(cudaSetDevice(device));
   return CL_OK;
 }
+struct Stream {
+  cudaStream_t s = nullptr;
+  ~Stream() { if (s) cudaStreamDestroy(s); }
+};
 }  // namespace
 
 extern "C" {
 
-int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, int32_t t, int32_t n, int32_t k, int32_t iters,
-                    float* ms) {
-  if (!x || !w || !y || t <= 0 || n <= 0 || k <= 0) return CL_ERR_INVALID_ARG;
+// epi 0: y[k_splits][t][n] = the split-K partials (k_splits 0: the batched step's count, pick_splits_public); y == NULL only
+//        reports that count through *k_splits_used.
+// epi 1: y[t][n] = resid + x w^T, added in place (the tile path's o / down projections).
+// epi 2: act[t][n/2] = bf16(silu(gate) * up) of the interleaved gate|up rows (launch_gemm_bf16_silu).
+// The residual and SiLU epilogues run unsplit (k_splits 0 or 1), as in the tile path, and the SiLU launcher has no PDL launch.
+// pdl = 1 launches with programmatic stream serialization, as the batched step does, so the kernel requests its first W tiles
+// before griddepcontrol.wait.  Every output element starts as NaN.
+int cl_op_gemm_bf16_epi(int device, int epi, int32_t k_splits, int pdl, const uint16_t* x, const uint16_t* w, const float* resid, float* y,
+                        uint16_t* act, int32_t t, int32_t n, int32_t k, int32_t* k_splits_used) {
+  if (!x || !w || t <= 0 || n <= 0 || k <= 0 || k_splits < 0 || epi < 0 || epi > 2 || (epi == 0 && !y && !k_splits_used) ||
+      (epi == 1 && (!resid || !y)) || (epi == 2 && (!act || (n & 1) || pdl)))
+    return CL_ERR_INVALID_ARG;
   int rc = check_device(device);
   if (rc) return rc;
   if (!gemm_tc_supported(t, n, k)) { set_last_error("shape not supported by the wgmma GEMM (K % 8)"); return CL_ERR_INVALID_ARG; }
+  const int ks = k_splits ? k_splits : epi == 0 ? pick_splits_public(n, k) : 1;
+  if (k_splits_used) *k_splits_used = ks;
+  if (epi == 0 && !y) return CL_OK;
+  if (epi != 0 && ks != 1) { set_last_error("the residual and SiLU epilogues run unsplit"); return CL_ERR_INVALID_ARG; }
+  if (!gemm_splits_supported(k, ks)) { set_last_error("launch_gemm_bf16 refuses this split count"); return CL_ERR_INVALID_ARG; }
+  const size_t out_bytes = epi == 0 ? (size_t)ks * t * n * 4 : epi == 1 ? (size_t)t * n * 4 : (size_t)t * (n / 2) * 2;
+  DevBuf dx, dw, dy;
+  CL_CUDA_OK(dx.upload(x, (size_t)t * k * 2));
+  CL_CUDA_OK(dw.upload(w, (size_t)n * k * 2));
+  if (epi == 1) CL_CUDA_OK(dy.upload(resid, out_bytes));
+  else {
+    CL_CUDA_OK(dy.alloc(out_bytes));
+    CL_CUDA_OK(cudaMemset(dy.p, 0xff, out_bytes));   // NaN pattern: every element must be written
+  }
+  // a pageable upload may return before its DMA lands and the fill is asynchronous: both must be done before the launch
+  CL_CUDA_OK(cudaDeviceSynchronize());
+  Stream st;
+  CL_CUDA_OK(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
+  const __nv_bfloat16 *X = dx.as<__nv_bfloat16>(), *W = dw.as<__nv_bfloat16>();
+  const int r = epi == 2 ? launch_gemm_bf16_silu(X, W, t, n, k, dy.as<__nv_bfloat16>(), n / 2, st.s)
+                         : launch_gemm_bf16(X, W, dy.as<float>(), epi == 1 ? dy.as<float>() : nullptr, t, n, k, st.s, ks, pdl != 0);
+  if (r < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("wgmma GEMM launch failed"); return CL_ERR_CUDA; }
+  CL_CUDA_OK(cudaStreamSynchronize(st.s));
+  CL_CUDA_OK(cudaMemcpy(epi == 2 ? (void*)act : (void*)y, dy.p, out_bytes, cudaMemcpyDeviceToHost));
+  return CL_OK;
+}
+
+int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, int32_t t, int32_t n, int32_t k, int32_t iters,
+                    float* ms) {
+  if (!y) return CL_ERR_INVALID_ARG;
+  const int rc = cl_op_gemm_bf16_epi(device, 0, 1, 0, x, w, nullptr, y, nullptr, t, n, k, nullptr);
+  if (rc || iters <= 0 || !ms) return rc;
   DevBuf dx, dw, dy;
   CL_CUDA_OK(dx.upload(x, (size_t)t * k * 2));
   CL_CUDA_OK(dw.upload(w, (size_t)n * k * 2));
   CL_CUDA_OK(dy.alloc((size_t)t * n * 4));
-  CL_CUDA_OK(cudaMemset(dy.p, 0xff, (size_t)t * n * 4));  // NaN pattern: every element must be written
-  if (launch_gemm_bf16(dx.as<__nv_bfloat16>(), dw.as<__nv_bfloat16>(), dy.as<float>(), nullptr, t, n, k, nullptr) < 0) {
-    CL_CUDA_OK(cudaGetLastError());
-    set_last_error("launch_gemm_bf16 failed");
-    return CL_ERR_CUDA;
-  }
+  cudaEvent_t e0, e1;
+  CL_CUDA_OK(cudaEventCreate(&e0));
+  CL_CUDA_OK(cudaEventCreate(&e1));
+  for (int i = 0; i < 3; ++i) launch_gemm_bf16(dx.as<__nv_bfloat16>(), dw.as<__nv_bfloat16>(), dy.as<float>(), nullptr, t, n, k, nullptr);
   CL_CUDA_OK(cudaDeviceSynchronize());
-  CL_CUDA_OK(cudaMemcpy(y, dy.p, (size_t)t * n * 4, cudaMemcpyDeviceToHost));
-  if (iters > 0 && ms) {
-    cudaEvent_t e0, e1;
-    CL_CUDA_OK(cudaEventCreate(&e0));
-    CL_CUDA_OK(cudaEventCreate(&e1));
-    for (int i = 0; i < 3; ++i) launch_gemm_bf16(dx.as<__nv_bfloat16>(), dw.as<__nv_bfloat16>(), dy.as<float>(), nullptr, t, n, k, nullptr);
-    CL_CUDA_OK(cudaDeviceSynchronize());
-    CL_CUDA_OK(cudaEventRecord(e0));
-    for (int i = 0; i < iters; ++i) launch_gemm_bf16(dx.as<__nv_bfloat16>(), dw.as<__nv_bfloat16>(), dy.as<float>(), nullptr, t, n, k, nullptr);
-    CL_CUDA_OK(cudaEventRecord(e1));
-    CL_CUDA_OK(cudaDeviceSynchronize());
-    float tm = 0.f;
-    CL_CUDA_OK(cudaEventElapsedTime(&tm, e0, e1));
-    *ms = tm / (float)iters;
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-  }
+  CL_CUDA_OK(cudaEventRecord(e0));
+  for (int i = 0; i < iters; ++i) launch_gemm_bf16(dx.as<__nv_bfloat16>(), dw.as<__nv_bfloat16>(), dy.as<float>(), nullptr, t, n, k, nullptr);
+  CL_CUDA_OK(cudaEventRecord(e1));
+  CL_CUDA_OK(cudaDeviceSynchronize());
+  float tm = 0.f;
+  CL_CUDA_OK(cudaEventElapsedTime(&tm, e0, e1));
+  *ms = tm / (float)iters;
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
   return CL_OK;
 }
 
-// variant: -1 auto (wgmma kernel when the shape allows), 0 mma.sync kernel, 1 wgmma kernel
-static int attn_prefill_impl(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t, int32_t n_heads, int32_t n_kv,
-                             int32_t head_dim, int variant, int iters, float* out, float* ms) {
-  if (!q || !k || !v || !out || t <= 0) return CL_ERR_INVALID_ARG;
+// Causal attention of the queries at positions pos0 .. pos0 + t - 1 (q [t][n_heads * head_dim]) over keys 0 .. pos0 + t - 1
+// (k, v [pos0 + t][n_kv][head_dim]), paged by op_build_kv_pool.  variant: -1 the engine's rule (Engine::attn_prefill: the wgmma
+// kernel when it takes the shape), 0 mma.sync kernel, 1 wgmma kernel.  out [t][n_heads * head_dim] = the kernel's bf16 output.
+static int attn_prefill_impl(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0, int32_t t,
+                             int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int iters, float* out, float* ms) {
+  if (!q || !k || !v || !out || t <= 0 || pos0 < 0 || variant < -1 || variant > 1) return CL_ERR_INVALID_ARG;
   int rc = check_device(device);
   if (rc) return rc;
-  if ((head_dim != 64 && head_dim != 128) || n_kv <= 0 || n_heads % n_kv) { set_last_error("unsupported attention shape"); return CL_ERR_INVALID_ARG; }
-  const int P = 32, HD = head_dim;
-  const int n_pages = (t + P - 1) / P;
-  std::vector<int> bt(n_pages);
-  for (int i = 0; i < n_pages; ++i) bt[i] = n_pages - 1 - i;  // reversed page order
-  const size_t pool = (size_t)n_pages * n_kv * P * HD;
-  std::vector<uint16_t> kp(pool, 0), vp(pool, 0);
-  for (int tt = 0; tt < t; ++tt)
-    for (int g = 0; g < n_kv; ++g) {
-      const size_t dst = (((size_t)bt[tt / P] * n_kv + g) * P + tt % P) * HD;
-      memcpy(&kp[dst], k + ((size_t)tt * n_kv + g) * HD, (size_t)HD * 2);
-      memcpy(&vp[dst], v + ((size_t)tt * n_kv + g) * HD, (size_t)HD * 2);
-    }
+  if ((head_dim != 64 && head_dim != 128) || n_kv <= 0 || n_heads % n_kv || (page_size != 16 && page_size != 32 && page_size != 64)) {
+    set_last_error("unsupported attention shape");
+    return CL_ERR_INVALID_ARG;
+  }
+  const int P = page_size, HD = head_dim, n_tok = pos0 + t;
+  OpKvPool pool;
+  op_build_kv_pool(k, v, &n_tok, 1, n_kv, HD, P, &pool);
   const size_t qd = (size_t)n_heads * HD;
   DevBuf dq, dk, dv, dbt, dout, dout32;
   CL_CUDA_OK(dq.upload(q, (size_t)t * qd * 2));
-  CL_CUDA_OK(dk.upload(kp.data(), pool * 2));
-  CL_CUDA_OK(dv.upload(vp.data(), pool * 2));
-  CL_CUDA_OK(dbt.upload(bt.data(), bt.size() * 4));
+  CL_CUDA_OK(dk.upload(pool.k.data(), pool.k.size() * 2));
+  CL_CUDA_OK(dv.upload(pool.v.data(), pool.v.size() * 2));
+  CL_CUDA_OK(dbt.upload(pool.bt.data(), pool.bt.size() * 4));
   CL_CUDA_OK(dout.alloc((size_t)t * qd * 2));
   CL_CUDA_OK(cudaMemset(dout.p, 0xff, (size_t)t * qd * 2));   // NaN pattern: every output must be written
   CL_CUDA_OK(dout32.alloc((size_t)t * qd * 4));
-  AttnPrefillArgs a{dq.as<__nv_bfloat16>(), dk.as<__nv_bfloat16>(), dv.as<__nv_bfloat16>(), dbt.as<int>(), P, 0, t, n_heads, n_kv, HD,
-                    dout.as<__nv_bfloat16>()};
+  AttnPrefillArgs a{dq.as<__nv_bfloat16>(), dk.as<__nv_bfloat16>() + pool.layer_elems, dv.as<__nv_bfloat16>() + pool.layer_elems,
+                    dbt.as<int>(), P, pos0, t, n_heads, n_kv, HD, dout.as<__nv_bfloat16>()};
+  const long long pool_rows = 2LL * pool.n_pages * n_kv * P;
   CUtensorMap km, vm;
-  bool tc = variant != 0 && attn_prefill_tc_supported(n_heads, n_kv, HD, P, 0, t);
-  if (tc) tc = make_tmap_2d_bf16(&km, dk.p, (uint64_t)n_pages * n_kv * P, HD, 64, 32) && make_tmap_2d_bf16(&vm, dv.p, (uint64_t)n_pages * n_kv * P, HD, 64, 32);
+  bool tc = variant != 0 && attn_prefill_tc_supported(n_heads, n_kv, HD, P, pos0, t);
+  if (tc) tc = make_tmap_2d_bf16(&km, dk.p, pool_rows, HD, 64, 32) && make_tmap_2d_bf16(&vm, dv.p, pool_rows, HD, 64, 32);
   if (variant == 1 && !tc) { set_last_error("wgmma prefill attention does not support this shape"); return CL_ERR_INVALID_ARG; }
-  auto run = [&]() { return tc ? launch_attn_prefill_tc(a, km, vm, 0, nullptr) : launch_attn_prefill(a, nullptr); };
+  auto run = [&]() { return tc ? launch_attn_prefill_tc(a, km, vm, pool_rows / 2, nullptr) : launch_attn_prefill(a, nullptr); };
   if (run() < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("prefill attention launch failed"); return CL_ERR_CUDA; }
   if (launch_bf16_to_f32(dout.as<__nv_bfloat16>(), dout32.as<float>(), (int64_t)t * qd, nullptr) < 0) return CL_ERR_CUDA;
   CL_CUDA_OK(cudaDeviceSynchronize());
@@ -389,11 +421,15 @@ static int attn_prefill_impl(int device, const uint16_t* q, const uint16_t* k, c
 
 int cl_op_attn_prefill(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t, int32_t n_heads, int32_t n_kv,
                        int32_t head_dim, float* out) {
-  return attn_prefill_impl(device, q, k, v, t, n_heads, n_kv, head_dim, -1, 0, out, nullptr);
+  return attn_prefill_impl(device, -1, q, k, v, 0, t, n_heads, n_kv, head_dim, 32, 0, out, nullptr);
 }
 int cl_op_attn_prefill_variant(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t, int32_t n_heads,
                                int32_t n_kv, int32_t head_dim, float* out, int32_t iters, float* ms) {
-  return attn_prefill_impl(device, q, k, v, t, n_heads, n_kv, head_dim, variant, iters, out, ms);
+  return attn_prefill_impl(device, variant, q, k, v, 0, t, n_heads, n_kv, head_dim, 32, iters, out, ms);
+}
+int cl_op_attn_prefill_cached(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0, int32_t t,
+                              int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, float* out) {
+  return attn_prefill_impl(device, variant, q, k, v, pos0, t, n_heads, n_kv, head_dim, page_size, 0, out, nullptr);
 }
 
 }  // extern "C"

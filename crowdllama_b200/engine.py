@@ -76,7 +76,8 @@ EXPORTS = [
     "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
     "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
-    "cl_op_gemm_bf16", "cl_op_attn_prefill", "cl_op_attn_prefill_variant", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
+    "cl_op_attn_decode_batch", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
+    "cl_op_attn_prefill_cached", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages",
     "cl_tokenizer_load", "cl_tokenizer_free", "cl_tokenizer_encode", "cl_tokenizer_decode", "cl_tokenizer_info", "cl_engine_load_tokenizer",
@@ -147,9 +148,13 @@ def lib():
         "cl_op_rmsnorm_gateup": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, f32, vp, i32, i32]),
         "cl_op_attn_decode": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
         "cl_op_qkv_rope_append": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, f32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
+        "cl_op_attn_decode_batch": (C.c_int, [C.c_int, C.c_int, i32, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp,
+                                              P(i32), P(i32)]),
         "cl_op_gemm_bf16": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, P(f32)]),
+        "cl_op_gemm_bf16_epi": (C.c_int, [C.c_int, C.c_int, i32, C.c_int, vp, vp, vp, vp, vp, i32, i32, i32, P(i32)]),
         "cl_op_attn_prefill": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, vp]),
         "cl_op_attn_prefill_variant": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, vp, i32, P(f32)]),
+        "cl_op_attn_prefill_cached": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
         "cl_op_sample": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), vp, vp, i32, vp, vp]),
         "cl_op_synth_weights": (C.c_int, [C.c_int, u64, i32, i64, f32, vp]),
         "cl_tokenizer_load": (C.c_int, [C.c_char_p, C.c_char_p, P(vp)]),
@@ -580,6 +585,28 @@ def op_attn_decode(q_roped, k_cache_bf16, v_cache_bf16, n_heads, n_kv, head_dim,
     return out
 
 
+def op_attn_decode_batch(q, k_cache_bf16, v_cache_bf16, ctx_lens, n_heads, n_kv, head_dim, page_size=32, slots=None, n_slots=None,
+                         out_init=None, variant=-1, nsplit=0, tc_small=-1, with_bf16=True, device=0):
+    """cl_op_attn_decode_batch: decode attention of the batched step.  q [B][H*D] fp32; k/v caches [sum(ctx_lens)][n_kv][D] bf16,
+    the sequences back to back.  Returns (out [n_slots][H*D] fp32 (starts as out_init, NaN when None), out_bf16 [B][H*D] uint16
+    or None, nsplit used, tc_small used (-1: the CUDA-core kernel ran))."""
+    q = np.ascontiguousarray(q, dtype=np.float32)
+    kc = np.ascontiguousarray(k_cache_bf16, dtype=np.uint16)
+    vc = np.ascontiguousarray(v_cache_bf16, dtype=np.uint16)
+    lens = np.ascontiguousarray(ctx_lens, dtype=np.int32)
+    B = len(lens)
+    n_slots = n_slots or B
+    sl = None if slots is None else np.ascontiguousarray(slots, dtype=np.int32)
+    out = np.full((n_slots, n_heads * head_dim), np.nan, np.float32) if out_init is None else \
+        np.array(out_init, dtype=np.float32, order="C", copy=True)
+    ob = np.empty((B, n_heads * head_dim), np.uint16) if with_bf16 else None
+    ns, small = C.c_int32(), C.c_int32()
+    _check(lib().cl_op_attn_decode_batch(device, variant, nsplit, tc_small, _ptr(q), _ptr(kc), _ptr(vc), _ptr(lens),
+                                         None if sl is None else _ptr(sl), B, n_slots, n_heads, n_kv, head_dim, page_size, _ptr(out),
+                                         None if ob is None else _ptr(ob), C.byref(ns), C.byref(small)), "cl_op_attn_decode_batch")
+    return out, ob, ns.value, small.value
+
+
 def op_qkv_rope_append(w_qkv_bf16, h, gain, eps, n_heads, n_kv, head_dim, pos, rope_theta, variant=0, device=0):
     w = np.ascontiguousarray(w_qkv_bf16, dtype=np.uint16)
     h = np.ascontiguousarray(h, dtype=np.float32)
@@ -600,6 +627,41 @@ def op_gemm_bf16(x_bf16, w_bf16, iters=0, device=0):
     _check(lib().cl_op_gemm_bf16(device, _ptr(x), _ptr(w), _ptr(y), x.shape[0], w.shape[0], w.shape[1], iters,
                                  C.byref(ms)), "cl_op_gemm_bf16")
     return (y, ms.value) if iters else y
+
+
+def op_gemm_bf16_epi(x_bf16, w_bf16, epi=0, k_splits=0, pdl=False, resid=None, device=0):
+    """cl_op_gemm_bf16_epi.  epi 0: (partials [k_splits][T][N] fp32, k_splits used); epi 1: (resid + X W^T [T][N] fp32, 1);
+    epi 2: (bf16(silu(gate) * up) [T][N/2] as uint16, 1) of interleaved gate|up rows of W."""
+    x = np.ascontiguousarray(x_bf16, dtype=np.uint16)
+    w = np.ascontiguousarray(w_bf16, dtype=np.uint16)
+    t, n, k = x.shape[0], w.shape[0], w.shape[1]
+    ks = C.c_int32()
+    L = lib()
+    if epi == 0:
+        _check(L.cl_op_gemm_bf16_epi(device, 0, k_splits, int(pdl), _ptr(x), _ptr(w), None, None, None, t, n, k, C.byref(ks)),
+               "cl_op_gemm_bf16_epi")
+        y, act, r = np.empty((ks.value, t, n), np.float32), None, None
+    elif epi == 1:
+        r = np.ascontiguousarray(resid, dtype=np.float32)
+        y, act = np.empty((t, n), np.float32), None
+    else:
+        y, act, r = None, np.empty((t, n // 2), np.uint16), None
+    _check(L.cl_op_gemm_bf16_epi(device, epi, k_splits, int(pdl), _ptr(x), _ptr(w), None if r is None else _ptr(r),
+                                 None if y is None else _ptr(y), None if act is None else _ptr(act), t, n, k, C.byref(ks)),
+           "cl_op_gemm_bf16_epi")
+    return (act if epi == 2 else y), ks.value
+
+
+def op_attn_prefill_cached(q_bf16, k_bf16, v_bf16, pos0, n_heads, n_kv, head_dim, page_size=32, variant=-1, device=0):
+    """cl_op_attn_prefill_cached: causal attention of q [T][H*D] (positions pos0 .. pos0+T-1) over k, v [pos0+T][n_kv][D]."""
+    q = np.ascontiguousarray(q_bf16, dtype=np.uint16)
+    k = np.ascontiguousarray(k_bf16, dtype=np.uint16)
+    v = np.ascontiguousarray(v_bf16, dtype=np.uint16)
+    t = q.shape[0]
+    out = np.empty((t, n_heads * head_dim), np.float32)
+    _check(lib().cl_op_attn_prefill_cached(device, variant, _ptr(q), _ptr(k), _ptr(v), pos0, t, n_heads, n_kv, head_dim, page_size,
+                                           _ptr(out)), "cl_op_attn_prefill_cached")
+    return out
 
 
 def op_attn_prefill(q_bf16, k_bf16, v_bf16, n_heads, n_kv, head_dim, device=0):

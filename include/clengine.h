@@ -334,9 +334,28 @@ int cl_op_qkv_rope_append(int device, int variant, const uint16_t* w_qkv, const 
 int cl_op_attn_decode(int device, const float* q, const uint16_t* k_cache, const uint16_t* v_cache,
                       int32_t ctx_len, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size,
                       float* out);
+/* decode attention of the batched step for `batch` sequences at once.  q [batch][n_heads*head_dim] fp32; k_cache/v_cache
+ * [sum of ctx_lens][n_kv][head_dim] bf16 = the sequences' tokens back to back (each one's current token last); slots[batch]
+ * (NULL: 0..batch-1) distinct and < n_slots; out [n_slots][n_heads*head_dim] fp32 is read and written: rows of the slots
+ * outside the batch come back unchanged; out_bf16 [batch][n_heads*head_dim] (may be NULL) = the bf16 copy the o-projection
+ * reads.  variant 0: CUDA-core kernel (decode_kernels.cu), 1: tensor-core kernel (attn_decode_tc.cu), -1: the step's choice.
+ * nsplit 0 / tc_small -1: the step's plan (attn_decode_tc_plan); other values are used as given.  *nsplit_used and
+ * *tc_small_used (-1: the CUDA-core kernel ran) report what ran.  The kernel runs twice without resetting its split counters;
+ * CL_ERR_INTERNAL when the two outputs differ in any bit. */
+int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_small, const float* q, const uint16_t* k_cache,
+                            const uint16_t* v_cache, const int32_t* ctx_lens, const int32_t* slots, int32_t batch, int32_t n_slots,
+                            int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, float* out, uint16_t* out_bf16,
+                            int32_t* nsplit_used, int32_t* tc_small_used);
 /* prefill GEMM on the tensor cores (wgmma): Y[t][n] = sum_k X[t][k] W[n][k]; X,W bf16, Y fp32 */
 int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, int32_t t,
                     int32_t n, int32_t k, int32_t iters, float* ms);
+/* the same GEMM with the epilogues and launches of the engine.  epi 0: y [k_splits][t][n] = the split-K partials (split s
+ * sums k-blocks of 64 s*ceil(nkb/k_splits) ..), k_splits 0 = the batched step's count; y == NULL only reports the count.
+ * epi 1: y [t][n] = resid + X W^T.  epi 2: act [t][n/2] bf16 = bf16(silu(gate) * up) of interleaved gate|up rows.  Epilogues
+ * 1 and 2 run unsplit (k_splits 0 or 1) and epi 2 without PDL.  pdl 1: programmatic dependent launch, as in the batched
+ * step.  *k_splits_used (may be NULL) reports the count; CL_ERR_INVALID_ARG for a count the GEMM refuses. */
+int cl_op_gemm_bf16_epi(int device, int epi, int32_t k_splits, int pdl, const uint16_t* x, const uint16_t* w, const float* resid,
+                        float* y, uint16_t* act, int32_t t, int32_t n, int32_t k, int32_t* k_splits_used);
 /* causal prefill attention: q [t][n_heads][d], k,v [t][n_kv][d] bf16 (roped), out bf16-rounded fp32 */
 int cl_op_attn_prefill(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v,
                        int32_t t, int32_t n_heads, int32_t n_kv, int32_t head_dim, float* out);
@@ -344,6 +363,10 @@ int cl_op_attn_prefill(int device, const uint16_t* q, const uint16_t* k, const u
  * 1: wgmma kernel (attn_prefill_tc.cu, head_dim 128), -1: what the engine would pick — and an optional timing loop */
 int cl_op_attn_prefill_variant(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t,
                                int32_t n_heads, int32_t n_kv, int32_t head_dim, float* out, int32_t iters, float* ms);
+/* the same behind a cached prefix: q [t][n_heads][d] for positions pos0 .. pos0+t-1, k,v [pos0+t][n_kv][d]; page_size 16,
+ * 32 or 64.  CL_ERR_INVALID_ARG when variant 1 does not take the shape. */
+int cl_op_attn_prefill_cached(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0,
+                              int32_t t, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, float* out);
 /* the decode step's device sampler (the step tail kernel) on host logits [n_rows][vocab]: row r draws with sp[r] at RNG
  * step step[r], with history row r = history + r * hist_stride, n_history[r] ids (history may be NULL when every
  * n_history[r] is 0).  ids_out[n_rows].  CL_ERR_INVALID_ARG for settings the device sampler does not cover. */
