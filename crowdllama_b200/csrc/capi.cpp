@@ -59,6 +59,12 @@ int cl_sample_token(const float* logits, int32_t vocab, const cl_sampling* s, co
   return CL_OK;
 }
 
+int cl_draft_ngram(const int32_t* hist, int32_t n, int32_t k, int32_t* out, int32_t* n_out) {
+  if (!out || !n_out || n < 0 || (n > 0 && !hist) || k < 1 || k > kSpecMaxDraft) return CL_ERR_INVALID_ARG;
+  *n_out = cl::ngram_draft(hist, n, k, out);
+  return CL_OK;
+}
+
 void cl_greedy_sampling(cl_sampling* s, int32_t max_new_tokens) {
   memset(s, 0, sizeof *s);
   s->temperature = 0.f;
@@ -122,6 +128,11 @@ int cl_engine_stats(cl_engine* e, cl_stats* out) {
 int cl_engine_prefix_stats(cl_engine* e, cl_prefix_stats* out) {
   if (!e || !out) return CL_ERR_INVALID_ARG;
   return e->impl.prefix_stats(out);   // like cl_engine_stats: no engine lock, so it never waits behind a scheduler iteration
+}
+
+int cl_engine_spec_stats(cl_engine* e, cl_spec_stats* out) {
+  if (!e || !out) return CL_ERR_INVALID_ARG;
+  return e->impl.spec_stats(out);   // atomics only, no engine lock
 }
 
 int cl_engine_set_tensor(cl_engine* e, int32_t layer, int32_t kind, const uint16_t* data, int64_t n) {
@@ -455,6 +466,17 @@ int cl_decode_step_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, con
   if (!e || !seqs || !ids) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
   CL_GUARD(return e->impl.decode_step_batch(seqs, n_seqs, ids, logits_out, argmax_out);)
+}
+int cl_decode_verify(cl_engine* e, cl_seq_t s, int32_t input_id, const int32_t* draft, int32_t k, const cl_sampling* sp, uint64_t step0,
+                     int32_t* ids_out, int32_t* n_out, float* logits_out) {
+  if (!e || !draft || !ids_out || !n_out) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(
+    int n = 0;
+    const int rc = e->impl.decode_verify(s, input_id, draft, k, sp, step0, ids_out, &n, logits_out);
+    *n_out = n;
+    return rc;
+  )
 }
 int cl_seq_fake_fill(cl_engine* e, cl_seq_t s, int32_t n_tokens) {
   if (!e) return CL_ERR_INVALID_ARG;

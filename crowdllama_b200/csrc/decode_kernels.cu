@@ -808,9 +808,21 @@ __device__ __forceinline__ double sample_uniform01(unsigned long long seed, unsi
   return __dmul_rn((double)(x >> 11), 1.0 / 9007199254740992.0);
 }
 
-// One block of a sampled slot: the top-k keys of its vocabulary slice (repeat penalty applied) -> a.sample.cand; the
-// last block to finish merges them, draws, and advances the slot.
-__device__ __forceinline__ void step_tail_sample(const StepTailArgs& a, int b, int slot) {
+// History of a draw: the slot's ring (ids 0 .. ring_len - 1, id i at ring[i % kSampleHistMax]) followed by n_extra ids
+// that are not in the ring yet (a decode step's input; the inputs of a verify pass up to its row).
+struct TailHist {
+  const int* ring;
+  int ring_len;
+  const int* extra;
+  int n_extra;
+};
+
+// The draw of one logits row, called by all kTailBlocks blocks of the row: each block keys its vocabulary slice (repeat
+// penalty applied) and leaves its top-k keys in cand[blockIdx.x]; the last block to finish merges them and draws at RNG
+// step *step + step_add.  Returns the id on thread 0 of the last block, -1 on every other thread.
+__device__ __forceinline__ int tail_draw(const float* lg_row, int V, const SampleParams& sp, const TailHist& h,
+                                         unsigned long long* cand_row, unsigned* counter, const unsigned long long* step,
+                                         int step_add) {
   __shared__ unsigned long long keys[kSampleSliceMax];
   __shared__ unsigned pen[kSampleSliceMax / 32];
   __shared__ unsigned long long top[kSampleTopKMax], sorted[kSampleTopKMax];
@@ -818,25 +830,20 @@ __device__ __forceinline__ void step_tail_sample(const StepTailArgs& a, int b, i
   __shared__ int n_out, is_last_s;
   __shared__ double s_den;
   const int tid = threadIdx.x;
-  const SampleState& S = a.sample;
-  const SampleParams sp = S.par[slot];
-  const int V = a.vocab, K = sp.top_k;
-  const int input = a.tok[slot];
-  const int hlen = S.hist_len[slot];
-  const int* ring = S.hist + (size_t)slot * kSampleHistMax;
+  const int K = sp.top_k;
   const int slice = (V + (int)gridDim.x - 1) / (int)gridDim.x;
   const int lo = blockIdx.x * slice, n = max(0, min(slice, V - lo));
-  const float* lg = a.logits + (size_t)slot * V + lo;
+  const float* lg = lg_row + lo;
 
   for (int i = tid; i < kSampleSliceMax / 32; i += 256) pen[i] = 0u;
   if (tid == 0) n_out = 0;
   __syncthreads();
   if (sp.repeat_penalty != 1.0f && sp.repeat_last_n != 0) {   // the distinct in-range ids of the last repeat_last_n
-    const int total = hlen + (S.push_input ? 1 : 0);
+    const int total = h.ring_len + h.n_extra;
     const int w = sp.repeat_last_n > 0 && total > sp.repeat_last_n ? sp.repeat_last_n : total;
     for (int j = tid; j < w; j += 256) {
       const int idx = total - w + j;
-      const int id = (S.push_input && idx == hlen) ? input : ring[idx % kSampleHistMax];
+      const int id = idx < h.ring_len ? h.ring[idx % kSampleHistMax] : h.extra[idx - h.ring_len];
       if (id >= lo && id < lo + n) atomicOr(&pen[(id - lo) >> 5], 1u << ((id - lo) & 31));
     }
   }
@@ -848,7 +855,7 @@ __device__ __forceinline__ void step_tail_sample(const StepTailArgs& a, int b, i
   }
   __syncthreads();
   const unsigned long long t1 = n > K ? block_topk_threshold([&](int i) { return keys[i]; }, n, K) : 1ull;
-  unsigned long long* cand = S.cand + ((size_t)slot * gridDim.x + blockIdx.x) * kSampleTopKMax;
+  unsigned long long* cand = cand_row + (size_t)blockIdx.x * kSampleTopKMax;
   for (int i = tid; i < n; i += 256)
     if (keys[i] >= t1) cand[atomicAdd(&n_out, 1)] = keys[i];
   __syncthreads();
@@ -856,17 +863,17 @@ __device__ __forceinline__ void step_tail_sample(const StepTailArgs& a, int b, i
   __threadfence();
   __syncthreads();
   if (tid == 0) {
-    const unsigned old = atomicAdd(a.counters + slot, 1u);
+    const unsigned old = atomicAdd(counter, 1u);
     is_last_s = (old == gridDim.x - 1);
-    if (is_last_s) a.counters[slot] = 0u;
+    if (is_last_s) *counter = 0u;
     n_out = 0;
   }
   __syncthreads();
-  if (!is_last_s) return;
+  if (!is_last_s) return -1;
   __threadfence();
 
   // merge: the k largest of the kTailBlocks * k candidates, sorted descending
-  const unsigned long long* cs = S.cand + (size_t)slot * gridDim.x * kSampleTopKMax;
+  const unsigned long long* cs = cand_row;
   auto cget = [&](int i) { return __ldcg(cs + (size_t)(i / K) * kSampleTopKMax + (i % K)); };
   const int nc = (int)gridDim.x * K;
   const unsigned long long t2 = block_topk_threshold(cget, nc, K);
@@ -895,7 +902,7 @@ __device__ __forceinline__ void step_tail_sample(const StepTailArgs& a, int b, i
   __shared__ double q[kSampleTopKMax];
   if (tid < K) q[tid] = __ddiv_rn(p[tid], s_den);
   __syncthreads();
-  if (tid != 0) return;
+  if (tid != 0) return -1;
   int keep = K;
   if (sp.top_p > 0.f && sp.top_p < 1.f) {
     double cum = 0.0;
@@ -903,33 +910,24 @@ __device__ __forceinline__ void step_tail_sample(const StepTailArgs& a, int b, i
   }
   double tot = 0.0;
   for (int i = 0; i < keep; ++i) tot = __dadd_rn(tot, p[i]);
-  const unsigned long long step = S.step[slot];
-  const double u = __dmul_rn(sample_uniform01(sp.seed, step), tot);
+  const double u = __dmul_rn(sample_uniform01(sp.seed, *step + (unsigned long long)step_add), tot);
   double cum = 0.0;
   int pick = sample_key_id(sorted[keep - 1]);
   for (int i = 0; i < keep; ++i) { cum = __dadd_rn(cum, p[i]); if (u < cum) { pick = sample_key_id(sorted[i]); break; } }
-  if (S.push_input) { S.hist[(size_t)slot * kSampleHistMax + hlen % kSampleHistMax] = input; S.hist_len[slot] = hlen + 1; }
-  S.step[slot] = step + 1;
-  a.tok[slot] = pick;
-  a.pos[slot] += 1;
-  const int sc = *a.step_counter;
-  a.ids_ring[(size_t)(sc % a.ring_steps) * a.ring_stride + b] = pick;
+  return pick;
 }
 
-__global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a) {
+// Greedy choice of one logits row (largest value, lowest index on ties), called by all kTailBlocks blocks of the row:
+// per-block partials in part_val / part_idx, merged by the last block to finish.  Returns the id on lane 0 of warp 0 of
+// the last block, -1 on every other thread.
+__device__ __forceinline__ int tail_argmax(const float* lg, int V, float* part_val, int* part_idx, unsigned* counter) {
   __shared__ float sv[8];
   __shared__ int si[8];
   __shared__ int is_last_s;
-  pdl_launch_dependents();
-  pdl_wait();
-  const int b = blockIdx.y;
-  const int slot = a.slots ? a.slots[b] : b;
-  if (a.sample.mode && a.sample.mode[slot]) { step_tail_sample(a, b, slot); return; }
-  const float* lg = a.logits + (size_t)slot * a.vocab;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float best = -INFINITY;
   int bi = 0x7fffffff;
-  for (int i = blockIdx.x * 256 + tid; i < a.vocab; i += gridDim.x * 256) {
+  for (int i = blockIdx.x * 256 + tid; i < V; i += gridDim.x * 256) {
     const float v = lg[i];
     if (v > best || (v == best && i < bi)) { best = v; bi = i; }
   }
@@ -944,20 +942,20 @@ __global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a)
   if (tid == 0) {
     for (int w = 1; w < 8; ++w)
       if (sv[w] > best || (sv[w] == best && si[w] < bi)) { best = sv[w]; bi = si[w]; }
-    a.part_val[(size_t)slot * gridDim.x + blockIdx.x] = best;
-    a.part_idx[(size_t)slot * gridDim.x + blockIdx.x] = bi;
+    part_val[blockIdx.x] = best;
+    part_idx[blockIdx.x] = bi;
     __threadfence();
-    const unsigned old = atomicAdd(a.counters + slot, 1u);
+    const unsigned old = atomicAdd(counter, 1u);
     is_last_s = (old == gridDim.x - 1);
-    if (is_last_s) a.counters[slot] = 0u;
+    if (is_last_s) *counter = 0u;
   }
   __syncthreads();
-  if (!is_last_s || warp != 0) return;
+  if (!is_last_s || warp != 0) return -1;
   __threadfence();
   best = -INFINITY; bi = 0x7fffffff;
   for (int i = lane; i < (int)gridDim.x; i += 32) {
-    const float v = __ldcg(a.part_val + (size_t)slot * gridDim.x + i);
-    const int id = __ldcg(a.part_idx + (size_t)slot * gridDim.x + i);
+    const float v = __ldcg(part_val + i);
+    const int id = __ldcg(part_idx + i);
     if (v > best || (v == best && id < bi)) { best = v; bi = id; }
   }
 #pragma unroll
@@ -966,13 +964,88 @@ __global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a)
     const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
     if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
   }
-  if (lane != 0) return;
-  if (bi == 0x7fffffff) bi = 0;  // all-NaN logits: stay in range
-  a.tok[slot] = bi;
+  if (lane != 0) return -1;
+  return bi == 0x7fffffff ? 0 : bi;   // all-NaN logits: stay in range
+}
+
+__global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.y;
+  const int slot = a.slots ? a.slots[b] : b;
+  const float* lg = a.logits + (size_t)slot * a.vocab;
+  const SampleState& S = a.sample;
+  const bool sampled = S.mode && S.mode[slot];
+  int pick;
+  if (sampled) {
+    const TailHist h{S.hist + (size_t)slot * kSampleHistMax, S.hist_len[slot], a.tok + slot, S.push_input};
+    pick = tail_draw(lg, a.vocab, S.par[slot], h, S.cand + (size_t)slot * gridDim.x * kSampleTopKMax, a.counters + slot,
+                     S.step + slot, 0);
+  } else {
+    pick = tail_argmax(lg, a.vocab, a.part_val + (size_t)slot * gridDim.x, a.part_idx + (size_t)slot * gridDim.x, a.counters + slot);
+  }
+  if (pick < 0) return;
+  if (sampled) {
+    if (S.push_input) {
+      const int hlen = S.hist_len[slot];
+      S.hist[(size_t)slot * kSampleHistMax + hlen % kSampleHistMax] = a.tok[slot];
+      S.hist_len[slot] = hlen + 1;
+    }
+    S.step[slot] += 1;
+  }
+  a.tok[slot] = pick;
   a.pos[slot] += 1;
   const int step = *a.step_counter;  // same value for every batch entry of this step
-  a.ids_ring[(size_t)(step % a.ring_steps) * a.ring_stride + b] = bi;
+  a.ids_ring[(size_t)(step % a.ring_steps) * a.ring_stride + b] = pick;
   // the step counter itself is bumped by step_bump_kernel after every batch entry has read it
+}
+
+// Verify pass (Engine::verify_draft): row r of the logits [T][vocab] makes the choice the step tail would make after the
+// inputs x0, d1 .. dr: greedy, or on an armed slot the draw with history = ring + inputs[0..r] and RNG step step + r.
+// Each row has its own partial, candidate and counter buffers.  Nothing of the slot is written here.
+__global__ void __launch_bounds__(256, 8) spec_tail_kernel(const SpecTailArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int r = blockIdx.y, slot = a.slot;
+  const float* lg = a.logits + (size_t)r * a.vocab;
+  const SampleState& S = a.sample;
+  int pick;
+  if (S.mode[slot]) {
+    const TailHist h{S.hist + (size_t)slot * kSampleHistMax, S.hist_len[slot], a.inputs, r + 1};
+    pick = tail_draw(lg, a.vocab, S.par[slot], h, a.cand + (size_t)r * gridDim.x * kSampleTopKMax, a.counters + r, S.step + slot, r);
+  } else {
+    pick = tail_argmax(lg, a.vocab, a.part_val + (size_t)r * gridDim.x, a.part_idx + (size_t)r * gridDim.x, a.counters + r);
+  }
+  if (pick >= 0) a.choice[r] = pick;
+}
+
+// One block after spec_tail_kernel: a = the drafts d_1 .. d_a that equal the choices y_1 .. y_a; the pass emits
+// y_1 .. y_{a+1} and leaves the slot as a + 1 decode steps would: next input y_{a+1} at position len + a + 1, and on an
+// armed slot x0, d1 .. da pushed into the history ring and the RNG step advanced by a + 1.
+__global__ void spec_accept_kernel(const SpecTailArgs a) {
+  __shared__ int s_acc;
+  pdl_wait();
+  const int tid = threadIdx.x, k = a.T - 1, slot = a.slot;
+  if (tid == 0) {
+    int acc = 0;
+    while (acc < k && a.choice[acc] == a.inputs[acc + 1]) ++acc;
+    s_acc = acc;
+    a.out[0] = acc + 1;
+    a.tok[slot] = a.choice[acc];
+    a.pos[slot] = a.len + acc + 1;
+  }
+  __syncthreads();
+  const int acc = s_acc;
+  if (tid <= acc) a.out[1 + tid] = a.choice[tid];
+  const SampleState& S = a.sample;
+  if (!S.mode[slot]) return;
+  const int hlen = S.hist_len[slot];
+  if (tid <= acc) S.hist[(size_t)slot * kSampleHistMax + (hlen + tid) % kSampleHistMax] = a.inputs[tid];
+  __syncthreads();   // every thread has read hist_len
+  if (tid == 0) {
+    S.hist_len[slot] = hlen + acc + 1;
+    S.step[slot] += (unsigned long long)(acc + 1);
+  }
 }
 
 // step counter bump: tiny kernel keeps the protocol obviously correct (1 thread).
@@ -990,6 +1063,13 @@ int launch_step_tail(const StepTailArgs& a, cudaStream_t st) {
   if (cudaGetLastError() != cudaSuccess) return -1;
   step_bump_kernel<<<1, 256, 0, st>>>(a.step_counter, a.sync_counters, a.n_sync_counters);
   return cudaGetLastError() == cudaSuccess ? 2 : -1;
+}
+
+int launch_spec_tail(const SpecTailArgs& a, cudaStream_t st, bool pdl) {
+  static PerDeviceOnce once;
+  if (once.pending()) { prefer_max_smem(spec_tail_kernel); prefer_max_smem(spec_accept_kernel); once.mark(); }
+  if (launch_ex(spec_tail_kernel, dim3(kTailBlocks, a.T), dim3(256), 0, st, pdl, a) != cudaSuccess) return -1;
+  return launch_ex(spec_accept_kernel, dim3(1), dim3(32), 0, st, true, a) == cudaSuccess ? 2 : -1;
 }
 
 __global__ void synth_bf16_kernel(__nv_bfloat16* out, int64_t n, int k_cols, int row_mult, int row_off, uint64_t seed,

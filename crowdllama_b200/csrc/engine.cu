@@ -186,6 +186,12 @@ int Engine::init(const cl_engine_config& c) {
   prefill_small_max_ = std::min(256, env_int("CL_PREFILL_SMALL_MAX", kDefaultPrefillSmallMax));
   device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
   prefix_cache_ = env_int("CL_PREFIX_CACHE", c.prefix_cache) != 0;
+  speculate_ = env_int("CL_SPECULATE", c.speculate);
+  if (speculate_ < 0 || speculate_ > kSpecMaxDraft) { set_last_error("speculate must be 0..15"); return CL_ERR_INVALID_ARG; }
+  if (speculate_ > 0 && !spec_path_ok()) {
+    fprintf(stderr, "[clengine] speculative decoding needs the tensor-core split-K path, which this model shape lacks: decoding normally\n");
+    speculate_ = 0;
+  }
   if (c.start_scheduler) start_scheduler();
   return CL_OK;
 }
@@ -1034,6 +1040,17 @@ int Engine::debug_hidden(float* out, int n) {
   if (n != cfg.d_model) return CL_ERR_INVALID_ARG;
   CL_CUDA_OK(cudaMemcpyAsync(out, d_h_ + (size_t)last_single_slot_ * cfg.d_model, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
   CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  return CL_OK;
+}
+
+int Engine::spec_stats(cl_spec_stats* out) {
+  memset(out, 0, sizeof *out);
+  out->enabled = speculate_ > 0 ? 1 : 0;
+  out->max_draft = speculate_;
+  out->verify_passes = spec_passes_;
+  out->tokens_drafted = spec_drafted_;
+  out->tokens_accepted = spec_accepted_;
+  out->tokens_emitted = spec_emitted_;
   return CL_OK;
 }
 

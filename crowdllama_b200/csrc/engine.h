@@ -26,6 +26,17 @@ constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts
 constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi)
 constexpr int kDefaultSchedLingerUs = 1000;     // CL_SCHED_LINGER_US: with an empty batch, keep collecting while requests arrive within this gap (max 8x in total)
 
+// Speculative decoding (cl_engine_config.speculate, Engine::verify_draft, ngram_draft): the constants of the drafter.
+constexpr int kSpecMaxDraft = 15;     // drafted tokens per verify pass at most (its rows: x0 + drafts <= 16)
+constexpr int kDraftNgramMax = 3;     // the drafter matches the history's last 3 ids, then its last 2
+constexpr int kDraftNgramMin = 2;
+constexpr int kSpecBackoff = 8;       // tokens a request decodes without drafting after a verify pass that accepted nothing
+
+// Prompt-lookup drafter: the longest suffix of hist[0..n) of length kDraftNgramMax .. kDraftNgramMin that also occurs
+// earlier in hist; from its most recent earlier occurrence, the up to k ids that followed it (stopping at the end of
+// hist) go to out.  Returns how many (0: no match).
+int ngram_draft(const int32_t* hist, int n, int k, int32_t* out);
+
 void set_last_error(const std::string& s);
 const char* get_last_error();
 
@@ -253,6 +264,15 @@ class Engine {
   int arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist);
   int disarm_sampling(cl_seq_t s);
   int read_next_token(cl_seq_t s, int32_t* out);   // d_tok_[s]: what the last step tail of `s` chose
+  // Speculative decoding: one verify pass of x0 and the drafts draft[0..k) (prefill.cu; contract in include/clengine.h,
+  // cl_decode_verify).  ids_out receives the *n_out = a + 1 emitted ids; logits_out (may be nullptr): [k + 1][vocab].
+  int verify_draft(cl_seq_t s, int32_t x0, const int32_t* draft, int k, int32_t* ids_out, int* n_out, float* logits_out);
+  // verify_draft with sp's draw armed for the pass (sp nullptr or temperature <= 0: greedy), as decode_sample does
+  int decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
+                    int* n_out, float* logits_out);
+  bool spec_path_ok() const;          // the verify pass runs on this model shape
+  int speculate() const { return speculate_; }
+  int spec_stats(cl_spec_stats* out);
   bool device_sample() const { return device_sample_; }
   int set_tensor(int layer, int kind, const uint16_t* data, int64_t n);
   int load_safetensors(const std::string& path);   // HF llama-layout checkpoint (file or directory) -> set_tensor (weights_io.cpp)
@@ -305,6 +325,9 @@ class Engine {
   int prefill_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, int& launches, LaunchProfiler& prof);
   int attn_prefill(const AttnPrefillArgs& a, int layer, int& launches, LaunchProfiler& prof);   // the one choice of prefill attention kernel
   int prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_out);    // short prompts: split-K projections (prefill.cu)
+  int ensure_small_ws();
+  // the split-K pass of prefill_small and verify_draft: T rows of s from pos0; leaves sws_->h and the final-norm rows sws_->xn
+  int small_pass(cl_seq_t s, const int* ids, int T, int pos0, int& launches, LaunchProfiler& prof);
   bool prefill_path_ok() const;
   int set_single_slot(cl_seq_t s);
 
@@ -367,6 +390,12 @@ class Engine {
   struct SmallPrefillWs { float* part = nullptr; __nv_bfloat16* xn = nullptr; __nv_bfloat16* q = nullptr; __nv_bfloat16* attn = nullptr;
                           float* h = nullptr; __nv_bfloat16* act = nullptr; int* iota = nullptr; };
   std::unique_ptr<SmallPrefillWs> sws_;
+  // verify pass (allocated lazily): rows of at most kSpecMaxDraft + 1
+  struct SpecWs { float* logits = nullptr; int* choice = nullptr; float* part_val = nullptr; int* part_idx = nullptr;
+                  unsigned* counters = nullptr; unsigned long long* cand = nullptr; int* out = nullptr; };
+  std::unique_ptr<SpecWs> spec_;
+  int speculate_ = 0;                 // most drafted tokens per verify pass in the scheduler / synchronous path (0 = off)
+  std::atomic<int64_t> spec_passes_{0}, spec_drafted_{0}, spec_accepted_{0}, spec_emitted_{0};
   int prefill_small_max_ = 0;         // prompts up to this many tokens take the split-K path (CL_PREFILL_SMALL_MAX, 0 = off)
   struct BatchWs { __nv_bfloat16* xn = nullptr; __nv_bfloat16* attn = nullptr; __nv_bfloat16* act = nullptr; float* part = nullptr; float* logits = nullptr; };
   std::unique_ptr<BatchWs> bws_;

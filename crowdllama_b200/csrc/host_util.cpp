@@ -177,6 +177,19 @@ static double uniform01(uint64_t seed, uint64_t step) {
   uint64_t x = mix64h(seed * 0x9E3779B97F4A7C15ull + step + 0x632BE59BD9B4E019ull);
   return (double)(x >> 11) * (1.0 / 9007199254740992.0);
 }
+int ngram_draft(const int32_t* hist, int n, int k, int32_t* out) {
+  for (int g = kDraftNgramMax; g >= kDraftNgramMin; --g) {
+    const int32_t* suffix = hist + n - g;
+    for (int i = n - g - 1; i >= 0; --i) {   // most recent earlier occurrence first; it may overlap the suffix
+      if (memcmp(hist + i, suffix, (size_t)g * 4) != 0) continue;
+      const int m = std::min(k, n - (i + g));
+      memcpy(out, hist + i + g, (size_t)m * 4);
+      return m;
+    }
+  }
+  return 0;
+}
+
 // HF transformers modeling_rope_utils.py, _compute_llama3_parameters (Llama-3.1 / 3.2): wavelengths beyond
 // original_max_pos / low_freq_factor are stretched by `factor`, those below original_max_pos / high_freq_factor are kept,
 // the band in between is blended linearly.

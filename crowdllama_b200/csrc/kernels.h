@@ -83,8 +83,8 @@ struct SampleState {
   unsigned long long* step = nullptr;    // [slot] RNG step of the next draw (+1 per draw)
   int* hist = nullptr;                   // [slot][kSampleHistMax] ring: id i of the history at i % kSampleHistMax
   int* hist_len = nullptr;               // [slot] ids in the history so far
-  unsigned long long* cand = nullptr;    // [slot][kTailBlocks][kSampleTopKMax] per-block top-k keys
-  int push_input = 0;                    // 1 (decode steps): tok[slot], the step's input, joins the history before the draw
+  unsigned long long* cand = nullptr;    // [slot][kTailBlocks][kSampleTopKMax] per-block top-k keys (step tail)
+  int push_input = 0;                   // 1 (decode steps): tok[slot], the step's input, joins the history before the draw
 };
 
 struct StepTailArgs {                // argmax (or a draw) over logits, advance the sequence
@@ -105,6 +105,25 @@ struct StepTailArgs {                // argmax (or a draw) over logits, advance 
   SampleState sample;
 };
 
+// Verify pass of speculative decoding for one slot (Engine::verify_draft): T = k + 1 rows with inputs x0, d1 .. dk.
+// spec_tail_kernel makes row r's step-tail choice into choice[r] (the draw: history = ring + inputs[0..r], RNG step
+// step[slot] + r); spec_accept_kernel then accepts the longest run of drafts equal to the choices and advances the slot.
+struct SpecTailArgs {
+  const float* logits = nullptr;     // [T][vocab]
+  int vocab = 0, T = 0, slot = 0;
+  int len = 0;                       // cached tokens of the sequence before the pass (x0 sits at position len)
+  const int* inputs = nullptr;       // [T] x0, d1 .. dk
+  int* choice = nullptr;             // [T] y_1 .. y_T
+  float* part_val = nullptr;         // [T][kTailBlocks]
+  int* part_idx = nullptr;
+  unsigned* counters = nullptr;      // [T], zero between passes
+  unsigned long long* cand = nullptr;   // [T][kTailBlocks][kSampleTopKMax]
+  int* tok = nullptr;                // [slot] next input (written: y_{a+1})
+  int* pos = nullptr;                // [slot] its position (written: len + a + 1)
+  int* out = nullptr;                // [1 + T] a + 1, then y_1 .. y_{a+1}
+  SampleState sample;                // mode / par / step / hist / hist_len of the slot (cand and push_input unused)
+};
+
 // every launcher returns the number of kernels it enqueued (for cl_stats.kernel_launches)
 int launch_gemv(int variant, int epi, bool norm, const GemvArgs& a, cudaStream_t st, bool pdl, int* n_ctas = nullptr);
 int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st, bool pdl);
@@ -117,6 +136,7 @@ int launch_attn_decode_tc(const AttnDecodeArgs& a, const CUtensorMap& kmap, cons
 int launch_embed(const __nv_bfloat16* table, int d, const int* tok, float* h, int h_stride, const int* slots,
                  int batch, cudaStream_t st);
 int launch_step_tail(const StepTailArgs& a, cudaStream_t st);
+int launch_spec_tail(const SpecTailArgs& a, cudaStream_t st, bool pdl);   // spec_tail_kernel + spec_accept_kernel (PDL)
 // rope_hd > 0: rows are written rope-pair-interleaved per head of rope_hd rows (see QkvEpi)
 int launch_synth_bf16(__nv_bfloat16* out, int64_t n_logical, int k_cols, int row_mult, int row_off, uint64_t seed,
                       int key, float scale, cudaStream_t st, int rope_hd = 0);

@@ -50,33 +50,64 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   auto& q = seqs_[s];
   int rc = ensure_capacity(s, q.len + n);
   if (rc) return rc;
-  const int d = cfg.d_model, F = cfg.d_ff, T = n, pos0 = q.len;
-  const int s_qkv = pick_splits_public(qkv_dim_, d), s_o = pick_splits_public(d, q_dim_), s_gu = pick_splits_public(2 * F, d), s_dn = pick_splits_public(d, F);
-  if (!sws_) {
-    sws_.reset(new SmallPrefillWs());
-    const size_t Tm = 256;
-    size_t part = 0;
-    part = std::max(part, (size_t)s_qkv * Tm * qkv_dim_);
-    part = std::max(part, (size_t)s_o * Tm * d);
-    part = std::max(part, (size_t)s_gu * Tm * 2 * F);
-    part = std::max(part, (size_t)s_dn * Tm * d);
-    if ((rc = ws_alloc(allocs_, sws_->part, part * 4)) || (rc = ws_alloc(allocs_, sws_->xn, Tm * d * 2)) ||
-        (rc = ws_alloc(allocs_, sws_->q, Tm * q_dim_ * 2)) || (rc = ws_alloc(allocs_, sws_->attn, Tm * q_dim_ * 2)) ||
-        (rc = ws_alloc(allocs_, sws_->h, Tm * d * 4)) || (rc = ws_alloc(allocs_, sws_->act, Tm * F * 2)) ||
-        (rc = ws_alloc(allocs_, sws_->iota, Tm * 4))) { sws_.reset(); return rc; }
-    std::vector<int> io(Tm);
-    for (size_t i = 0; i < Tm; ++i) io[i] = (int)i;
-    CL_CUDA_OK(cudaMemcpy(sws_->iota, io.data(), Tm * 4, cudaMemcpyHostToDevice));
-  }
-  SmallPrefillWs& w = *sws_;
+  if ((rc = ensure_small_ws())) return rc;
+  const int d = cfg.d_model;
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
-  const int* bt = d_bt_ + (size_t)s * max_pages_per_seq_;
   int launches = 0;
+  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
+  if ((rc = small_pass(s, d_prompt_, n, q.len, launches, prof))) return rc;
+  // the last row -> the slot's residual row, then the shared tail (its own final norm + GEMV head)
+  CL_CUDA_OK(cudaMemcpyAsync(d_h_ + (size_t)s * d, sws_->h + (size_t)(n - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, stream_));
+  const int last_pos = q.len + n - 1;
+  CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &last_pos, 4, cudaMemcpyHostToDevice, stream_));
+  rc = set_single_slot(s);
+  if (rc) return rc;
+  CL_LAUNCH(enqueue_lm_head(1, false));
+  CL_LAUNCH(enqueue_step_tail(1, false));
+  prof.report("prefill profile", 32, "short-prompt path, " + std::to_string(n) + " tokens");
+  launches_ += launches;
+  seq_advance(s, ids, n, n);
+  if (logits_out) return read_logits(s, logits_out);
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  return CL_OK;
+}
+
+int Engine::ensure_small_ws() {
+  if (sws_) return CL_OK;
+  const int d = cfg.d_model, F = cfg.d_ff;
+  const int s_qkv = pick_splits_public(qkv_dim_, d), s_o = pick_splits_public(d, q_dim_), s_gu = pick_splits_public(2 * F, d), s_dn = pick_splits_public(d, F);
+  sws_.reset(new SmallPrefillWs());
+  const size_t Tm = 256;
+  size_t part = 0;
+  part = std::max(part, (size_t)s_qkv * Tm * qkv_dim_);
+  part = std::max(part, (size_t)s_o * Tm * d);
+  part = std::max(part, (size_t)s_gu * Tm * 2 * F);
+  part = std::max(part, (size_t)s_dn * Tm * d);
+  int rc;
+  if ((rc = ws_alloc(allocs_, sws_->part, part * 4)) || (rc = ws_alloc(allocs_, sws_->xn, Tm * d * 2)) ||
+      (rc = ws_alloc(allocs_, sws_->q, Tm * q_dim_ * 2)) || (rc = ws_alloc(allocs_, sws_->attn, Tm * q_dim_ * 2)) ||
+      (rc = ws_alloc(allocs_, sws_->h, Tm * d * 4)) || (rc = ws_alloc(allocs_, sws_->act, Tm * F * 2)) ||
+      (rc = ws_alloc(allocs_, sws_->iota, Tm * 4))) { sws_.reset(); return rc; }
+  std::vector<int> io(Tm);
+  for (size_t i = 0; i < Tm; ++i) io[i] = (int)i;
+  CL_CUDA_OK(cudaMemcpy(sws_->iota, io.data(), Tm * 4, cudaMemcpyHostToDevice));
+  return CL_OK;
+}
+
+// One split-K pass over T <= 256 rows of sequence s at positions pos0 .. pos0 + T - 1, token ids at ids (device):
+// embedding, every layer (K/V written into the sequence's pages), and the final norm.  Leaves the final residual rows in
+// sws_->h and their normalised bf16 rows, the LM head's input, in sws_->xn.  A row's results do not depend on the rows
+// after it.  prefill_small and the verify pass of speculative decoding (verify_draft) both run it.
+int Engine::small_pass(cl_seq_t s, const int* ids, int T, int pos0, int& launches, LaunchProfiler& prof) {
+  const int d = cfg.d_model, F = cfg.d_ff;
+  const int s_qkv = pick_splits_public(qkv_dim_, d), s_o = pick_splits_public(d, q_dim_), s_gu = pick_splits_public(2 * F, d), s_dn = pick_splits_public(d, F);
+  SmallPrefillWs& w = *sws_;
+  const int* bt = d_bt_ + (size_t)s * max_pages_per_seq_;
+  int rc;
   // programmatic dependent launch between the GEMMs and the per-row glue kernels, as in the batched decode step (the two
   // prefill kernels in between are launched normally and order the stream)
   const bool bp = use_pdl_;
-  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
-  CL_LAUNCH(launch_embed_rows(embed_, d, d_prompt_, w.h, T, stream_));
+  CL_LAUNCH(launch_embed_rows(embed_, d, ids, w.h, T, stream_));
   const float* pending = nullptr;   // split-K partials of the previous residual projection, folded in by the next norm
   int pending_s = 0;
   for (int l = 0; l < cfg.n_layers; ++l) {
@@ -97,21 +128,82 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
     CL_LAUNCH(launch_gemm_bf16(w.act, L.wdown, w.part, nullptr, T, d, F, stream_, s_dn, bp));
     pending = w.part; pending_s = s_dn;
   }
-  // fold the last down-projection into the residual rows (the normalised copy it also writes is not used), then the shared tail
+  // fold the last down-projection into the residual rows; the final-norm rows it also writes feed the verify pass's head
   CL_LAUNCH(launch_batch_resid_norm(w.h, d, pending, pending_s, T, final_norm_, cfg.rms_eps, w.xn, w.iota, stream_, bp));
-  CL_CUDA_OK(cudaMemcpyAsync(d_h_ + (size_t)s * d, w.h + (size_t)(T - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, stream_));
-  const int last_pos = q.len + n - 1;
-  CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &last_pos, 4, cudaMemcpyHostToDevice, stream_));
-  rc = set_single_slot(s);
-  if (rc) return rc;
-  CL_LAUNCH(enqueue_lm_head(1, false));
-  CL_LAUNCH(enqueue_step_tail(1, false));
-  prof.report("prefill profile", 32, "short-prompt path, " + std::to_string(n) + " tokens");
-  launches_ += launches;
-  seq_advance(s, ids, n, n);
-  if (logits_out) return read_logits(s, logits_out);
-  CL_CUDA_OK(cudaStreamSynchronize(stream_));
   return CL_OK;
+}
+
+bool Engine::spec_path_ok() const {
+  return prefill_path_ok() && cfg.d_model <= 8192 && cfg.d_model % 4 == 0 && gemm_tc_supported(kSpecMaxDraft + 1, cfg.vocab_size, cfg.d_model);
+}
+
+// Verify pass of speculative decoding (include/clengine.h, cl_decode_verify): rows x0, d1 .. dk at positions len .. len + k
+// through small_pass, one GEMM over the final-norm rows for their logits, then the spec tail (row r's step-tail choice
+// y_{r+1}) and the accept kernel (a = longest run with y_j == d_j; next input y_{a+1}; an armed slot's history and RNG
+// step advanced as a + 1 steps would).  Only {a + 1, y_1 .. y_{a+1}} is read back.  Rejected rows leave K/V at positions
+// >= the new length, on the sequence's private pages.
+int Engine::verify_draft(cl_seq_t s, int32_t x0, const int32_t* draft, int k, int32_t* ids_out, int* n_out, float* logits_out) {
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  if (k < 1 || k > kSpecMaxDraft || !draft || !ids_out || !n_out) { set_last_error("verify: k must be 1..15"); return CL_ERR_INVALID_ARG; }
+  if (!spec_path_ok()) { set_last_error("verify: the model shape has no tensor-core split-K path"); return CL_ERR_INVALID_ARG; }
+  const int V = cfg.vocab_size, d = cfg.d_model, T = k + 1;
+  int32_t in[kSpecMaxDraft + 1];
+  in[0] = x0;
+  memcpy(in + 1, draft, (size_t)k * 4);
+  for (int i = 0; i < T; ++i)
+    if (in[i] < 0 || in[i] >= V) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
+  auto& q = seqs_[s];
+  int rc = ensure_capacity(s, q.len + T);
+  if (rc) return rc;
+  if ((rc = ensure_small_ws())) return rc;
+  if (!spec_) {
+    const size_t R = kSpecMaxDraft + 1;
+    spec_.reset(new SpecWs());
+    if ((rc = ws_alloc(allocs_, spec_->logits, R * V * 4)) || (rc = ws_alloc(allocs_, spec_->choice, R * 4)) ||
+        (rc = ws_alloc(allocs_, spec_->part_val, R * kTailBlocks * 4)) || (rc = ws_alloc(allocs_, spec_->part_idx, R * kTailBlocks * 4)) ||
+        (rc = ws_alloc(allocs_, spec_->counters, R * 4)) || (rc = ws_alloc(allocs_, spec_->cand, R * kTailBlocks * kSampleTopKMax * 8)) ||
+        (rc = ws_alloc(allocs_, spec_->out, (R + 1) * 4))) { spec_.reset(); return rc; }
+    CL_CUDA_OK(cudaMemsetAsync(spec_->counters, 0, R * 4, stream_));
+  }
+  CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, in, (size_t)T * 4, cudaMemcpyHostToDevice, stream_));
+  int launches = 0;
+  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
+  if ((rc = small_pass(s, d_prompt_, T, q.len, launches, prof))) return rc;
+  CL_LAUNCH(launch_gemm_bf16(sws_->xn, lm_head_, spec_->logits, nullptr, T, V, d, stream_, 1, false));
+  SpecTailArgs t;
+  t.logits = spec_->logits; t.vocab = V; t.T = T; t.slot = s; t.len = q.len; t.inputs = d_prompt_; t.choice = spec_->choice;
+  t.part_val = spec_->part_val; t.part_idx = spec_->part_idx; t.counters = spec_->counters; t.cand = spec_->cand;
+  t.tok = d_tok_; t.pos = d_pos_; t.out = spec_->out;
+  t.sample.mode = d_samp_mode_; t.sample.par = d_samp_par_; t.sample.step = d_samp_step_; t.sample.hist = d_samp_hist_;
+  t.sample.hist_len = d_samp_hlen_;
+  CL_LAUNCH(launch_spec_tail(t, stream_, use_pdl_));
+  CL_CUDA_OK(cudaMemcpyAsync(h_ids_pinned_, spec_->out, (size_t)(T + 1) * 4, cudaMemcpyDeviceToHost, stream_));
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  prof.report("prefill profile", 32, "verify pass, " + std::to_string(T) + " rows");
+  launches_ += launches;
+  const int n = h_ids_pinned_[0];
+  if (n < 1 || n > T) { set_last_error("verify: accept kernel returned a bad count"); return CL_ERR_INTERNAL; }
+  memcpy(ids_out, h_ids_pinned_ + 1, (size_t)n * 4);
+  *n_out = n;
+  seq_advance(s, in, n, n);   // x0, d1 .. da: only accepted tokens join the history and the prefix cache
+  spec_passes_++; spec_drafted_ += k; spec_accepted_ += n - 1; spec_emitted_ += n;
+  if (logits_out) CL_CUDA_OK(cudaMemcpy(logits_out, spec_->logits, (size_t)T * V * 4, cudaMemcpyDeviceToHost));
+  return CL_OK;
+}
+
+// cl_decode_verify: verify_draft with the device sampler armed for the pass when sp asks for a draw
+int Engine::decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
+                          int* n_out, float* logits_out) {
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  const bool sampled = sp && sp->temperature > 0.f;
+  int rc = CL_OK;
+  if (sampled) rc = arm_sampling(s, *sp, step0, seqs_[s].history.data(), (int)seqs_[s].history.size());
+  if (rc == CL_OK) rc = verify_draft(s, x0, draft, k, ids_out, n_out, logits_out);
+  if (sampled) {
+    const int r2 = disarm_sampling(s);
+    if (rc == CL_OK) rc = r2;
+  }
+  return rc;
 }
 
 // (Re)allocate the tile-path workspace for passes of up to `tokens` rows; old buffers stay in allocs_ until the engine dies

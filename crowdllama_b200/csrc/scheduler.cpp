@@ -40,6 +40,7 @@ struct Request {
   std::vector<int32_t> full;        // prompt + tokens generated before a preemption: what the (re-)prefill has to process
   size_t prefilled = 0;             // tokens of `full` already in the cache (chunked admission)
   bool dev_sample = false;          // sampled, and the step tail draws its tokens (device_sampling_ok, CL_DEVICE_SAMPLE)
+  int spec_backoff = 0;             // tokens to decode without drafting (after a verify pass that accepted nothing)
   bool greedy() const { return sp.temperature <= 0.f; }
   bool device_next() const { return greedy() || dev_sample; }   // the next id is d_tok_ after the step: no host sampler
 };
@@ -76,6 +77,35 @@ static bool finished(Request& r, const Tokenizer& tok, int max_seq_len) {
   return false;
 }
 
+// Speculative round of a greedy or device-sampled request decoding alone (Engine::speculate() > 0): draft from its prompt
+// and output (ngram_draft), clipped so that the request passes neither max_new nor max_seq_len, and check the draft in one
+// verify pass.  The emitted ids join r.out one at a time until the request finishes.  Returns how many joined, 0 when the
+// request takes a normal step instead (no draft, back-off, KV pool out of pages), or an error status.
+static int spec_round(Engine& e, Request& r) {
+  if (e.speculate() <= 0 || !r.device_next() || r.spec_backoff > 0 || r.out.empty()) return 0;
+  int len = 0;
+  if (e.seq_len(r.seq, &len)) return 0;
+  const int k_max = std::min({e.speculate(), r.max_new - (int)r.out.size() - 1, e.cfg.max_seq_len - len - 1});
+  if (k_max < 1) return 0;
+  std::vector<int32_t> hist(r.prompt);
+  hist.insert(hist.end(), r.out.begin(), r.out.end());   // ends with the next input x0
+  int32_t draft[kSpecMaxDraft], ids[kSpecMaxDraft + 1];
+  const int k = ngram_draft(hist.data(), (int)hist.size(), k_max, draft);
+  if (k == 0) return 0;
+  int n = 0;
+  const int rc = e.verify_draft(r.seq, r.out.back(), draft, k, ids, &n, nullptr);
+  if (rc == CL_ERR_OOM) return 0;
+  if (rc) return rc;
+  if (n == 1) r.spec_backoff = kSpecBackoff;
+  int joined = 0;
+  while (joined < n) {
+    r.out.push_back(ids[joined++]);
+    publish(r, r.out.back());
+    if (finished(r, *e.tok, e.cfg.max_seq_len)) break;
+  }
+  return joined;
+}
+
 // ---- synchronous path (no scheduler thread): one request at a time under the engine lock --------
 static int generate_sync(Engine& e, Request& r, const Engine::TokenSink* sink) {
   size_t emitted = 0;
@@ -107,9 +137,16 @@ static int generate_sync(Engine& e, Request& r, const Engine::TokenSink* sink) {
   r.out.push_back(next);
   emit();
   while (!finished(r, *e.tok, e.cfg.max_seq_len)) {
-    if (r.device_next()) {   // greedy or device-sampled: the token loop stays on the device
+    const int spec = spec_round(e, r);
+    if (spec < 0) { rc = spec; break; }
+    if (spec > 0) {
+      next = r.out.back();
+    } else if (r.device_next()) {   // greedy or device-sampled: the token loop stays on the device
       int room = std::min(r.max_new - (int)r.out.size(), e.cfg.max_seq_len - (int)(r.prompt.size() + r.out.size()));
       int chunk = std::min(room, sink ? 8 : 32);
+      // speculating: back to drafting after the back-off, or after one step when the history had no match
+      if (e.speculate() > 0) chunk = std::min(chunk, std::max(1, r.spec_backoff));
+      r.spec_backoff = std::max(0, r.spec_backoff - chunk);
       std::vector<int32_t> ids(chunk);
       rc = e.decode_greedy(&r.seq, 1, &next, chunk, ids.data(), nullptr);
       if (rc) break;
@@ -465,6 +502,31 @@ void Engine::scheduler_main() {
       ++i;
     }
     if (active_.empty()) continue;
+    // ---- speculative decoding: one request decoding alone with nothing to admit takes a verify pass instead of a step
+    if (speculate_ > 0 && active_.size() == 1 && !prefilling_ && [&] { std::lock_guard<std::mutex> lk(q_mu_); return queue_.empty(); }()) {
+      auto r = active_[0];
+      const int64_t t0 = now_ns();
+      const int n = spec_round(*this, *r);
+      if (n != 0) {
+        const int64_t dt = now_ns() - t0;
+        if (n < 0) {
+          seq_free(r->seq);
+          active_.clear();
+          complete(r, n, get_last_error());
+          continue;
+        }
+        r->decode_ns += dt;
+        tokens_generated_ += n;
+        sched_decode_steps_++; sched_decode_ns_ += dt;
+        if (finished(*r, *tok, cfg.max_seq_len)) {
+          seq_free(r->seq);
+          active_.clear();
+          requests_completed_++;
+          complete(r, CL_OK, "");
+        }
+        continue;
+      }
+    }
     // ---- one batched decode step
     const int B = (int)active_.size();
     slots.resize(B);
@@ -508,6 +570,7 @@ void Engine::scheduler_main() {
       }
       r->out.push_back(next);
       publish(*r, next);
+      if (r->spec_backoff > 0) r->spec_backoff--;
     }
     const int64_t dt = now_ns() - t0;
     for (auto& r : active_) r->decode_ns += dt;

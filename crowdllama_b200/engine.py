@@ -37,7 +37,8 @@ class EngineConfig(C.Structure):
                 ("model", ModelConfig), ("weights_path", C.c_char_p), ("weights_seed", C.c_uint64),
                 ("kv_pool_bytes", C.c_int64), ("page_size", C.c_int32), ("max_batch", C.c_int32),
                 ("max_seqs", C.c_int32), ("use_cuda_graph", C.c_int32), ("decode_path", C.c_int32),
-                ("start_scheduler", C.c_int32), ("prefix_cache", C.c_int32), ("reserved", C.c_int32 * 7)]
+                ("start_scheduler", C.c_int32), ("prefix_cache", C.c_int32), ("speculate", C.c_int32),
+                ("reserved", C.c_int32 * 6)]
 
 
 class Sampling(C.Structure):
@@ -67,11 +68,16 @@ class PrefixStats(C.Structure):
                 ("tokens_reused", C.c_int64), ("pages_evicted", C.c_int64), ("reserved", C.c_int64 * 4)]
 
 
+class SpecStats(C.Structure):
+    _fields_ = [("enabled", C.c_int32), ("max_draft", C.c_int32), ("verify_passes", C.c_int64), ("tokens_drafted", C.c_int64),
+                ("tokens_accepted", C.c_int64), ("tokens_emitted", C.c_int64), ("reserved", C.c_int64 * 4)]
+
+
 # every symbol include/clengine.h declares (tests check the library exports all of them)
 EXPORTS = [
     "cl_abi_version", "cl_strerror", "cl_last_error", "cl_default_engine_config", "cl_default_sampling",
     "cl_greedy_sampling", "cl_sample_token", "cl_model_preset", "cl_engine_create", "cl_engine_destroy", "cl_engine_model_config",
-    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
+    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_draft_ngram", "cl_decode_verify", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
     "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
     "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_timeline",
@@ -114,6 +120,9 @@ def lib():
         "cl_engine_model_config": (C.c_int, [vp, P(ModelConfig)]),
         "cl_engine_stats": (C.c_int, [vp, P(Stats)]),
         "cl_engine_prefix_stats": (C.c_int, [vp, P(PrefixStats)]),
+        "cl_engine_spec_stats": (C.c_int, [vp, P(SpecStats)]),
+        "cl_draft_ngram": (C.c_int, [vp, i32, i32, vp, P(i32)]),
+        "cl_decode_verify": (C.c_int, [vp, i32, i32, vp, i32, P(Sampling), u64, vp, P(i32), vp]),
         "cl_engine_set_tensor": (C.c_int, [vp, i32, i32, vp, i64]),
         "cl_checkpoint_info": (C.c_int, [C.c_char_p, P(ModelConfig), P(i32), P(i64)]),
         "cl_generate": (C.c_int, [vp, C.c_char_p, C.c_char_p, sz, P(Sampling), P(Result)]),
@@ -242,6 +251,16 @@ def sample_token(logits, sampling: Sampling, history=(), step: int = 0) -> int:
     return int(out.value)
 
 
+def draft_ngram(hist, k: int) -> np.ndarray:
+    """The prompt-lookup drafter of speculative decoding (cl_draft_ngram; no GPU involved): the up to k ids that followed
+    the most recent earlier occurrence of hist's last 3 (else 2) ids; empty when there is none."""
+    h = np.ascontiguousarray(hist, dtype=np.int32)
+    out = np.empty(max(k, 1), np.int32)
+    n = C.c_int32(0)
+    _check(lib().cl_draft_ngram(_ptr(h) if h.size else None, h.size, k, _ptr(out), C.byref(n)), "cl_draft_ngram")
+    return out[:n.value].copy()
+
+
 def ollama_default_sampling(seed: int = 0, max_new_tokens: int = -1) -> Sampling:
     s = Sampling()
     lib().cl_default_sampling(C.byref(s))
@@ -267,7 +286,8 @@ class Engine:
     def __init__(self, preset: str | None = None, model: dict | None = None, model_name: str | None = None,
                  device: int = 0, seed: int = 1234, max_batch: int = 8, max_seqs: int | None = None,
                  page_size: int = 32, kv_pool_bytes: int = 0, use_cuda_graph: bool = True, decode_path: int = 0,
-                 start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False):
+                 start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False,
+                 speculate: int = 0):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -290,6 +310,7 @@ class Engine:
         cfg.decode_path = decode_path
         cfg.start_scheduler = 1 if start_scheduler else 0
         cfg.prefix_cache = 1 if prefix_cache else 0     # env CL_PREFIX_CACHE=0|1 overrides
+        cfg.speculate = speculate                       # 0 off, 1..15 drafted tokens per verify pass; env CL_SPECULATE overrides
         h = C.c_void_p()
         _check(L.cl_engine_create(C.byref(cfg), C.byref(h)), "cl_engine_create")
         self._h = h
@@ -401,6 +422,18 @@ class Engine:
         _check(lib().cl_decode_step_batch(self._h, _ptr(seqs), len(seqs), _ptr(toks), _ptr(out) if want_logits else None, _ptr(am)),
                "cl_decode_step_batch")
         return out, am
+
+    def decode_verify(self, s: int, input_id: int, draft, sampling: Sampling | None = None, step0: int = 0,
+                      want_logits: bool = False):
+        """cl_decode_verify: one verify pass of input_id (the next input) and the drafted ids after it.  Returns (emitted ids
+        y_1 .. y_{a+1}, logits [k + 1][vocab] or None); the sequence advances by a + 1 tokens."""
+        d = np.ascontiguousarray(draft, dtype=np.int32)
+        ids = np.empty(max(len(d), 0) + 1, np.int32)
+        n = C.c_int32(0)
+        out = np.empty((len(d) + 1, self.cfg["vocab_size"]), np.float32) if want_logits else None
+        _check(lib().cl_decode_verify(self._h, s, int(input_id), _ptr(d), len(d), C.byref(sampling) if sampling else None, step0,
+                                      _ptr(ids), C.byref(n), _ptr(out) if want_logits else None), "cl_decode_verify")
+        return ids[:n.value].copy(), out
 
     def seq_fake_fill(self, s: int, n_tokens: int):
         """Fill the sequence's paged KV (all layers) with the synthetic cache pattern the parity tests' CPU checker also
@@ -526,6 +559,12 @@ class Engine:
         d = {n: getattr(st, n) for n, _ in st._fields_}
         d["gpu_model"] = st.gpu_model.decode(errors="replace")
         return d
+
+    def spec_stats(self) -> dict:
+        """cl_engine_spec_stats: enabled, max_draft, verify_passes, tokens_drafted, tokens_accepted, tokens_emitted."""
+        st = SpecStats()
+        _check(lib().cl_engine_spec_stats(self._h, C.byref(st)), "cl_engine_spec_stats")
+        return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved"}
 
     def prefix_stats(self) -> dict:
         """cl_engine_prefix_stats: enabled, cached_pages, lookups, tokens_looked_up, tokens_reused, pages_evicted."""

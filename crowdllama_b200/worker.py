@@ -73,9 +73,10 @@ class _Conn(socketserver.BaseRequestHandler):
 
 
 def serve(device: int, port: int, preset: str, model_name: str, max_batch: int = 8, greedy_tokens: int = 0, host="127.0.0.1",
-          ready_event=None, seed: int = 1234, tokenizer: str | None = None, chat_family: str | None = None, prefix_cache: bool = False):
+          ready_event=None, seed: int = 1234, tokenizer: str | None = None, chat_family: str | None = None, prefix_cache: bool = False,
+          speculate: int = 0):
     e = eng.Engine(preset=preset, model_name=model_name, device=device, seed=seed, max_batch=max_batch, start_scheduler=True,
-                   prefix_cache=prefix_cache)
+                   prefix_cache=prefix_cache, speculate=speculate)
     if tokenizer:
         e.load_tokenizer(tokenizer, chat_family)      # HF tokenizer.json instead of the byte-level fallback
     sampling = eng.greedy(greedy_tokens, ignore_eos=True) if greedy_tokens > 0 else None   # None = Ollama defaults
@@ -101,10 +102,13 @@ def main():
     ap.add_argument("--chat-family", default=None, help="llama3 | mistral | zephyr | chatml (default: auto-detect)")
     ap.add_argument("--prefix-cache", action="store_true",
                     help="reuse the cached KV pages of earlier requests that share a prompt prefix (env CL_PREFIX_CACHE overrides)")
+    ap.add_argument("--speculate", type=int, default=0,
+                    help="1..15: a request decoding alone drafts up to this many ids from its own history and verifies them in "
+                         "one pass (0 = off; env CL_SPECULATE overrides)")
     a = ap.parse_args()
     print(f"worker on cuda:{a.device} port {a.port} serving {a.model_name}", flush=True)
     serve(a.device, a.port, a.preset, a.model_name, a.max_batch, a.greedy_tokens, tokenizer=a.tokenizer, chat_family=a.chat_family,
-          prefix_cache=a.prefix_cache)
+          prefix_cache=a.prefix_cache, speculate=a.speculate)
 
 
 if __name__ == "__main__":

@@ -97,7 +97,14 @@ typedef struct cl_engine_config {
                               sequence is freed and are evicted least recently used first when the pool runs dry, so a
                               request whose prompt starts with an earlier prompt (or a preempted request coming back)
                               prefills only the rest.  See cl_seq_attach_prefix / cl_engine_prefix_stats. */
-  int32_t reserved[7];
+  int32_t speculate;       /* speculative decoding: 0 => off (default), 1..15 => the most drafted tokens per verify pass
+                              (env CL_SPECULATE overrides; other values make cl_engine_create fail with CL_ERR_INVALID_ARG).
+                              While exactly one request is running and nothing waits, a greedy or device-sampled request
+                              drafts the ids that followed the latest earlier occurrence of its last 3 (or 2) ids in its
+                              prompt and output (cl_draft_ngram) and checks them in one pass over the weights
+                              (cl_decode_verify).  The ids are the ones single steps would produce, up to near-tie flips
+                              between the two kernel paths.  Model shapes without the verify path decode normally. */
+  int32_t reserved[6];
 } cl_engine_config;
 
 /* Sampler.  The reference sends no options (api.go:109-118), so Ollama defaults apply upstream:
@@ -165,6 +172,17 @@ typedef struct cl_prefix_stats {
   int64_t reserved[4];
 } cl_prefix_stats;
 
+/* Speculative decoding accounting since engine creation (cl_engine_config.speculate). */
+typedef struct cl_spec_stats {
+  int32_t enabled;           /* the scheduler and the synchronous path speculate */
+  int32_t max_draft;         /* most drafted tokens per verify pass */
+  int64_t verify_passes;     /* verify passes run (cl_decode_verify calls included) */
+  int64_t tokens_drafted;    /* drafted tokens they checked */
+  int64_t tokens_accepted;   /* of which accepted */
+  int64_t tokens_emitted;    /* tokens they emitted: tokens_accepted + verify_passes */
+  int64_t reserved[4];
+} cl_spec_stats;
+
 typedef struct cl_engine cl_engine;
 typedef int32_t cl_seq_t;
 
@@ -183,6 +201,10 @@ void cl_greedy_sampling(cl_sampling* s, int32_t max_new_tokens);
 int cl_sample_token(const float* logits, int32_t vocab, const cl_sampling* s, const int32_t* history, int32_t n_history,
                     uint64_t step, int32_t* id);
 int cl_model_preset(const char* name, cl_model_config* out);
+/* The prompt-lookup drafter of speculative decoding (host only, no GPU involved): the longest suffix of hist[0..n) of
+ * length 3, else 2, that also occurs earlier in hist; from its most recent earlier occurrence, the up to k ids that
+ * followed it, stopping at the end of hist, go to out.  *n_out = their count (0: no match).  k: 1..15. */
+int cl_draft_ngram(const int32_t* hist, int32_t n, int32_t k, int32_t* out, int32_t* n_out);
 
 /* replaces: embedded Ollama server start, /root/reference/cmd/crowdllama/main.go:283-297 */
 int cl_engine_create(const cl_engine_config* cfg, cl_engine** out);
@@ -190,6 +212,7 @@ void cl_engine_destroy(cl_engine* e);
 int cl_engine_model_config(const cl_engine* e, cl_model_config* out);
 int cl_engine_stats(cl_engine* e, cl_stats* out);
 int cl_engine_prefix_stats(cl_engine* e, cl_prefix_stats* out);
+int cl_engine_spec_stats(cl_engine* e, cl_spec_stats* out);
 /* Overwrite one weight tensor from host memory (bf16 bits, logical [out][in] row-major; norm
  * gains as bf16 too).  kind: 0 embed, 1 lm_head, 2 final_norm, 3 attn_norm, 4 wq, 5 wk, 6 wv,
  * 7 wo, 8 ffn_norm, 9 w_gate, 10 w_up, 11 w_down (same numbering as the synthetic generator).
@@ -285,6 +308,23 @@ int cl_decode_sample_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, c
  * the greedy next ids. */
 int cl_decode_step_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* ids, float* logits_out,
                          int32_t* argmax_out);
+/* Speculative decoding, token level: one verify pass.  The sequence has len cached tokens and the next input input_id
+ * (x0: the last generated id, not cached yet); draft[0..k) = d1 .. dk, 1 <= k <= 15, are the guessed ids after it.
+ *   - The pass runs x0, d1 .. dk at positions len .. len + k through every layer (their K/V are written) and computes the
+ *     logits of all k + 1 rows.  Row r makes the decode step tail's choice y_{r+1}: greedy argmax (lowest index on ties),
+ *     or with a sampled sp the draw of cl_sample_token with history = the sequence's history + x0, d1 .. dr and RNG step
+ *     step0 + r.
+ *   - a = the largest count with y_j == d_j for every j <= a.  ids_out receives y_1 .. y_{a+1}, *n_out = a + 1.
+ *   - Afterwards len += a + 1 (x0, d1 .. da are cached) and the next input is y_{a+1}: exactly the state a + 1
+ *     cl_decode_step calls would leave, so the ids equal sequential decoding's up to logit differences between the two
+ *     kernel paths (near-tie flips).  K/V of rejected rows lies at positions >= the new length: nothing reads it, the
+ *     next writes overwrite it, and pages attached from the prefix cache are never written.
+ * sp may be NULL, or have temperature <= 0, for greedy; a sampled sp arms the device sampler for the pass and disarms it
+ * afterwards, like cl_decode_sample_batch.  logits_out (host, may be NULL): [k + 1][vocab_size].  Works whatever
+ * cl_engine_config.speculate is.  CL_ERR_INVALID_ARG for k outside 1..15, settings that need the host sampler, or a
+ * model shape without the verify path; CL_ERR_TOO_LONG past max_seq_len. */
+int cl_decode_verify(cl_engine* e, cl_seq_t seq, int32_t input_id, const int32_t* draft, int32_t k, const cl_sampling* sp,
+                     uint64_t step0, int32_t* ids_out, int32_t* n_out, float* logits_out);
 /* Parity aid: make the sequence hold n_tokens cached tokens whose K/V, in every layer, are the CPU oracle's
  * synthetic cache pattern (oracle/llama_oracle.c oc_seq_fake_fill: k[i] = (((i * 2654435761) >> 24 & 255) - 128) / 128,
  * v[i] = (((i * 40503) >> 8 & 255) - 128) / 128 with i = token * n_kv * head_dim + head * head_dim + dim; exact in
