@@ -135,6 +135,11 @@ int cl_engine_spec_stats(cl_engine* e, cl_spec_stats* out) {
   return e->impl.spec_stats(out);   // atomics only, no engine lock
 }
 
+int cl_engine_set_speculate_batch(cl_engine* e, int32_t n) {
+  if (!e) return CL_ERR_INVALID_ARG;
+  return e->impl.set_speculate_batch(n);   // an atomic the scheduler reads once per iteration, no engine lock
+}
+
 int cl_engine_set_tensor(cl_engine* e, int32_t layer, int32_t kind, const uint16_t* data, int64_t n) {
   if (!e || !data) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
@@ -477,6 +482,13 @@ int cl_decode_verify(cl_engine* e, cl_seq_t s, int32_t input_id, const int32_t* 
     *n_out = n;
     return rc;
   )
+}
+int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* input_ids, const int32_t* drafts,
+                           const int32_t* ks, const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int32_t* n_out,
+                           float* logits_out) {
+  if (!e || !seqs || !input_ids || !ks || !ids_out || !n_out || n_seqs < 1) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(return e->impl.decode_verify_batch(seqs, n_seqs, input_ids, drafts, ks, sp, step0, ids_out, n_out, logits_out);)
 }
 int cl_seq_fake_fill(cl_engine* e, cl_seq_t s, int32_t n_tokens) {
   if (!e) return CL_ERR_INVALID_ARG;

@@ -192,6 +192,9 @@ int Engine::init(const cl_engine_config& c) {
     fprintf(stderr, "[clengine] speculative decoding needs the tensor-core split-K path, which this model shape lacks: decoding normally\n");
     speculate_ = 0;
   }
+  if (const char* v = getenv("CL_SPECULATE_BATCH")) {
+    if (set_speculate_batch(atoi(v))) return CL_ERR_INVALID_ARG;
+  }
   if (c.start_scheduler) start_scheduler();
   return CL_OK;
 }
@@ -366,7 +369,8 @@ int Engine::alloc_state() {
     DMALLOC(bws_->logits, Bm * (size_t)cfg.vocab_size * 4);
   }
   prompt_cap_ = cfg.max_seq_len;
-  DMALLOC(d_prompt_, (size_t)prompt_cap_ * 4);
+  // also the input ids of a verify pass over several sequences, up to kSpecMaxRows even when max_seq_len is smaller
+  DMALLOC(d_prompt_, (size_t)std::max(prompt_cap_, kSpecMaxRows) * 4);
   CL_CUDA_OK(cudaMemsetAsync(d_tok_, 0, S * 4, stream_));
   CL_CUDA_OK(cudaMemsetAsync(d_pos_, 0, S * 4, stream_));
   CL_CUDA_OK(cudaMemsetAsync(d_bt_, 0, S * max_pages_per_seq_ * 4, stream_));
@@ -1051,6 +1055,16 @@ int Engine::spec_stats(cl_spec_stats* out) {
   out->tokens_drafted = spec_drafted_;
   out->tokens_accepted = spec_accepted_;
   out->tokens_emitted = spec_emitted_;
+  out->multi_passes = spec_multi_passes_;
+  return CL_OK;
+}
+
+int Engine::set_speculate_batch(int n) {
+  if (n < 1 || n > std::min(max_batch_, kSpecBatchMax)) {
+    set_last_error("speculate_batch must be 1..min(max_batch, 32)");
+    return CL_ERR_INVALID_ARG;
+  }
+  speculate_batch_ = n;
   return CL_OK;
 }
 

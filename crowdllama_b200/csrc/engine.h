@@ -31,6 +31,8 @@ constexpr int kSpecMaxDraft = 15;     // drafted tokens per verify pass at most 
 constexpr int kDraftNgramMax = 3;     // the drafter matches the history's last 3 ids, then its last 2
 constexpr int kDraftNgramMin = 2;
 constexpr int kSpecBackoff = 8;       // tokens a request decodes without drafting after a verify pass that accepted nothing
+constexpr int kSpecMaxRows = 128;     // rows of one verify pass over several sequences (Engine::verify_batch) at most
+constexpr int kSpecBatchMax = 32;     // sequences the scheduler verifies in one pass at most (cl_engine_set_speculate_batch)
 
 // Prompt-lookup drafter: the longest suffix of hist[0..n) of length kDraftNgramMax .. kDraftNgramMin that also occurs
 // earlier in hist; from its most recent earlier occurrence, the up to k ids that followed it (stopping at the end of
@@ -270,8 +272,19 @@ class Engine {
   // verify_draft with sp's draw armed for the pass (sp nullptr or temperature <= 0: greedy), as decode_sample does
   int decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
                     int* n_out, float* logits_out);
+  // One verify pass over n_seqs distinct sequences (contract in include/clengine.h, cl_decode_verify_batch): sequence i
+  // verifies x0[i] and ks[i] (0..15) drafts, taken back to back from drafts.  Its ids land at ids_out + its first row (the
+  // sum of k_j + 1 over the sequences before it), n_out[i] of them; logits_out (may be nullptr): [rows][vocab].
+  int verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks, int32_t* ids_out,
+                   int* n_out, float* logits_out);
+  // verify_batch with the device sampler armed for the pass on every sequence whose sp[i] draws (sp, step0 may be nullptr)
+  int decode_verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks, const cl_sampling* sp,
+                          const uint64_t* step0, int32_t* ids_out, int* n_out, float* logits_out);
   bool spec_path_ok() const;          // the verify pass runs on this model shape
   int speculate() const { return speculate_; }
+  int speculate_batch() const { return speculate_batch_; }
+  int set_speculate_batch(int n);     // 1..min(max_batch, kSpecBatchMax), else CL_ERR_INVALID_ARG
+  int64_t spec_multi_passes() const { return spec_multi_passes_; }
   int spec_stats(cl_spec_stats* out);
   bool device_sample() const { return device_sample_; }
   int set_tensor(int layer, int kind, const uint16_t* data, int64_t n);
@@ -290,6 +303,7 @@ class Engine {
   struct TokenSink { int (*fn)(void* user, const int32_t* ids, int n) = nullptr; void* user = nullptr; };
   int generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink = nullptr);
   void scheduler_main();
+  int spec_batch_round();   // one verify pass over the running requests (scheduler.cpp)
   void start_scheduler();
   void stop_scheduler();
 
@@ -326,8 +340,14 @@ class Engine {
   int attn_prefill(const AttnPrefillArgs& a, int layer, int& launches, LaunchProfiler& prof);   // the one choice of prefill attention kernel
   int prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_out);    // short prompts: split-K projections (prefill.cu)
   int ensure_small_ws();
-  // the split-K pass of prefill_small and verify_draft: T rows of s from pos0; leaves sws_->h and the final-norm rows sws_->xn
-  int small_pass(cl_seq_t s, const int* ids, int T, int pos0, int& launches, LaunchProfiler& prof);
+  // the split-K pass of prefill_small, verify_draft and verify_batch: T rows made of n_segs segments; leaves sws_->h and the
+  // final-norm rows sws_->xn.  row_map (device, or nullptr with one segment): [2][T] the sequence, then the position of every
+  // row; seg_table (device, may be nullptr): the segments as AttnVerifyArgs::segs, which selects the multi-row attention
+  // kernel where the shape allows it.
+  int small_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, const int* row_map, const int* seg_table, int& launches,
+                 LaunchProfiler& prof);
+  int ensure_spec_ws();
+  SpecTailArgs spec_tail_args(const PrefillSegment& g, int out_off) const;   // the spec tail of one verify segment
   bool prefill_path_ok() const;
   int set_single_slot(cl_seq_t s);
 
@@ -390,12 +410,16 @@ class Engine {
   struct SmallPrefillWs { float* part = nullptr; __nv_bfloat16* xn = nullptr; __nv_bfloat16* q = nullptr; __nv_bfloat16* attn = nullptr;
                           float* h = nullptr; __nv_bfloat16* act = nullptr; int* iota = nullptr; };
   std::unique_ptr<SmallPrefillWs> sws_;
-  // verify pass (allocated lazily): rows of at most kSpecMaxDraft + 1
+  // verify passes (allocated lazily): rows of at most kSpecMaxRows; out holds 1 + T ints per sequence, row_map [2][rows];
+  // segs [rows][8], attn_part and attn_cnt: the multi-row attention's segment table, split partials and counters
   struct SpecWs { float* logits = nullptr; int* choice = nullptr; float* part_val = nullptr; int* part_idx = nullptr;
-                  unsigned* counters = nullptr; unsigned long long* cand = nullptr; int* out = nullptr; };
+                  unsigned* counters = nullptr; unsigned long long* cand = nullptr; int* out = nullptr; int* row_map = nullptr;
+                  int* segs = nullptr; float* attn_part = nullptr; unsigned* attn_cnt = nullptr; };
+  int verify_split_pages() const;     // pages per split of the multi-row attention (a function of max_seq_len only)
   std::unique_ptr<SpecWs> spec_;
   int speculate_ = 0;                 // most drafted tokens per verify pass in the scheduler / synchronous path (0 = off)
-  std::atomic<int64_t> spec_passes_{0}, spec_drafted_{0}, spec_accepted_{0}, spec_emitted_{0};
+  std::atomic<int> speculate_batch_{1};   // most sequences the scheduler verifies in one pass (1: only a request running alone)
+  std::atomic<int64_t> spec_passes_{0}, spec_drafted_{0}, spec_accepted_{0}, spec_emitted_{0}, spec_multi_passes_{0};
   int prefill_small_max_ = 0;         // prompts up to this many tokens take the split-K path (CL_PREFILL_SMALL_MAX, 0 = off)
   struct BatchWs { __nv_bfloat16* xn = nullptr; __nv_bfloat16* attn = nullptr; __nv_bfloat16* act = nullptr; float* part = nullptr; float* logits = nullptr; };
   std::unique_ptr<BatchWs> bws_;

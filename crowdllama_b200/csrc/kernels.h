@@ -217,6 +217,9 @@ struct RopeScatterArgs {
   __nv_bfloat16* kpool; __nv_bfloat16* vpool; const int* block_table; int page_size;
   int n_heads, n_kv, head_dim;
   int n_split = 1; size_t split_stride = 0;   // qkv = sum of n_split split-K partials, split_stride floats apart (fixed order)
+  // optional per-row (sequence, position) map of a pass over several sequences: row t goes to position row_pos[t] of
+  // sequence row_seq[t], whose block table is block_table + row_seq[t] * bt_stride (pos0 unused).  nullptr: one sequence.
+  const int* row_seq = nullptr; const int* row_pos = nullptr; int bt_stride = 0;
 };
 int launch_rope_scatter(const RopeScatterArgs& a, cudaStream_t st);
 // causal attention of T new tokens (positions pos0..pos0+T-1) against the paged cache
@@ -230,6 +233,26 @@ int launch_attn_prefill(const AttnPrefillArgs& a, cudaStream_t st);
 // wgmma variant (attn_prefill_tc.cu): head_dim 128, page 32; kmap / vmap = pool-wide 2-D tensor maps (box {64, 32})
 bool attn_prefill_tc_supported(int n_heads, int n_kv, int head_dim, int page_size, int pos0, int T);
 int launch_attn_prefill_tc(const AttnPrefillArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st);
+// multi-row split-KV attention (attn_verify_tc.cu): segment s holds len_s cached tokens and R_s <= kVerifyMaxRows new rows at
+// positions len_s .. len_s + R_s - 1 (their K/V already in the pages); row r sees keys < len_s + r + 1
+constexpr int kVerifyMaxRows = 16;
+struct AttnVerifyArgs {
+  const __nv_bfloat16* q = nullptr;      // [rows][q_stride] roped
+  int q_stride = 0;
+  const int* segs = nullptr;             // [n_segs][8]: block-table row, first row, rows R, cached len, partial offset (floats), splits, 0, 0
+  const int* block_tables = nullptr;     // [seq][bt_stride]
+  int bt_stride = 0;
+  __nv_bfloat16* out = nullptr;          // [rows][out_stride]
+  int out_stride = 0;
+  float* part = nullptr;                 // per segment at its offset: [n_kv][splits][4 R][head_dim + 2]
+  unsigned* counters = nullptr;          // [n_segs][n_kv], zero between launches (the kernel re-arms them)
+  int n_segs = 0, n_heads = 0, n_kv = 0, head_dim = 0, page_size = 0;
+  int nsplit = 1;                        // grid splits: the largest of the segments' split counts
+  int split_pages = 0;                   // > 0: every split covers this many pages; 0: a segment's pages spread over its splits
+};
+bool attn_verify_tc_supported(int n_heads, int n_kv, int head_dim, int page_size);
+int attn_verify_max_splits();
+int launch_attn_verify_tc(const AttnVerifyArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st);
 // ---- batched decode glue (batch_kernels.cu) ------------------------------------------------------
 int launch_batch_resid_norm(float* h, int d, const float* ypart, int n_split, int B, const float* gain, float eps, __nv_bfloat16* xn,
                             const int* slots, cudaStream_t st, bool pdl = false);

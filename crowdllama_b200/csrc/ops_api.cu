@@ -302,6 +302,84 @@ int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_
   return CL_OK;
 }
 
+int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, const uint16_t* v_cache, const int32_t* ctx_lens,
+                      const int32_t* rows, int32_t n_segs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit,
+                      uint16_t* out, int32_t* nsplit_used) {
+  if (!q || !k_cache || !v_cache || !ctx_lens || !rows || !out || n_segs <= 0 || nsplit < 0) return CL_ERR_INVALID_ARG;
+  int rc = check_device(device);
+  if (rc) return rc;
+  if (!attn_verify_tc_supported(n_heads, n_kv, head_dim, page_size) || nsplit > attn_verify_max_splits()) {
+    set_last_error("the multi-row attention kernel does not take this shape or split count");
+    return CL_ERR_INVALID_ARG;
+  }
+  const int P = page_size, HD = head_dim;
+  const size_t qd = (size_t)n_heads * HD;
+  std::vector<int> toks(n_segs);
+  int T = 0, max_pages = 0;
+  for (int s = 0; s < n_segs; ++s) {
+    if (ctx_lens[s] < 0 || rows[s] < 1 || rows[s] > kVerifyMaxRows) {
+      set_last_error("cl_op_attn_verify: every segment needs 1..16 rows and a cached length >= 0");
+      return CL_ERR_INVALID_ARG;
+    }
+    toks[s] = ctx_lens[s] + rows[s];
+    T += rows[s];
+    max_pages = std::max(max_pages, (toks[s] + P - 1) / P);
+  }
+  OpKvPool pool;
+  op_build_kv_pool(k_cache, v_cache, toks.data(), n_segs, n_kv, HD, P, &pool);
+  // the engine's plan (Engine::verify_split_pages) unless nsplit is given: then every segment spreads its pages over nsplit
+  const int split_pages = nsplit ? 0 : std::max(8, (max_pages + attn_verify_max_splits() - 1) / attn_verify_max_splits());
+  std::vector<int> table(8 * (size_t)n_segs, 0);
+  long long part = 0;
+  int grid_splits = 1;
+  for (int s = 0, r0 = 0; s < n_segs; r0 += rows[s], ++s) {
+    const int pages = (toks[s] + P - 1) / P, ns = nsplit ? nsplit : (pages + split_pages - 1) / split_pages;
+    int* e = &table[8 * (size_t)s];
+    e[0] = s; e[1] = r0; e[2] = rows[s]; e[3] = ctx_lens[s]; e[4] = (int)part; e[5] = ns;
+    if (ns > 1) part += (long long)n_kv * ns * 4 * rows[s] * (HD + 2);
+    grid_splits = std::max(grid_splits, ns);
+  }
+  DevBuf dq, dk, dv, dbt, dseg, dout, dpart, dcnt;
+  CL_CUDA_OK(dq.upload(q, (size_t)T * qd * 2));
+  CL_CUDA_OK(dk.upload(pool.k.data(), pool.k.size() * 2));
+  CL_CUDA_OK(dv.upload(pool.v.data(), pool.v.size() * 2));
+  CL_CUDA_OK(dbt.upload(pool.bt.data(), pool.bt.size() * 4));
+  CL_CUDA_OK(dseg.upload(table.data(), table.size() * 4));
+  CL_CUDA_OK(dout.alloc((size_t)T * qd * 2));
+  CL_CUDA_OK(dpart.alloc((size_t)part * 4));
+  CL_CUDA_OK(dcnt.alloc((size_t)n_segs * n_kv * 4));
+  CL_CUDA_OK(cudaMemset(dcnt.p, 0, (size_t)n_segs * n_kv * 4));
+  const long long pool_rows = 2LL * pool.n_pages * n_kv * P;
+  CUtensorMap km, vm;
+  if (!make_tmap_2d_bf16(&km, dk.p, pool_rows, HD, 64, 32) || !make_tmap_2d_bf16(&vm, dv.p, pool_rows, HD, 64, 32)) {
+    set_last_error("cl_op_attn_verify: tensor map creation failed");
+    return CL_ERR_CUDA;
+  }
+  AttnVerifyArgs a;
+  a.q = dq.as<__nv_bfloat16>(); a.q_stride = (int)qd; a.segs = dseg.as<int>(); a.block_tables = dbt.as<int>(); a.bt_stride = pool.bt_stride;
+  a.out = dout.as<__nv_bfloat16>(); a.out_stride = (int)qd; a.part = dpart.as<float>(); a.counters = dcnt.as<unsigned>();
+  a.n_segs = n_segs; a.n_heads = n_heads; a.n_kv = n_kv; a.head_dim = HD; a.page_size = P; a.nsplit = grid_splits; a.split_pages = split_pages;
+  // two launches without re-arming the split counters in between must give the same bits
+  std::vector<uint16_t> first((size_t)T * qd);
+  for (int run = 0; run < 2; ++run) {
+    CL_CUDA_OK(cudaMemset(dout.p, 0xff, (size_t)T * qd * 2));   // NaN: every element must be written
+    CL_CUDA_OK(cudaDeviceSynchronize());
+    if (launch_attn_verify_tc(a, km, vm, pool_rows / 2, nullptr) < 0) {
+      CL_CUDA_OK(cudaGetLastError());
+      set_last_error("multi-row attention launch failed");
+      return CL_ERR_CUDA;
+    }
+    CL_CUDA_OK(cudaDeviceSynchronize());
+    CL_CUDA_OK(cudaMemcpy(run ? out : first.data(), dout.p, (size_t)T * qd * 2, cudaMemcpyDeviceToHost));
+  }
+  if (nsplit_used) *nsplit_used = grid_splits;
+  if (memcmp(out, first.data(), first.size() * 2)) {
+    set_last_error("cl_op_attn_verify: the second launch (split counters not reset) changed the output");
+    return CL_ERR_INTERNAL;
+  }
+  return CL_OK;
+}
+
 int cl_op_qkv_rope_append(int device, int variant, const uint16_t* w_qkv, const float* h, const float* gain, float eps, int32_t d_model,
                           int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t pos, float rope_theta, float* q_out,
                           uint16_t* k_out, uint16_t* v_out) {

@@ -55,7 +55,8 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
   int launches = 0;
   LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
-  if ((rc = small_pass(s, d_prompt_, n, q.len, launches, prof))) return rc;
+  const PrefillSegment seg{s, 0, n, q.len};
+  if ((rc = small_pass(&seg, 1, d_prompt_, n, nullptr, nullptr, launches, prof))) return rc;
   // the last row -> the slot's residual row, then the shared tail (its own final norm + GEMV head)
   CL_CUDA_OK(cudaMemcpyAsync(d_h_ + (size_t)s * d, sws_->h + (size_t)(n - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, stream_));
   const int last_pos = q.len + n - 1;
@@ -94,16 +95,30 @@ int Engine::ensure_small_ws() {
   return CL_OK;
 }
 
-// One split-K pass over T <= 256 rows of sequence s at positions pos0 .. pos0 + T - 1, token ids at ids (device):
-// embedding, every layer (K/V written into the sequence's pages), and the final norm.  Leaves the final residual rows in
-// sws_->h and their normalised bf16 rows, the LM head's input, in sws_->xn.  A row's results do not depend on the rows
-// after it.  prefill_small and the verify pass of speculative decoding (verify_draft) both run it.
-int Engine::small_pass(cl_seq_t s, const int* ids, int T, int pos0, int& launches, LaunchProfiler& prof) {
+// One split-K pass over T <= 256 rows, token ids at ids (device): embedding, every layer (K/V written into the sequences'
+// pages), and the final norm.  The rows are the segments' tokens, back to back.  Everything row-wise runs once over all
+// rows; RoPE + cache scatter runs in one launch (through row_map when it is given).  The causal attention runs in one launch
+// of the multi-row split-KV kernel (attn_verify_tc.cu) when seg_table is given and the shape is one it takes, else per
+// segment (attn_prefill).  Leaves the final residual rows in sws_->h and their normalised bf16 rows, the LM head's input,
+// in sws_->xn.  A row's results depend only on its own segment's rows before it.  prefill_small and the verify passes of
+// speculative decoding (verify_draft: one segment, no map or table; verify_batch) run it.
+int Engine::small_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, const int* row_map, const int* seg_table,
+                       int& launches, LaunchProfiler& prof) {
   const int d = cfg.d_model, F = cfg.d_ff;
   const int s_qkv = pick_splits_public(qkv_dim_, d), s_o = pick_splits_public(d, q_dim_), s_gu = pick_splits_public(2 * F, d), s_dn = pick_splits_public(d, F);
   SmallPrefillWs& w = *sws_;
-  const int* bt = d_bt_ + (size_t)s * max_pages_per_seq_;
   int rc;
+  AttnVerifyArgs va;
+  const bool multi_row = seg_table && have_kv_maps_ && attn_verify_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_);
+  if (multi_row) {
+    va.q = w.q; va.q_stride = q_dim_; va.segs = seg_table; va.block_tables = d_bt_; va.bt_stride = max_pages_per_seq_;
+    va.out = w.attn; va.out_stride = q_dim_; va.part = spec_->attn_part; va.counters = spec_->attn_cnt;
+    va.n_segs = n_segs; va.n_heads = cfg.n_heads; va.n_kv = cfg.n_kv_heads; va.head_dim = cfg.head_dim; va.page_size = page_size_;
+    va.split_pages = verify_split_pages();
+    va.nsplit = 1;
+    for (int i = 0; i < n_segs; ++i)
+      va.nsplit = std::max(va.nsplit, ((segs[i].pos0 + segs[i].n + page_size_ - 1) / page_size_ + va.split_pages - 1) / va.split_pages);
+  }
   // programmatic dependent launch between the GEMMs and the per-row glue kernels, as in the batched decode step (the two
   // prefill kernels in between are launched normally and order the stream)
   const bool bp = use_pdl_;
@@ -114,13 +129,20 @@ int Engine::small_pass(cl_seq_t s, const int* ids, int T, int pos0, int& launche
     const auto& L = layers_[l];
     CL_LAUNCH(launch_batch_resid_norm(w.h, d, pending, pending_s, T, L.attn_norm, cfg.rms_eps, w.xn, w.iota, stream_, bp));
     CL_LAUNCH(launch_gemm_bf16(w.xn, L.wqkv, w.part, nullptr, T, qkv_dim_, d, stream_, s_qkv, bp));
-    RopeScatterArgs ra{w.part, qkv_dim_, rope_, pos0, T, w.q, kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_,
-                       bt, page_size_, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim};
+    RopeScatterArgs ra{w.part, qkv_dim_, rope_, segs[0].pos0, T, w.q, kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_,
+                       d_bt_ + (row_map ? 0 : (size_t)segs[0].seq * max_pages_per_seq_), page_size_, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim};
     ra.n_split = s_qkv; ra.split_stride = (size_t)T * qkv_dim_;
+    if (row_map) { ra.row_seq = row_map; ra.row_pos = row_map + T; ra.bt_stride = max_pages_per_seq_; }
     CL_LAUNCH(launch_rope_scatter(ra, stream_));
-    AttnPrefillArgs aa{w.q, kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_, bt, page_size_,
-                       pos0, T, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, w.attn};
-    if ((rc = attn_prefill(aa, l, launches, prof))) return rc;
+    if (multi_row)
+      CL_LAUNCH(launch_attn_verify_tc(va, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_));
+    for (int i = 0; i < n_segs && !multi_row; ++i) {
+      const PrefillSegment& g = segs[i];
+      AttnPrefillArgs aa{w.q + (size_t)g.row0 * q_dim_, kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_,
+                         d_bt_ + (size_t)g.seq * max_pages_per_seq_, page_size_, g.pos0, g.n, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim,
+                         w.attn + (size_t)g.row0 * q_dim_};
+      if ((rc = attn_prefill(aa, l, launches, prof))) return rc;
+    }
     CL_LAUNCH(launch_gemm_bf16(w.attn, L.wo, w.part, nullptr, T, d, q_dim_, stream_, s_o, bp));
     CL_LAUNCH(launch_batch_resid_norm(w.h, d, w.part, s_o, T, L.ffn_norm, cfg.rms_eps, w.xn, w.iota, stream_, bp));
     CL_LAUNCH(launch_gemm_bf16(w.xn, L.wgu, w.part, nullptr, T, 2 * F, d, stream_, s_gu, bp));
@@ -131,6 +153,48 @@ int Engine::small_pass(cl_seq_t s, const int* ids, int T, int pos0, int& launche
   // fold the last down-projection into the residual rows; the final-norm rows it also writes feed the verify pass's head
   CL_LAUNCH(launch_batch_resid_norm(w.h, d, pending, pending_s, T, final_norm_, cfg.rms_eps, w.xn, w.iota, stream_, bp));
   return CL_OK;
+}
+
+int Engine::ensure_spec_ws() {
+  if (spec_) return CL_OK;
+  const size_t R = kSpecMaxRows, V = cfg.vocab_size;
+  int rc;
+  spec_.reset(new SpecWs());
+  if ((rc = ws_alloc(allocs_, spec_->logits, R * V * 4)) || (rc = ws_alloc(allocs_, spec_->choice, R * 4)) ||
+      (rc = ws_alloc(allocs_, spec_->part_val, R * kTailBlocks * 4)) || (rc = ws_alloc(allocs_, spec_->part_idx, R * kTailBlocks * 4)) ||
+      (rc = ws_alloc(allocs_, spec_->counters, R * 4)) || (rc = ws_alloc(allocs_, spec_->cand, R * kTailBlocks * kSampleTopKMax * 8)) ||
+      (rc = ws_alloc(allocs_, spec_->out, 2 * R * 4)) || (rc = ws_alloc(allocs_, spec_->row_map, 2 * R * 4)) ||
+      (rc = ws_alloc(allocs_, spec_->segs, R * 8 * 4)) || (rc = ws_alloc(allocs_, spec_->attn_cnt, R * cfg.n_kv_heads * 4))) { spec_.reset(); return rc; }
+  // the multi-row attention's split partials: at most 4 query rows per pass row, per kv head and split
+  if (attn_verify_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_)) {
+    const size_t max_splits = (max_pages_per_seq_ + verify_split_pages() - 1) / verify_split_pages();
+    if ((rc = ws_alloc(allocs_, spec_->attn_part, R * 4 * cfg.n_kv_heads * max_splits * (cfg.head_dim + 2) * 4))) { spec_.reset(); return rc; }
+  }
+  CL_CUDA_OK(cudaMemsetAsync(spec_->counters, 0, R * 4, stream_));
+  CL_CUDA_OK(cudaMemsetAsync(spec_->attn_cnt, 0, R * cfg.n_kv_heads * 4, stream_));
+  return CL_OK;
+}
+
+// Every split of the multi-row attention covers 8 pages (256 tokens at page 32), more only when a sequence of max_seq_len
+// would need more than the kernel's 64 splits.  A segment's split plan thus depends on its own length alone, so a sequence's
+// attention rows are the same bits whatever other sequences share the pass.
+int Engine::verify_split_pages() const {
+  return std::max(8, (max_pages_per_seq_ + attn_verify_max_splits() - 1) / attn_verify_max_splits());
+}
+
+// The spec tail of one segment of a verify pass: its rows' logits, inputs and tail buffers, and its 1 + n ints of output at
+// out_off.  The segment's sequence is its slot; the sequence's cached length is g.pos0.
+SpecTailArgs Engine::spec_tail_args(const PrefillSegment& g, int out_off) const {
+  const size_t r0 = g.row0;
+  SpecTailArgs t;
+  t.logits = spec_->logits + r0 * cfg.vocab_size; t.vocab = cfg.vocab_size; t.T = g.n; t.slot = g.seq; t.len = g.pos0;
+  t.inputs = d_prompt_ + r0; t.choice = spec_->choice + r0;
+  t.part_val = spec_->part_val + r0 * kTailBlocks; t.part_idx = spec_->part_idx + r0 * kTailBlocks; t.counters = spec_->counters + r0;
+  t.cand = spec_->cand + r0 * kTailBlocks * kSampleTopKMax;
+  t.tok = d_tok_; t.pos = d_pos_; t.out = spec_->out + out_off;
+  t.sample.mode = d_samp_mode_; t.sample.par = d_samp_par_; t.sample.step = d_samp_step_; t.sample.hist = d_samp_hist_;
+  t.sample.hist_len = d_samp_hlen_;
+  return t;
 }
 
 bool Engine::spec_path_ok() const {
@@ -155,28 +219,14 @@ int Engine::verify_draft(cl_seq_t s, int32_t x0, const int32_t* draft, int k, in
   auto& q = seqs_[s];
   int rc = ensure_capacity(s, q.len + T);
   if (rc) return rc;
-  if ((rc = ensure_small_ws())) return rc;
-  if (!spec_) {
-    const size_t R = kSpecMaxDraft + 1;
-    spec_.reset(new SpecWs());
-    if ((rc = ws_alloc(allocs_, spec_->logits, R * V * 4)) || (rc = ws_alloc(allocs_, spec_->choice, R * 4)) ||
-        (rc = ws_alloc(allocs_, spec_->part_val, R * kTailBlocks * 4)) || (rc = ws_alloc(allocs_, spec_->part_idx, R * kTailBlocks * 4)) ||
-        (rc = ws_alloc(allocs_, spec_->counters, R * 4)) || (rc = ws_alloc(allocs_, spec_->cand, R * kTailBlocks * kSampleTopKMax * 8)) ||
-        (rc = ws_alloc(allocs_, spec_->out, (R + 1) * 4))) { spec_.reset(); return rc; }
-    CL_CUDA_OK(cudaMemsetAsync(spec_->counters, 0, R * 4, stream_));
-  }
+  if ((rc = ensure_small_ws()) || (rc = ensure_spec_ws())) return rc;
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, in, (size_t)T * 4, cudaMemcpyHostToDevice, stream_));
   int launches = 0;
   LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
-  if ((rc = small_pass(s, d_prompt_, T, q.len, launches, prof))) return rc;
+  const PrefillSegment seg{s, 0, T, q.len};
+  if ((rc = small_pass(&seg, 1, d_prompt_, T, nullptr, nullptr, launches, prof))) return rc;
   CL_LAUNCH(launch_gemm_bf16(sws_->xn, lm_head_, spec_->logits, nullptr, T, V, d, stream_, 1, false));
-  SpecTailArgs t;
-  t.logits = spec_->logits; t.vocab = V; t.T = T; t.slot = s; t.len = q.len; t.inputs = d_prompt_; t.choice = spec_->choice;
-  t.part_val = spec_->part_val; t.part_idx = spec_->part_idx; t.counters = spec_->counters; t.cand = spec_->cand;
-  t.tok = d_tok_; t.pos = d_pos_; t.out = spec_->out;
-  t.sample.mode = d_samp_mode_; t.sample.par = d_samp_par_; t.sample.step = d_samp_step_; t.sample.hist = d_samp_hist_;
-  t.sample.hist_len = d_samp_hlen_;
-  CL_LAUNCH(launch_spec_tail(t, stream_, use_pdl_));
+  CL_LAUNCH(launch_spec_tail(spec_tail_args(seg, 0), stream_, use_pdl_));
   CL_CUDA_OK(cudaMemcpyAsync(h_ids_pinned_, spec_->out, (size_t)(T + 1) * 4, cudaMemcpyDeviceToHost, stream_));
   CL_CUDA_OK(cudaStreamSynchronize(stream_));
   prof.report("prefill profile", 32, "verify pass, " + std::to_string(T) + " rows");
@@ -200,6 +250,110 @@ int Engine::decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, c
   if (sampled) rc = arm_sampling(s, *sp, step0, seqs_[s].history.data(), (int)seqs_[s].history.size());
   if (rc == CL_OK) rc = verify_draft(s, x0, draft, k, ids_out, n_out, logits_out);
   if (sampled) {
+    const int r2 = disarm_sampling(s);
+    if (rc == CL_OK) rc = r2;
+  }
+  return rc;
+}
+
+// Verify pass over several sequences (include/clengine.h, cl_decode_verify_batch): sequence i is segment i of one small_pass,
+// rows x0[i], d_1 .. d_{k_i} at positions len_i .. len_i + k_i.  One GEMM computes the logits of all rows, then each segment
+// runs verify_draft's spec tail and accept kernel on its own rows and slot.  Every row's computation is the one it has in a
+// pass of its sequence alone, so each sequence's ids, logits and K/V equal verifying it alone.  Everything is checked before
+// anything is enqueued; on an error no sequence's length changes.
+int Engine::verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks, int32_t* ids_out,
+                         int* n_out, float* logits_out) {
+  if (n_seqs < 1 || !ss || !x0 || !ks || !ids_out || !n_out) { set_last_error("verify_batch: bad arguments"); return CL_ERR_INVALID_ARG; }
+  if (!spec_path_ok()) { set_last_error("verify: the model shape has no tensor-core split-K path"); return CL_ERR_INVALID_ARG; }
+  const int V = cfg.vocab_size, d = cfg.d_model;
+  std::vector<PrefillSegment> segs(n_seqs);
+  std::vector<int32_t> in;
+  int T = 0, n_drafted = 0;
+  for (int i = 0; i < n_seqs; ++i) {
+    const int s = ss[i];
+    if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+    for (int j = 0; j < i; ++j) if (ss[j] == s) { set_last_error("duplicate sequence in batch"); return CL_ERR_INVALID_ARG; }
+    if (ks[i] < 0 || ks[i] > kSpecMaxDraft || (ks[i] > 0 && !drafts)) { set_last_error("verify: k must be 0..15"); return CL_ERR_INVALID_ARG; }
+    if (T + ks[i] + 1 > kSpecMaxRows) { set_last_error("verify: more than 128 rows in one pass"); return CL_ERR_INVALID_ARG; }
+    segs[i] = PrefillSegment{s, T, ks[i] + 1, seqs_[s].len};
+    in.push_back(x0[i]);
+    in.insert(in.end(), drafts + n_drafted, drafts + n_drafted + ks[i]);
+    T += ks[i] + 1;
+    n_drafted += ks[i];
+  }
+  for (int t = 0; t < T; ++t)
+    if (in[t] < 0 || in[t] >= V) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
+  for (const auto& g : segs)
+    if (g.pos0 + g.n > cfg.max_seq_len) { set_last_error("sequence exceeds max_seq_len"); return CL_ERR_TOO_LONG; }
+  int rc;
+  for (const auto& g : segs)
+    if ((rc = ensure_capacity(g.seq, g.pos0 + g.n))) return rc;
+  if ((rc = ensure_small_ws()) || (rc = ensure_spec_ws())) return rc;
+  std::vector<int> row_map(2 * (size_t)T), table(8 * (size_t)n_seqs, 0);
+  const int split_pages = verify_split_pages();
+  long long part_off = 0;
+  for (int i = 0; i < n_seqs; ++i) {
+    const PrefillSegment& g = segs[i];
+    for (int r = 0; r < g.n; ++r) { row_map[g.row0 + r] = g.seq; row_map[T + g.row0 + r] = g.pos0 + r; }
+    const int pages = (g.pos0 + g.n + page_size_ - 1) / page_size_, ns = (pages + split_pages - 1) / split_pages;
+    int* e = &table[8 * (size_t)i];
+    e[0] = g.seq; e[1] = g.row0; e[2] = g.n; e[3] = g.pos0; e[4] = (int)part_off; e[5] = ns;
+    if (ns > 1) part_off += (long long)cfg.n_kv_heads * ns * 4 * g.n * (cfg.head_dim + 2);
+  }
+  CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, in.data(), (size_t)T * 4, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaMemcpyAsync(spec_->row_map, row_map.data(), row_map.size() * 4, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaMemcpyAsync(spec_->segs, table.data(), table.size() * 4, cudaMemcpyHostToDevice, stream_));
+  int launches = 0;
+  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
+  if ((rc = small_pass(segs.data(), n_seqs, d_prompt_, T, spec_->row_map, spec_->segs, launches, prof))) return rc;
+  CL_LAUNCH(launch_gemm_bf16(sws_->xn, lm_head_, spec_->logits, nullptr, T, V, d, stream_, 1, false));
+  // segment i's output {n_i, ids} sits at out[row0_i + i]: one int more per segment than its rows
+  for (int i = 0; i < n_seqs; ++i) CL_LAUNCH(launch_spec_tail(spec_tail_args(segs[i], segs[i].row0 + i), stream_, use_pdl_));
+  CL_CUDA_OK(cudaMemcpyAsync(h_ids_pinned_, spec_->out, (size_t)(T + n_seqs) * 4, cudaMemcpyDeviceToHost, stream_));
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  prof.report("prefill profile", 32, "verify pass, " + std::to_string(n_seqs) + " sequences, " + std::to_string(T) + " rows");
+  launches_ += launches;
+  for (int i = 0; i < n_seqs; ++i) {
+    const int n = h_ids_pinned_[segs[i].row0 + i];
+    if (n < 1 || n > segs[i].n) { set_last_error("verify: accept kernel returned a bad count"); return CL_ERR_INTERNAL; }
+  }
+  int accepted = 0, emitted = 0;
+  for (int i = 0; i < n_seqs; ++i) {
+    const PrefillSegment& g = segs[i];
+    const int n = h_ids_pinned_[g.row0 + i];
+    memcpy(ids_out + g.row0, h_ids_pinned_ + g.row0 + i + 1, (size_t)n * 4);
+    n_out[i] = n;
+    seq_advance(g.seq, in.data() + g.row0, n, n);   // x0, d1 .. da: only accepted tokens join the history and the prefix cache
+    accepted += n - 1; emitted += n;
+  }
+  spec_passes_ += n_seqs; spec_drafted_ += n_drafted; spec_accepted_ += accepted; spec_emitted_ += emitted;
+  if (n_seqs > 1) spec_multi_passes_++;
+  if (logits_out) CL_CUDA_OK(cudaMemcpy(logits_out, spec_->logits, (size_t)T * V * 4, cudaMemcpyDeviceToHost));
+  return CL_OK;
+}
+
+// cl_decode_verify_batch: verify_batch with the device sampler armed for the pass on the sequences whose sp[i] draws
+int Engine::decode_verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks,
+                                const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int* n_out, float* logits_out) {
+  if (n_seqs < 1 || !ss) { set_last_error("verify_batch: bad arguments"); return CL_ERR_INVALID_ARG; }
+  for (int i = 0; i < n_seqs; ++i) {
+    if (ss[i] < 0 || ss[i] >= max_seqs_ || !seqs_[ss[i]].live) return CL_ERR_BAD_SEQ;
+    if (sp && sp[i].temperature > 0.f && !device_sampling_ok(sp[i], cfg.vocab_size)) {
+      set_last_error("sampling settings need the host sampler");
+      return CL_ERR_INVALID_ARG;
+    }
+  }
+  std::vector<cl_seq_t> armed;
+  int rc = CL_OK;
+  for (int i = 0; i < n_seqs && rc == CL_OK && sp; ++i) {
+    if (!(sp[i].temperature > 0.f)) continue;
+    const cl_seq_t s = ss[i];
+    if (std::find(armed.begin(), armed.end(), s) != armed.end()) continue;   // a duplicate: verify_batch refuses it
+    rc = arm_sampling(s, sp[i], step0 ? step0[i] : 0, seqs_[s].history.data(), (int)seqs_[s].history.size());
+    if (rc == CL_OK) armed.push_back(s);
+  }
+  if (rc == CL_OK) rc = verify_batch(ss, n_seqs, x0, drafts, ks, ids_out, n_out, logits_out);
+  for (cl_seq_t s : armed) {
     const int r2 = disarm_sampling(s);
     if (rc == CL_OK) rc = r2;
   }

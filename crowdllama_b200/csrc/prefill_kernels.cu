@@ -63,7 +63,8 @@ int launch_rmsnorm_bf16(const float* h, const float* gain, float eps, __nv_bfloa
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) rope_scatter_kernel(const RopeScatterArgs a) {
   const int t = blockIdx.x;
-  const int pos = a.pos0 + t;
+  const int pos = a.row_seq ? a.row_pos[t] : a.pos0 + t;
+  const int* bt = a.row_seq ? a.block_table + (size_t)a.row_seq[t] * a.bt_stride : a.block_table;
   const int HD = a.head_dim, half = HD / 2;
   const float* row = a.qkv + (size_t)t * a.qkv_stride;
   const float2* rope = a.rope + (size_t)pos * half;
@@ -82,7 +83,7 @@ __global__ void __launch_bounds__(256) rope_scatter_kernel(const RopeScatterArgs
     a.q_out[(size_t)t * qd + hh * HD + j] = __float2bfloat16_rn(x0 * cs.x - x1 * cs.y);
     a.q_out[(size_t)t * qd + hh * HD + j + half] = __float2bfloat16_rn(x1 * cs.x + x0 * cs.y);
   }
-  const int page = a.block_table[pos / a.page_size], off = pos % a.page_size;
+  const int page = bt[pos / a.page_size], off = pos % a.page_size;
   for (int i = threadIdx.x; i < a.n_kv * half; i += blockDim.x) {
     const int g = i / half, j = i % half;
     const float2 cs = rope[j];

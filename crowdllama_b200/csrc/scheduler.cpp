@@ -106,6 +106,60 @@ static int spec_round(Engine& e, Request& r) {
   return joined;
 }
 
+// Speculative round of the 2 .. speculate_batch running requests, every one greedy or device-sampled: each drafts as
+// spec_round would (k = 0 while backing off, without a match, or when the pool has no pages for its draft), and one
+// verify_batch pass checks all of them.  Drafts are clipped so that the pass stays within kSpecMaxRows: every k is capped at
+// the largest c with sum(min(k_i, c) + 1) <= kSpecMaxRows, so no request loses a drafted token while another keeps more
+// than c.  Returns the ids that joined the requests' outputs, 0 when nobody drafted (the batch takes a normal step), or an
+// error status.
+int Engine::spec_batch_round() {
+  const int B = (int)active_.size();
+  std::vector<int> ks(B, 0);
+  std::vector<int32_t> drafts((size_t)B * kSpecMaxDraft);
+  for (int b = 0; b < B; ++b) {
+    Request& r = *active_[b];
+    if (r.spec_backoff > 0 || r.out.empty()) continue;
+    const int k_max = std::min({speculate_, r.max_new - (int)r.out.size() - 1, cfg.max_seq_len - seqs_[r.seq].len - 1});
+    if (k_max < 1) continue;
+    std::vector<int32_t> hist(r.prompt);
+    hist.insert(hist.end(), r.out.begin(), r.out.end());   // ends with the next input x0
+    ks[b] = ngram_draft(hist.data(), (int)hist.size(), k_max, drafts.data() + (size_t)b * kSpecMaxDraft);
+  }
+  int cap = kSpecMaxDraft;
+  auto rows = [&](int c) { int t = 0; for (int k : ks) t += std::min(k, c) + 1; return t; };
+  while (cap > 0 && rows(cap) > kSpecMaxRows) --cap;
+  for (int b = 0; b < B; ++b) {
+    ks[b] = std::min(ks[b], cap);
+    // pages for the drafted rows (x0's are reserved already): a request the pool cannot serve drafts nothing this round
+    const cl_seq_t s = active_[b]->seq;
+    if (ks[b] > 0 && ensure_capacity(s, seqs_[s].len + ks[b] + 1)) ks[b] = 0;
+  }
+  if (std::all_of(ks.begin(), ks.end(), [](int k) { return k == 0; })) return 0;
+  std::vector<cl_seq_t> ss(B);
+  std::vector<int32_t> x0(B), packed, ids(kSpecMaxRows);
+  std::vector<int> n(B);
+  for (int b = 0; b < B; ++b) {
+    ss[b] = active_[b]->seq;
+    x0[b] = active_[b]->out.back();
+    packed.insert(packed.end(), drafts.begin() + (size_t)b * kSpecMaxDraft, drafts.begin() + (size_t)b * kSpecMaxDraft + ks[b]);
+  }
+  const int rc = verify_batch(ss.data(), B, x0.data(), packed.data(), ks.data(), ids.data(), n.data(), nullptr);
+  if (rc) return rc;
+  int joined = 0;
+  for (int b = 0, row0 = 0; b < B; row0 += ks[b] + 1, ++b) {
+    Request& r = *active_[b];
+    if (ks[b] > 0) r.spec_backoff = n[b] == 1 ? kSpecBackoff : 0;
+    else if (r.spec_backoff > 0) r.spec_backoff--;   // one token, as in a decode step
+    for (int j = 0; j < n[b]; ++j) {
+      r.out.push_back(ids[row0 + j]);
+      publish(r, r.out.back());
+      ++joined;
+      if (finished(r, *tok, cfg.max_seq_len)) break;
+    }
+  }
+  return joined;
+}
+
 // ---- synchronous path (no scheduler thread): one request at a time under the engine lock --------
 static int generate_sync(Engine& e, Request& r, const Engine::TokenSink* sink) {
   size_t emitted = 0;
@@ -527,6 +581,42 @@ void Engine::scheduler_main() {
         continue;
       }
     }
+    auto retire_finished = [&] {
+      for (size_t i = 0; i < active_.size();) {
+        auto r = active_[i];
+        if (finished(*r, *tok, cfg.max_seq_len)) {
+          seq_free(r->seq);
+          active_.erase(active_.begin() + i);
+          requests_completed_++;
+          complete(r, CL_OK, "");
+        } else {
+          ++i;
+        }
+      }
+    };
+    auto fail_active = [&](int rc) {
+      const std::string err = get_last_error();
+      for (auto& r : active_) { seq_free(r->seq); complete(r, rc, err); }
+      active_.clear();
+      last_slots.clear();
+    };
+    // ---- speculative decoding over 2 .. speculate_batch_ requests, all greedy or device-sampled, with nothing to admit:
+    // one verify pass for all of them instead of a step (it counts as one decode step)
+    if (speculate_ > 0 && active_.size() >= 2 && (int)active_.size() <= speculate_batch_ && !prefilling_ &&
+        std::all_of(active_.begin(), active_.end(), [](const std::shared_ptr<Request>& r) { return r->device_next(); }) &&
+        [&] { std::lock_guard<std::mutex> lk(q_mu_); return queue_.empty(); }()) {
+      const int64_t t0 = now_ns();
+      const int n = spec_batch_round();
+      if (n < 0) { fail_active(n); continue; }
+      if (n > 0) {
+        const int64_t dt = now_ns() - t0;
+        for (auto& r : active_) r->decode_ns += dt;
+        tokens_generated_ += n;
+        sched_decode_steps_++; sched_decode_ns_ += dt;
+        retire_finished();
+        continue;
+      }
+    }
     // ---- one batched decode step
     const int B = (int)active_.size();
     slots.resize(B);
@@ -550,13 +640,7 @@ void Engine::scheduler_main() {
         if (cudaEventRecord(step_done_ev_, stream_) != cudaSuccess || cudaEventSynchronize(step_done_ev_) != cudaSuccess) rc = CL_ERR_CUDA;
       } else if (cudaStreamSynchronize(stream_) != cudaSuccess) rc = CL_ERR_CUDA;
     }
-    if (rc) {
-      const std::string err = get_last_error();
-      for (auto& r : active_) { seq_free(r->seq); complete(r, rc, err); }
-      active_.clear();
-      last_slots.clear();
-      continue;
-    }
+    if (rc) { fail_active(rc); continue; }
     for (int b = 0; b < B; ++b) {
       auto& r = active_[b];
       auto& st = seqs_[r->seq];
@@ -578,18 +662,7 @@ void Engine::scheduler_main() {
     sched_decode_steps_++; sched_decode_ns_ += dt;
     const double tps = (double)max_batch_ / ((double)dt * 1e-9);   // capacity at the current step time (engine.cu, init)
     tok_per_sec_ewma_ = tok_per_sec_ewma_ == 0.0 ? tps : 0.9 * tok_per_sec_ewma_ + 0.1 * tps;
-    // ---- retire finished requests
-    for (size_t i = 0; i < active_.size();) {
-      auto r = active_[i];
-      if (finished(*r, *tok, cfg.max_seq_len)) {
-        seq_free(r->seq);
-        active_.erase(active_.begin() + i);
-        requests_completed_++;
-        complete(r, CL_OK, "");
-      } else {
-        ++i;
-      }
-    }
+    retire_finished();
   }
   // shutdown: fail whatever is left
   std::lock_guard<std::mutex> elk(mu_);

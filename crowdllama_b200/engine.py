@@ -7,6 +7,7 @@ of the binding fails loudly, and if no sm_90 device is visible `Engine(...)` rai
 from __future__ import annotations
 
 import ctypes as C
+import os
 from pathlib import Path
 
 import numpy as np
@@ -70,19 +71,20 @@ class PrefixStats(C.Structure):
 
 class SpecStats(C.Structure):
     _fields_ = [("enabled", C.c_int32), ("max_draft", C.c_int32), ("verify_passes", C.c_int64), ("tokens_drafted", C.c_int64),
-                ("tokens_accepted", C.c_int64), ("tokens_emitted", C.c_int64), ("reserved", C.c_int64 * 4)]
+                ("tokens_accepted", C.c_int64), ("tokens_emitted", C.c_int64), ("multi_passes", C.c_int64),
+                ("reserved", C.c_int64 * 3)]
 
 
 # every symbol include/clengine.h declares (tests check the library exports all of them)
 EXPORTS = [
     "cl_abi_version", "cl_strerror", "cl_last_error", "cl_default_engine_config", "cl_default_sampling",
     "cl_greedy_sampling", "cl_sample_token", "cl_model_preset", "cl_engine_create", "cl_engine_destroy", "cl_engine_model_config",
-    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_draft_ngram", "cl_decode_verify", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
+    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_engine_set_speculate_batch", "cl_draft_ngram", "cl_decode_verify", "cl_decode_verify_batch", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
     "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
     "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
-    "cl_op_attn_decode_batch", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
+    "cl_op_attn_decode_batch", "cl_op_attn_verify", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
     "cl_op_attn_prefill_cached", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages",
@@ -123,6 +125,8 @@ def lib():
         "cl_engine_spec_stats": (C.c_int, [vp, P(SpecStats)]),
         "cl_draft_ngram": (C.c_int, [vp, i32, i32, vp, P(i32)]),
         "cl_decode_verify": (C.c_int, [vp, i32, i32, vp, i32, P(Sampling), u64, vp, P(i32), vp]),
+        "cl_engine_set_speculate_batch": (C.c_int, [vp, i32]),
+        "cl_decode_verify_batch": (C.c_int, [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
         "cl_engine_set_tensor": (C.c_int, [vp, i32, i32, vp, i64]),
         "cl_checkpoint_info": (C.c_int, [C.c_char_p, P(ModelConfig), P(i32), P(i64)]),
         "cl_generate": (C.c_int, [vp, C.c_char_p, C.c_char_p, sz, P(Sampling), P(Result)]),
@@ -159,6 +163,7 @@ def lib():
         "cl_op_qkv_rope_append": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, f32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
         "cl_op_attn_decode_batch": (C.c_int, [C.c_int, C.c_int, i32, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp,
                                               P(i32), P(i32)]),
+        "cl_op_attn_verify": (C.c_int, [C.c_int, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, P(i32)]),
         "cl_op_gemm_bf16": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, P(f32)]),
         "cl_op_gemm_bf16_epi": (C.c_int, [C.c_int, C.c_int, i32, C.c_int, vp, vp, vp, vp, vp, i32, i32, i32, P(i32)]),
         "cl_op_attn_prefill": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -287,7 +292,7 @@ class Engine:
                  device: int = 0, seed: int = 1234, max_batch: int = 8, max_seqs: int | None = None,
                  page_size: int = 32, kv_pool_bytes: int = 0, use_cuda_graph: bool = True, decode_path: int = 0,
                  start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False,
-                 speculate: int = 0):
+                 speculate: int = 0, speculate_batch: int = 1):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -314,6 +319,9 @@ class Engine:
         h = C.c_void_p()
         _check(L.cl_engine_create(C.byref(cfg), C.byref(h)), "cl_engine_create")
         self._h = h
+        # requests verified in one pass; env CL_SPECULATE_BATCH overrides the argument, as CL_SPECULATE does `speculate`
+        if speculate_batch != 1 and "CL_SPECULATE_BATCH" not in os.environ:
+            self.set_speculate_batch(speculate_batch)
         mc = ModelConfig()
         _check(L.cl_engine_model_config(self._h, C.byref(mc)), "cl_engine_model_config")
         self.cfg = mc.as_dict()
@@ -434,6 +442,32 @@ class Engine:
         _check(lib().cl_decode_verify(self._h, s, int(input_id), _ptr(d), len(d), C.byref(sampling) if sampling else None, step0,
                                       _ptr(ids), C.byref(n), _ptr(out) if want_logits else None), "cl_decode_verify")
         return ids[:n.value].copy(), out
+
+    def decode_verify_batch(self, seqs, input_ids, drafts, samplings=None, step0=None, want_logits: bool = False):
+        """cl_decode_verify_batch: one verify pass over several sequences; drafts[i] (0..15 ids) follow input_ids[i].
+        samplings (None, or one Sampling or None per sequence: greedy) and step0 as in decode_verify.  Returns (a list of the
+        emitted ids of every sequence, logits [sum(k_i + 1)][vocab] or None)."""
+        seqs = np.ascontiguousarray(seqs, dtype=np.int32)
+        x0 = np.ascontiguousarray(input_ids, dtype=np.int32)
+        ks = np.array([len(d) for d in drafts], np.int32)
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(d, np.int64) for d in drafts] + [np.zeros(1, np.int64)]), dtype=np.int32)
+        rows = int(ks.sum()) + len(seqs)
+        sp = None
+        if samplings is not None:
+            sp = (Sampling * len(seqs))(*[s if s is not None else greedy(-1) for s in samplings])
+        st = np.ascontiguousarray(step0 if step0 is not None else np.zeros(len(seqs)), dtype=np.uint64)
+        ids = np.empty(rows, np.int32)
+        n = np.zeros(len(seqs), np.int32)
+        out = np.empty((rows, self.cfg["vocab_size"]), np.float32) if want_logits else None
+        _check(lib().cl_decode_verify_batch(self._h, _ptr(seqs), len(seqs), _ptr(x0), _ptr(flat), _ptr(ks), sp, _ptr(st), _ptr(ids),
+                                            _ptr(n), _ptr(out) if want_logits else None), "cl_decode_verify_batch")
+        r0 = np.concatenate([[0], np.cumsum(ks + 1)])
+        return [ids[r0[i]:r0[i] + n[i]].copy() for i in range(len(seqs))], out
+
+    def set_speculate_batch(self, n: int):
+        """cl_engine_set_speculate_batch: how many running requests the scheduler may verify in one pass (1 = only a
+        request running alone)."""
+        _check(lib().cl_engine_set_speculate_batch(self._h, n), "cl_engine_set_speculate_batch")
 
     def seq_fake_fill(self, s: int, n_tokens: int):
         """Fill the sequence's paged KV (all layers) with the synthetic cache pattern the parity tests' CPU checker also
@@ -564,7 +598,13 @@ class Engine:
         """cl_engine_spec_stats: enabled, max_draft, verify_passes, tokens_drafted, tokens_accepted, tokens_emitted."""
         st = SpecStats()
         _check(lib().cl_engine_spec_stats(self._h, C.byref(st)), "cl_engine_spec_stats")
-        return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved"}
+        return {n: getattr(st, n) for n, _ in st._fields_ if n not in ("reserved", "multi_passes")}
+
+    def spec_multi_passes(self) -> int:
+        """cl_spec_stats.multi_passes: verify passes that checked two or more sequences at once."""
+        st = SpecStats()
+        _check(lib().cl_engine_spec_stats(self._h, C.byref(st)), "cl_engine_spec_stats")
+        return st.multi_passes
 
     def prefix_stats(self) -> dict:
         """cl_engine_prefix_stats: enabled, cached_pages, lookups, tokens_looked_up, tokens_reused, pages_evicted."""
@@ -644,6 +684,21 @@ def op_attn_decode_batch(q, k_cache_bf16, v_cache_bf16, ctx_lens, n_heads, n_kv,
                                          None if sl is None else _ptr(sl), B, n_slots, n_heads, n_kv, head_dim, page_size, _ptr(out),
                                          None if ob is None else _ptr(ob), C.byref(ns), C.byref(small)), "cl_op_attn_decode_batch")
     return out, ob, ns.value, small.value
+
+
+def op_attn_verify(q_bf16, k_cache_bf16, v_cache_bf16, ctx_lens, rows, n_heads, n_kv, head_dim, page_size=32, nsplit=0, device=0):
+    """cl_op_attn_verify: the multi-row split-KV attention of a verify pass.  q [sum(rows)][H*D] bf16; k/v caches
+    [sum(ctx_lens + rows)][n_kv][D] bf16, the segments back to back.  Returns (out [sum(rows)][H*D] bf16 as uint16, splits)."""
+    q = np.ascontiguousarray(q_bf16, dtype=np.uint16)
+    kc = np.ascontiguousarray(k_cache_bf16, dtype=np.uint16)
+    vc = np.ascontiguousarray(v_cache_bf16, dtype=np.uint16)
+    lens = np.ascontiguousarray(ctx_lens, dtype=np.int32)
+    rw = np.ascontiguousarray(rows, dtype=np.int32)
+    out = np.empty((int(rw.sum()), n_heads * head_dim), np.uint16)
+    ns = C.c_int32()
+    _check(lib().cl_op_attn_verify(device, _ptr(q), _ptr(kc), _ptr(vc), _ptr(lens), _ptr(rw), len(lens), n_heads, n_kv, head_dim,
+                                   page_size, nsplit, _ptr(out), C.byref(ns)), "cl_op_attn_verify")
+    return out, ns.value
 
 
 def op_qkv_rope_append(w_qkv_bf16, h, gain, eps, n_heads, n_kv, head_dim, pos, rope_theta, variant=0, device=0):

@@ -176,11 +176,12 @@ typedef struct cl_prefix_stats {
 typedef struct cl_spec_stats {
   int32_t enabled;           /* the scheduler and the synchronous path speculate */
   int32_t max_draft;         /* most drafted tokens per verify pass */
-  int64_t verify_passes;     /* verify passes run (cl_decode_verify calls included) */
+  int64_t verify_passes;     /* sequences verified: a pass over n sequences counts n (cl_decode_verify[_batch] calls included) */
   int64_t tokens_drafted;    /* drafted tokens they checked */
   int64_t tokens_accepted;   /* of which accepted */
   int64_t tokens_emitted;    /* tokens they emitted: tokens_accepted + verify_passes */
-  int64_t reserved[4];
+  int64_t multi_passes;      /* passes that verified two or more sequences at once (cl_engine_set_speculate_batch) */
+  int64_t reserved[3];
 } cl_spec_stats;
 
 typedef struct cl_engine cl_engine;
@@ -213,6 +214,13 @@ int cl_engine_model_config(const cl_engine* e, cl_model_config* out);
 int cl_engine_stats(cl_engine* e, cl_stats* out);
 int cl_engine_prefix_stats(cl_engine* e, cl_prefix_stats* out);
 int cl_engine_spec_stats(cl_engine* e, cl_spec_stats* out);
+/* How many running requests the scheduler may verify in one pass (speculative decoding, cl_engine_config.speculate > 0).
+ * n = 1 (the default): a request speculates only while it runs alone.  n >= 2: while 2 .. n requests are running, nothing
+ * waits or is being prefilled, every one of them is greedy or device-sampled and at least one has a draft, each drafts as
+ * it would alone and one pass over the weights verifies all of them (cl_decode_verify_batch); otherwise they take batched
+ * steps.  n: 1 .. min(max_batch, 32), else CL_ERR_INVALID_ARG.  Env CL_SPECULATE_BATCH sets it at cl_engine_create (an
+ * invalid value makes the create fail with CL_ERR_INVALID_ARG). */
+int cl_engine_set_speculate_batch(cl_engine* e, int32_t n);
 /* Overwrite one weight tensor from host memory (bf16 bits, logical [out][in] row-major; norm
  * gains as bf16 too).  kind: 0 embed, 1 lm_head, 2 final_norm, 3 attn_norm, 4 wq, 5 wk, 6 wv,
  * 7 wo, 8 ffn_norm, 9 w_gate, 10 w_up, 11 w_down (same numbering as the synthetic generator).
@@ -325,6 +333,20 @@ int cl_decode_step_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, con
  * model shape without the verify path; CL_ERR_TOO_LONG past max_seq_len. */
 int cl_decode_verify(cl_engine* e, cl_seq_t seq, int32_t input_id, const int32_t* draft, int32_t k, const cl_sampling* sp,
                      uint64_t step0, int32_t* ids_out, int32_t* n_out, float* logits_out);
+/* Speculative decoding, token level: one verify pass over n_seqs distinct sequences, so that one pass over the weights
+ * checks the drafts of all of them.  Sequence seqs[i] has the contract of cl_decode_verify with input_ids[i], its ks[i]
+ * drafts (0 <= ks[i] <= 15; the drafts of all sequences back to back in `drafts`), sp[i] and step0[i] (sp and step0 may be
+ * NULL: greedy, step 0).  ks[i] = 0 is allowed: the sequence then advances by exactly the one id a decode step would choose.
+ * Its rows are r0_i .. r0_i + ks[i], r0_i = the sum of ks[j] + 1 over j < i, at most 128 rows in all:
+ *   - ids_out [rows]: the emitted ids of sequence i start at ids_out + r0_i; n_out[i] = their count (a_i + 1).
+ *   - logits_out (host, may be NULL): [rows][vocab_size].
+ * Each sequence's ids, logits and K/V are those of the same call with that sequence alone.  CL_ERR_INVALID_ARG for a
+ * duplicate sequence, k outside 0..15, more than 128 rows, an id out of range, settings that need the host sampler or a
+ * model shape without the verify path; CL_ERR_TOO_LONG if a sequence would pass max_seq_len.  On an error no sequence's
+ * length changes. */
+int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* input_ids, const int32_t* drafts,
+                           const int32_t* ks, const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int32_t* n_out,
+                           float* logits_out);
 /* Parity aid: make the sequence hold n_tokens cached tokens whose K/V, in every layer, are the CPU oracle's
  * synthetic cache pattern (oracle/llama_oracle.c oc_seq_fake_fill: k[i] = (((i * 2654435761) >> 24 & 255) - 128) / 128,
  * v[i] = (((i * 40503) >> 8 & 255) - 128) / 128 with i = token * n_kv * head_dim + head * head_dim + dim; exact in
@@ -386,6 +408,17 @@ int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_
                             const uint16_t* v_cache, const int32_t* ctx_lens, const int32_t* slots, int32_t batch, int32_t n_slots,
                             int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, float* out, uint16_t* out_bf16,
                             int32_t* nsplit_used, int32_t* tc_small_used);
+/* The multi-row split-KV attention of a verify pass over several sequences (cl_decode_verify_batch): segment s has
+ * ctx_lens[s] cached tokens and rows[s] (1..16) new query rows at positions ctx_lens[s] .. ctx_lens[s] + rows[s] - 1; row r
+ * sees keys < ctx_lens[s] + r + 1.  q [sum(rows)][n_heads * head_dim] bf16 (roped), the segments' rows back to back;
+ * k/v caches [sum(ctx_lens + rows)][n_kv][head_dim] bf16, the segments back to back, paged by the engine's rules into a
+ * scrambled pool.  out [sum(rows)][n_heads * head_dim] bf16.  nsplit 0: the engine's split plan (every split 8 pages),
+ * else every segment spreads its pages over nsplit (1..64) splits; *nsplit_used (may be NULL) = the grid's splits.  The
+ * kernel launches twice without re-arming its split counters and the call fails with CL_ERR_INTERNAL if the two outputs
+ * differ in any bit.  Shapes: head_dim 128, 4 query heads per kv head, page 32; others return CL_ERR_INVALID_ARG. */
+int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, const uint16_t* v_cache, const int32_t* ctx_lens,
+                      const int32_t* rows, int32_t n_segs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit,
+                      uint16_t* out, int32_t* nsplit_used);
 /* prefill GEMM on the tensor cores (wgmma): Y[t][n] = sum_k X[t][k] W[n][k]; X,W bf16, Y fp32 */
 int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, int32_t t,
                     int32_t n, int32_t k, int32_t iters, float* ms);
