@@ -135,6 +135,11 @@ int cl_engine_spec_stats(cl_engine* e, cl_spec_stats* out) {
   return e->impl.spec_stats(out);   // atomics only, no engine lock
 }
 
+int cl_engine_set_prefix_host_cache(cl_engine* e, int64_t bytes) {
+  if (!e) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  return e->impl.set_prefix_host_cache(bytes);
+}
 int cl_engine_set_speculate_batch(cl_engine* e, int32_t n) {
   if (!e) return CL_ERR_INVALID_ARG;
   return e->impl.set_speculate_batch(n);   // an atomic the scheduler reads once per iteration, no engine lock
@@ -571,6 +576,31 @@ int cl_kvpool_cached_pages(cl_kvpool* p) {
   if (!p) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(p->mu);
   return p->pool.cached_pages();
+}
+int cl_kvpool_set_host_pages(cl_kvpool* p, int32_t n) {
+  if (!p) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(p->mu);
+  return p->pool.set_host_pages(n);
+}
+int cl_kvpool_take_moves(cl_kvpool* p, int32_t* moves, int32_t cap, int32_t* n_out) {
+  if (!p || !n_out) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(p->mu);
+  const auto& mv = p->pool.moves();
+  *n_out = (int32_t)mv.size();
+  if (!moves) return CL_OK;
+  if (cap < (int32_t)mv.size()) return CL_ERR_INVALID_ARG;
+  for (size_t i = 0; i < mv.size(); ++i) {
+    moves[3 * i] = mv[i].kind;
+    moves[3 * i + 1] = mv[i].page;
+    moves[3 * i + 2] = mv[i].host;
+  }
+  p->pool.clear_moves();
+  return CL_OK;
+}
+int cl_kvpool_host_cached_pages(cl_kvpool* p) {
+  if (!p) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(p->mu);
+  return p->pool.host_cached_pages();
 }
 
 }  // extern "C"

@@ -8,6 +8,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <set>
 
 #include <sys/stat.h>
 
@@ -35,6 +36,7 @@ Engine::~Engine() {
   if (step_done_ev_) cudaEventDestroy(step_done_ev_);
   for (void* p : allocs_) cudaFree(p);
   if (h_logits_pinned_) cudaFreeHost(h_logits_pinned_);
+  if (host_kv_) cudaFreeHost(host_kv_);
   if (h_ids_pinned_) cudaFreeHost(h_ids_pinned_);
   if (ev0_) cudaEventDestroy(ev0_);
   if (ev1_) cudaEventDestroy(ev1_);
@@ -194,6 +196,10 @@ int Engine::init(const cl_engine_config& c) {
   }
   if (const char* v = getenv("CL_SPECULATE_BATCH")) {
     if (set_speculate_batch(atoi(v))) return CL_ERR_INVALID_ARG;
+  }
+  if (const char* v = getenv("CL_PREFIX_CACHE_HOST_MIB")) {
+    const int rc = set_prefix_host_cache(atoll(v) * (1LL << 20));
+    if (rc) return rc;
   }
   if (c.start_scheduler) start_scheduler();
   return CL_OK;
@@ -440,6 +446,7 @@ int Engine::ensure_capacity(cl_seq_t s, int n_tokens) {
   const size_t before = pool_->pages_of(s).size();
   const int rc = pool_->reserve(s, n_tokens);
   if (rc) { set_last_error("KV page pool exhausted"); return rc; }
+  if (const int mrc = drain_kv_moves()) return mrc;
   const auto& pages = pool_->pages_of(s);
   if (pages.size() != before)
     CL_CUDA_OK(cudaMemcpyAsync(d_bt_ + (size_t)s * max_pages_per_seq_ + before, pages.data() + before,
@@ -463,6 +470,7 @@ int Engine::attach_prefix(cl_seq_t s, const int32_t* ids, int n, int* reused) {
   auto& q = seqs_[s];
   if (q.len != 0 || !pool_->pages_of(s).empty()) { set_last_error("attach_prefix needs a new sequence (no tokens, no pages)"); return CL_ERR_INVALID_ARG; }
   const int r = pool_->attach(s, ids, std::min(n, cfg.max_seq_len));   // >= 0: the owner has no pages
+  if (const int mrc = drain_kv_moves()) return mrc;
   prefix_lookups_++;
   prefix_tokens_looked_up_ += n;
   prefix_tokens_reused_ += r;
@@ -484,6 +492,71 @@ int Engine::prefix_stats(cl_prefix_stats* out) {
   out->tokens_looked_up = prefix_tokens_looked_up_;
   out->tokens_reused = prefix_tokens_reused_;
   out->pages_evicted = pool_ ? pool_->evicted_pages() : 0;
+  if (pool_) {
+    out->host_pages = pool_->host_pages();
+    out->host_pages_cached = pool_->host_cached_pages();
+    out->pages_to_host = pool_->pages_to_host();
+    out->pages_from_host = pool_->pages_from_host();
+  }
+  return CL_OK;
+}
+
+int Engine::set_prefix_host_cache(int64_t bytes) {
+  const int64_t page_bytes = 2LL * (int64_t)kv_layer_elems_ / n_pages_ * cfg.n_layers * 2;   // K and V of every layer
+  if (bytes < 0 || (bytes > 0 && bytes < page_bytes)) { set_last_error("prefix host cache: bytes must be 0 or at least one page"); return CL_ERR_INVALID_ARG; }
+  if (!prefix_cache_) { set_last_error("prefix host cache needs the prefix cache"); return CL_ERR_INVALID_ARG; }
+  bool busy = std::any_of(seqs_.begin(), seqs_.end(), [](const SeqState& q) { return q.live; });
+  {
+    std::lock_guard<std::mutex> lk(q_mu_);
+    busy = busy || !queue_.empty() || !active_.empty() || prefilling_;
+  }
+  if (busy) { set_last_error("prefix host cache can only be resized with no sequence live or queued"); return CL_ERR_INVALID_ARG; }
+  const int64_t n = bytes / page_bytes;
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  pool_->set_host_pages(0);   // no moves are pending: every reserve and attach drains its own
+  if (host_kv_) {
+    CL_CUDA_OK(cudaFreeHost(host_kv_));
+    host_kv_ = nullptr;
+  }
+  if (n == 0) return CL_OK;
+  if (!d_moves_) DMALLOC(d_moves_, (size_t)2 * n_pages_ * sizeof(int2));
+  void* h = nullptr;
+  if (n > INT32_MAX || cudaHostAlloc(&h, (size_t)(n * page_bytes), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
+    cudaGetLastError();
+    set_last_error("prefix host cache: cannot pin " + std::to_string(n * page_bytes) + " bytes of host memory");
+    return CL_ERR_OOM;
+  }
+  host_kv_ = static_cast<uint4*>(h);
+  pool_->set_host_pages((int)n);
+  return CL_OK;
+}
+
+int Engine::drain_kv_moves() {
+  const auto& mv = pool_->moves();
+  if (mv.empty()) return CL_OK;   // always so with the host tier off
+  std::vector<int2> buf(mv.size());
+  for (size_t i = 0; i < mv.size(); ++i) buf[i] = make_int2(mv[i].page, mv[i].host);
+  CL_CUDA_OK(cudaMemcpyAsync(d_moves_, buf.data(), buf.size() * sizeof(int2), cudaMemcpyHostToDevice, stream_));
+  KvMoveArgs a;
+  a.kpool = kpool_; a.vpool = vpool_; a.layer_elems = kv_layer_elems_; a.host = host_kv_; a.n_layers = cfg.n_layers;
+  a.blk_vec = (int)(kv_layer_elems_ / n_pages_ * 2 / 16);
+  int launches = 0;
+  LaunchProfiler prof(stream_, nullptr);
+  // one launch per run of same-kind moves in which no device page and no host page repeats
+  std::set<int> pages, hosts;
+  size_t i0 = 0;
+  for (size_t i = 0; i <= mv.size(); ++i) {
+    if (i < mv.size() && mv[i].kind == mv[i0].kind && pages.insert(mv[i].page).second && hosts.insert(mv[i].host).second) continue;
+    a.moves = d_moves_ + i0;
+    a.n_moves = (int)(i - i0);
+    CL_LAUNCH(launch_kv_move(mv[i0].kind == KvPool::kSpill, a, stream_));
+    if (i == mv.size()) break;
+    pages = {mv[i].page};
+    hosts = {mv[i].host};
+    i0 = i;
+  }
+  launches_ += launches;
+  pool_->clear_moves();
   return CL_OK;
 }
 

@@ -97,17 +97,32 @@ class LaunchProfiler {
 // once the free list is empty.  Attached pages are read-only for their owners: every kernel writes K/V only at positions
 // >= the sequence's length, and attach() leaves at least one token of the prompt to compute.  Without attach / publish
 // the allocator hands out exactly the pages it always did.
+//
+// Host tier (set_host_pages(H), H > 0): an index entry lives on a device page or on one of H host pages, each holding one
+// device page's K and V of every layer.  Evicting a cached device page then moves its entry to a free host page (a spill)
+// instead of erasing it; with no host page free, the host LRU front is dropped first (deepest page of a chain first, as
+// release orders them).  attach() walks the chain as before and gives every host entry on it a device page, from the free
+// list or by evicting the device LRU (which may spill in turn), and frees the host page (a fill).  Before making room it
+// references the chain's device entries and takes its host entries off the host LRU, so it never evicts or drops its own
+// chain; it takes the longest prefix whose host entries can all get a device page now.  Every spill and fill is recorded
+// as a Move, in decision order, and the caller must execute the moves in exactly that order before anything reads or
+// writes the pages involved: a device page may be spilled and then filled in one call, and a host page freed by a fill
+// may be reused by a later spill of the same call.  A spill run may also name one host page twice (the entry spilled
+// first was dropped again to make room), so moves of one kind run concurrently only while no page repeats.
 class KvPool {
  public:
   static constexpr uint64_t kRootUid = 0;
+  enum MoveKind { kSpill = 0, kFill = 1 };
+  struct Move { int kind, page, host; };   // kSpill: device page -> host page; kFill: host page -> device page
   KvPool(int n_pages, int page_size);
   int reserve(int owner, int n_tokens);  // CL_OK / CL_ERR_OOM (atomic: nothing taken on failure); evicts cached pages last
   int release(int owner);                // published pages whose refcount drops to 0 become cached, the rest free
   // Only on an owner without pages: takes the longest indexed chain matching ids[0..n), at most P * floor((n - 1) / P)
-  // tokens.  Returns the tokens reused (>= 0) or CL_ERR_INVALID_ARG.
+  // tokens (host-tier entries only as far as device pages can be found for them).  Returns the tokens reused (>= 0) or
+  // CL_ERR_INVALID_ARG.
   int attach(int owner, const int32_t* ids, int n);
   // Tokens attach() would reuse, without taking anything; *cached_pages (may be nullptr): how many of the matching pages
-  // are cached (attaching them takes them out of free_pages()).
+  // are cached on the device or held by the host tier (attaching either takes a page out of free_pages()).
   int lookup(const int32_t* ids, int n, int* cached_pages) const;
   // Index the owner's full pages covering ids[0..n_known) not published yet.  A page whose key is already indexed stays private.
   int publish(int owner, const int32_t* ids, int n_known);
@@ -118,6 +133,14 @@ class KvPool {
   int64_t evicted_pages() const { return evicted_; }
   int n_pages() const { return n_pages_; }
   int page_size() const { return page_size_; }
+  // Host tier of n pages (0: off).  Drops every entry the tier held.  CL_ERR_INVALID_ARG for n < 0 or while moves are pending.
+  int set_host_pages(int n);
+  int host_pages() const { return host_n_; }
+  int host_cached_pages() const { return host_n_ - (int)host_free_.size(); }
+  int64_t pages_to_host() const { return to_host_; }
+  int64_t pages_from_host() const { return from_host_; }
+  const std::vector<Move>& moves() const { return moves_; }   // recorded since the last clear_moves(), in order
+  void clear_moves() { moves_.clear(); }
 
  private:
   struct Key {
@@ -125,22 +148,33 @@ class KvPool {
     std::vector<int32_t> ids;
     bool operator<(const Key& o) const { return parent != o.parent ? parent < o.parent : ids < o.ids; }
   };
+  struct Entry { int loc; uint64_t uid; };   // loc >= 0: device page; loc < 0: host page ~loc
+  using Index = std::map<Key, Entry>;
   struct Chain { int published = 0; uint64_t tail = kRootUid; };   // leading pages indexed (or matched), uid of the last
-  int walk(const int32_t* ids, int n, std::vector<int>* pages) const;
+  int walk(const int32_t* ids, int n, std::vector<int>* locs) const;   // the chain's entry locations
+  int take_page();        // a free page, else the device LRU front, evicted (spilled when a host page can be had)
+  int take_host_page();   // a free host page, else the host LRU front, dropped; -1 when there is none
   int n_pages_, page_size_;
   std::vector<int> free_;  // stack; low page ids are handed out first
   std::map<int, std::vector<int>> owned_;
   std::vector<int> empty_;
   // prefix sharing
-  std::map<Key, int> index_;                       // -> page
-  std::vector<std::map<Key, int>::iterator> entry_;   // page -> its index entry (index_.end(): not published)
-  std::vector<uint64_t> uid_;                      // page -> uid of its entry
+  Index index_;
+  std::vector<Index::iterator> entry_;             // page -> its index entry (index_.end(): not published)
   std::vector<int> ref_;                           // page -> owners holding it
   std::list<int> lru_;                             // cached pages, evicted from the front
   std::vector<std::list<int>::iterator> lru_pos_;
   std::map<int, Chain> chain_;
   uint64_t next_uid_ = kRootUid + 1;
   int64_t evicted_ = 0;
+  // host tier
+  int host_n_ = 0;
+  std::vector<int> host_free_;                     // stack; low host page ids first
+  std::vector<Index::iterator> host_entry_;        // host page -> its index entry (index_.end(): free)
+  std::list<int> host_lru_;                        // host pages holding an entry, dropped from the front
+  std::vector<std::list<int>::iterator> host_lru_pos_;
+  std::vector<Move> moves_;
+  int64_t to_host_ = 0, from_host_ = 0;
 };
 
 // ---- tokenizers ---------------------------------------------------------------------------------
@@ -251,6 +285,8 @@ class Engine {
   int attach_prefix(cl_seq_t s, const int32_t* ids, int n, int* reused);
   bool prefix_cache() const { return prefix_cache_; }
   int prefix_stats(cl_prefix_stats* out);
+  // Host tier of the prefix cache (contract in include/clengine.h, cl_engine_set_prefix_host_cache); callers hold mu_
+  int set_prefix_host_cache(int64_t bytes);
   int prefill(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
   // several prompts in one pass of the tile path (prefill.cu); logits_out: [n_seqs][vocab] or nullptr
   int prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* ids, const int* lens, float* logits_out);
@@ -317,6 +353,10 @@ class Engine {
   int fill_synthetic(uint64_t seed);
   int alloc_state();
   int ensure_capacity(cl_seq_t s, int n_tokens);  // reserve pages + upload block table row
+  // Enqueue the KvPool's pending spills and fills on stream_, in the order the pool decided them, and clear them.  Every
+  // call that reserves or attaches pages ends here, so the copies sit on the stream ahead of any kernel that writes an
+  // evicted page or reads an attached one.  Eager launches: never inside a captured graph.
+  int drain_kv_moves();
   // Every call that appends K/V to sequence s ends here: len += n, ids join the history, and with the prefix cache on the
   // full pages whose tokens are all known are published.  The first n_known ids are real tokens; a placeholder stops
   // publishing for the rest of the sequence.  The work that wrote the pages is already on stream_, ahead of any reader.
@@ -428,6 +468,8 @@ class Engine {
   int prefill_chunk_tokens_ = 4096;
 
   std::unique_ptr<KvPool> pool_;
+  uint4* host_kv_ = nullptr;          // host tier of the prefix cache: pinned, mapped pages (KvMoveArgs::host)
+  int2* d_moves_ = nullptr;           // the moves of one drain (at most 2 per pool page), uploaded for the transfer kernels
   std::vector<SeqState> seqs_;
   bool prefix_cache_ = false;         // share full KV pages across sequences with the same prefix (CL_PREFIX_CACHE)
   std::atomic<int64_t> prefix_lookups_{0}, prefix_tokens_looked_up_{0}, prefix_tokens_reused_{0};

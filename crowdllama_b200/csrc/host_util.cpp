@@ -19,9 +19,49 @@ KvPool::KvPool(int n_pages, int page_size) : n_pages_(n_pages), page_size_(page_
   free_.reserve(n_pages);
   for (int i = n_pages - 1; i >= 0; --i) free_.push_back(i);
   entry_.assign(n_pages, index_.end());
-  uid_.assign(n_pages, kRootUid);
   ref_.assign(n_pages, 0);
   lru_pos_.assign(n_pages, lru_.end());
+}
+int KvPool::take_host_page() {
+  int h;
+  if (!host_free_.empty()) {
+    h = host_free_.back();
+    host_free_.pop_back();
+  } else if (!host_lru_.empty()) {   // drop the least recently spilled entry
+    h = host_lru_.front();
+    host_lru_.pop_front();
+    host_lru_pos_[h] = host_lru_.end();
+    index_.erase(host_entry_[h]);
+    host_entry_[h] = index_.end();
+  } else {
+    return -1;
+  }
+  return h;
+}
+int KvPool::take_page() {
+  if (!free_.empty()) {
+    const int p = free_.back();
+    free_.pop_back();
+    return p;
+  }
+  // evict the least recently released cached page: its entry moves to a host page, or goes when there is none
+  const int p = lru_.front();
+  lru_.pop_front();
+  lru_pos_[p] = lru_.end();
+  const Index::iterator e = entry_[p];
+  entry_[p] = index_.end();
+  ++evicted_;
+  const int h = take_host_page();
+  if (h < 0) {
+    index_.erase(e);
+  } else {
+    e->second.loc = ~h;
+    host_entry_[h] = e;
+    host_lru_pos_[h] = host_lru_.insert(host_lru_.end(), h);
+    moves_.push_back(Move{kSpill, p, h});
+    ++to_host_;
+  }
+  return p;
 }
 int KvPool::reserve(int owner, int n_tokens) {
   auto& v = owned_[owner];
@@ -30,21 +70,22 @@ int KvPool::reserve(int owner, int n_tokens) {
   if (extra <= 0) return CL_OK;
   if (extra > free_pages()) return CL_ERR_OOM;
   for (int i = 0; i < extra; ++i) {
-    int p;
-    if (!free_.empty()) {
-      p = free_.back();
-      free_.pop_back();
-    } else {   // evict the least recently released cached page; its index entry goes with it
-      p = lru_.front();
-      lru_.pop_front();
-      lru_pos_[p] = lru_.end();
-      index_.erase(entry_[p]);
-      entry_[p] = index_.end();
-      ++evicted_;
-    }
+    const int p = take_page();
     ref_[p] = 1;
     v.push_back(p);
   }
+  return CL_OK;
+}
+int KvPool::set_host_pages(int n) {
+  if (n < 0 || !moves_.empty()) return CL_ERR_INVALID_ARG;
+  for (int h = 0; h < host_n_; ++h)
+    if (host_entry_[h] != index_.end()) index_.erase(host_entry_[h]);
+  host_n_ = n;
+  host_free_.clear();
+  for (int h = n - 1; h >= 0; --h) host_free_.push_back(h);
+  host_entry_.assign(n, index_.end());
+  host_lru_.clear();
+  host_lru_pos_.assign(n, host_lru_.end());
   return CL_OK;
 }
 int KvPool::release(int owner) {
@@ -61,35 +102,67 @@ int KvPool::release(int owner) {
   owned_.erase(it);
   return CL_OK;
 }
-int KvPool::walk(const int32_t* ids, int n, std::vector<int>* pages) const {
+int KvPool::walk(const int32_t* ids, int n, std::vector<int>* locs) const {
   const int max_pages = n > 1 ? (n - 1) / page_size_ : 0;   // at least one token is left to compute
   Key key{kRootUid, {}};
   for (int k = 0; k < max_pages; ++k) {
     key.ids.assign(ids + (size_t)k * page_size_, ids + (size_t)(k + 1) * page_size_);
     auto it = index_.find(key);
     if (it == index_.end()) break;
-    pages->push_back(it->second);
-    key.parent = uid_[it->second];
+    locs->push_back(it->second.loc);
+    key.parent = it->second.uid;
   }
-  return (int)pages->size() * page_size_;
+  return (int)locs->size() * page_size_;
 }
 int KvPool::lookup(const int32_t* ids, int n, int* cached_pages) const {
-  std::vector<int> pages;
-  const int tokens = walk(ids, n, &pages);
-  if (cached_pages) *cached_pages = (int)std::count_if(pages.begin(), pages.end(), [&](int p) { return ref_[p] == 0; });
+  std::vector<int> locs;
+  const int tokens = walk(ids, n, &locs);
+  if (cached_pages) *cached_pages = (int)std::count_if(locs.begin(), locs.end(), [&](int l) { return l < 0 || ref_[l] == 0; });
   return tokens;
 }
 int KvPool::attach(int owner, const int32_t* ids, int n) {
   auto& v = owned_[owner];
   if (!v.empty()) return CL_ERR_INVALID_ARG;
-  const int tokens = walk(ids, n, &v);
-  for (int p : v)
-    if (ref_[p]++ == 0) {   // cached -> referenced
-      lru_.erase(lru_pos_[p]);
-      lru_pos_[p] = lru_.end();
+  std::vector<int> locs;
+  walk(ids, n, &locs);
+  // the longest prefix whose host entries can all get a device page now: each takes one of the allocatable pages, and
+  // each cached device entry leaves the LRU, so it is no longer one of them
+  size_t k = 0;
+  for (int avail = free_pages(); k < locs.size(); ++k) {
+    const int l = locs[k];
+    if (l < 0 || ref_[l] == 0) {
+      if (avail == 0) break;
+      --avail;
     }
-  chain_[owner] = Chain{(int)v.size(), v.empty() ? kRootUid : uid_[v.back()]};
-  return tokens;
+  }
+  locs.resize(k);
+  for (int l : locs) {
+    if (l >= 0 && ref_[l]++ == 0) {   // cached -> referenced
+      lru_.erase(lru_pos_[l]);
+      lru_pos_[l] = lru_.end();
+    } else if (l < 0) {               // off the host LRU: making room below must not drop it
+      host_lru_.erase(host_lru_pos_[~l]);
+      host_lru_pos_[~l] = host_lru_.end();
+    }
+  }
+  for (int l : locs) {
+    if (l >= 0) {
+      v.push_back(l);
+      continue;
+    }
+    const int h = ~l, p = take_page();
+    const Index::iterator e = host_entry_[h];
+    host_entry_[h] = index_.end();
+    e->second.loc = p;
+    entry_[p] = e;
+    ref_[p] = 1;
+    moves_.push_back(Move{kFill, p, h});
+    ++from_host_;
+    host_free_.push_back(h);
+    v.push_back(p);
+  }
+  chain_[owner] = Chain{(int)v.size(), v.empty() ? kRootUid : entry_[v.back()]->second.uid};
+  return (int)v.size() * page_size_;
 }
 int KvPool::publish(int owner, const int32_t* ids, int n_known) {
   auto it = owned_.find(owner);
@@ -100,12 +173,11 @@ int KvPool::publish(int owner, const int32_t* ids, int n_known) {
     Key key{c.tail, std::vector<int32_t>(ids + (size_t)k * page_size_, ids + (size_t)(k + 1) * page_size_)};
     auto f = index_.find(key);
     if (f != index_.end()) {   // the same tokens are indexed on another page: this one stays private, the chain goes on there
-      c.tail = uid_[f->second];
+      c.tail = f->second.uid;
     } else {
       const int p = v[k];
-      entry_[p] = index_.emplace(std::move(key), p).first;
-      uid_[p] = next_uid_++;
-      c.tail = uid_[p];
+      entry_[p] = index_.emplace(std::move(key), Entry{p, next_uid_++}).first;
+      c.tail = entry_[p]->second.uid;
     }
     c.published = k + 1;
   }

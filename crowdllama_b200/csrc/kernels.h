@@ -146,6 +146,22 @@ int launch_bf16_to_f32(const __nv_bfloat16* in, float* out, int64_t n, cudaStrea
 int launch_fake_fill_kv(__nv_bfloat16* kpool, __nv_bfloat16* vpool, size_t layer_elems, int n_layers, const int* block_table,
                         int page_size, int n_kv, int head_dim, int n_tokens, cudaStream_t st);
 
+// Host tier of the prefix cache (kv_host.cu): copies of whole pages, every layer's K and V, between the pool and pinned,
+// mapped host pages.  to_host: kv_spill_kernel (pool -> host), else kv_fill_kernel (host -> pool).  One launch copies
+// n_moves pages; no page, device or host, may appear twice in one launch.  Never launched with PDL, and neither kernel
+// triggers its dependents early.
+struct KvMoveArgs {
+  const int2* moves = nullptr;       // [n_moves] (device page, host page), device memory
+  int n_moves = 0;
+  __nv_bfloat16* kpool = nullptr;    // [n_layers][n_pages][n_kv][page][head_dim]
+  __nv_bfloat16* vpool = nullptr;
+  size_t layer_elems = 0;            // elements of one layer of the pool
+  uint4* host = nullptr;             // device view of the host pages: [host page][K|V][n_layers][n_kv][page][head_dim]
+  int n_layers = 0;
+  int blk_vec = 0;                   // one page of one layer (n_kv * page * head_dim bf16) in 16-byte units
+};
+int launch_kv_move(bool to_host, const KvMoveArgs& a, cudaStream_t st);
+
 int launch_gather_kv(const __nv_bfloat16* pool_layer, const int* block_table, int page_size, int n_kv, int head_dim, int t0, int n,
                      float* out, cudaStream_t st);
 

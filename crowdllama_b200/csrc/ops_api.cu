@@ -302,6 +302,102 @@ int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_
   return CL_OK;
 }
 
+int cl_op_kv_host_roundtrip(int device, int32_t n_layers, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t n_moves,
+                            int32_t iters, float* ms) {
+  if (n_layers <= 0 || n_kv <= 0 || n_moves <= 0 || iters < 0 || (head_dim != 64 && head_dim != 128) ||
+      (page_size != 16 && page_size != 32 && page_size != 64)) {
+    set_last_error("cl_op_kv_host_roundtrip: unsupported shape");
+    return CL_ERR_INVALID_ARG;
+  }
+  int rc = check_device(device);
+  if (rc) return rc;
+  // pool of 2 n + 2 pages, scattered: the n spilled pages hold random bits, their n destinations and two pages nothing
+  // names the largest finite bf16 (+ for K, - for V), so a block copied short, to the wrong place or not at all shows
+  const int n = n_moves, n_pages = 2 * n + 2;
+  const size_t blk = (size_t)n_kv * page_size * head_dim, layer_elems = (size_t)n_pages * blk;
+  std::vector<int> perm(n_pages);
+  std::iota(perm.begin(), perm.end(), 0);
+  std::shuffle(perm.begin(), perm.end(), std::mt19937(0x5eed));
+  std::vector<int2> spill(n), fill(n);
+  for (int i = 0; i < n; ++i) {
+    spill[i] = make_int2(perm[2 * i], n - 1 - i);   // host pages in the other order
+    fill[i] = make_int2(perm[2 * i + 1], n - 1 - i);
+  }
+  const size_t pool_elems = (size_t)n_layers * layer_elems;
+  std::vector<uint16_t> k(pool_elems, 0x7F7F), v(pool_elems, 0xFF7F);
+  std::mt19937 rng(0xc0ffee);
+  for (int i = 0; i < n; ++i)
+    for (int l = 0; l < n_layers; ++l)
+      for (size_t e = 0; e < blk; ++e) {
+        const size_t at = l * layer_elems + (size_t)spill[i].x * blk + e;
+        k[at] = (uint16_t)rng();
+        v[at] = (uint16_t)rng();
+      }
+  DevBuf dk, dv, dmv;
+  CL_CUDA_OK(dk.upload(k.data(), pool_elems * 2));
+  CL_CUDA_OK(dv.upload(v.data(), pool_elems * 2));
+  std::vector<int2> moves(spill);
+  moves.insert(moves.end(), fill.begin(), fill.end());
+  CL_CUDA_OK(dmv.upload(moves.data(), moves.size() * sizeof(int2)));
+  const size_t host_bytes = (size_t)n * 2 * n_layers * blk * 2;
+  void* host = nullptr;
+  CL_CUDA_OK(cudaHostAlloc(&host, host_bytes, cudaHostAllocMapped | cudaHostAllocPortable));
+  struct HostFree { void* p; ~HostFree() { cudaFreeHost(p); } } host_guard{host};
+  memset(host, 0xff, host_bytes);
+  KvMoveArgs a;
+  a.n_moves = n; a.kpool = dk.as<__nv_bfloat16>(); a.vpool = dv.as<__nv_bfloat16>(); a.layer_elems = layer_elems;
+  a.host = static_cast<uint4*>(host); a.n_layers = n_layers; a.blk_vec = (int)(blk * 2 / 16);
+  KvMoveArgs f = a;
+  a.moves = dmv.as<int2>();
+  f.moves = dmv.as<int2>() + n;
+  if (launch_kv_move(true, a, nullptr) < 0 || launch_kv_move(false, f, nullptr) < 0) {
+    CL_CUDA_OK(cudaGetLastError());
+    return CL_ERR_CUDA;
+  }
+  CL_CUDA_OK(cudaDeviceSynchronize());
+  std::vector<uint16_t> k2(pool_elems), v2(pool_elems);
+  CL_CUDA_OK(cudaMemcpy(k2.data(), dk.p, pool_elems * 2, cudaMemcpyDeviceToHost));
+  CL_CUDA_OK(cudaMemcpy(v2.data(), dv.p, pool_elems * 2, cudaMemcpyDeviceToHost));
+  // expected: every destination page equals its source, every other page is unchanged, host page h = [K|V][layer] blocks
+  std::vector<uint16_t> kw(k), vw(v);
+  const uint16_t* hp = static_cast<const uint16_t*>(host);
+  bool host_ok = true;
+  for (int i = 0; i < n; ++i)
+    for (int l = 0; l < n_layers; ++l) {
+      const size_t src = l * layer_elems + (size_t)spill[i].x * blk, dst = l * layer_elems + (size_t)fill[i].x * blk;
+      memcpy(&kw[dst], &k[src], blk * 2);
+      memcpy(&vw[dst], &v[src], blk * 2);
+      const size_t h = (size_t)spill[i].y * 2 * n_layers;
+      host_ok = host_ok && !memcmp(hp + (h + l) * blk, &k[src], blk * 2) && !memcmp(hp + (h + n_layers + l) * blk, &v[src], blk * 2);
+    }
+  if (!host_ok || k2 != kw || v2 != vw) {
+    set_last_error(std::string("cl_op_kv_host_roundtrip: ") + (host_ok ? "the pool" : "a host page") + " differs from the expected bytes");
+    return CL_ERR_INTERNAL;
+  }
+  if (iters > 0 && ms) {
+    cudaEvent_t e0, e1, e2;
+    CL_CUDA_OK(cudaEventCreate(&e0));
+    CL_CUDA_OK(cudaEventCreate(&e1));
+    CL_CUDA_OK(cudaEventCreate(&e2));
+    CL_CUDA_OK(cudaEventRecord(e0, nullptr));
+    for (int i = 0; i < iters; ++i) launch_kv_move(true, a, nullptr);
+    CL_CUDA_OK(cudaEventRecord(e1, nullptr));
+    for (int i = 0; i < iters; ++i) launch_kv_move(false, f, nullptr);
+    CL_CUDA_OK(cudaEventRecord(e2, nullptr));
+    CL_CUDA_OK(cudaEventSynchronize(e2));
+    CL_CUDA_OK(cudaGetLastError());
+    float t0 = 0.f, t1 = 0.f;
+    CL_CUDA_OK(cudaEventElapsedTime(&t0, e0, e1));
+    CL_CUDA_OK(cudaEventElapsedTime(&t1, e1, e2));
+    ms[0] = t0 / (float)iters;
+    ms[1] = t1 / (float)iters;
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    cudaEventDestroy(e2);
+  }
+  return CL_OK;
+}
+
 int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, const uint16_t* v_cache, const int32_t* ctx_lens,
                       const int32_t* rows, int32_t n_segs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit,
                       uint16_t* out, int32_t* nsplit_used) {

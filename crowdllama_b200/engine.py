@@ -66,7 +66,8 @@ class Stats(C.Structure):
 
 class PrefixStats(C.Structure):
     _fields_ = [("enabled", C.c_int32), ("cached_pages", C.c_int32), ("lookups", C.c_int64), ("tokens_looked_up", C.c_int64),
-                ("tokens_reused", C.c_int64), ("pages_evicted", C.c_int64), ("reserved", C.c_int64 * 4)]
+                ("tokens_reused", C.c_int64), ("pages_evicted", C.c_int64), ("host_pages", C.c_int64), ("host_pages_cached", C.c_int64),
+                ("pages_to_host", C.c_int64), ("pages_from_host", C.c_int64)]
 
 
 class SpecStats(C.Structure):
@@ -79,15 +80,16 @@ class SpecStats(C.Structure):
 EXPORTS = [
     "cl_abi_version", "cl_strerror", "cl_last_error", "cl_default_engine_config", "cl_default_sampling",
     "cl_greedy_sampling", "cl_sample_token", "cl_model_preset", "cl_engine_create", "cl_engine_destroy", "cl_engine_model_config",
-    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_engine_set_speculate_batch", "cl_draft_ngram", "cl_decode_verify", "cl_decode_verify_batch", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
+    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_engine_set_speculate_batch", "cl_engine_set_prefix_host_cache", "cl_draft_ngram", "cl_decode_verify", "cl_decode_verify_batch", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
     "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
     "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
     "cl_op_attn_decode_batch", "cl_op_attn_verify", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
-    "cl_op_attn_prefill_cached", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
+    "cl_op_attn_prefill_cached", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
-    "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages",
+    "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages", "cl_kvpool_set_host_pages", "cl_kvpool_take_moves",
+    "cl_kvpool_host_cached_pages",
     "cl_tokenizer_load", "cl_tokenizer_free", "cl_tokenizer_encode", "cl_tokenizer_decode", "cl_tokenizer_info", "cl_engine_load_tokenizer",
 ]
 
@@ -126,6 +128,7 @@ def lib():
         "cl_draft_ngram": (C.c_int, [vp, i32, i32, vp, P(i32)]),
         "cl_decode_verify": (C.c_int, [vp, i32, i32, vp, i32, P(Sampling), u64, vp, P(i32), vp]),
         "cl_engine_set_speculate_batch": (C.c_int, [vp, i32]),
+        "cl_engine_set_prefix_host_cache": (C.c_int, [vp, i64]),
         "cl_decode_verify_batch": (C.c_int, [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
         "cl_engine_set_tensor": (C.c_int, [vp, i32, i32, vp, i64]),
         "cl_checkpoint_info": (C.c_int, [C.c_char_p, P(ModelConfig), P(i32), P(i64)]),
@@ -169,6 +172,7 @@ def lib():
         "cl_op_attn_prefill": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, vp]),
         "cl_op_attn_prefill_variant": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, vp, i32, P(f32)]),
         "cl_op_attn_prefill_cached": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+        "cl_op_kv_host_roundtrip": (C.c_int, [C.c_int, i32, i32, i32, i32, i32, i32, P(f32)]),
         "cl_op_sample": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), vp, vp, i32, vp, vp]),
         "cl_op_synth_weights": (C.c_int, [C.c_int, u64, i32, i64, f32, vp]),
         "cl_tokenizer_load": (C.c_int, [C.c_char_p, C.c_char_p, P(vp)]),
@@ -187,6 +191,9 @@ def lib():
         "cl_kvpool_attach": (C.c_int, [vp, i32, vp, i32, P(i32)]),
         "cl_kvpool_publish": (C.c_int, [vp, i32, vp, i32]),
         "cl_kvpool_cached_pages": (C.c_int, [vp]),
+        "cl_kvpool_set_host_pages": (C.c_int, [vp, i32]),
+        "cl_kvpool_take_moves": (C.c_int, [vp, vp, i32, P(i32)]),
+        "cl_kvpool_host_cached_pages": (C.c_int, [vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -292,7 +299,7 @@ class Engine:
                  device: int = 0, seed: int = 1234, max_batch: int = 8, max_seqs: int | None = None,
                  page_size: int = 32, kv_pool_bytes: int = 0, use_cuda_graph: bool = True, decode_path: int = 0,
                  start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False,
-                 speculate: int = 0, speculate_batch: int = 1):
+                 speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -322,6 +329,9 @@ class Engine:
         # requests verified in one pass; env CL_SPECULATE_BATCH overrides the argument, as CL_SPECULATE does `speculate`
         if speculate_batch != 1 and "CL_SPECULATE_BATCH" not in os.environ:
             self.set_speculate_batch(speculate_batch)
+        # host tier of the prefix cache; env CL_PREFIX_CACHE_HOST_MIB sizes it at create and overrides the argument
+        if prefix_cache_host_bytes and "CL_PREFIX_CACHE_HOST_MIB" not in os.environ:
+            self.set_prefix_host_cache(prefix_cache_host_bytes)
         mc = ModelConfig()
         _check(L.cl_engine_model_config(self._h, C.byref(mc)), "cl_engine_model_config")
         self.cfg = mc.as_dict()
@@ -469,6 +479,11 @@ class Engine:
         request running alone)."""
         _check(lib().cl_engine_set_speculate_batch(self._h, n), "cl_engine_set_speculate_batch")
 
+    def set_prefix_host_cache(self, nbytes: int):
+        """cl_engine_set_prefix_host_cache: pinned host memory behind the prefix cache (whole pages; 0 frees it).  Only with
+        the prefix cache on and no sequence live or queued."""
+        _check(lib().cl_engine_set_prefix_host_cache(self._h, nbytes), "cl_engine_set_prefix_host_cache")
+
     def seq_fake_fill(self, s: int, n_tokens: int):
         """Fill the sequence's paged KV (all layers) with the synthetic cache pattern the parity tests' CPU checker also
         generates (include/clengine.h: cl_seq_fake_fill) — a parity aid."""
@@ -606,11 +621,12 @@ class Engine:
         _check(lib().cl_engine_spec_stats(self._h, C.byref(st)), "cl_engine_spec_stats")
         return st.multi_passes
 
-    def prefix_stats(self) -> dict:
-        """cl_engine_prefix_stats: enabled, cached_pages, lookups, tokens_looked_up, tokens_reused, pages_evicted."""
+    def prefix_stats(self, host: bool = False) -> dict:
+        """cl_engine_prefix_stats: enabled, cached_pages, lookups, tokens_looked_up, tokens_reused, pages_evicted; with
+        host=True also the host tier's host_pages, host_pages_cached, pages_to_host and pages_from_host."""
         st = PrefixStats()
         _check(lib().cl_engine_prefix_stats(self._h, C.byref(st)), "cl_engine_prefix_stats")
-        return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved"}
+        return {n: getattr(st, n) for n, _ in st._fields_[:None if host else 6]}
 
 
 # ---- single-op wrappers (host numpy in / out) -----------------------------------------------------
@@ -800,6 +816,16 @@ def op_sample(logits, samplings, histories, steps, device=0):
     return out
 
 
+def op_kv_host_roundtrip(n_layers, n_kv, head_dim, page_size, n_moves, iters=0, device=0):
+    """cl_op_kv_host_roundtrip: spill n_moves pages of a scrambled pool to host pages and fill them into other pages; raises
+    unless the round trip is bit-exact and no other page changed.  Returns (spill ms, fill ms) per launch over `iters` timed
+    launches of each, or None when iters is 0."""
+    ms = (C.c_float * 2)()
+    _check(lib().cl_op_kv_host_roundtrip(device, n_layers, n_kv, head_dim, page_size, n_moves, iters, ms if iters else None),
+           "cl_op_kv_host_roundtrip")
+    return (ms[0], ms[1]) if iters else None
+
+
 def op_synth_weights(seed, key, n, scale, device=0):
     out = np.empty(n, np.uint16)
     _check(lib().cl_op_synth_weights(device, seed, key, n, scale, _ptr(out)), "cl_op_synth_weights")
@@ -901,3 +927,20 @@ class KvPool:
     @property
     def cached_pages(self) -> int:
         return lib().cl_kvpool_cached_pages(self._h)
+
+    def set_host_pages(self, n: int):
+        """Host tier of n pages (0: off); drops every entry it held."""
+        _check(lib().cl_kvpool_set_host_pages(self._h, n), "cl_kvpool_set_host_pages")
+
+    def take_moves(self):
+        """The spills (kind 0) and fills (kind 1) recorded since the last call, in order: a list of (kind, device page,
+        host page)."""
+        n = C.c_int32()
+        _check(lib().cl_kvpool_take_moves(self._h, None, 0, C.byref(n)), "cl_kvpool_take_moves")
+        a = np.empty((max(n.value, 1), 3), np.int32)
+        _check(lib().cl_kvpool_take_moves(self._h, _ptr(a), n.value, C.byref(n)), "cl_kvpool_take_moves")
+        return [tuple(int(x) for x in r) for r in a[:n.value]]
+
+    @property
+    def host_cached_pages(self) -> int:
+        return lib().cl_kvpool_host_cached_pages(self._h)

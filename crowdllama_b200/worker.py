@@ -74,9 +74,10 @@ class _Conn(socketserver.BaseRequestHandler):
 
 def serve(device: int, port: int, preset: str, model_name: str, max_batch: int = 8, greedy_tokens: int = 0, host="127.0.0.1",
           ready_event=None, seed: int = 1234, tokenizer: str | None = None, chat_family: str | None = None, prefix_cache: bool = False,
-          speculate: int = 0, speculate_batch: int = 1):
+          speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0):
     e = eng.Engine(preset=preset, model_name=model_name, device=device, seed=seed, max_batch=max_batch, start_scheduler=True,
-                   prefix_cache=prefix_cache, speculate=speculate, speculate_batch=speculate_batch)
+                   prefix_cache=prefix_cache, speculate=speculate, speculate_batch=speculate_batch,
+                   prefix_cache_host_bytes=prefix_cache_host_bytes)
     if tokenizer:
         e.load_tokenizer(tokenizer, chat_family)      # HF tokenizer.json instead of the byte-level fallback
     sampling = eng.greedy(greedy_tokens, ignore_eos=True) if greedy_tokens > 0 else None   # None = Ollama defaults
@@ -108,10 +109,16 @@ def main():
     ap.add_argument("--speculate-batch", type=int, default=1,
                     help="1..min(max_batch, 32): with --speculate, up to this many running requests verify their drafts in one "
                          "pass (1 = only a request running alone; env CL_SPECULATE_BATCH overrides)")
+    ap.add_argument("--prefix-cache-host-gib", type=float, default=0.0,
+                    help="with --prefix-cache: GiB of pinned host memory that keeps evicted cached KV pages for reuse "
+                         "(0 = off; env CL_PREFIX_CACHE_HOST_MIB overrides)")
     a = ap.parse_args()
+    if a.prefix_cache_host_gib and not a.prefix_cache:
+        ap.error("--prefix-cache-host-gib requires --prefix-cache")
     print(f"worker on cuda:{a.device} port {a.port} serving {a.model_name}", flush=True)
     serve(a.device, a.port, a.preset, a.model_name, a.max_batch, a.greedy_tokens, tokenizer=a.tokenizer, chat_family=a.chat_family,
-          prefix_cache=a.prefix_cache, speculate=a.speculate, speculate_batch=a.speculate_batch)
+          prefix_cache=a.prefix_cache, speculate=a.speculate, speculate_batch=a.speculate_batch,
+          prefix_cache_host_bytes=int(a.prefix_cache_host_gib * 2**30))
 
 
 if __name__ == "__main__":

@@ -96,7 +96,8 @@ typedef struct cl_engine_config {
                               env CL_PREFIX_CACHE=0|1 overrides).  Full pages of known tokens stay indexed after their
                               sequence is freed and are evicted least recently used first when the pool runs dry, so a
                               request whose prompt starts with an earlier prompt (or a preempted request coming back)
-                              prefills only the rest.  See cl_seq_attach_prefix / cl_engine_prefix_stats. */
+                              prefills only the rest.  See cl_seq_attach_prefix / cl_engine_prefix_stats, and
+                              cl_engine_set_prefix_host_cache for a host-memory tier behind the pool. */
   int32_t speculate;       /* speculative decoding: 0 => off (default), 1..15 => the most drafted tokens per verify pass
                               (env CL_SPECULATE overrides; other values make cl_engine_create fail with CL_ERR_INVALID_ARG).
                               While exactly one request is running and nothing waits, a greedy or device-sampled request
@@ -169,7 +170,11 @@ typedef struct cl_prefix_stats {
   int64_t tokens_looked_up;  /* prompt tokens of those lookups */
   int64_t tokens_reused;     /* of which found in the cache: their prefill was skipped */
   int64_t pages_evicted;     /* cached pages handed out again because the pool ran dry */
-  int64_t reserved[4];
+  /* host tier (cl_engine_set_prefix_host_cache); pages dropped from it = pages_to_host - pages_from_host - host_pages_cached */
+  int64_t host_pages;        /* capacity in pages (0: off) */
+  int64_t host_pages_cached; /* now: host pages holding an evicted page that stays indexed */
+  int64_t pages_to_host;     /* evicted pages copied to the host tier (spills) */
+  int64_t pages_from_host;   /* of which copied back to HBM because a sequence attached them (fills) */
 } cl_prefix_stats;
 
 /* Speculative decoding accounting since engine creation (cl_engine_config.speculate). */
@@ -221,6 +226,16 @@ int cl_engine_spec_stats(cl_engine* e, cl_spec_stats* out);
  * steps.  n: 1 .. min(max_batch, 32), else CL_ERR_INVALID_ARG.  Env CL_SPECULATE_BATCH sets it at cl_engine_create (an
  * invalid value makes the create fail with CL_ERR_INVALID_ARG). */
 int cl_engine_set_speculate_batch(cl_engine* e, int32_t n);
+/* Host tier of the prefix cache: `bytes` of pinned, mapped host memory (rounded down to whole pages; a page holds one pool
+ * page's K and V of every layer) behind the HBM page pool.  A cached page the pool evicts is copied there and stays
+ * indexed instead of being forgotten (the least recently evicted one is dropped when the tier is full), and a sequence
+ * whose prompt reaches it copies it back into a free pool page instead of prefilling it again.  Reuse stays bit-identical:
+ * a restored page holds the bytes that were evicted.  Off by default; 0 frees the tier.  Copies run on the engine's
+ * stream inside the calls that reserve or attach pages (cl_seq_attach_prefix, prefill, decode, request admission).
+ * CL_ERR_INVALID_ARG while any sequence is live or a request is queued, with the prefix cache off, for bytes < 0 and
+ * for 0 < bytes < one page; CL_ERR_OOM when the memory cannot be pinned (the tier is then off).  Env
+ * CL_PREFIX_CACHE_HOST_MIB sets it at cl_engine_create (a failure there makes the create fail with that status). */
+int cl_engine_set_prefix_host_cache(cl_engine* e, int64_t bytes);
 /* Overwrite one weight tensor from host memory (bf16 bits, logical [out][in] row-major; norm
  * gains as bf16 too).  kind: 0 embed, 1 lm_head, 2 final_norm, 3 attn_norm, 4 wq, 5 wk, 6 wv,
  * 7 wo, 8 ffn_norm, 9 w_gate, 10 w_up, 11 w_down (same numbering as the synthetic generator).
@@ -419,6 +434,14 @@ int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_
 int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, const uint16_t* v_cache, const int32_t* ctx_lens,
                       const int32_t* rows, int32_t n_segs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit,
                       uint16_t* out, int32_t* nsplit_used);
+/* The host tier's transfer kernels (cl_engine_set_prefix_host_cache): a pool of n_layers layers and 2 n_moves + 2 pages,
+ * scattered, in which n_moves pages hold random bits and every other element the largest finite bf16 (+ K, - V).  One
+ * kv_spill_kernel launch copies the n_moves pages to pinned, mapped host pages, one kv_fill_kernel launch copies those
+ * into the n_moves other pages.  CL_ERR_INTERNAL unless every destination and every host page holds exactly the source's
+ * bytes and every other page is unchanged.  iters > 0: ms[0] / ms[1] = CUDA-event time of one spill / fill launch, the
+ * mean over iters launches of each.  head_dim 64 or 128, page_size 16, 32 or 64. */
+int cl_op_kv_host_roundtrip(int device, int32_t n_layers, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t n_moves,
+                            int32_t iters, float* ms);
 /* prefill GEMM on the tensor cores (wgmma): Y[t][n] = sum_k X[t][k] W[n][k]; X,W bf16, Y fp32 */
 int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, int32_t t,
                     int32_t n, int32_t k, int32_t iters, float* ms);
@@ -485,6 +508,17 @@ int cl_kvpool_used_pages(cl_kvpool* p);   /* held by some owner */
 int cl_kvpool_attach(cl_kvpool* p, int32_t owner, const int32_t* ids, int32_t n, int32_t* n_reused);
 int cl_kvpool_publish(cl_kvpool* p, int32_t owner, const int32_t* ids, int32_t n_known);
 int cl_kvpool_cached_pages(cl_kvpool* p);
+/* Host tier (what cl_engine_set_prefix_host_cache runs on).  set_host_pages: n host pages (0: off), dropping every entry
+ * the tier held; CL_ERR_INVALID_ARG for n < 0 or while moves are pending.  With the tier on, reserve and attach record
+ * moves: kind 0 (spill) copies a cached device page that reserve or attach evicts to a host page, which keeps its index
+ * entry; kind 1 (fill) copies a host page back into a device page when attach takes its entry.  With no host page free, the
+ * least recently spilled entry is dropped.  The moves must be executed in the order given: a device page can be spilled and
+ * then filled, and a host page freed by a fill reused by a later spill, within one call.  take_moves: *n_out = the moves
+ * pending; with moves != NULL (cap >= *n_out, else CL_ERR_INVALID_ARG) they are written as [n][3] (kind, device page,
+ * host page) and cleared.  host_cached_pages: host pages holding an entry now. */
+int cl_kvpool_set_host_pages(cl_kvpool* p, int32_t n);
+int cl_kvpool_take_moves(cl_kvpool* p, int32_t* moves, int32_t cap, int32_t* n_out);
+int cl_kvpool_host_cached_pages(cl_kvpool* p);
 
 #ifdef __cplusplus
 }

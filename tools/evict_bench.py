@@ -76,7 +76,7 @@ def main():
         t_window = time.time()
         for t in threads:
             t.join(timeout=120)
-        st1, ps1 = e.stats(), e.prefix_stats()
+        st1, ps1 = e.stats(), e.prefix_stats(host=True)
         with lock:
             ok = [d for d in done if "error" not in d]
             errs = [d for d in done if "error" in d]
@@ -127,7 +127,10 @@ def main():
                    prefix_cache=dict(enabled=ps1["enabled"], lookups=ps1["lookups"] - ps0["lookups"],
                                      tokens_looked_up=ps1["tokens_looked_up"] - ps0["tokens_looked_up"],
                                      tokens_reused=ps1["tokens_reused"] - ps0["tokens_reused"],
-                                     pages_evicted=ps1["pages_evicted"] - ps0["pages_evicted"], cached_pages_at_end=ps1["cached_pages"]))
+                                     pages_evicted=ps1["pages_evicted"] - ps0["pages_evicted"], cached_pages_at_end=ps1["cached_pages"],
+                                     # host tier (CL_PREFIX_CACHE_HOST_MIB): pages copied out on eviction and back on a hit
+                                     host_pages=ps1["host_pages"], pages_to_host=ps1["pages_to_host"],
+                                     pages_from_host=ps1["pages_from_host"], host_pages_cached_at_end=ps1["host_pages_cached"]))
         print(json.dumps(out))
 
 
