@@ -493,7 +493,7 @@ int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, c
                            float* logits_out) {
   if (!e || !seqs || !input_ids || !ks || !ids_out || !n_out || n_seqs < 1) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
-  CL_GUARD(return e->impl.decode_verify_batch(seqs, n_seqs, input_ids, drafts, ks, sp, step0, ids_out, n_out, logits_out);)
+  CL_GUARD(return e->impl.decode_verify_batch(seqs, n_seqs, input_ids, drafts, ks, sp, step0, ids_out, n_out, logits_out, true);)
 }
 int cl_seq_fake_fill(cl_engine* e, cl_seq_t s, int32_t n_tokens) {
   if (!e) return CL_ERR_INVALID_ARG;

@@ -1000,7 +1000,7 @@ __global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a)
   // the step counter itself is bumped by step_bump_kernel after every batch entry has read it
 }
 
-// Verify pass (Engine::verify_draft): row r of the logits [T][vocab] makes the choice the step tail would make after the
+// Verify pass (Engine::verify_batch): row r of the logits [T][vocab] makes the choice the step tail would make after the
 // inputs x0, d1 .. dr: greedy, or on an armed slot the draw with history = ring + inputs[0..r] and RNG step step + r.
 // Each row has its own partial, candidate and counter buffers.  Nothing of the slot is written here.
 __global__ void __launch_bounds__(256, 8) spec_tail_kernel(const SpecTailArgs a) {

@@ -26,7 +26,7 @@ constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts
 constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi)
 constexpr int kDefaultSchedLingerUs = 1000;     // CL_SCHED_LINGER_US: with an empty batch, keep collecting while requests arrive within this gap (max 8x in total)
 
-// Speculative decoding (cl_engine_config.speculate, Engine::verify_draft, ngram_draft): the constants of the drafter.
+// Speculative decoding (cl_engine_config.speculate, Engine::verify_batch, ngram_draft): the constants of the drafter.
 constexpr int kSpecMaxDraft = 15;     // drafted tokens per verify pass at most (its rows: x0 + drafts <= 16)
 constexpr int kDraftNgramMax = 3;     // the drafter matches the history's last 3 ids, then its last 2
 constexpr int kDraftNgramMin = 2;
@@ -302,20 +302,20 @@ class Engine {
   int arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist);
   int disarm_sampling(cl_seq_t s);
   int read_next_token(cl_seq_t s, int32_t* out);   // d_tok_[s]: what the last step tail of `s` chose
-  // Speculative decoding: one verify pass of x0 and the drafts draft[0..k) (prefill.cu; contract in include/clengine.h,
-  // cl_decode_verify).  ids_out receives the *n_out = a + 1 emitted ids; logits_out (may be nullptr): [k + 1][vocab].
-  int verify_draft(cl_seq_t s, int32_t x0, const int32_t* draft, int k, int32_t* ids_out, int* n_out, float* logits_out);
-  // verify_draft with sp's draw armed for the pass (sp nullptr or temperature <= 0: greedy), as decode_sample does
-  int decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
-                    int* n_out, float* logits_out);
-  // One verify pass over n_seqs distinct sequences (contract in include/clengine.h, cl_decode_verify_batch): sequence i
-  // verifies x0[i] and ks[i] (0..15) drafts, taken back to back from drafts.  Its ids land at ids_out + its first row (the
-  // sum of k_j + 1 over the sequences before it), n_out[i] of them; logits_out (may be nullptr): [rows][vocab].
+  // Speculative decoding: one verify pass over n_seqs distinct sequences (prefill.cu; contract in include/clengine.h,
+  // cl_decode_verify_batch): sequence i verifies x0[i] and ks[i] (0..15) drafts, taken back to back from drafts.  Its ids
+  // land at ids_out + its first row (the sum of k_j + 1 over the sequences before it), n_out[i] = a + 1 of them; logits_out
+  // (may be nullptr): [rows][vocab].  seg_table: the attention takes the multi-row kernel (small_pass); false only with
+  // one sequence, whose attention then runs per segment as in cl_decode_verify.
   int verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks, int32_t* ids_out,
-                   int* n_out, float* logits_out);
+                   int* n_out, float* logits_out, bool seg_table);
   // verify_batch with the device sampler armed for the pass on every sequence whose sp[i] draws (sp, step0 may be nullptr)
   int decode_verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks, const cl_sampling* sp,
-                          const uint64_t* step0, int32_t* ids_out, int* n_out, float* logits_out);
+                          const uint64_t* step0, int32_t* ids_out, int* n_out, float* logits_out, bool seg_table);
+  // cl_decode_verify: decode_verify_batch of one sequence with k in 1..15, without the segment table (sp nullptr or
+  // temperature <= 0: greedy)
+  int decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
+                    int* n_out, float* logits_out);
   bool spec_path_ok() const;          // the verify pass runs on this model shape
   int speculate() const { return speculate_; }
   int speculate_batch() const { return speculate_batch_; }
@@ -339,7 +339,6 @@ class Engine {
   struct TokenSink { int (*fn)(void* user, const int32_t* ids, int n) = nullptr; void* user = nullptr; };
   int generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink = nullptr);
   void scheduler_main();
-  int spec_batch_round();   // one verify pass over the running requests (scheduler.cpp)
   void start_scheduler();
   void stop_scheduler();
 
@@ -380,7 +379,7 @@ class Engine {
   int attn_prefill(const AttnPrefillArgs& a, int layer, int& launches, LaunchProfiler& prof);   // the one choice of prefill attention kernel
   int prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_out);    // short prompts: split-K projections (prefill.cu)
   int ensure_small_ws();
-  // the split-K pass of prefill_small, verify_draft and verify_batch: T rows made of n_segs segments; leaves sws_->h and the
+  // the split-K pass of prefill_small and verify_batch: T rows made of n_segs segments; leaves sws_->h and the
   // final-norm rows sws_->xn.  row_map (device, or nullptr with one segment): [2][T] the sequence, then the position of every
   // row; seg_table (device, may be nullptr): the segments as AttnVerifyArgs::segs, which selects the multi-row attention
   // kernel where the shape allows it.
@@ -390,6 +389,25 @@ class Engine {
   SpecTailArgs spec_tail_args(const PrefillSegment& g, int out_off) const;   // the spec tail of one verify segment
   bool prefill_path_ok() const;
   int set_single_slot(cl_seq_t s);
+
+  // request-level transitions and scheduler phases (scheduler.cpp); callers hold mu_
+  bool join(Request& r, const int32_t* ids, int n, bool admission);
+  void retire(Request& r, int status, const std::string& err);
+  void preempt(std::shared_ptr<Request> r);
+  int host_next_token(Request& r, float* logits, bool read_back, const int32_t* hist, int n_hist, int32_t* next);
+  int spec_round(const std::shared_ptr<Request>* rs, int n);
+  int generate_sync(const std::shared_ptr<Request>& r, const TokenSink* sink);
+  int admission_pages(Request& r, int* hit);
+  bool wait_for_work();
+  bool admit_group(int budget);
+  void admit_chunked(int budget);
+  void admitted(const std::shared_ptr<Request>& r, int32_t next);
+  void make_room();
+  bool speculate_running();
+  int step_running();
+  void retire_finished();
+  void fail_running(int rc);
+  void shutdown_requests();
 
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
@@ -499,6 +517,10 @@ class Engine {
   std::vector<std::shared_ptr<Request>> active_;
   std::shared_ptr<Request> prefilling_;   // the one request whose prompt is being prefilled chunk by chunk (scheduler.cpp)
   int sched_prefill_chunk_ = 0;           // admission token budget per iteration while other sequences are decoding (CL_SCHED_PREFILL_CHUNK; 0 = unlimited)
+  // the scheduler thread's host buffers: a host-sampled request's logits, d_tok_ read back, the slot list last uploaded to d_slots_
+  std::vector<float> sched_logits_;
+  std::vector<int32_t> sched_toks_;
+  std::vector<int> sched_slots_;
   std::atomic<bool> stop_{false};
   bool sched_started_ = false;
   friend struct Request;

@@ -105,7 +105,7 @@ struct StepTailArgs {                // argmax (or a draw) over logits, advance 
   SampleState sample;
 };
 
-// Verify pass of speculative decoding for one slot (Engine::verify_draft): T = k + 1 rows with inputs x0, d1 .. dk.
+// Verify pass of speculative decoding for one slot (a segment of Engine::verify_batch): T = k + 1 rows with inputs x0, d1 .. dk.
 // spec_tail_kernel makes row r's step-tail choice into choice[r] (the draw: history = ring + inputs[0..r], RNG step
 // step[slot] + r); spec_accept_kernel then accepts the longest run of drafts equal to the choices and advances the slot.
 struct SpecTailArgs {

@@ -101,7 +101,7 @@ int Engine::ensure_small_ws() {
 // of the multi-row split-KV kernel (attn_verify_tc.cu) when seg_table is given and the shape is one it takes, else per
 // segment (attn_prefill).  Leaves the final residual rows in sws_->h and their normalised bf16 rows, the LM head's input,
 // in sws_->xn.  A row's results depend only on its own segment's rows before it.  prefill_small and the verify passes of
-// speculative decoding (verify_draft: one segment, no map or table; verify_batch) run it.
+// speculative decoding (verify_batch; without the segment table: one segment, no map or table) run it.
 int Engine::small_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, const int* row_map, const int* seg_table,
                        int& launches, LaunchProfiler& prof) {
   const int d = cfg.d_model, F = cfg.d_ff;
@@ -201,68 +201,18 @@ bool Engine::spec_path_ok() const {
   return prefill_path_ok() && cfg.d_model <= 8192 && cfg.d_model % 4 == 0 && gemm_tc_supported(kSpecMaxDraft + 1, cfg.vocab_size, cfg.d_model);
 }
 
-// Verify pass of speculative decoding (include/clengine.h, cl_decode_verify): rows x0, d1 .. dk at positions len .. len + k
-// through small_pass, one GEMM over the final-norm rows for their logits, then the spec tail (row r's step-tail choice
-// y_{r+1}) and the accept kernel (a = longest run with y_j == d_j; next input y_{a+1}; an armed slot's history and RNG
-// step advanced as a + 1 steps would).  Only {a + 1, y_1 .. y_{a+1}} is read back.  Rejected rows leave K/V at positions
-// >= the new length, on the sequence's private pages.
-int Engine::verify_draft(cl_seq_t s, int32_t x0, const int32_t* draft, int k, int32_t* ids_out, int* n_out, float* logits_out) {
-  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
-  if (k < 1 || k > kSpecMaxDraft || !draft || !ids_out || !n_out) { set_last_error("verify: k must be 1..15"); return CL_ERR_INVALID_ARG; }
-  if (!spec_path_ok()) { set_last_error("verify: the model shape has no tensor-core split-K path"); return CL_ERR_INVALID_ARG; }
-  const int V = cfg.vocab_size, d = cfg.d_model, T = k + 1;
-  int32_t in[kSpecMaxDraft + 1];
-  in[0] = x0;
-  memcpy(in + 1, draft, (size_t)k * 4);
-  for (int i = 0; i < T; ++i)
-    if (in[i] < 0 || in[i] >= V) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
-  auto& q = seqs_[s];
-  int rc = ensure_capacity(s, q.len + T);
-  if (rc) return rc;
-  if ((rc = ensure_small_ws()) || (rc = ensure_spec_ws())) return rc;
-  CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, in, (size_t)T * 4, cudaMemcpyHostToDevice, stream_));
-  int launches = 0;
-  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
-  const PrefillSegment seg{s, 0, T, q.len};
-  if ((rc = small_pass(&seg, 1, d_prompt_, T, nullptr, nullptr, launches, prof))) return rc;
-  CL_LAUNCH(launch_gemm_bf16(sws_->xn, lm_head_, spec_->logits, nullptr, T, V, d, stream_, 1, false));
-  CL_LAUNCH(launch_spec_tail(spec_tail_args(seg, 0), stream_, use_pdl_));
-  CL_CUDA_OK(cudaMemcpyAsync(h_ids_pinned_, spec_->out, (size_t)(T + 1) * 4, cudaMemcpyDeviceToHost, stream_));
-  CL_CUDA_OK(cudaStreamSynchronize(stream_));
-  prof.report("prefill profile", 32, "verify pass, " + std::to_string(T) + " rows");
-  launches_ += launches;
-  const int n = h_ids_pinned_[0];
-  if (n < 1 || n > T) { set_last_error("verify: accept kernel returned a bad count"); return CL_ERR_INTERNAL; }
-  memcpy(ids_out, h_ids_pinned_ + 1, (size_t)n * 4);
-  *n_out = n;
-  seq_advance(s, in, n, n);   // x0, d1 .. da: only accepted tokens join the history and the prefix cache
-  spec_passes_++; spec_drafted_ += k; spec_accepted_ += n - 1; spec_emitted_ += n;
-  if (logits_out) CL_CUDA_OK(cudaMemcpy(logits_out, spec_->logits, (size_t)T * V * 4, cudaMemcpyDeviceToHost));
-  return CL_OK;
-}
-
-// cl_decode_verify: verify_draft with the device sampler armed for the pass when sp asks for a draw
-int Engine::decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
-                          int* n_out, float* logits_out) {
-  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
-  const bool sampled = sp && sp->temperature > 0.f;
-  int rc = CL_OK;
-  if (sampled) rc = arm_sampling(s, *sp, step0, seqs_[s].history.data(), (int)seqs_[s].history.size());
-  if (rc == CL_OK) rc = verify_draft(s, x0, draft, k, ids_out, n_out, logits_out);
-  if (sampled) {
-    const int r2 = disarm_sampling(s);
-    if (rc == CL_OK) rc = r2;
-  }
-  return rc;
-}
-
-// Verify pass over several sequences (include/clengine.h, cl_decode_verify_batch): sequence i is segment i of one small_pass,
-// rows x0[i], d_1 .. d_{k_i} at positions len_i .. len_i + k_i.  One GEMM computes the logits of all rows, then each segment
-// runs verify_draft's spec tail and accept kernel on its own rows and slot.  Every row's computation is the one it has in a
-// pass of its sequence alone, so each sequence's ids, logits and K/V equal verifying it alone.  Everything is checked before
-// anything is enqueued; on an error no sequence's length changes.
+// Verify pass of speculative decoding over n_seqs distinct sequences (include/clengine.h, cl_decode_verify and
+// cl_decode_verify_batch): sequence i is segment i of one small_pass, rows x0[i], d_1 .. d_{k_i} at positions len_i ..
+// len_i + k_i.  One GEMM computes the logits of all rows, then each segment runs the spec tail (row r's step-tail choice
+// y_{r+1}) and the accept kernel (a = longest run with y_j == d_j; next input y_{a+1}; an armed slot's history and RNG step
+// advanced as a + 1 steps would) on its own rows and slot.  Only {a + 1, y_1 .. y_{a+1}} of each sequence is read back.
+// seg_table: small_pass gets the row map and the segment table, so the attention runs in the multi-row kernel where the
+// shape allows it; without it (one sequence only) the segment goes through attn_prefill, as cl_decode_verify always has.
+// Every row's computation is the one it has in a pass of its sequence alone, so each sequence's ids, logits and K/V equal
+// verifying it alone.  Everything is checked before anything is enqueued; on an error no sequence's length changes.
+// Rejected rows leave K/V at positions >= the new length, on the sequence's private pages.
 int Engine::verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks, int32_t* ids_out,
-                         int* n_out, float* logits_out) {
+                         int* n_out, float* logits_out, bool seg_table) {
   if (n_seqs < 1 || !ss || !x0 || !ks || !ids_out || !n_out) { set_last_error("verify_batch: bad arguments"); return CL_ERR_INVALID_ARG; }
   if (!spec_path_ok()) { set_last_error("verify: the model shape has no tensor-core split-K path"); return CL_ERR_INVALID_ARG; }
   const int V = cfg.vocab_size, d = cfg.d_model;
@@ -289,23 +239,27 @@ int Engine::verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, cons
   for (const auto& g : segs)
     if ((rc = ensure_capacity(g.seq, g.pos0 + g.n))) return rc;
   if ((rc = ensure_small_ws()) || (rc = ensure_spec_ws())) return rc;
-  std::vector<int> row_map(2 * (size_t)T), table(8 * (size_t)n_seqs, 0);
-  const int split_pages = verify_split_pages();
-  long long part_off = 0;
-  for (int i = 0; i < n_seqs; ++i) {
-    const PrefillSegment& g = segs[i];
-    for (int r = 0; r < g.n; ++r) { row_map[g.row0 + r] = g.seq; row_map[T + g.row0 + r] = g.pos0 + r; }
-    const int pages = (g.pos0 + g.n + page_size_ - 1) / page_size_, ns = (pages + split_pages - 1) / split_pages;
-    int* e = &table[8 * (size_t)i];
-    e[0] = g.seq; e[1] = g.row0; e[2] = g.n; e[3] = g.pos0; e[4] = (int)part_off; e[5] = ns;
-    if (ns > 1) part_off += (long long)cfg.n_kv_heads * ns * 4 * g.n * (cfg.head_dim + 2);
-  }
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, in.data(), (size_t)T * 4, cudaMemcpyHostToDevice, stream_));
-  CL_CUDA_OK(cudaMemcpyAsync(spec_->row_map, row_map.data(), row_map.size() * 4, cudaMemcpyHostToDevice, stream_));
-  CL_CUDA_OK(cudaMemcpyAsync(spec_->segs, table.data(), table.size() * 4, cudaMemcpyHostToDevice, stream_));
+  if (seg_table) {
+    std::vector<int> row_map(2 * (size_t)T), table(8 * (size_t)n_seqs, 0);
+    const int split_pages = verify_split_pages();
+    long long part_off = 0;
+    for (int i = 0; i < n_seqs; ++i) {
+      const PrefillSegment& g = segs[i];
+      for (int r = 0; r < g.n; ++r) { row_map[g.row0 + r] = g.seq; row_map[T + g.row0 + r] = g.pos0 + r; }
+      const int pages = (g.pos0 + g.n + page_size_ - 1) / page_size_, ns = (pages + split_pages - 1) / split_pages;
+      int* e = &table[8 * (size_t)i];
+      e[0] = g.seq; e[1] = g.row0; e[2] = g.n; e[3] = g.pos0; e[4] = (int)part_off; e[5] = ns;
+      if (ns > 1) part_off += (long long)cfg.n_kv_heads * ns * 4 * g.n * (cfg.head_dim + 2);
+    }
+    CL_CUDA_OK(cudaMemcpyAsync(spec_->row_map, row_map.data(), row_map.size() * 4, cudaMemcpyHostToDevice, stream_));
+    CL_CUDA_OK(cudaMemcpyAsync(spec_->segs, table.data(), table.size() * 4, cudaMemcpyHostToDevice, stream_));
+  }
   int launches = 0;
   LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
-  if ((rc = small_pass(segs.data(), n_seqs, d_prompt_, T, spec_->row_map, spec_->segs, launches, prof))) return rc;
+  if ((rc = small_pass(segs.data(), n_seqs, d_prompt_, T, seg_table ? spec_->row_map : nullptr, seg_table ? spec_->segs : nullptr,
+                       launches, prof)))
+    return rc;
   CL_LAUNCH(launch_gemm_bf16(sws_->xn, lm_head_, spec_->logits, nullptr, T, V, d, stream_, 1, false));
   // segment i's output {n_i, ids} sits at out[row0_i + i]: one int more per segment than its rows
   for (int i = 0; i < n_seqs; ++i) CL_LAUNCH(launch_spec_tail(spec_tail_args(segs[i], segs[i].row0 + i), stream_, use_pdl_));
@@ -332,9 +286,19 @@ int Engine::verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, cons
   return CL_OK;
 }
 
-// cl_decode_verify_batch: verify_batch with the device sampler armed for the pass on the sequences whose sp[i] draws
+// cl_decode_verify: one sequence with 1..15 drafts, verified without the segment table
+int Engine::decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
+                          int* n_out, float* logits_out) {
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  if (k < 1 || k > kSpecMaxDraft) { set_last_error("verify: k must be 1..15"); return CL_ERR_INVALID_ARG; }
+  return decode_verify_batch(&s, 1, &x0, draft, &k, sp, &step0, ids_out, n_out, logits_out, false);
+}
+
+// cl_decode_verify_batch (seg_table = true) and cl_decode_verify: verify_batch with the device sampler armed for the pass
+// on the sequences whose sp[i] draws
 int Engine::decode_verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, const int32_t* drafts, const int* ks,
-                                const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int* n_out, float* logits_out) {
+                                const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int* n_out, float* logits_out,
+                                bool seg_table) {
   if (n_seqs < 1 || !ss) { set_last_error("verify_batch: bad arguments"); return CL_ERR_INVALID_ARG; }
   for (int i = 0; i < n_seqs; ++i) {
     if (ss[i] < 0 || ss[i] >= max_seqs_ || !seqs_[ss[i]].live) return CL_ERR_BAD_SEQ;
@@ -352,7 +316,7 @@ int Engine::decode_verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x
     rc = arm_sampling(s, sp[i], step0 ? step0[i] : 0, seqs_[s].history.data(), (int)seqs_[s].history.size());
     if (rc == CL_OK) armed.push_back(s);
   }
-  if (rc == CL_OK) rc = verify_batch(ss, n_seqs, x0, drafts, ks, ids_out, n_out, logits_out);
+  if (rc == CL_OK) rc = verify_batch(ss, n_seqs, x0, drafts, ks, ids_out, n_out, logits_out, seg_table);
   for (cl_seq_t s : armed) {
     const int r2 = disarm_sampling(s);
     if (rc == CL_OK) rc = r2;

@@ -327,21 +327,26 @@ def test_short_request_admitted_during_a_long_one_does_not_disturb_it():
     long_prompt = _prompt(20, V)
     shorts = [np.array([(7 * i + 3 * j + 1) % V for j in range(5 + i % 4)], np.int32) for i in range(24)]
     with eng.Engine(preset="tiny-test", seed=11, max_batch=4, max_seqs=4, start_scheduler=True) as e:
-        solo = e.generate_ids(long_prompt, eng.greedy(400, ignore_eos=True)).token_ids
-        short_solo = [int(e.generate_ids(p, eng.greedy(1, ignore_eos=True)).token_ids[0]) for p in shorts]
+        solo_r = e.generate_ids(long_prompt, eng.greedy(400, ignore_eos=True))
+        solo = solo_r.token_ids
+        short_r = [e.generate_ids(p, eng.greedy(1, ignore_eos=True)) for p in shorts]
+        short_solo = [int(r.token_ids[0]) for r in short_r]
         out = {}
 
         def run_long():
             out["long"] = e.generate_ids(long_prompt, eng.greedy(400, ignore_eos=True))
         th = threading.Thread(target=run_long)
         th.start()
-        got = [int(e.generate_ids(p, eng.greedy(1, ignore_eos=True)).token_ids[0]) for p in shorts]
+        got_r = [e.generate_ids(p, eng.greedy(1, ignore_eos=True)) for p in shorts]
+        got = [int(r.token_ids[0]) for r in got_r]
         th.join()
         assert out["long"].n_generated == 400
         np.testing.assert_array_equal(out["long"].token_ids, solo)
         assert got == short_solo
         st = e.stats()
         assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0
+        results = [solo_r, out["long"], *short_r, *got_r]
+        assert st["requests_completed"] == len(results) and st["preemptions"] == sum(r.n_preempted for r in results)
 
 
 def test_long_prompt_is_admitted_in_chunks_between_decode_steps(monkeypatch):
@@ -358,9 +363,9 @@ def test_long_prompt_is_admitted_in_chunks_between_decode_steps(monkeypatch):
     a_prompt = _prompt(12, V)
     shorts = [np.array([(11 * i + 5 * j + 2) % V for j in range(6 + i)], np.int32) for i in range(5)]
     with eng.Engine(preset="tiny-test", seed=21, max_batch=8, max_seqs=8, start_scheduler=True) as e:
-        a_solo = e.generate_ids(a_prompt, eng.greedy(400, ignore_eos=True)).token_ids
-        b_solo = e.generate_ids(long_prompt, eng.greedy(24, ignore_eos=True)).token_ids
-        s_solo = [e.generate_ids(p, eng.greedy(10, ignore_eos=True)).token_ids for p in shorts]
+        solo_r = [e.generate_ids(p, eng.greedy(n, ignore_eos=True)) for p, n in [(a_prompt, 400), (long_prompt, 24)] + [(p, 10) for p in shorts]]
+        a_solo, b_solo = solo_r[0].token_ids, solo_r[1].token_ids
+        s_solo = [r.token_ids for r in solo_r[2:]]
         out, stamps = {}, []
 
         def run_a():
@@ -383,7 +388,8 @@ def test_long_prompt_is_admitted_in_chunks_between_decode_steps(monkeypatch):
         for i in range(len(shorts)):
             assert out[f"s{i}"].n_generated == 10 and out[f"s{i}"].token_ids[0] == s_solo[i][0]
         st = e.stats()
-        assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0 and st["requests_completed"] >= 7 + 7
+        assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0 and st["requests_completed"] == 7 + 7
+        assert st["preemptions"] == sum(r.n_preempted for r in solo_r + list(out.values()))
 
 
 def test_group_admission_of_a_burst_matches_requests_run_alone(monkeypatch):
@@ -413,6 +419,7 @@ def test_group_admission_of_a_burst_matches_requests_run_alone(monkeypatch):
             assert out[i].n_generated == 24 and out[i].token_ids[0] == solo[i][0], i
             assert (out[i].token_ids == solo[i]).mean() > 0.7, i
         assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0 and st["requests_completed"] - before["requests_completed"] == len(prompts)
+        assert st["preemptions"] - before["preemptions"] == sum(r.n_preempted for r in out)
         # fewer prefill calls than requests: groups were formed
         assert st["sched_prefill_calls"] - before["sched_prefill_calls"] < len(prompts)
         # sampled requests go through the group path too (host sampler on the pass's logits): deterministic per seed

@@ -82,6 +82,7 @@ def test_eviction_and_recompute_reproduces_tokens():
         st = e.stats()
         assert st["preemptions"] > 0, "the pool was meant to be too small"
         assert st["kv_pages_used"] == 0 and st["requests_completed"] == len(prompts)
+        assert st["preemptions"] == sum(r.n_preempted for r in out)
         exact = 0
         for i, r in enumerate(out):
             assert r.n_generated == 60 and r.done_reason == "length"

@@ -200,6 +200,7 @@ def test_scheduler_reuses_a_shared_prefix():
         ps, st = e.prefix_stats(), e.stats()
         assert ps["lookups"] == 16 and ps["tokens_reused"] >= 15 * 1024, ps
         assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0 and st["requests_completed"] == 16
+        assert st["preemptions"] == sum(o.n_preempted for o in out)
     with eng.Engine(model=cfg, seed=31, max_batch=1, max_seqs=1) as ref:
         assert ref.prefix_stats()["lookups"] == 0
         for i in range(16):
@@ -229,6 +230,7 @@ def test_preempted_requests_reattach_their_pages():
         print(f"preemptions {st['preemptions']}, prefix stats {ps}")
         assert st["preemptions"] > 0 and ps["tokens_reused"] > 0 and ps["pages_evicted"] > 0
         assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0 and st["requests_completed"] == len(prompts)
+        assert st["preemptions"] == sum(o.n_preempted for o in out)
     with eng.Engine(model=cfg, seed=8, max_batch=1, max_seqs=1) as ref:
         for i, p in enumerate(prompts):
             assert out[i].n_generated == 160

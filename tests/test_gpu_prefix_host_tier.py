@@ -271,6 +271,7 @@ def test_scheduler_brings_preempted_requests_back_from_the_host():
         print(f"preemptions {st['preemptions']}, prefix stats {ps}")
         assert st["preemptions"] > 0 and ps["pages_from_host"] > 0 and ps["tokens_reused"] > 0
         assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0 and st["requests_completed"] == len(prompts)
+        assert st["preemptions"] == sum(o.n_preempted for o in out)
         assert ps["pages_to_host"] - ps["pages_from_host"] - ps["host_pages_cached"] >= 0
         assert ps["host_pages_cached"] <= ps["host_pages"] == 250
     with eng.Engine(model=cfg, seed=8, max_batch=1, max_seqs=1) as ref:

@@ -213,7 +213,8 @@ def test_requests_match_between_device_and_host_sampling(monkeypatch, scheduler)
 def test_concurrent_sampled_requests_complete_without_leaks():
     reqs = _requests() * 3
     with eng.Engine(preset="tiny-test", seed=31, max_batch=4, max_seqs=4, start_scheduler=True) as e:
-        solo = [e.generate_ids(p, sp).token_ids for p, sp in reqs]
+        solo_r = [e.generate_ids(p, sp) for p, sp in reqs]
+        solo = [r.token_ids for r in solo_r]
         res = [None] * len(reqs)
 
         def run(i):
@@ -229,3 +230,4 @@ def test_concurrent_sampled_requests_complete_without_leaks():
             assert r.token_ids[0] == solo[i][0]
         st = e.stats()
         assert st["kv_pages_used"] == 0 and st["active_seqs"] == 0
+        assert st["requests_completed"] == 2 * len(reqs) and st["preemptions"] == sum(r.n_preempted for r in solo_r + res)

@@ -324,7 +324,7 @@ def _spec_prompt(V, salt):
 
 
 def _token_level_replay(e, prompt, sp, k_spec, max_new):
-    """What a speculating request does, through cl_decode_verify and single steps (scheduler.cpp spec_round)."""
+    """What a speculating request does, through cl_decode_verify and single steps (scheduler.cpp Engine::spec_round with one request)."""
     s = e.seq_create()
     lg = e.prefill(s, prompt)
     out = [eng.sample_token(lg, sp, list(prompt), 0)]
@@ -391,6 +391,7 @@ def test_second_request_switches_to_batched_steps():
         ta.join()
         st = e.stats()
         assert st["sched_decode_steps"] > before and st["kv_pages_used"] == 0 and st["requests_completed"] == 2
+        assert st["preemptions"] == out["a"].n_preempted + out["b"].n_preempted
         assert e.spec_stats()["verify_passes"] > 0
     with eng.Engine(model=cfg, seed=41, max_batch=4, max_seqs=4) as ref:
         for p, r, n in ((pa, out["a"], 400), (pb, out["b"], 48)):
