@@ -520,6 +520,11 @@ int cl_debug_hidden(cl_engine* e, float* out, int32_t n) {
   std::lock_guard<std::mutex> lk(e->impl.mu_);
   return e->impl.debug_hidden(out, n);
 }
+int cl_debug_seq_hidden(cl_engine* e, cl_seq_t s, int32_t what, float* out, int32_t n, int32_t* mega_out) {
+  if (!e) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(return e->impl.debug_seq_hidden(s, what, out, n, mega_out);)
+}
 
 // ---- paged-KV allocator (host logic) ---------------------------------------------------------------
 int cl_kvpool_create(int32_t n_pages, int32_t page_size, cl_kvpool** out) {

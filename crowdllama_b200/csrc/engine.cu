@@ -919,6 +919,7 @@ int Engine::decode_greedy(const cl_seq_t* ss, int B, const int32_t* first_ids, i
   }
   CL_CUDA_OK(cudaMemcpyAsync(d_slots_, ss, (size_t)B * 4, cudaMemcpyHostToDevice, stream_));
   last_single_slot_ = B == 1 ? ss[0] : -1;
+  if (B > 1) last_batch_slots_.assign(ss, ss + B);
   slots_dirty_ = true;
   float total_ms = 0.f;
   for (int done = 0; done < n_steps;) {
@@ -1030,6 +1031,7 @@ int Engine::decode_step_batch(const cl_seq_t* ss, int B, const int32_t* ids, flo
   }
   CL_CUDA_OK(cudaMemcpyAsync(d_slots_, ss, (size_t)B * 4, cudaMemcpyHostToDevice, stream_));
   last_single_slot_ = B == 1 ? ss[0] : -1;
+  if (B > 1) last_batch_slots_.assign(ss, ss + B);
   slots_dirty_ = true;
   const int rc = run_step_graph(B);
   if (rc) return rc;
@@ -1106,17 +1108,30 @@ int Engine::debug_hidden(float* out, int n) {
   if (last_single_slot_ < 0) return CL_ERR_INVALID_ARG;
   // negative n selects a last-layer intermediate of the most recent single-sequence step (diagnostics):
   // -1 = q (roped), -2 = attention output, -3 = SwiGLU activation
-  if (n < 0) {
-    const float* src = n == -1 ? d_q_ + (size_t)last_single_slot_ * q_dim_ : n == -2 ? d_attn_ + (size_t)last_single_slot_ * q_dim_
-                                                                              : d_act_ + (size_t)last_single_slot_ * cfg.d_ff;
-    const int cnt = n == -3 ? cfg.d_ff : q_dim_;
-    CL_CUDA_OK(cudaMemcpyAsync(out, src, (size_t)cnt * 4, cudaMemcpyDeviceToHost, stream_));
-    CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  if (n < 0 && n >= -3) return debug_seq_hidden(last_single_slot_, -n, out, n == -3 ? cfg.d_ff : q_dim_, nullptr);
+  return debug_seq_hidden(last_single_slot_, 0, out, n, nullptr);
+}
+
+int Engine::debug_seq_hidden(cl_seq_t s, int what, float* out, int n, int32_t* mega_out) {
+  if (mega_out) *mega_out = use_mega_ && d_mega_layers_ != nullptr ? 1 : 0;
+  if (!out && n == 0) return CL_OK;   // only the flag was asked for
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  const int want = what == 0 ? cfg.d_model : what == 3 || what == 5 ? cfg.d_ff : q_dim_;
+  if (what < 0 || what > 5 || n != want || !out) { set_last_error("debug_seq_hidden: bad buffer selector or element count"); return CL_ERR_INVALID_ARG; }
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  if (what <= 3) {   // per-slot fp32 state: written by every step that contains the sequence
+    const float* src = what == 0 ? d_h_ + (size_t)s * cfg.d_model : what == 1 ? d_q_ + (size_t)s * q_dim_
+                     : what == 2 ? d_attn_ + (size_t)s * q_dim_ : d_act_ + (size_t)s * cfg.d_ff;
+    CL_CUDA_OK(cudaMemcpy(out, src, (size_t)n * 4, cudaMemcpyDeviceToHost));
     return CL_OK;
   }
-  if (n != cfg.d_model) return CL_ERR_INVALID_ARG;
-  CL_CUDA_OK(cudaMemcpyAsync(out, d_h_ + (size_t)last_single_slot_ * cfg.d_model, (size_t)n * 4, cudaMemcpyDeviceToHost, stream_));
-  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  // bf16 operands of the batched step's GEMMs: rows in batch order
+  int b = -1;
+  for (size_t i = 0; i < last_batch_slots_.size(); ++i) if (last_batch_slots_[i] == s) b = (int)i;
+  if (b < 0 || !bws_) { set_last_error("debug_seq_hidden: the sequence was not part of the latest batched step"); return CL_ERR_INVALID_ARG; }
+  std::vector<uint16_t> tmp((size_t)n);
+  CL_CUDA_OK(cudaMemcpy(tmp.data(), (what == 4 ? bws_->attn : bws_->act) + (size_t)b * n, (size_t)n * 2, cudaMemcpyDeviceToHost));
+  for (int i = 0; i < n; ++i) { const uint32_t u = (uint32_t)tmp[(size_t)i] << 16; memcpy(&out[i], &u, 4); }
   return CL_OK;
 }
 

@@ -331,6 +331,7 @@ class Engine {
   int decode_step_batch(const cl_seq_t* seqs, int n_seqs, const int32_t* ids, float* logits_out, int32_t* argmax_out);
   int time_dominant_kernel(cl_seq_t s, int32_t first_id, int n_steps, float* kernel_ms, float* step_ms);
   int debug_hidden(float* out, int n);
+  int debug_seq_hidden(cl_seq_t s, int what, float* out, int n, int32_t* mega_out);   // contract in include/clengine.h
   int debug_timeline(long long* out, int n);   // CL_TIMELINE=1: globaltimer stamps of the last step (CTA 0 of every node)
   int stats(cl_stats* out);
 
@@ -496,6 +497,7 @@ class Engine {
   int prefill_min_tokens_ = 16;
   bool graph_failed_ = false;
   int last_single_slot_ = -1;
+  std::vector<int> last_batch_slots_;  // sequences of the latest step over two or more sequences, in batch order (debug_seq_hidden)
   bool slots_dirty_ = false;          // d_slots_ was rewritten outside the scheduler loop: its cached copy is stale
   cudaEvent_t* probe_ev_ = nullptr;   // time_dominant_kernel: event pair recorded around the dominant kernel of an eager step
   int probe_idx_ = 0;

@@ -587,6 +587,7 @@ int Engine::step_running() {
     cudaMemcpyAsync(d_slots_, sched_slots_.data(), (size_t)B * 4, cudaMemcpyHostToDevice, stream_);
     slots_dirty_ = false;
     last_single_slot_ = B == 1 ? sched_slots_[0] : -1;
+    if (B > 1) last_batch_slots_ = sched_slots_;
   }
   const int64_t t0 = now_ns();
   int rc = run_step_graph(B);

@@ -83,7 +83,7 @@ EXPORTS = [
     "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_engine_set_speculate_batch", "cl_engine_set_prefix_host_cache", "cl_draft_ngram", "cl_decode_verify", "cl_decode_verify_batch", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
     "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
-    "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_timeline",
+    "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_seq_hidden", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
     "cl_op_attn_decode_batch", "cl_op_attn_verify", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
     "cl_op_attn_prefill_cached", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
@@ -157,6 +157,7 @@ def lib():
         "cl_time_dominant_kernel": (C.c_int, [vp, i32, i32, i32, P(f32), P(f32)]),
         "cl_debug_kv": (C.c_int, [vp, i32, i32, i32, i32, i32, vp]),
         "cl_debug_hidden": (C.c_int, [vp, vp, i32]),
+        "cl_debug_seq_hidden": (C.c_int, [vp, i32, i32, vp, i32, P(i32)]),
         "cl_debug_timeline": (C.c_int, [vp, vp, i32]),
         "cl_op_gemv": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, P(f32)]),
         "cl_op_gemv_residual": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, vp, i32, i32]),
@@ -505,6 +506,22 @@ class Engine:
         out = np.empty(self.cfg["d_model"], np.float32)
         _check(lib().cl_debug_hidden(self._h, _ptr(out), out.size), "cl_debug_hidden")
         return out
+
+    def debug_seq_hidden(self, s: int, what: str) -> np.ndarray:
+        """cl_debug_seq_hidden: one buffer of sequence s after the latest decode step that contained it.  what: "h" (residual
+        stream), "q" (roped q), "attn" (attention output, fp32), "act" (SwiGLU activation of a single-sequence step),
+        "attn_bf16" / "act_bf16" (the rows the batched step's o / down projections read)."""
+        i = ("h", "q", "attn", "act", "attn_bf16", "act_bf16").index(what)
+        n = self.cfg["d_model"] if i == 0 else self.cfg["d_ff"] if i in (3, 5) else self.cfg["n_heads"] * self.cfg["head_dim"]
+        out = np.empty(n, np.float32)
+        _check(lib().cl_debug_seq_hidden(self._h, s, i, _ptr(out), n, None), "cl_debug_seq_hidden")
+        return out
+
+    def runs_mega_kernel(self) -> bool:
+        """Whether single-sequence steps of this engine run decode_mega_kernel (else the per-op kernels)."""
+        m = C.c_int32(-1)
+        _check(lib().cl_debug_seq_hidden(self._h, 0, 0, None, 0, C.byref(m)), "cl_debug_seq_hidden")
+        return m.value == 1
 
     def debug_timeline(self) -> np.ndarray:
         n = (self.cfg["n_layers"] * 5 + 1) * 4

@@ -377,6 +377,17 @@ int cl_time_dominant_kernel(cl_engine* e, cl_seq_t seq, int32_t first_id, int32_
 /* debugging / parity: copy the residual stream after `layer` (or the final norm input when
  * layer == n_layers) of the most recent single-sequence step to host (d_model floats). */
 int cl_debug_hidden(cl_engine* e, float* out, int32_t n);
+/* The same buffers for any live sequence, after the latest decode step (single or batched) that contained it; the stream is
+ * synchronised first.  what: 0 = the residual stream after the last layer (d_model floats); 1 = the last layer's roped q
+ * (n_heads * head_dim); 2 = its attention output, fp32 (n_heads * head_dim); 3 = its SwiGLU activation as a single-sequence
+ * step leaves it (d_ff; a batched step does not write this buffer).  After a step over two or more sequences, until the next
+ * such step or multi-prompt prefill: 4 = the bf16 attention row the o-projection GEMM read, 5 = the bf16 activation row
+ * the down-projection GEMM read (as floats).  n must be the buffer's element count.  *mega_out (may be NULL): 1 when this
+ * engine's single-sequence steps run decode_mega_kernel, 0 when they run the per-op kernels (the shape, CL_MEGA=0 or the
+ * device ruled the persistent kernel out); out == NULL with n == 0 reports only that.  cl_debug_hidden(out, n) is this call
+ * on the sequence of the most recent single-sequence step.  CL_ERR_INVALID_ARG for a wrong n or `what`, and for 4 / 5 when
+ * the sequence was not in the latest batched step. */
+int cl_debug_seq_hidden(cl_engine* e, cl_seq_t seq, int32_t what, float* out, int32_t n, int32_t* mega_out);
 /* profiling aid (engine created with env CL_TIMELINE=1): %globaltimer stamps [node][4] = {CTA start,
  * dependency satisfied, inputs loaded / pages consumed, outputs written} of CTA 0 of every kernel node of
  * the most recent token step; nodes = n_layers * {qkv, attn, o, gate|up, down} + lm_head.  Returns the
