@@ -162,6 +162,15 @@ int cl_generate_ids(cl_engine* e, const int32_t* prompt_ids, int32_t n_prompt, c
   CL_GUARD(return e->impl.generate_ids(prompt_ids, n_prompt, sp, out);)
 }
 
+int cl_generate_ids_logprobs(cl_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const cl_sampling* s, int32_t top_n,
+                             cl_result* out, cl_token_logprob** lps) {
+  if (!e || !out || !lps || top_n < 0 || top_n > CL_MAX_TOP_LOGPROBS) return CL_ERR_INVALID_ARG;
+  *lps = nullptr;
+  cl_sampling sp;
+  if (s) sp = *s; else cl_default_sampling(&sp);
+  CL_GUARD(return e->impl.generate_ids(prompt_ids, n_prompt, sp, out, nullptr, top_n, lps);)
+}
+
 namespace {
 // incremental detokeniser: emits only text that later tokens cannot change (an incomplete UTF-8 tail is held back)
 struct StreamText {
@@ -196,8 +205,26 @@ int text_sink(void* u, const int32_t* ids, int n) {
 int64_t wall_ns() {
   return std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::system_clock::now().time_since_epoch()).count();
 }
-std::vector<uint8_t> response_frame(const std::string& model, const std::string& text, bool done, const std::string& reason) {
+// the wire form of records: token = the id's surface bytes alone (cl_tokenizer_decode of that id) as lossy UTF-8, bytes exact
+std::vector<PbTokenLogprob> wire_logprobs(const Tokenizer& tok, const cl_token_logprob* lp, size_t n) {
+  auto one = [&](int32_t id, float v) {
+    PbTokenLogprob t;
+    t.bytes = tok.decode_bytes({id});
+    t.token = Tokenizer::sanitize(t.bytes);
+    t.logprob = v;
+    return t;
+  };
+  std::vector<PbTokenLogprob> out;
+  for (size_t i = 0; i < n; ++i) {
+    out.push_back(one(lp[i].id, lp[i].logprob));
+    for (int j = 0; j < lp[i].n_top; ++j) out.back().top.push_back(one(lp[i].top_ids[j], lp[i].top_logprobs[j]));
+  }
+  return out;
+}
+std::vector<uint8_t> response_frame(const std::string& model, const std::string& text, bool done, const std::string& reason,
+                                    std::vector<PbTokenLogprob> logprobs = {}) {
   PbGenerateResponse pr;
+  pr.logprobs = std::move(logprobs);
   pr.model = model;
   const int64_t ns = wall_ns();
   pr.created_at_sec = ns / 1000000000ll;
@@ -209,13 +236,22 @@ std::vector<uint8_t> response_frame(const std::string& model, const std::string&
   pr.total_duration = done ? ns : 0;       // api.go:84: the reference stores time.Now().UnixNano() here
   return pb_encode_response(pr);
 }
-struct FrameSinkCtx { StreamText st; cl_frame_cb cb; void* user; std::string model; };
+// A frame goes out when the text has a stable delta; the records of its ids ride along.  Records of ids whose text is held
+// back (an open UTF-8 sequence) wait for the next frame, the last ones for the Done=true frame, so the frames' records
+// concatenate to one per generated token.
+struct FrameSinkCtx { StreamText st; cl_frame_cb cb; void* user; std::string model; std::vector<cl_token_logprob> lps; };
 int frame_sink(void* u, const int32_t* ids, int n) {
   auto* c = (FrameSinkCtx*)u;
   const std::string delta = c->st.feed(ids, n, false);
   if (delta.empty()) return 0;
-  const std::vector<uint8_t> f = response_frame(c->model, delta, false, "");
+  const std::vector<uint8_t> f = response_frame(c->model, delta, false, "", wire_logprobs(*c->st.tok, c->lps.data(), c->lps.size()));
+  c->lps.clear();
   return c->cb(c->user, f.data(), f.size());
+}
+int frame_lp_sink(void* u, const cl_token_logprob* lp, int n) {
+  auto* c = (FrameSinkCtx*)u;
+  c->lps.insert(c->lps.end(), lp, lp + n);
+  return 0;
 }
 int check_model(cl_engine* e, const char* model) {
   // exact string match, like Resource.SupportedModels (manager.go:349-354)
@@ -279,23 +315,33 @@ static int handle_message_impl(cl_engine* e, const uint8_t* req, size_t req_len,
   cl_sampling sp;
   if (s) sp = *s; else cl_default_sampling(&sp);
   apply_options(gr.opt, &sp);                                   // request options win over the worker's defaults
+  // logprobs (Ollama's rules): top_logprobs 0..20, and more than 0 only together with logprobs
+  if (gr.opt.top_logprobs < 0 || gr.opt.top_logprobs > CL_MAX_TOP_LOGPROBS || (gr.opt.top_logprobs > 0 && !gr.opt.logprobs)) {
+    set_last_error("top_logprobs must be 0..20 and needs logprobs");
+    return CL_ERR_INVALID_ARG;
+  }
+  const int top_n = gr.opt.logprobs ? gr.opt.top_logprobs : -1;
   std::vector<int32_t> ids = prompt_ids(e, gr.prompt.data(), gr.prompt.size(), gr.opt.raw);
   cl_result r;
+  cl_token_logprob* lps = nullptr;
   if (gr.stream && allow_stream) {
     // streaming (SURVEY.md §8f row 4): Done=false frames carrying text deltas, then one Done=true frame
-    FrameSinkCtx ctx{StreamText{e->impl.tok.get(), {}, 0}, cb, user, gr.model};
-    Engine::TokenSink sink{frame_sink, &ctx};
-    const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r, &sink);
+    FrameSinkCtx ctx{StreamText{e->impl.tok.get(), {}, 0}, cb, user, gr.model, {}};
+    Engine::TokenSink sink{frame_sink, &ctx, top_n >= 0 ? frame_lp_sink : nullptr};
+    const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r, &sink, top_n, top_n >= 0 ? &lps : nullptr);
     if (rc) return rc;
+    free(lps);
     const std::string tail = ctx.st.feed(nullptr, 0, true);
-    const std::vector<uint8_t> f = response_frame(gr.model, tail, true, r.done_reason);
+    const std::vector<uint8_t> f = response_frame(gr.model, tail, true, r.done_reason, wire_logprobs(*e->impl.tok, ctx.lps.data(), ctx.lps.size()));
     cl_result_free(&r);
     cb(user, f.data(), f.size());
     return CL_OK;
   }
-  const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r);
+  const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r, nullptr, top_n, top_n >= 0 ? &lps : nullptr);
   if (rc) return rc;
-  const std::vector<uint8_t> f = response_frame(gr.model, std::string(r.text, r.text_len), true, r.done_reason);
+  std::vector<PbTokenLogprob> wl = lps ? wire_logprobs(*e->impl.tok, lps, (size_t)r.n_generated) : std::vector<PbTokenLogprob>();
+  free(lps);
+  const std::vector<uint8_t> f = response_frame(gr.model, std::string(r.text, r.text_len), true, r.done_reason, std::move(wl));
   cl_result_free(&r);
   cb(user, f.data(), f.size());
   return CL_OK;
@@ -494,6 +540,21 @@ int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, c
   if (!e || !seqs || !input_ids || !ks || !ids_out || !n_out || n_seqs < 1) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
   CL_GUARD(return e->impl.decode_verify_batch(seqs, n_seqs, input_ids, drafts, ks, sp, step0, ids_out, n_out, logits_out, true);)
+}
+int cl_seq_set_logprobs(cl_engine* e, cl_seq_t s, int32_t top_n) {
+  if (!e) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(return e->impl.set_logprobs(s, top_n);)
+}
+int cl_seq_take_logprobs(cl_engine* e, cl_seq_t s, cl_token_logprob* out, int32_t cap, int32_t* n_out) {
+  if (!e || !n_out) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(
+    int n = 0;
+    const int rc = e->impl.take_logprobs(s, out, cap, &n);
+    *n_out = n;
+    return rc;
+  )
 }
 int cl_seq_fake_fill(cl_engine* e, cl_seq_t s, int32_t n_tokens) {
   if (!e) return CL_ERR_INVALID_ARG;

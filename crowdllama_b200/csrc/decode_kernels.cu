@@ -968,6 +968,125 @@ __device__ __forceinline__ int tail_argmax(const float* lg, int V, float* part_v
   return bi == 0x7fffffff ? 0 : bi;   // all-NaN logits: stay in range
 }
 
+// Log-probabilities of one logits row (kernels.h LogprobRecord), called by all kTailBlocks blocks of the row before the
+// choice: each block leaves its slice's (max, sum of expf(v - max)) in part_row and its top-n keys in cand_row; the last
+// block to finish merges them and writes lse, n_top and the top-n into rec (and rec2 when not nullptr).  The id and its
+// logprob are written by the choosing block afterwards (tail_logprob_pick): every record write of this function is fenced
+// before this block takes part in the choice, whose last block therefore sees lse.
+//
+// The top-n are n rounds of "largest key below the previous one" (keys as sample_key: value descending, id ascending): per
+// block over its slice, then one warp merges the kTailBlocks sorted lists.  A radix select (block_topk_threshold) needs
+// its own histogram per instantiation, and the tail kernels' shared memory would then no longer fit 8 blocks per SM.
+__device__ __forceinline__ void tail_logprobs(const float* lg_row, int V, int N, float2* part_row, unsigned long long* cand_row,
+                                           unsigned* counter, LogprobRecord* rec, LogprobRecord* rec2) {
+  __shared__ float red[8];
+  __shared__ unsigned long long kred[2][8];
+  __shared__ int is_last_s;
+  __shared__ double s_lse;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int slice = (V + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int lo = blockIdx.x * slice, n = max(0, min(slice, V - lo));
+  const float* x = lg_row + lo;
+  if (N > V) N = V;
+
+  float m = -INFINITY;
+  for (int i = tid; i < n; i += 256) m = fmaxf(m, x[i]);
+  m = warp_max(m);
+  if (lane == 0) red[warp] = m;
+  __syncthreads();
+  m = red[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) m = fmaxf(m, red[w]);
+  __syncthreads();
+  float s = 0.f;
+  if (m > -INFINITY)
+    for (int i = tid; i < n; i += 256) s += expf(x[i] - m);
+  s = warp_sum(s);
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  if (tid == 0) {
+    float tot = 0.f;
+    for (int w = 0; w < 8; ++w) tot += red[w];
+    part_row[blockIdx.x] = make_float2(m, tot);
+  }
+  unsigned long long* cand = cand_row + (size_t)blockIdx.x * kLogprobTopMax;
+  unsigned long long below = ~0ull;
+  for (int j = 0; j < N; ++j) {   // a short slice leaves empty (0) entries
+    unsigned long long best = 0ull;
+    for (int i = tid; i < n; i += 256) {
+      const unsigned long long k = sample_key(x[i], lo + i);
+      if (k < below && k > best) best = k;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+    if (lane == 0) kred[j & 1][warp] = best;
+    __syncthreads();
+    best = kred[j & 1][0];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) best = max(best, kred[j & 1][w]);
+    if (tid == 0) cand[j] = best;
+    below = best;
+  }
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned old = atomicAdd(counter, 1u);
+    is_last_s = (old == gridDim.x - 1);
+    if (is_last_s) *counter = 0u;
+  }
+  __syncthreads();
+  if (!is_last_s) return;
+  __threadfence();
+
+  // lse = M + log(sum_b s_b exp(m_b - M)), in double and in block order
+  if (tid == 0) {
+    float M = -INFINITY;
+    for (int b = 0; b < (int)gridDim.x; ++b) M = fmaxf(M, __ldcg(&part_row[b].x));
+    double S = 0.0;
+    for (int b = 0; b < (int)gridDim.x; ++b) {
+      const float2 p = __ldcg(part_row + b);
+      if (p.y > 0.f) S += (double)p.y * exp((double)p.x - (double)M);
+    }
+    s_lse = (double)M + log(S);
+    rec->lse = s_lse;
+    rec->n_top = N;
+    if (rec2) { rec2->lse = s_lse; rec2->n_top = N; }
+  }
+  __syncthreads();
+  if (N > 0 && warp == 0) {
+    // k-way merge of the blocks' descending lists: lane l holds the heads of lists l and l + 32 (kTailBlocks = 64)
+    static_assert(kTailBlocks == 64, "two lists per lane");
+    const double lse = s_lse;
+    int h0 = 0, h1 = 0;
+    const unsigned long long* c0 = cand_row + (size_t)lane * kLogprobTopMax;
+    const unsigned long long* c1 = cand_row + (size_t)(lane + 32) * kLogprobTopMax;
+    unsigned long long k0 = __ldcg(c0), k1 = __ldcg(c1);
+    for (int j = 0; j < N; ++j) {
+      unsigned long long best = max(k0, k1);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+      // keys are distinct, so exactly one head equals best
+      if (k0 == best) k0 = ++h0 < N ? __ldcg(c0 + h0) : 0ull;
+      else if (k1 == best) k1 = ++h1 < N ? __ldcg(c1 + h1) : 0ull;
+      if (lane == 0) {
+        const int id = sample_key_id(best);
+        const float lp = __double2float_rn(__dsub_rn((double)sample_key_value(best), lse));
+        rec->top_ids[j] = id; rec->top_logprobs[j] = lp;
+        if (rec2) { rec2->top_ids[j] = id; rec2->top_logprobs[j] = lp; }
+      }
+    }
+  }
+  __threadfence();
+  __syncthreads();
+}
+
+// The choosing thread of an armed row: the chosen id and logit[id] - lse into the record(s) tail_logprobs filled.
+__device__ __forceinline__ void tail_logprob_pick(const float* lg_row, int pick, LogprobRecord* rec, LogprobRecord* rec2) {
+  const float lp = __double2float_rn(__dsub_rn((double)lg_row[pick], __ldcg(&rec->lse)));
+  rec->id = pick; rec->logprob = lp;
+  if (rec2) { rec2->id = pick; rec2->logprob = lp; }
+}
+
 __global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a) {
   pdl_launch_dependents();
   pdl_wait();
@@ -976,6 +1095,14 @@ __global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a)
   const float* lg = a.logits + (size_t)slot * a.vocab;
   const SampleState& S = a.sample;
   const bool sampled = S.mode && S.mode[slot];
+  const LogprobState& P = a.lp;
+  const int lp_n = P.top_n ? P.top_n[slot] : -1;
+  LogprobRecord* lp_ring = nullptr;
+  if (lp_n >= 0) {
+    if (P.ring) lp_ring = P.ring + (size_t)(*a.step_counter % a.ring_steps) * a.ring_stride + b;
+    tail_logprobs(lg, a.vocab, lp_n, P.part + (size_t)slot * gridDim.x, P.cand + (size_t)slot * gridDim.x * kLogprobTopMax,
+                  P.counters + slot, P.last + slot, lp_ring);
+  }
   int pick;
   if (sampled) {
     const TailHist h{S.hist + (size_t)slot * kSampleHistMax, S.hist_len[slot], a.tok + slot, S.push_input};
@@ -985,6 +1112,7 @@ __global__ void __launch_bounds__(256, 8) step_tail_kernel(const StepTailArgs a)
     pick = tail_argmax(lg, a.vocab, a.part_val + (size_t)slot * gridDim.x, a.part_idx + (size_t)slot * gridDim.x, a.counters + slot);
   }
   if (pick < 0) return;
+  if (lp_n >= 0) tail_logprob_pick(lg, pick, P.last + slot, lp_ring);
   if (sampled) {
     if (S.push_input) {
       const int hlen = S.hist_len[slot];
@@ -1009,6 +1137,11 @@ __global__ void __launch_bounds__(256, 8) spec_tail_kernel(const SpecTailArgs a)
   const int r = blockIdx.y, slot = a.slot;
   const float* lg = a.logits + (size_t)r * a.vocab;
   const SampleState& S = a.sample;
+  const LogprobState& P = a.lp;
+  const int lp_n = P.top_n ? P.top_n[slot] : -1;
+  if (lp_n >= 0)
+    tail_logprobs(lg, a.vocab, lp_n, P.part + (size_t)r * gridDim.x, P.cand + (size_t)r * gridDim.x * kLogprobTopMax, P.counters + r,
+                  P.last + r, nullptr);
   int pick;
   if (S.mode[slot]) {
     const TailHist h{S.hist + (size_t)slot * kSampleHistMax, S.hist_len[slot], a.inputs, r + 1};
@@ -1016,7 +1149,10 @@ __global__ void __launch_bounds__(256, 8) spec_tail_kernel(const SpecTailArgs a)
   } else {
     pick = tail_argmax(lg, a.vocab, a.part_val + (size_t)r * gridDim.x, a.part_idx + (size_t)r * gridDim.x, a.counters + r);
   }
-  if (pick >= 0) a.choice[r] = pick;
+  if (pick >= 0) {
+    a.choice[r] = pick;
+    if (lp_n >= 0) tail_logprob_pick(lg, pick, P.last + r, nullptr);
+  }
 }
 
 // One block after spec_tail_kernel: a = the drafts d_1 .. d_a that equal the choices y_1 .. y_a; the pass emits

@@ -38,6 +38,7 @@ Engine::~Engine() {
   if (h_logits_pinned_) cudaFreeHost(h_logits_pinned_);
   if (host_kv_) cudaFreeHost(host_kv_);
   if (h_ids_pinned_) cudaFreeHost(h_ids_pinned_);
+  if (h_lp_pinned_) cudaFreeHost(h_lp_pinned_);
   if (ev0_) cudaEventDestroy(ev0_);
   if (ev1_) cudaEventDestroy(ev1_);
   if (stream_) cudaStreamDestroy(stream_);
@@ -343,6 +344,17 @@ int Engine::alloc_state() {
   DMALLOC(d_samp_cand_, S * kTailBlocks * kSampleTopKMax * 8);
   CL_CUDA_OK(cudaMemsetAsync(d_samp_mode_, 0, S * 4, stream_));
   samp_hlen_.assign(S, -1);
+  // logprobs: the captured step graphs point at these, so they exist from the start (the ring and its pinned mirror hold
+  // ring_steps_ x max_batch_ records of 184 bytes: 24.1 MB each at max_batch 128)
+  DMALLOC(d_lp_n_, S * 4);
+  DMALLOC(d_lp_part_, S * kTailBlocks * sizeof(float2));
+  DMALLOC(d_lp_cand_, S * kTailBlocks * kLogprobTopMax * 8);
+  DMALLOC(d_lp_cnt_, S * 4);
+  DMALLOC(d_lp_last_, S * sizeof(LogprobRecord));
+  DMALLOC(d_lp_ring_, (size_t)ring_steps_ * max_batch_ * sizeof(LogprobRecord));
+  CL_CUDA_OK(cudaMemsetAsync(d_lp_n_, 0xFF, S * 4, stream_));   // -1: off
+  CL_CUDA_OK(cudaMemsetAsync(d_lp_cnt_, 0, S * 4, stream_));
+  lp_n_.assign(S, -1);
   DMALLOC(d_ids_ring_, (size_t)ring_steps_ * max_batch_ * 4);
   DMALLOC(d_step_counter_, 4);
   n_sync_ = cfg.n_layers * 10 + 1;   // persistent kernel: 6 grid barriers + 4 tile counters per layer + the lookahead frontier
@@ -386,6 +398,7 @@ int Engine::alloc_state() {
   CL_CUDA_OK(cudaMemsetAsync(d_step_counter_, 0, 4, stream_));
   CL_CUDA_OK(cudaMallocHost(&h_logits_pinned_, (size_t)cfg.vocab_size * 4));
   CL_CUDA_OK(cudaMallocHost(&h_ids_pinned_, (size_t)ring_steps_ * max_batch_ * 4));
+  CL_CUDA_OK(cudaMallocHost(&h_lp_pinned_, (size_t)std::max(ring_steps_ * max_batch_, max_seqs_) * sizeof(LogprobRecord)));
   return CL_OK;
 }
 
@@ -396,7 +409,8 @@ int Engine::seq_create(cl_seq_t* out) {
       seqs_[i] = SeqState();
       seqs_[i].live = true;
       *out = i;
-      return disarm_sampling(i);
+      const int rc = disarm_sampling(i);
+      return rc ? rc : upload_logprobs(i, -1);
     }
   set_last_error("no free sequence slot (max_seqs)");
   return CL_ERR_OOM;
@@ -405,7 +419,46 @@ int Engine::seq_free(cl_seq_t s) {
   if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
   pool_->release(s);
   seqs_[s] = SeqState();
-  return disarm_sampling(s);
+  const int rc = disarm_sampling(s);
+  return rc ? rc : upload_logprobs(s, -1);
+}
+
+int Engine::set_logprobs(cl_seq_t s, int top_n) {
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  if (top_n < -1 || top_n > kLogprobTopMax) { set_last_error("logprobs: top_n must be -1..20"); return CL_ERR_INVALID_ARG; }
+  if (top_n >= 0 && cfg.vocab_size > kTailBlocks * kSampleSliceMax) { set_last_error("logprobs: vocabulary above 163840"); return CL_ERR_INVALID_ARG; }
+  seqs_[s].lps.clear();
+  return upload_logprobs(s, top_n);
+}
+
+int Engine::upload_logprobs(cl_seq_t s, int top_n) {
+  if (lp_n_[s] == top_n) return CL_OK;
+  CL_CUDA_OK(cudaMemcpyAsync(d_lp_n_ + s, &top_n, 4, cudaMemcpyHostToDevice, stream_));
+  lp_n_[s] = top_n;
+  return CL_OK;
+}
+
+int Engine::take_logprobs(cl_seq_t s, cl_token_logprob* out, int cap, int* n_out) {
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  auto& q = seqs_[s].lps;
+  if (!out) { *n_out = (int)q.size(); return CL_OK; }
+  if (cap < 0) return CL_ERR_INVALID_ARG;
+  const int n = std::min(cap, (int)q.size());
+  for (int i = 0; i < n; ++i) out[i] = to_token_logprob(q[(size_t)i]);
+  q.erase(q.begin(), q.begin() + n);
+  *n_out = n;
+  return CL_OK;
+}
+
+int Engine::collect_logprobs(const cl_seq_t* ss, int n) {
+  bool any = false;
+  for (int i = 0; i < n; ++i) any = any || lp_n_[ss[i]] >= 0;
+  if (!any) return CL_OK;
+  CL_CUDA_OK(cudaMemcpyAsync(h_lp_pinned_, d_lp_last_, (size_t)max_seqs_ * sizeof(LogprobRecord), cudaMemcpyDeviceToHost, stream_));
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  for (int i = 0; i < n; ++i)
+    if (lp_n_[ss[i]] >= 0) seqs_[ss[i]].lps.push_back(h_lp_pinned_[ss[i]]);
+  return CL_OK;
 }
 
 int Engine::arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist) {
@@ -686,6 +739,8 @@ int Engine::enqueue_step_tail(int B, bool push_input) {
   SampleState& smp = t.sample;
   smp.mode = d_samp_mode_; smp.par = d_samp_par_; smp.step = d_samp_step_; smp.hist = d_samp_hist_; smp.hist_len = d_samp_hlen_;
   smp.cand = d_samp_cand_; smp.push_input = push_input ? 1 : 0;
+  LogprobState& lp = t.lp;
+  lp.top_n = d_lp_n_; lp.part = d_lp_part_; lp.cand = d_lp_cand_; lp.counters = d_lp_cnt_; lp.last = d_lp_last_; lp.ring = d_lp_ring_;
   return launch_step_tail(t, stream_);
 }
 
@@ -849,6 +904,7 @@ int Engine::decode_step(cl_seq_t s, int32_t id, float* logits_out, int32_t* argm
   rc = run_step_graph(1);
   if (rc) return rc;
   seq_advance(s, &id, 1, 1);
+  if ((rc = collect_logprobs(&s, 1))) return rc;
   if (logits_out) { rc = read_logits(s, logits_out); if (rc) return rc; }
   if (argmax_out) {
     CL_CUDA_OK(cudaMemcpyAsync(h_ids_pinned_, d_tok_ + s, 4, cudaMemcpyDeviceToHost, stream_));
@@ -873,12 +929,16 @@ int Engine::prefill_tokenwise(cl_seq_t s, const int32_t* ids, int n, float* logi
   const int armed_hlen = samp_hlen_[s];
   const int off = 0, on = 1, hlen_before_last = std::max(0, armed_hlen - 1);
   if (armed_hlen >= 0 && n > 1) CL_CUDA_OK(cudaMemcpyAsync(d_samp_mode_ + s, &off, 4, cudaMemcpyHostToDevice, stream_));
+  // likewise only the last token's tail records logprobs
+  const int lp_off = -1, lp_on = lp_n_[s];
+  if (lp_on >= 0 && n > 1) CL_CUDA_OK(cudaMemcpyAsync(d_lp_n_ + s, &lp_off, 4, cudaMemcpyHostToDevice, stream_));
   for (int i = 0; i < n; ++i) {
     CL_CUDA_OK(cudaMemcpyAsync(d_tok_ + s, d_prompt_ + i, 4, cudaMemcpyDeviceToDevice, stream_));
     if (armed_hlen >= 0 && i == n - 1) {
       CL_CUDA_OK(cudaMemcpyAsync(d_samp_mode_ + s, &on, 4, cudaMemcpyHostToDevice, stream_));
       CL_CUDA_OK(cudaMemcpyAsync(d_samp_hlen_ + s, &hlen_before_last, 4, cudaMemcpyHostToDevice, stream_));
     }
+    if (lp_on >= 0 && n > 1 && i == n - 1) CL_CUDA_OK(cudaMemcpyAsync(d_lp_n_ + s, &lp_on, 4, cudaMemcpyHostToDevice, stream_));
     rc = run_step_graph(1);
     if (rc) return rc;
   }
@@ -894,12 +954,15 @@ int Engine::prefill(cl_seq_t s, const int32_t* ids, int n, float* logits_out) {
   for (int i = 0; i < n; ++i)
     if (ids[i] < 0 || ids[i] >= cfg.vocab_size) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
   if (seqs_[s].len + n > cfg.max_seq_len) { set_last_error("sequence exceeds max_seq_len"); return CL_ERR_TOO_LONG; }
+  int rc;
   if (n >= prefill_min_tokens_ && prefill_path_ok()) {
     // short prompts: split-K projections so that every SM streams weights (d_model <= 8192: one 1024-thread CTA per row in the glue)
-    if (n <= prefill_small_max_ && cfg.d_model <= 8192 && cfg.d_model % 4 == 0) return prefill_small(s, ids, n, logits_out);
-    return prefill_chunked(s, ids, n, logits_out);
+    if (n <= prefill_small_max_ && cfg.d_model <= 8192 && cfg.d_model % 4 == 0) rc = prefill_small(s, ids, n, logits_out);
+    else rc = prefill_chunked(s, ids, n, logits_out);
+  } else {
+    rc = prefill_tokenwise(s, ids, n, logits_out);
   }
-  return prefill_tokenwise(s, ids, n, logits_out);
+  return rc ? rc : collect_logprobs(&s, 1);
 }
 
 int Engine::decode_greedy(const cl_seq_t* ss, int B, const int32_t* first_ids, int n_steps, int32_t* ids_out, float* device_ms) {
@@ -938,6 +1001,12 @@ int Engine::decode_greedy(const cl_seq_t* ss, int B, const int32_t* first_ids, i
     total_ms += ms;
     for (int i = 0; i < chunk; ++i)
       for (int b = 0; b < B; ++b) ids_out[(size_t)(done + i) * B + b] = h_ids_pinned_[(size_t)i * max_batch_ + b];
+    if (std::any_of(ss, ss + B, [&](cl_seq_t s) { return lp_n_[s] >= 0; })) {   // the record ring, only when a slot records
+      CL_CUDA_OK(cudaMemcpy(h_lp_pinned_, d_lp_ring_, (size_t)chunk * max_batch_ * sizeof(LogprobRecord), cudaMemcpyDeviceToHost));
+      for (int i = 0; i < chunk; ++i)
+        for (int b = 0; b < B; ++b)
+          if (lp_n_[ss[b]] >= 0) seqs_[ss[b]].lps.push_back(h_lp_pinned_[(size_t)i * max_batch_ + b]);
+    }
     done += chunk;
   }
   std::vector<int32_t> fed((size_t)n_steps);
@@ -1033,8 +1102,9 @@ int Engine::decode_step_batch(const cl_seq_t* ss, int B, const int32_t* ids, flo
   last_single_slot_ = B == 1 ? ss[0] : -1;
   if (B > 1) last_batch_slots_.assign(ss, ss + B);
   slots_dirty_ = true;
-  const int rc = run_step_graph(B);
+  int rc = run_step_graph(B);
   if (rc) return rc;
+  if ((rc = collect_logprobs(ss, B))) return rc;
   for (int b = 0; b < B; ++b) {
     seq_advance(ss[b], &ids[b], 1, 1);
     if (logits_out) { const int r2 = read_logits(ss[b], logits_out + (size_t)b * cfg.vocab_size); if (r2) return r2; }

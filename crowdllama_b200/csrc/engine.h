@@ -39,6 +39,16 @@ constexpr int kSpecBatchMax = 32;     // sequences the scheduler verifies in one
 // hist) go to out.  Returns how many (0: no match).
 int ngram_draft(const int32_t* hist, int n, int k, int32_t* out);
 
+// the C-ABI view of a step tail record (lse stays internal)
+inline cl_token_logprob to_token_logprob(const LogprobRecord& r) {
+  cl_token_logprob o{};
+  o.id = r.id; o.logprob = r.logprob; o.n_top = r.n_top;
+  for (int j = 0; j < r.n_top && j < kLogprobTopMax; ++j) { o.top_ids[j] = r.top_ids[j]; o.top_logprobs[j] = r.top_logprobs[j]; }
+  return o;
+}
+static_assert(sizeof(cl_token_logprob) == 172, "cl_token_logprob is 172 bytes");
+static_assert(kLogprobTopMax == CL_MAX_TOP_LOGPROBS, "one top-n limit");
+
 void set_last_error(const std::string& s);
 const char* get_last_error();
 
@@ -240,14 +250,17 @@ struct PbGenerateOptions {
   uint32_t has = 0;   // bit i set <=> field number i present
   uint64_t seed = 0; float temperature = 0.f; int32_t top_k = 0; float top_p = 0.f; float repeat_penalty = 0.f;
   int32_t repeat_last_n = 0; int32_t num_predict = 0; bool raw = false;
+  bool logprobs = false; int32_t top_logprobs = 0;   // Ollama's top-level logprobs / top_logprobs (fields 9, 10)
 };
 struct PbGenerateRequest { std::string model, prompt; bool stream = false; PbGenerateOptions opt; };
 // request options override the caller's default sampling field by field
 void apply_options(const PbGenerateOptions& o, cl_sampling* sp);
+struct PbTokenLogprob { std::string token, bytes; float logprob = 0.f; std::vector<PbTokenLogprob> top; };
 struct PbGenerateResponse {
   std::string model, response, done_reason, worker_id;
   int64_t created_at_sec = 0; int32_t created_at_nanos = 0;
   bool done = false; int64_t total_duration = 0;
+  std::vector<PbTokenLogprob> logprobs;   // field 8: the records of this frame's tokens
 };
 bool pb_decode_request(const uint8_t* data, size_t len, PbGenerateRequest* out);  // false: not a GenerateRequest
 std::vector<uint8_t> pb_encode_response(const PbGenerateResponse& r);
@@ -266,6 +279,7 @@ struct SeqState {
   int len = 0;            // tokens whose K/V are in the cache
   int known = 0;          // leading history ids that are the real tokens of the cached K/V (seq_fake_fill's are not)
   std::vector<int32_t> history;
+  std::vector<LogprobRecord> lps;   // records of the ids the step tail chose while logprobs were on, not taken yet
 };
 
 struct Request;  // scheduler.cpp
@@ -302,6 +316,11 @@ class Engine {
   int arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist);
   int disarm_sampling(cl_seq_t s);
   int read_next_token(cl_seq_t s, int32_t* out);   // d_tok_[s]: what the last step tail of `s` chose
+  // Log-probabilities (contract in include/clengine.h, cl_seq_set_logprobs): top_n -1 = off, 0..kLogprobTopMax = every
+  // later step tail of `s` leaves a record, which the call that ran it appends to seqs_[s].lps.  seq_create / seq_free disarm.
+  int set_logprobs(cl_seq_t s, int top_n);
+  int take_logprobs(cl_seq_t s, cl_token_logprob* out, int cap, int* n_out);
+  bool logprobs_on(cl_seq_t s) const { return lp_n_[s] >= 0; }
   // Speculative decoding: one verify pass over n_seqs distinct sequences (prefill.cu; contract in include/clengine.h,
   // cl_decode_verify_batch): sequence i verifies x0[i] and ks[i] (0..15) drafts, taken back to back from drafts.  Its ids
   // land at ids_out + its first row (the sum of k_j + 1 over the sequences before it), n_out[i] = a + 1 of them; logits_out
@@ -337,8 +356,14 @@ class Engine {
 
   // request-level (scheduler.cpp)
   // sink (optional): called on the CALLING thread with every batch of newly generated ids; nonzero return cancels
-  struct TokenSink { int (*fn)(void* user, const int32_t* ids, int n) = nullptr; void* user = nullptr; };
-  int generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink = nullptr);
+  // lp_fn (optional, with logprobs on): called just before fn with the records of the same ids
+  struct TokenSink {
+    int (*fn)(void* user, const int32_t* ids, int n) = nullptr; void* user = nullptr;
+    int (*lp_fn)(void* user, const cl_token_logprob* lps, int n) = nullptr;
+  };
+  // top_n >= 0: logprobs on for the request; *lps (malloc'd, one record per generated id) when lps is not nullptr
+  int generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink = nullptr,
+                   int top_n = -1, cl_token_logprob** lps = nullptr);
   void scheduler_main();
   void start_scheduler();
   void stop_scheduler();
@@ -371,6 +396,10 @@ class Engine {
   bool ensure_graph(int B);
   void precapture_graphs();                       // graph launch (or eager enqueue)
   int read_logits(int slot, float* out);
+  // After a call whose step tail ran once for the sequences ss[0..n): each one with logprobs on appends its record
+  // (d_lp_last_) to its pending list.  Nothing is copied when none is on.  Synchronises the stream.
+  int collect_logprobs(const cl_seq_t* ss, int n);
+  int upload_logprobs(cl_seq_t s, int top_n);     // d_lp_n_[s] = top_n unless it holds it already
   int prefill_tokenwise(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
   int prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits_out);
   int ensure_prefill_ws(int tokens);  // tensor-core path (prefill.cu)
@@ -453,6 +482,10 @@ class Engine {
   int* d_samp_mode_ = nullptr; SampleParams* d_samp_par_ = nullptr; unsigned long long* d_samp_step_ = nullptr;
   int* d_samp_hist_ = nullptr; int* d_samp_hlen_ = nullptr; unsigned long long* d_samp_cand_ = nullptr;
   std::vector<int> samp_hlen_;        // host: history length uploaded by arm_sampling, -1 = disarmed
+  // log-probabilities (kernels.h LogprobState), indexed by sequence handle; the ring runs parallel to the id ring
+  int* d_lp_n_ = nullptr; float2* d_lp_part_ = nullptr; unsigned long long* d_lp_cand_ = nullptr; unsigned* d_lp_cnt_ = nullptr;
+  LogprobRecord* d_lp_last_ = nullptr; LogprobRecord* d_lp_ring_ = nullptr; LogprobRecord* h_lp_pinned_ = nullptr;
+  std::vector<int> lp_n_;             // host mirror of d_lp_n_
   bool device_sample_ = true;         // CL_DEVICE_SAMPLE: the scheduler and the synchronous path draw on the device where they can
 
   // prefill workspace (allocated lazily)
@@ -473,7 +506,8 @@ class Engine {
   // segs [rows][8], attn_part and attn_cnt: the multi-row attention's segment table, split partials and counters
   struct SpecWs { float* logits = nullptr; int* choice = nullptr; float* part_val = nullptr; int* part_idx = nullptr;
                   unsigned* counters = nullptr; unsigned long long* cand = nullptr; int* out = nullptr; int* row_map = nullptr;
-                  int* segs = nullptr; float* attn_part = nullptr; unsigned* attn_cnt = nullptr; };
+                  int* segs = nullptr; float* attn_part = nullptr; unsigned* attn_cnt = nullptr;
+                  float2* lp_part = nullptr; unsigned long long* lp_cand = nullptr; unsigned* lp_cnt = nullptr; LogprobRecord* lp_rows = nullptr; };
   int verify_split_pages() const;     // pages per split of the multi-row attention (a function of max_seq_len only)
   std::unique_ptr<SpecWs> spec_;
   int speculate_ = 0;                 // most drafted tokens per verify pass in the scheduler / synchronous path (0 = off)

@@ -87,6 +87,30 @@ struct SampleState {
   int push_input = 0;                   // 1 (decode steps): tok[slot], the step's input, joins the history before the draw
 };
 
+// Per-token log-probabilities of the step tail: natural-log log_softmax of the raw fp32 logits row (before the repeat
+// penalty, temperature, top-k and top-p), whatever the sampler then does with it.  Every block of the row keys its slice
+// (slice max, sum of expf(v - max), its top-n keys), the row's last block merges the kTailBlocks partials in fixed block
+// order (lse in double) and writes lse and the top-n (value descending, id ascending); the block that makes the row's choice
+// then writes the chosen id and logit[id] - lse.  Every logprob is (double)logit - lse rounded to fp32: an fp32 lse would
+// carry half an ulp of the row's largest logits (5e-4 at 1e4).  A record thus depends on its logits row alone.
+constexpr int kLogprobTopMax = 20;
+struct LogprobRecord {                   // 184 bytes
+  double lse;                            // log of the row's softmax denominator, max included
+  int id;                                // the chosen id
+  float logprob;                         // (double)logit[id] - lse, rounded to fp32
+  int n_top;
+  int top_ids[kLogprobTopMax];
+  float top_logprobs[kLogprobTopMax];    // (double)logit - lse, rounded to fp32
+};
+struct LogprobState {
+  const int* top_n = nullptr;            // [slot] -1: off, 0..kLogprobTopMax: on with that many alternatives (nullptr: off everywhere)
+  float2* part = nullptr;                // [row][kTailBlocks] slice (max, sum of exp(v - max))
+  unsigned long long* cand = nullptr;    // [row][kTailBlocks][kLogprobTopMax] slice top-n keys
+  unsigned* counters = nullptr;          // [row], zero between launches
+  LogprobRecord* last = nullptr;         // [row]: the row's latest record
+  LogprobRecord* ring = nullptr;         // step tail only (may be nullptr): [ring_steps][ring_stride], parallel to the id ring
+};
+
 struct StepTailArgs {                // argmax (or a draw) over logits, advance the sequence
   const float* logits = nullptr;     // [slot][vocab]
   int vocab = 0;
@@ -103,6 +127,7 @@ struct StepTailArgs {                // argmax (or a draw) over logits, advance 
   const int* slots = nullptr;
   int batch = 1;
   SampleState sample;
+  LogprobState lp;                   // rows = slots
 };
 
 // Verify pass of speculative decoding for one slot (a segment of Engine::verify_batch): T = k + 1 rows with inputs x0, d1 .. dk.
@@ -122,6 +147,7 @@ struct SpecTailArgs {
   int* pos = nullptr;                // [slot] its position (written: len + a + 1)
   int* out = nullptr;                // [1 + T] a + 1, then y_1 .. y_{a+1}
   SampleState sample;                // mode / par / step / hist / hist_len of the slot (cand and push_input unused)
+  LogprobState lp;                   // top_n of the slot; part / cand / counters / last per row of the pass (row r = y_{r+1}'s record)
 };
 
 // every launcher returns the number of kernels it enqueued (for cl_stats.kernel_launches)

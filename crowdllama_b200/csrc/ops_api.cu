@@ -530,14 +530,18 @@ int cl_op_qkv_rope_append(int device, int variant, const uint16_t* w_qkv, const 
   return CL_OK;
 }
 
-int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
-                 const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out) {
+// cl_op_sample, and with top_n >= 0 cl_op_sample_logprobs (rows with temperature <= 0 then take the greedy choice)
+static int op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
+                     const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t top_n, int32_t* ids_out,
+                     cl_token_logprob* lp_out) {
   if (!logits || n_rows <= 0 || vocab <= 1 || !sp || !n_history || !step || !ids_out) return CL_ERR_INVALID_ARG;
+  if (top_n >= 0 && (top_n > kLogprobTopMax || !lp_out || vocab > kTailBlocks * kSampleSliceMax)) return CL_ERR_INVALID_ARG;
   const size_t R = (size_t)n_rows;
   std::vector<SampleParams> par(R);
   std::vector<int> ring(R * kSampleHistMax, 0), hlen(R), mode(R, 1);
   for (size_t r = 0; r < R; ++r) {
-    if (!device_sampling_ok(sp[r], vocab)) { set_last_error("cl_op_sample: settings the device sampler does not cover"); return CL_ERR_INVALID_ARG; }
+    if (top_n >= 0 && !(sp[r].temperature > 0.f)) mode[r] = 0;
+    else if (!device_sampling_ok(sp[r], vocab)) { set_last_error("cl_op_sample: settings the device sampler does not cover"); return CL_ERR_INVALID_ARG; }
     const int n = n_history[r];
     if (n < 0 || (n > 0 && (!history || n > hist_stride))) return CL_ERR_INVALID_ARG;
     par[r].temperature = sp[r].temperature; par[r].top_p = sp[r].top_p; par[r].repeat_penalty = sp[r].repeat_penalty;
@@ -573,10 +577,39 @@ int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab,
   t.sample.mode = dmode.as<int>(); t.sample.par = dpar.as<SampleParams>(); t.sample.step = dstep.as<unsigned long long>();
   t.sample.hist = dhist.as<int>(); t.sample.hist_len = dhlen.as<int>(); t.sample.cand = dcand.as<unsigned long long>();
   t.sample.push_input = 0;
+  DevBuf dlpn, dlpart, dlcand, dlcnt, dlrec;
+  if (top_n >= 0) {
+    const std::vector<int> lpn(R, top_n);
+    CL_CUDA_OK(dlpn.upload(lpn.data(), R * 4));
+    CL_CUDA_OK(dlpart.alloc(R * kTailBlocks * sizeof(float2)));
+    CL_CUDA_OK(dlcand.alloc(R * kTailBlocks * kLogprobTopMax * 8));
+    CL_CUDA_OK(dlcnt.alloc(R * 4));
+    CL_CUDA_OK(dlrec.alloc(R * sizeof(LogprobRecord)));
+    CL_CUDA_OK(cudaMemset(dlcnt.p, 0, R * 4));
+    t.lp.top_n = dlpn.as<int>(); t.lp.part = dlpart.as<float2>(); t.lp.cand = dlcand.as<unsigned long long>();
+    t.lp.counters = dlcnt.as<unsigned>(); t.lp.last = dlrec.as<LogprobRecord>();
+  }
   if (launch_step_tail(t, nullptr) < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("launch_step_tail failed"); return CL_ERR_CUDA; }
   CL_CUDA_OK(cudaDeviceSynchronize());
   CL_CUDA_OK(cudaMemcpy(ids_out, dtok.p, R * 4, cudaMemcpyDeviceToHost));
+  if (top_n >= 0) {
+    std::vector<LogprobRecord> rec(R);
+    CL_CUDA_OK(cudaMemcpy(rec.data(), dlrec.p, R * sizeof(LogprobRecord), cudaMemcpyDeviceToHost));
+    for (size_t r = 0; r < R; ++r) lp_out[r] = to_token_logprob(rec[r]);
+  }
   return CL_OK;
+}
+
+int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
+                 const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out) {
+  return op_sample(device, logits, n_rows, vocab, sp, history, n_history, hist_stride, step, -1, ids_out, nullptr);
+}
+
+int cl_op_sample_logprobs(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
+                          const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t top_n, int32_t* ids_out,
+                          cl_token_logprob* lp_out) {
+  if (top_n < 0) return CL_ERR_INVALID_ARG;
+  return op_sample(device, logits, n_rows, vocab, sp, history, n_history, hist_stride, step, top_n, ids_out, lp_out);
 }
 
 int cl_op_synth_weights(int device, uint64_t seed, int32_t tensor_key, int64_t n, float scale, uint16_t* out_bf16) {

@@ -164,13 +164,17 @@ int Engine::ensure_spec_ws() {
       (rc = ws_alloc(allocs_, spec_->part_val, R * kTailBlocks * 4)) || (rc = ws_alloc(allocs_, spec_->part_idx, R * kTailBlocks * 4)) ||
       (rc = ws_alloc(allocs_, spec_->counters, R * 4)) || (rc = ws_alloc(allocs_, spec_->cand, R * kTailBlocks * kSampleTopKMax * 8)) ||
       (rc = ws_alloc(allocs_, spec_->out, 2 * R * 4)) || (rc = ws_alloc(allocs_, spec_->row_map, 2 * R * 4)) ||
-      (rc = ws_alloc(allocs_, spec_->segs, R * 8 * 4)) || (rc = ws_alloc(allocs_, spec_->attn_cnt, R * cfg.n_kv_heads * 4))) { spec_.reset(); return rc; }
+      (rc = ws_alloc(allocs_, spec_->segs, R * 8 * 4)) || (rc = ws_alloc(allocs_, spec_->attn_cnt, R * cfg.n_kv_heads * 4)) ||
+      (rc = ws_alloc(allocs_, spec_->lp_part, R * kTailBlocks * sizeof(float2))) ||
+      (rc = ws_alloc(allocs_, spec_->lp_cand, R * kTailBlocks * kLogprobTopMax * 8)) || (rc = ws_alloc(allocs_, spec_->lp_cnt, R * 4)) ||
+      (rc = ws_alloc(allocs_, spec_->lp_rows, R * sizeof(LogprobRecord)))) { spec_.reset(); return rc; }
   // the multi-row attention's split partials: at most 4 query rows per pass row, per kv head and split
   if (attn_verify_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_)) {
     const size_t max_splits = (max_pages_per_seq_ + verify_split_pages() - 1) / verify_split_pages();
     if ((rc = ws_alloc(allocs_, spec_->attn_part, R * 4 * cfg.n_kv_heads * max_splits * (cfg.head_dim + 2) * 4))) { spec_.reset(); return rc; }
   }
   CL_CUDA_OK(cudaMemsetAsync(spec_->counters, 0, R * 4, stream_));
+  CL_CUDA_OK(cudaMemsetAsync(spec_->lp_cnt, 0, R * 4, stream_));
   CL_CUDA_OK(cudaMemsetAsync(spec_->attn_cnt, 0, R * cfg.n_kv_heads * 4, stream_));
   return CL_OK;
 }
@@ -194,6 +198,8 @@ SpecTailArgs Engine::spec_tail_args(const PrefillSegment& g, int out_off) const 
   t.tok = d_tok_; t.pos = d_pos_; t.out = spec_->out + out_off;
   t.sample.mode = d_samp_mode_; t.sample.par = d_samp_par_; t.sample.step = d_samp_step_; t.sample.hist = d_samp_hist_;
   t.sample.hist_len = d_samp_hlen_;
+  t.lp.top_n = d_lp_n_; t.lp.part = spec_->lp_part + r0 * kTailBlocks; t.lp.cand = spec_->lp_cand + r0 * kTailBlocks * kLogprobTopMax;
+  t.lp.counters = spec_->lp_cnt + r0; t.lp.last = spec_->lp_rows + r0;
   return t;
 }
 
@@ -271,10 +277,14 @@ int Engine::verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, cons
     const int n = h_ids_pinned_[segs[i].row0 + i];
     if (n < 1 || n > segs[i].n) { set_last_error("verify: accept kernel returned a bad count"); return CL_ERR_INTERNAL; }
   }
+  // the records of a sequence's emitted ids y_1 .. y_{a+1} are those of its leading rows
+  if (std::any_of(ss, ss + n_seqs, [&](cl_seq_t s) { return lp_n_[s] >= 0; }))
+    CL_CUDA_OK(cudaMemcpy(h_lp_pinned_, spec_->lp_rows, (size_t)T * sizeof(LogprobRecord), cudaMemcpyDeviceToHost));
   int accepted = 0, emitted = 0;
   for (int i = 0; i < n_seqs; ++i) {
     const PrefillSegment& g = segs[i];
     const int n = h_ids_pinned_[g.row0 + i];
+    if (lp_n_[g.seq] >= 0) seqs_[g.seq].lps.insert(seqs_[g.seq].lps.end(), h_lp_pinned_ + g.row0, h_lp_pinned_ + g.row0 + n);
     memcpy(ids_out + g.row0, h_ids_pinned_ + g.row0 + i + 1, (size_t)n * 4);
     n_out[i] = n;
     seq_advance(g.seq, in.data() + g.row0, n, n);   // x0, d1 .. da: only accepted tokens join the history and the prefix cache
@@ -463,6 +473,7 @@ int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* 
   prof.report("prefill profile", 32, "multi-prompt tile path, " + std::to_string(total) + " tokens");
   launches_ += launches;
   for (int i = 0; i < n_seqs; ++i) seq_advance(ss[i], ids[i], lens[i], lens[i]);
+  if ((rc = collect_logprobs(ss, n_seqs))) return rc;
   if (logits_out) {
     for (int i = 0; i < n_seqs; ++i)
       if ((rc = read_logits(ss[i], logits_out + (size_t)i * V))) return rc;

@@ -41,6 +41,10 @@ struct Request {
   std::vector<int32_t> full;        // prompt + out as of the last sync_full()
   size_t prefilled = 0;             // tokens of `full` already in the cache (chunked admission)
   bool dev_sample = false;          // sampled, and the step tail draws its tokens (device_sampling_ok, CL_DEVICE_SAMPLE)
+  int top_n = -1;                   // logprobs: -1 off, else the alternatives per record (the sequence is armed with it)
+  std::vector<LogprobRecord> lps;   // one record per id of `out` (kept across preemptions)
+  std::vector<LogprobRecord> pub_lps;   // streaming: the records of `pub` (guarded by m)
+  bool lp_mismatch = false;         // an id joined without its own record: the request fails with CL_ERR_INTERNAL
   int spec_backoff = 0;             // tokens to decode without drafting (after a verify pass that accepted nothing)
   bool greedy() const { return sp.temperature <= 0.f; }
   bool device_next() const { return greedy() || dev_sample; }   // the next id is d_tok_ after the step: no host sampler
@@ -83,25 +87,43 @@ static bool finished(Request& r, const Tokenizer& tok, int max_seq_len) {
 // only, by one rule.  An id from a decode step or verify pass of the scheduler counts as it joins.  An id chosen at
 // admission counts only when the request finishes with it: a request that goes on decoding never counts its admission id.
 // The synchronous path counts r.out.size() when it retires successfully.
+// With logprobs on, the i-th id takes the i-th record the calls since the last join left on r's sequence (the step tail's
+// record of exactly that id); records of ids that did not join are dropped.  A missing record, or one of another id, is a
+// defect: the request then fails when it retires instead of returning a wrong record.
 bool Engine::join(Request& r, const int32_t* ids, int n, bool admission) {
+  std::vector<LogprobRecord>* pending = r.top_n >= 0 ? &seqs_[r.seq].lps : nullptr;
   int joined = 0;
   bool fin = false;
   while (joined < n && !fin) {
+    if (pending) {
+      LogprobRecord rec{};
+      rec.id = -1;
+      if (joined < (int)pending->size()) rec = (*pending)[(size_t)joined];
+      if (rec.id != ids[joined]) r.lp_mismatch = true;
+      r.lps.push_back(rec);
+    }
     r.out.push_back(ids[joined++]);
     if (r.streaming) {
       std::lock_guard<std::mutex> lk(r.m);
       r.pub.push_back(r.out.back());
+      if (pending) r.pub_lps.push_back(r.lps.back());
       r.cv.notify_all();
     }
     fin = finished(r, *tok, cfg.max_seq_len);
   }
+  if (pending) pending->clear();
   if (!r.sync && (!admission || fin)) tokens_generated_ += joined;
   return fin;
 }
 
 // Retire: r leaves the engine with `status` (CL_OK: finished or cancelled; else failed, with err): its sequence is freed, a
 // successful request is counted, and the waiting client thread wakes.  requests_completed_ moves here only.
-void Engine::retire(Request& r, int status, const std::string& err) {
+void Engine::retire(Request& r, int status, const std::string& err_in) {
+  std::string err = err_in;
+  if (status == CL_OK && r.lp_mismatch) {
+    status = CL_ERR_INTERNAL;
+    err = "logprobs: a generated id has no record of its own";
+  }
   if (r.seq >= 0) seq_free(r.seq);
   r.seq = -1;
   if (status == CL_OK) {
@@ -144,6 +166,12 @@ int Engine::host_next_token(Request& r, float* logits, bool read_back, const int
     if (rc) return rc;
   }
   *next = sample_token(logits, cfg.vocab_size, r.sp, hist, n_hist, (uint64_t)r.out.size());
+  auto& pending = seqs_[r.seq].lps;
+  if (r.top_n >= 0 && !pending.empty()) {   // lse and the top list are the device's; the host's id gets logit - lse as there
+    LogprobRecord& rec = pending.back();
+    rec.id = *next;
+    rec.logprob = (float)((double)logits[*next] - rec.lse);
+  }
   if (!r.device_next()) CL_CUDA_OK(cudaMemcpyAsync(d_tok_ + r.seq, next, 4, cudaMemcpyHostToDevice, stream_));
   return CL_OK;
 }
@@ -206,10 +234,17 @@ int Engine::generate_sync(const std::shared_ptr<Request>& rp, const TokenSink* s
   size_t emitted = 0;
   auto emit = [&]() {
     if (!sink || !sink->fn || r.out.size() <= emitted) return;
-    if (sink->fn(sink->user, r.out.data() + emitted, (int)(r.out.size() - emitted))) r.cancel = true;
+    const int n = (int)(r.out.size() - emitted);
+    if (sink->lp_fn && r.top_n >= 0) {
+      std::vector<cl_token_logprob> lp((size_t)n);
+      for (int i = 0; i < n; ++i) lp[(size_t)i] = to_token_logprob(r.lps[emitted + (size_t)i]);
+      if (sink->lp_fn(sink->user, lp.data(), n)) r.cancel = true;
+    }
+    if (sink->fn(sink->user, r.out.data() + emitted, n)) r.cancel = true;
     emitted = r.out.size();
   };
   int rc = seq_create(&r.seq);
+  if (rc == CL_OK && r.top_n >= 0) rc = set_logprobs(r.seq, r.top_n);
   if (rc) return rc;
   std::vector<float> logits(cfg.vocab_size);
   int64_t t0 = now_ns();
@@ -257,8 +292,13 @@ int Engine::generate_sync(const std::shared_ptr<Request>& rp, const TokenSink* s
   return rc;
 }
 
-int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink) {
+int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink, int top_n,
+                         cl_token_logprob** lps) {
   if (!prompt || n_prompt <= 0 || !out) { set_last_error("empty prompt"); return CL_ERR_INVALID_ARG; }
+  if (top_n < -1 || top_n > kLogprobTopMax || (top_n >= 0 && cfg.vocab_size > kTailBlocks * kSampleSliceMax)) {
+    set_last_error("logprobs: top_n must be -1..20 and the vocabulary at most 163840");
+    return CL_ERR_INVALID_ARG;
+  }
   if (n_prompt >= cfg.max_seq_len) { set_last_error("prompt longer than max_seq_len"); return CL_ERR_TOO_LONG; }
   for (int i = 0; i < n_prompt; ++i)
     if (prompt[i] < 0 || prompt[i] >= cfg.vocab_size) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
@@ -271,6 +311,7 @@ int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling&
   r->sync = !sched_started_;
   r->streaming = !r->sync && sink && sink->fn;   // the synchronous path calls the sink itself
   r->dev_sample = device_sample_ && device_sampling_ok(sp, cfg.vocab_size);
+  r->top_n = top_n;
   if (r->sync) {
     std::lock_guard<std::mutex> lk(mu_);
     const int rc = generate_sync(r, sink);
@@ -287,12 +328,16 @@ int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling&
     std::unique_lock<std::mutex> lk(r->m);
     size_t seen = 0;
     std::vector<int32_t> fresh;
+    std::vector<cl_token_logprob> fresh_lp;
     while (true) {
       r->cv.wait(lk, [&] { return r->done || r->pub.size() > seen; });
       if (r->pub.size() > seen) {
         fresh.assign(r->pub.begin() + seen, r->pub.end());
+        fresh_lp.clear();
+        for (size_t i = seen; i < r->pub_lps.size(); ++i) fresh_lp.push_back(to_token_logprob(r->pub_lps[i]));
         seen = r->pub.size();
         lk.unlock();                       // the callback runs on this (the caller's) thread, outside every lock
+        if (sink->lp_fn && r->top_n >= 0 && sink->lp_fn(sink->user, fresh_lp.data(), (int)fresh_lp.size())) r->cancel = true;
         if (sink->fn(sink->user, fresh.data(), (int)fresh.size())) r->cancel = true;
         lk.lock();
         continue;
@@ -306,6 +351,10 @@ int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling&
     return r->status;
   }
   fill_result(*r, out, tok.get());
+  if (lps) {
+    *lps = (cl_token_logprob*)malloc(sizeof(cl_token_logprob) * std::max<size_t>(1, r->lps.size()));
+    for (size_t i = 0; i < r->lps.size(); ++i) (*lps)[i] = to_token_logprob(r->lps[i]);
+  }
   return CL_OK;
 }
 
@@ -423,6 +472,7 @@ bool Engine::admit_group(int budget) {
   for (size_t i = 0; rc == CL_OK && i < group.size(); ++i) {
     auto& r = group[i];
     rc = ensure_capacity(r->seq, (int)r->full.size() + 1);
+    if (rc == CL_OK && r->top_n >= 0) rc = set_logprobs(r->seq, r->top_n);
     // the pass's tail draws the next token of a device-sampled request (step = tokens generated before a preemption)
     if (rc == CL_OK && r->dev_sample) rc = arm_sampling(r->seq, r->sp, r->out.size(), r->full.data(), (int)r->full.size());
     if (rc) break;
@@ -500,6 +550,7 @@ void Engine::admit_chunked(int budget) {
     const int64_t t0 = now_ns();
     // only the last chunk's tail draws: earlier chunks run with the slot disarmed
     int rc = last && r->dev_sample ? arm_sampling(r->seq, r->sp, r->out.size(), r->full.data(), (int)r->full.size()) : CL_OK;
+    if (rc == CL_OK && last && r->top_n >= 0) rc = set_logprobs(r->seq, r->top_n);
     if (rc == CL_OK) rc = prefill(r->seq, r->full.data() + r->prefilled, (int)chunk, last && !r->dev_sample ? sched_logits_.data() : nullptr);
     int32_t next = 0;
     if (rc == CL_OK && last && r->dev_sample) rc = read_next_token(r->seq, &next);
@@ -601,6 +652,7 @@ int Engine::step_running() {
   } else if (cudaStreamSynchronize(stream_) != cudaSuccess) {
     return CL_ERR_CUDA;
   }
+  if ((rc = collect_logprobs(sched_slots_.data(), B))) return rc;
   for (auto& r : active_) {
     seq_advance(r->seq, &r->out.back(), 1, 1);
     const std::vector<int32_t>& hist = seqs_[r->seq].history;

@@ -76,6 +76,12 @@ class SpecStats(C.Structure):
                 ("reserved", C.c_int64 * 3)]
 
 
+# cl_token_logprob (include/clengine.h): one record of the step tail's log-probabilities, 172 bytes
+MAX_TOP_LOGPROBS = 20
+TOKEN_LOGPROB = np.dtype([("id", np.int32), ("logprob", np.float32), ("n_top", np.int32),
+                          ("top_ids", np.int32, (MAX_TOP_LOGPROBS,)), ("top_logprobs", np.float32, (MAX_TOP_LOGPROBS,))])
+assert TOKEN_LOGPROB.itemsize == 172
+
 # every symbol include/clengine.h declares (tests check the library exports all of them)
 EXPORTS = [
     "cl_abi_version", "cl_strerror", "cl_last_error", "cl_default_engine_config", "cl_default_sampling",
@@ -89,7 +95,7 @@ EXPORTS = [
     "cl_op_attn_prefill_cached", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages", "cl_kvpool_set_host_pages", "cl_kvpool_take_moves",
-    "cl_kvpool_host_cached_pages",
+    "cl_kvpool_host_cached_pages", "cl_seq_set_logprobs", "cl_seq_take_logprobs", "cl_generate_ids_logprobs", "cl_op_sample_logprobs",
     "cl_tokenizer_load", "cl_tokenizer_free", "cl_tokenizer_encode", "cl_tokenizer_decode", "cl_tokenizer_info", "cl_engine_load_tokenizer",
 ]
 
@@ -175,6 +181,10 @@ def lib():
         "cl_op_attn_prefill_cached": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
         "cl_op_kv_host_roundtrip": (C.c_int, [C.c_int, i32, i32, i32, i32, i32, i32, P(f32)]),
         "cl_op_sample": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), vp, vp, i32, vp, vp]),
+        "cl_op_sample_logprobs": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), vp, vp, i32, vp, i32, vp, vp]),
+        "cl_seq_set_logprobs": (C.c_int, [vp, i32, i32]),
+        "cl_seq_take_logprobs": (C.c_int, [vp, i32, vp, i32, P(i32)]),
+        "cl_generate_ids_logprobs": (C.c_int, [vp, vp, i32, P(Sampling), i32, P(Result), P(vp)]),
         "cl_op_synth_weights": (C.c_int, [C.c_int, u64, i32, i64, f32, vp]),
         "cl_tokenizer_load": (C.c_int, [C.c_char_p, C.c_char_p, P(vp)]),
         "cl_tokenizer_free": (None, [vp]),
@@ -369,6 +379,18 @@ class Engine:
     def seq_free(self, s: int):
         _check(lib().cl_seq_free(self._h, s), "cl_seq_free")
 
+    def set_logprobs(self, s: int, top_n: int):
+        """cl_seq_set_logprobs: -1 off, 0..20 = every later step tail of s leaves a record with top_n alternatives."""
+        _check(lib().cl_seq_set_logprobs(self._h, s, top_n), "cl_seq_set_logprobs")
+
+    def take_logprobs(self, s: int) -> np.ndarray:
+        """cl_seq_take_logprobs: the records of the ids chosen for s since the last take (a TOKEN_LOGPROB array)."""
+        n = C.c_int32()
+        _check(lib().cl_seq_take_logprobs(self._h, s, None, 0, C.byref(n)), "cl_seq_take_logprobs")
+        out = np.zeros(n.value, TOKEN_LOGPROB)
+        _check(lib().cl_seq_take_logprobs(self._h, s, out.ctypes.data, n.value, C.byref(n)), "cl_seq_take_logprobs")
+        return out[:n.value]
+
     def seq_len(self, s: int) -> int:
         n = C.c_int32()
         _check(lib().cl_seq_len(self._h, s, C.byref(n)), "cl_seq_len")
@@ -540,6 +562,21 @@ class Engine:
             return GenerateResult(r)
         finally:
             lib().cl_result_free(C.byref(r))
+
+    def generate_ids_logprobs(self, prompt_ids, sampling: Sampling, top_n: int):
+        """cl_generate_ids_logprobs: (GenerateResult, records), records a TOKEN_LOGPROB array with one entry per generated id."""
+        ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
+        r = Result()
+        lp = C.c_void_p()
+        _check(lib().cl_generate_ids_logprobs(self._h, _ptr(ids), len(ids), C.byref(sampling), top_n, C.byref(r), C.byref(lp)),
+               "cl_generate_ids_logprobs")
+        try:
+            res = GenerateResult(r)
+            recs = np.frombuffer(C.string_at(lp, res.n_generated * TOKEN_LOGPROB.itemsize), TOKEN_LOGPROB).copy()
+            return res, recs
+        finally:
+            lib().cl_result_free(C.byref(r))
+            lib().cl_buffer_free(lp)
 
     def generate(self, model: str, prompt: str, sampling: Sampling | None = None) -> GenerateResult:
         r = Result()
@@ -831,6 +868,25 @@ def op_sample(logits, samplings, histories, steps, device=0):
     _check(lib().cl_op_sample(device, _ptr(lg), rows, lg.shape[1], sp, _ptr(hist), _ptr(nh), stride, _ptr(st), _ptr(out)),
            "cl_op_sample")
     return out
+
+
+def op_sample_logprobs(logits, samplings, histories, steps, top_n, device=0):
+    """cl_op_sample_logprobs: op_sample with every row's logprobs on (a row with temperature <= 0 takes the greedy choice).
+    Returns (ids [n_rows], records: a TOKEN_LOGPROB array [n_rows])."""
+    lg = np.ascontiguousarray(np.atleast_2d(logits), dtype=np.float32)
+    rows = lg.shape[0]
+    stride = max(1, max(len(h) for h in histories))
+    hist = np.zeros((rows, stride), np.int32)
+    for r, h in enumerate(histories):
+        hist[r, :len(h)] = np.asarray(h, np.int32)
+    nh = np.ascontiguousarray([len(h) for h in histories], dtype=np.int32)
+    st = np.ascontiguousarray(steps, dtype=np.uint64)
+    sp = (Sampling * rows)(*samplings)
+    out = np.empty(rows, np.int32)
+    recs = np.zeros(rows, TOKEN_LOGPROB)
+    _check(lib().cl_op_sample_logprobs(device, _ptr(lg), rows, lg.shape[1], sp, _ptr(hist), _ptr(nh), stride, _ptr(st), top_n,
+                                       _ptr(out), recs.ctypes.data), "cl_op_sample_logprobs")
+    return out, recs
 
 
 def op_kv_host_roundtrip(n_layers, n_kv, head_dim, page_size, n_moves, iters=0, device=0):

@@ -141,6 +141,15 @@ class _Handler(BaseHTTPRequestHandler):
         if not chat and req.get("raw"):
             options = options or GenerateOptions()
             options.raw = True
+        # Ollama's top-level logprobs / top_logprobs (0..20; alternatives only together with logprobs)
+        want_lp, top_lp = req.get("logprobs"), req.get("top_logprobs")
+        if top_lp is not None and (isinstance(top_lp, bool) or not isinstance(top_lp, int) or not 0 <= top_lp <= 20):
+            return self._json(400, {"error": "top_logprobs must be an integer from 0 to 20"})
+        if top_lp and not want_lp:
+            return self._json(400, {"error": "top_logprobs requires logprobs to be true"})
+        if want_lp:
+            options = options or GenerateOptions()
+            options.logprobs, options.top_logprobs = True, int(top_lp or 0)
         stream = bool(req.get("stream", False))
         addr, worker = self.server.table.best(model)
         if worker is None:                                                # gateway.go:192-199
@@ -157,6 +166,8 @@ class _Handler(BaseHTTPRequestHandler):
                 o = {"model": g.model or model, "created_at": now, "response": g.response, "done": g.done}
             if g.done:
                 o["done_reason"] = g.done_reason
+            if want_lp:
+                o["logprobs"] = [t.to_json() for t in g.logprobs]
             return o
 
         if stream:

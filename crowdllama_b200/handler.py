@@ -71,8 +71,14 @@ def worker_api_handler(engine: "eng.Engine", sampling: "eng.Sampling | None" = N
         return generate_req
 
     def _raw(generate_req) -> bool:
-        # raw = "do not apply the chat template": only the byte-level entry points of libclengine know how
-        return bool(generate_req.options and generate_req.options.raw and hasattr(engine, "handle_message_stream"))
+        # raw = "do not apply the chat template" and logprobs: only the byte-level entry points of libclengine carry them,
+        # so such requests take that path instead of assembling frames a second way here
+        o = generate_req.options
+        if o is not None and (o.logprobs or o.top_logprobs is not None):
+            if not hasattr(engine, "handle_message_stream"):
+                raise HandlerError("logprobs need the byte-level engine entry points")
+            return True
+        return bool(o and o.raw and hasattr(engine, "handle_message_stream"))
 
     def handler(ctx, req: BaseMessage) -> BaseMessage:
         generate_req = _request(req)

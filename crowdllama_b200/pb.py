@@ -15,9 +15,14 @@ FIELDS = {
     # EXTENSION (SURVEY.md §8f row 3): request options the reference's wire cannot express (api.go:193-197);
     # every field has explicit presence (proto3 `optional`): temperature 0 = greedy is not "unset"
     "GenerateOptions": {"seed": 1, "temperature": 2, "top_k": 3, "top_p": 4, "repeat_penalty": 5, "repeat_last_n": 6,
-                        "num_predict": 7, "raw": 8},
+                        "num_predict": 7, "raw": 8,
+                        # EXTENSION: Ollama's top-level `logprobs` / `top_logprobs` (0..20) of a request
+                        "logprobs": 9, "top_logprobs": 10},
     "GenerateResponse": {"model": 1, "created_at": 2, "response": 3, "done": 4, "done_reason": 5, "worker_id": 6,
-                         "total_duration": 7},
+                         "total_duration": 7,
+                         "logprobs": 8},          # EXTENSION: repeated TokenLogprob, one per token of this frame
+    # EXTENSION: token = the id's surface bytes as lossy UTF-8, bytes = the exact bytes, top_logprobs = the alternatives
+    "TokenLogprob": {"token": 1, "logprob": 2, "bytes": 3, "top_logprobs": 4},
     "Timestamp": {"seconds": 1, "nanos": 2},
 }
 
@@ -90,6 +95,8 @@ class GenerateOptions:
     repeat_last_n: int | None = None
     num_predict: int | None = None
     raw: bool | None = None
+    logprobs: bool | None = None
+    top_logprobs: int | None = None
 
     def encode(self) -> bytes:
         F, out = FIELDS["GenerateOptions"], b""
@@ -114,8 +121,8 @@ class GenerateOptions:
             if name in _OPT_FLOAT and wt == 5:
                 setattr(m, name, struct.unpack("<f", v)[0])
             elif name not in _OPT_FLOAT and wt == 0:
-                if name == "raw":
-                    m.raw = bool(v)
+                if name in ("raw", "logprobs"):
+                    setattr(m, name, bool(v))
                 elif name == "seed":
                     m.seed = v
                 else:
@@ -138,6 +145,49 @@ class GenerateOptions:
 
     def is_empty(self) -> bool:
         return all(getattr(self, k) is None for k in FIELDS["GenerateOptions"])
+
+
+@dataclass
+class TokenLogprob:
+    token: str = ""
+    logprob: float = 0.0
+    bytes: bytes = b""
+    top_logprobs: list = field(default_factory=list)    # of TokenLogprob (without their own top_logprobs)
+
+    def encode(self) -> bytes:
+        F = FIELDS["TokenLogprob"]
+        out = b""
+        if self.token:
+            out += _ld(F["token"], self.token.encode())
+        out += _varint(F["logprob"] << 3 | 5) + struct.pack("<f", float(self.logprob))
+        if self.bytes:
+            out += _ld(F["bytes"], bytes(self.bytes))
+        for t in self.top_logprobs:
+            out += _ld(F["top_logprobs"], t.encode())
+        return out
+
+    @classmethod
+    def decode(cls, b: bytes) -> "TokenLogprob":
+        F, m = FIELDS["TokenLogprob"], cls()
+        for f, wt, v in _fields(b):
+            if f == F["token"] and wt == 2:
+                m.token = v.decode("utf-8", "replace")
+            elif f == F["logprob"] and wt == 5:
+                m.logprob = struct.unpack("<f", v)[0]
+            elif f == F["bytes"] and wt == 2:
+                m.bytes = bytes(v)
+            elif f == F["top_logprobs"] and wt == 2:
+                m.top_logprobs.append(TokenLogprob.decode(v))
+        return m
+
+    def to_json(self) -> dict:
+        """Ollama's shape: {"token", "logprob", "bytes": [ints], "top_logprobs": [...]} (top entries without their own list)."""
+        o = {"token": self.token, "logprob": self.logprob, "bytes": list(self.bytes)}
+        if self.top_logprobs:
+            o["top_logprobs"] = [{"token": t.token, "logprob": t.logprob, "bytes": list(t.bytes)} for t in self.top_logprobs]
+        else:
+            o["top_logprobs"] = []
+        return o
 
 
 @dataclass
@@ -185,6 +235,7 @@ class GenerateResponse:
     done_reason: str = ""
     worker_id: str = ""
     total_duration: int = 0
+    logprobs: list = field(default_factory=list)        # of TokenLogprob
 
     def encode(self) -> bytes:
         F, T = FIELDS["GenerateResponse"], FIELDS["Timestamp"]
@@ -208,6 +259,8 @@ class GenerateResponse:
             out += _ld(F["worker_id"], self.worker_id.encode())
         if self.total_duration:
             out += _varint(F["total_duration"] << 3) + _varint(self.total_duration)
+        for t in self.logprobs:
+            out += _ld(F["logprobs"], t.encode())
         return out
 
     @classmethod
@@ -232,6 +285,8 @@ class GenerateResponse:
                 m.worker_id = v.decode("utf-8", "replace")
             elif f == F["total_duration"] and wt == 0:
                 m.total_duration = v if v < 1 << 63 else v - (1 << 64)
+            elif f == F["logprobs"] and wt == 2:
+                m.logprobs.append(TokenLogprob.decode(v))
         return m
 
 

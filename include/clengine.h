@@ -362,6 +362,39 @@ int cl_decode_verify(cl_engine* e, cl_seq_t seq, int32_t input_id, const int32_t
 int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* input_ids, const int32_t* drafts,
                            const int32_t* ks, const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int32_t* n_out,
                            float* logits_out);
+
+/* ---- per-token log-probabilities (Ollama's `logprobs` / `top_logprobs`) -----------------------------------------------
+ * What is computed: the natural-log log_softmax of the logits row the step tail chose the id from, taken over the raw fp32
+ * logits, i.e. BEFORE the repeat penalty, temperature, top-k and top-p: the model's distribution, whatever the sampler
+ * then does with it.  (Which distribution Ollama reports could not be pinned against its source; this is the choice.)
+ * The step tail kernel computes it on the device: lse = M + log(sum_b s_b exp(m_b - M)) over its 64 vocabulary slices
+ * (slice max m_b, slice sum s_b of expf(v - m_b); the merge in double, in fixed slice order), logprob(id) = logit[id] - lse
+ * in double rounded to fp32, and the top n_top ids by logit (value descending, id ascending, the greedy tie rule).  A record depends on its
+ * logits row alone: it is the same bits run to run, whatever other sequences share the step, and whether the id was
+ * chosen greedily or drawn.  A sequence without logprobs runs exactly the step tail it ran before. */
+#define CL_MAX_TOP_LOGPROBS 20
+typedef struct cl_token_logprob {  /* 172 bytes */
+  int32_t id;          /* the chosen id */
+  float logprob;       /* its log-probability (<= 0) */
+  int32_t n_top;       /* entries of top_ids / top_logprobs in use */
+  int32_t top_ids[CL_MAX_TOP_LOGPROBS];
+  float top_logprobs[CL_MAX_TOP_LOGPROBS];
+} cl_token_logprob;
+/* top_n -1: off (the default of a new sequence; cl_seq_free disarms too), 0..20: every later id the step tail chooses for
+ * the sequence leaves a record with top_n alternatives.  Pending records are dropped.  CL_ERR_INVALID_ARG for top_n outside
+ * -1..20, and for arming a model whose vocabulary exceeds 163 840 (64 slices of 2 560, the device sampler's limit). */
+int cl_seq_set_logprobs(cl_engine* e, cl_seq_t seq, int32_t top_n);
+/* The records of the ids the step tail chose for the sequence since the last take, in order: one per id chosen by
+ * cl_prefill (its last token), cl_prefill_batch, cl_decode_step[_batch], cl_decode_greedy[_batch], cl_decode_sample_batch
+ * and cl_decode_verify[_batch] (the emitted ids).  Up to cap records go to out and are removed; *n_out = how many.
+ * out == NULL: *n_out = the count pending, nothing is removed. */
+int cl_seq_take_logprobs(cl_engine* e, cl_seq_t seq, cl_token_logprob* out, int32_t cap, int32_t* n_out);
+/* cl_generate_ids with logprobs on (top_n 0..20): *lps (malloc'd, free with cl_buffer_free) = one record per generated id,
+ * out->n_generated of them.  The ids equal those of the same request through cl_generate_ids.  A host-sampled request
+ * (settings the device sampler does not cover) takes lse and the top list from the device and sets logprob = logit[id] - lse
+ * with the same double subtraction and fp32 rounding. */
+int cl_generate_ids_logprobs(cl_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const cl_sampling* s, int32_t top_n,
+                             cl_result* out, cl_token_logprob** lps);
 /* Parity aid: make the sequence hold n_tokens cached tokens whose K/V, in every layer, are the CPU oracle's
  * synthetic cache pattern (oracle/llama_oracle.c oc_seq_fake_fill: k[i] = (((i * 2654435761) >> 24 & 255) - 128) / 128,
  * v[i] = (((i * 40503) >> 8 & 255) - 128) / 128 with i = token * n_kv * head_dim + head * head_dim + dim; exact in
@@ -479,6 +512,11 @@ int cl_op_attn_prefill_cached(int device, int variant, const uint16_t* q, const 
  * n_history[r] is 0).  ids_out[n_rows].  CL_ERR_INVALID_ARG for settings the device sampler does not cover. */
 int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
                  const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out);
+/* cl_op_sample with every row's logprobs on (top_n 0..20): the same step tail kernel; lp_out[n_rows] = the records.  A row
+ * whose sp[r].temperature <= 0 takes the greedy choice instead of a draw.  vocab <= 163 840. */
+int cl_op_sample_logprobs(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
+                          const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t top_n, int32_t* ids_out,
+                          cl_token_logprob* lp_out);
 /* synthetic weight generator (device kernel) -> host copy, for known-answer tests */
 int cl_op_synth_weights(int device, uint64_t seed, int32_t tensor_key, int64_t n, float scale,
                         uint16_t* out_bf16);
