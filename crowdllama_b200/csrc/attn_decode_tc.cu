@@ -11,7 +11,6 @@
 //   (same tail as attn_decode_kernel: fp32 output for the GEMV path, bf16 copy = X operand of the o-projection).
 // Shapes: head_dim 128, 4 query heads per kv head, page 32 (Llama-3-8B / Mistral-7B); others use the CUDA-core kernel.
 #include <algorithm>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -57,7 +56,7 @@ attn_decode_tc_kernel(const __grid_constant__ CUtensorMap kmap, const __grid_con
     fence_barrier_init();
   }
   __syncthreads();
-  if (a.pdl_early) pdl_launch_dependents();
+  pdl_launch_dependents();
   const bool is_producer = warp == NW;
   if (is_producer) {
     if (!elect_one()) return;
@@ -314,27 +313,19 @@ int launch_variant(const AttnDecodeArgs& a, const CUtensorMap& kmap, const CUten
     attr.mark();
   }
   TcArgs t{a, layer_row0};
-  cudaLaunchConfig_t cfg{};
   // persistent launch (single split, more items than resident CTAs): MINB CTAs per SM walk the items instead of one CTA
-  // per item (CL_BATCH_ATTN_PERSIST=0 restores one CTA per item).
-  static const int persist = getenv("CL_BATCH_ATTN_PERSIST") ? atoi(getenv("CL_BATCH_ATTN_PERSIST")) : 1;
+  // per item.
   const int n_items = a.n_kv * a.nsplit * a.batch, resident = MINB * sm_count();
-  const int grid = (persist && a.nsplit == 1 && n_items > resident) ? resident : n_items;
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3((NW + 1) * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute la[1];
-  la[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  la[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = la; cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, kmap, vmap, t) == cudaSuccess ? 1 : -1;
+  const int grid = (a.nsplit == 1 && n_items > resident) ? resident : n_items;
+  return launch_pdl(kern, dim3(grid), dim3((NW + 1) * 32), smem, st, pdl, kmap, vmap, t) == cudaSuccess ? 1 : -1;
 }
 }  // namespace
 
 // KV splits per sequence and kernel shape for a batched step of `batch` sequences: one wave of 8-warp CTAs while the
-// items fit the machine, otherwise the 4-warp shape with two CTAs per SM (CL_BATCH_ATTN_SMALL = 0 / 1 forces one).
+// items fit the machine, otherwise the 4-warp shape with two CTAs per SM.
 void attn_decode_tc_plan(int n_kv, int batch, int nsplit_max, int cta_budget, int* nsplit, int* small) {
-  static const int force = getenv("CL_BATCH_ATTN_SMALL") ? atoi(getenv("CL_BATCH_ATTN_SMALL")) : -1;
   const int items = n_kv * batch;
-  *small = force >= 0 ? (force != 0) : (items > cta_budget);   // small shape once the items exceed one wave
+  *small = items > cta_budget;   // small shape once the items exceed one wave
   const int budget = *small ? 2 * cta_budget : cta_budget;
   *nsplit = std::max(1, std::min(std::min(nsplit_max, MAXS), budget / std::max(items, 1)));
 }

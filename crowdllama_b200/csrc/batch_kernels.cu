@@ -7,18 +7,6 @@
 
 namespace cl {
 
-// launch with or without the programmatic-dependent-launch attribute (the kernels call griddepcontrol.* either way)
-template <typename Kern, typename... Args>
-static int launch_k(Kern kern, dim3 grid, dim3 block, cudaStream_t st, bool pdl, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, args...) == cudaSuccess ? 1 : -1;
-}
-
 // h[slot] += sum_s ypart[s][b]  (fixed order);  xn[b] = bf16(rmsnorm(h[slot]) * gain)
 // one CTA of 1024 threads per sequence: every thread owns <= 2 float4 of the row, all loads of a pass are independent
 __global__ void __launch_bounds__(1024) batch_resid_norm_kernel(float* __restrict__ h, int d, const float* __restrict__ ypart, int n_split,
@@ -72,7 +60,7 @@ __global__ void __launch_bounds__(1024) batch_resid_norm_kernel(float* __restric
 int launch_batch_resid_norm(float* h, int d, const float* ypart, int n_split, int B, const float* gain, float eps, __nv_bfloat16* xn,
                             const int* slots, cudaStream_t st, bool pdl) {
   if (d > 8192 || d % 4) return -1;
-  return launch_k(batch_resid_norm_kernel, dim3(B), dim3(1024), st, pdl, h, d, ypart, n_split, B, gain, eps, xn, slots);
+  return launch_pdl(batch_resid_norm_kernel, dim3(B), dim3(1024), 0, st, pdl, h, d, ypart, n_split, B, gain, eps, xn, slots) == cudaSuccess ? 1 : -1;
 }
 
 // q|k|v partials (rope-pair-interleaved columns) -> RoPE at pos[slot] -> q (fp32, bf16-rounded) and the paged cache
@@ -113,7 +101,8 @@ __global__ void __launch_bounds__(256) batch_rope_append_kernel(const float* __r
 int launch_batch_rope_append(const float* ypart, int n_split, int B, const QkvEpi& e, float* q_out, int q_stride, const int* slots,
                              cudaStream_t st, bool pdl) {
   const int pairs = (e.n_heads + 2 * e.n_kv) * e.head_dim / 2;
-  return launch_k(batch_rope_append_kernel, dim3((pairs + 255) / 256, B), dim3(256), st, pdl, ypart, n_split, B, e, q_out, q_stride, slots);
+  return launch_pdl(batch_rope_append_kernel, dim3((pairs + 255) / 256, B), dim3(256), 0, st, pdl, ypart, n_split, B, e, q_out, q_stride, slots) ==
+                 cudaSuccess ? 1 : -1;
 }
 
 // gate|up partials (interleaved pairs) -> act[b][i] = bf16(silu(g) * u)
@@ -131,7 +120,7 @@ __global__ void batch_silu_kernel(const float* __restrict__ ypart, int n_split, 
   }
 }
 int launch_batch_silu(const float* ypart, int n_split, int B, int d_ff, __nv_bfloat16* act, cudaStream_t st, bool pdl) {
-  return launch_k(batch_silu_kernel, dim3((d_ff + 255) / 256, B), dim3(256), st, pdl, ypart, n_split, B, d_ff, act);
+  return launch_pdl(batch_silu_kernel, dim3((d_ff + 255) / 256, B), dim3(256), 0, st, pdl, ypart, n_split, B, d_ff, act) == cudaSuccess ? 1 : -1;
 }
 
 // logits partial/tmp [b][vocab] -> logits[slot][vocab]

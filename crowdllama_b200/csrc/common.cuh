@@ -57,6 +57,18 @@ __device__ __forceinline__ float warp_max(float v) {
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+// Launch with the programmatic-stream-serialization attribute when pdl is set.  The kernels call griddepcontrol.* either
+// way: without the attribute both instructions are no-ops.
+template <typename Kern, typename... Args>
+static inline cudaError_t launch_pdl(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, const Args&... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kern, args...);
+}
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   unsigned v;

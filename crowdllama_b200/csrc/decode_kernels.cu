@@ -11,22 +11,17 @@
 //                                keep their x slice in registers.  The producer never waits for
 //                                activations, so with PDL the next kernel's ring fills while the
 //                                previous kernel drains.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.h"
 
 namespace cl {
 
 static int g_sm_count[64] = {0};   // per device ordinal (one engine per GPU process, but a process may open several)
-static bool g_carveout_max = true;
 int sm_count() {
   int dev = 0;
   cudaGetDevice(&dev);
   int& n = g_sm_count[dev & 63];
   if (!n) {
-    const char* cv = getenv("CL_CARVEOUT_MAX");
-    if (cv && *cv == '0') g_carveout_max = false;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     if (n <= 0) n = 132;
   }
@@ -38,22 +33,7 @@ int sm_count() {
 // which defeats the PDL overlap (and a 101 KB ring kernel would not co-reside with its successor).
 template <typename Kern>
 static void prefer_max_smem(Kern kern) {
-  if (g_carveout_max) cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-}
-
-template <typename Kern, typename Args>
-static cudaError_t launch_ex(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, const Args& args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, args);
+  cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 }
 
 // ================================================================================================
@@ -115,7 +95,7 @@ __global__ void __launch_bounds__(256, 2) gemv_ldg_kernel(const GemvArgs a) {
   __shared__ float red[8];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.y;
-  if (a.pdl_early) pdl_launch_dependents();
+  pdl_launch_dependents();
   pdl_wait();
   const int slot = a.slots ? a.slots[b] : b;
   const int K = a.K;
@@ -177,7 +157,6 @@ __global__ void __launch_bounds__(256, 2) gemv_ldg_kernel(const GemvArgs a) {
     acc0 = warp_sum(acc0);
     acc1 = warp_sum(acc1);
     if (lane == 0) gemv_epilogue<EPI>(a, slot, 2 * p, acc0, acc1);
-    if (!a.pdl_early && p == p1 - 2) pdl_launch_dependents();   // about to start the last row pair
   }
 }
 
@@ -214,7 +193,7 @@ __global__ void __launch_bounds__(288, 1) gemv_ring_kernel(const GemvArgs a) {
     fence_barrier_init();
   }
   __syncthreads();
-  if (a.pdl_early) pdl_launch_dependents();
+  pdl_launch_dependents();
   const bool stamp = a.tl != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tid == 0;
   if (stamp) a.tl[0] = gtime_ns();
 
@@ -230,9 +209,6 @@ __global__ void __launch_bounds__(288, 1) gemv_ring_kernel(const GemvArgs a) {
         mbar_arrive_expect_tx(&full[st], STAGE_BYTES);
         bulk_g2s(ring + (size_t)st * STAGE_BYTES, src + (size_t)it * STAGE_BYTES, STAGE_BYTES, &full[st], pol);
       }
-      // every byte this CTA will ever read from HBM is now in flight: let the next kernel's CTAs
-      // become resident and start streaming THEIR weights while this one drains
-      if (!a.pdl_early) pdl_launch_dependents();
     }
     // the producer warp must stay until the consumers are done with the barriers it arms
   } else {
@@ -365,7 +341,7 @@ static cudaError_t launch_ring_inst(const GemvArgs& a, cudaStream_t st, bool pdl
   }
   if (smem > 160 * 1024) return cudaErrorInvalidValue;
   g_last_gemv_ctas = G * a.batch;
-  return launch_ex(kern, dim3(G, a.batch), dim3(288), smem, st, pdl, a);
+  return launch_pdl(kern, dim3(G, a.batch), dim3(288), smem, st, pdl, a);
 }
 
 template <int EPI, bool NORM>
@@ -397,7 +373,7 @@ static cudaError_t launch_ldg(const GemvArgs& a, cudaStream_t st, bool pdl) {
   int npairs = a.N / 2;
   if (G * 8 > npairs) G = (npairs + 7) / 8;
   g_last_gemv_ctas = G * a.batch;
-  return launch_ex(kern, dim3(G, a.batch), dim3(256), smem, st, pdl, a);
+  return launch_pdl(kern, dim3(G, a.batch), dim3(256), smem, st, pdl, a);
 }
 
 int launch_gemv(int variant, int epi, bool norm, const GemvArgs& a, cudaStream_t st, bool pdl, int* n_ctas) {
@@ -426,8 +402,7 @@ int launch_gemv(int variant, int epi, bool norm, const GemvArgs& a, cudaStream_t
 //   q|k|v GEMV that precedes it; only the page holding the current token is fetched after the wait.
 //   The consumers' short latency-bound phase then overlaps the o-projection's weight prefetch.
 // ================================================================================================
-static int g_attn_ring_bytes = 64 * 1024;    // + 96 KB GEMV ring of the neighbouring kernel = co-resident under PDL (env CL_ATTN_RING_KB)
-constexpr int kAttnRingBytesMax = 128 * 1024;
+constexpr int kAttnRingBytes = 64 * 1024;    // + 96 KB GEMV ring of the neighbouring kernel = co-resident under PDL
 constexpr int kAttnMaxStages = 8;
 
 template <int REP, int HD>
@@ -458,7 +433,7 @@ __global__ void __launch_bounds__(288) attn_decode_kernel(const AttnDecodeArgs a
     fence_barrier_init();
   }
   __syncthreads();
-  if (a.pdl_early) pdl_launch_dependents();
+  pdl_launch_dependents();
   const bool stamp = a.tl != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && tid == 0;
   if (stamp) a.tl[0] = gtime_ns();
 
@@ -686,16 +661,14 @@ __global__ void __launch_bounds__(288) attn_decode_kernel(const AttnDecodeArgs a
 int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st, bool pdl) {
   const int rep = a.n_heads / a.n_kv;
   dim3 grid(a.n_kv, a.nsplit, a.batch), block(288);
-  static bool env_read = false;
-  if (!env_read) { const char* v = getenv("CL_ATTN_RING_KB"); if (v && atoi(v) >= 16 && atoi(v) <= 128) g_attn_ring_bytes = atoi(v) * 1024; env_read = true; }
-  if (a.nsplit > 64 || 2 * a.page_size * a.head_dim * 2 * 2 > g_attn_ring_bytes) return -1;
-  const size_t smem = g_attn_ring_bytes;
+  if (a.nsplit > 64 || 2 * a.page_size * a.head_dim * 2 * 2 > kAttnRingBytes) return -1;
+  const size_t smem = kAttnRingBytes;
   AttnDecodeArgs a2 = a;
-  a2.ring_bytes = g_attn_ring_bytes;
+  a2.ring_bytes = kAttnRingBytes;
   cudaError_t e = cudaErrorInvalidValue;
 #define CL_ATT(R, D) do { static PerDeviceOnce once; if (once.pending()) { prefer_max_smem(attn_decode_kernel<R, D>);     \
-      cudaFuncSetAttribute(attn_decode_kernel<R, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnRingBytesMax); once.mark(); } \
-    e = launch_ex(attn_decode_kernel<R, D>, grid, block, smem, st, pdl, a2); } while (0)
+      cudaFuncSetAttribute(attn_decode_kernel<R, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnRingBytes); once.mark(); } \
+    e = launch_pdl(attn_decode_kernel<R, D>, grid, block, smem, st, pdl, a2); } while (0)
   if (a.head_dim == 128) {
     if (rep == 1) CL_ATT(1, 128); else if (rep == 2) CL_ATT(2, 128); else if (rep == 4) CL_ATT(4, 128);
     else if (rep == 8) CL_ATT(8, 128);
@@ -1204,8 +1177,8 @@ int launch_step_tail(const StepTailArgs& a, cudaStream_t st) {
 int launch_spec_tail(const SpecTailArgs& a, cudaStream_t st, bool pdl) {
   static PerDeviceOnce once;
   if (once.pending()) { prefer_max_smem(spec_tail_kernel); prefer_max_smem(spec_accept_kernel); once.mark(); }
-  if (launch_ex(spec_tail_kernel, dim3(kTailBlocks, a.T), dim3(256), 0, st, pdl, a) != cudaSuccess) return -1;
-  return launch_ex(spec_accept_kernel, dim3(1), dim3(32), 0, st, true, a) == cudaSuccess ? 2 : -1;
+  if (launch_pdl(spec_tail_kernel, dim3(kTailBlocks, a.T), dim3(256), 0, st, pdl, a) != cudaSuccess) return -1;
+  return launch_pdl(spec_accept_kernel, dim3(1), dim3(32), 0, st, true, a) == cudaSuccess ? 2 : -1;
 }
 
 __global__ void synth_bf16_kernel(__nv_bfloat16* out, int64_t n, int k_cols, int row_mult, int row_off, uint64_t seed,

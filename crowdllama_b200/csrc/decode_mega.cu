@@ -17,8 +17,6 @@
 // The LM head and the argmax tail stay separate kernels (decode_kernels.cu).
 // Built for the Llama-3-8B / Mistral-7B layer shape (d 4096, d_ff 14336, head_dim 128, 4 q heads per kv
 // head, page 32); other shapes use the per-op path.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.h"
 
@@ -80,28 +78,28 @@ constexpr int CH = 1;
 // a norm prologue or attention, with HBM idle) it pulls weight tiles that lie AHEAD of every
 // CTA's ring into the L2 (50 MB on H100) with cp.async.bulk.prefetch.L2.  All weight tiles of the step form one sequence
 // in consumption order (per layer: q|k|v, o, gate|up, down); `ctr` is the global prefetch frontier in that
-// numbering.  The frontier is kept between (own demand position + min_ahead) and (+ budget) tiles, so the
+// numbering.  The frontier is kept between (own demand position + kPfMin) and (+ kPfBudget) tiles, so the
 // lookahead never outgrows L2.  When the consumers resume, the ring refills from L2 faster than HBM could feed
 // it, the producers block again and the frontier moves on: HBM keeps streaming through the barriers.
 constexpr int PFCH = 2;
+constexpr int kPfMin = 900, kPfBudget = 4096;   // tiles
 struct Lookahead {
-  unsigned* ctr;
+  unsigned* ctr;         // nullptr: no lookahead
   unsigned known;        // lower bound of the frontier as last seen by this CTA
-  int min_ahead, budget; // tiles
   unsigned total;        // n_layers * tiles per layer
   int t_qkv, tl;         // tiles in the q|k|v segment / per layer
   unsigned n_pf, n_lim, n_jump, n_calls;   // diagnostics (CL_TIMELINE)
 };
 __device__ __forceinline__ void lookahead_step(Lookahead& la, const MegaArgs& a, unsigned mypos) {
-  if (la.budget <= 0) return;
+  if (!la.ctr) return;
   ++la.n_calls;
-  const unsigned lim = mypos + (unsigned)la.budget;
+  const unsigned lim = mypos + (unsigned)kPfBudget;
   if (la.known >= lim || la.known >= la.total) { ++la.n_lim; return; }
   const unsigned p = atomicAdd(la.ctr, (unsigned)PFCH);
   la.known = p + PFCH;
-  if (p < mypos + (unsigned)la.min_ahead) {      // frontier fell behind the demand stream: jump ahead
-    atomicMax(la.ctr, mypos + (unsigned)la.min_ahead);
-    la.known = mypos + (unsigned)la.min_ahead;
+  if (p < mypos + (unsigned)kPfMin) {      // frontier fell behind the demand stream: jump ahead
+    atomicMax(la.ctr, mypos + (unsigned)kPfMin);
+    la.known = mypos + (unsigned)kPfMin;
     ++la.n_jump;
     return;
   }
@@ -127,6 +125,7 @@ __device__ __forceinline__ void lookahead_step(Lookahead& la, const MegaArgs& a,
 // a few 32 KB copies per SM already saturate HBM (tools/bench_barrier.cu measures it), while every further tile in
 // flight only deepens the queues in front of the L2 slices — and the grid barriers' red/poll round trips wait in
 // those queues.  The ring still fills all NS slots.
+constexpr int kMaxFlight = 2;
 __device__ __forceinline__ void wait_slot(Ring& r, int st, Lookahead& la, const MegaArgs& a, unsigned mypos) {
   // (try_wait, not test_wait: a tightly polling producer warp measurably slows the two consumer warps that share
   // its scheduler)
@@ -138,7 +137,7 @@ __device__ __forceinline__ void wait_slot(Ring& r, int st, Lookahead& la, const 
     volatile int* pause = r.tile_id + 7;
     for (uint32_t spins = 0; *pause; ++spins) if (spins > (1u << 26)) __trap();
   }
-  for (uint32_t spins = 0; (int)(r.git - r.tail) >= a.max_flight; ++spins) {
+  for (uint32_t spins = 0; (int)(r.git - r.tail) >= kMaxFlight; ++spins) {
     const uint32_t n = r.tail;
     if (mbar_try_wait(&r.full[n % NS], (n / NS) & 1u)) ++r.tail;
     else lookahead_step(la, a, mypos);
@@ -322,7 +321,7 @@ __global__ void __launch_bounds__(288, 1) decode_mega_kernel(const __grid_consta
     const uint64_t pol = policy_evict_first();
     const int cur_page = pos / P;
     const int TL = T_QKV + T_O + T_GU + T_DN;
-    Lookahead la{a.pf_ctr, 0u, a.pf_min, a.pf_ctr ? a.pf_budget : 0, (unsigned)(a.n_layers * TL), T_QKV, TL, 0u, 0u, 0u, 0u};
+    Lookahead la{a.pf_ctr, 0u, (unsigned)(a.n_layers * TL), T_QKV, TL, 0u, 0u, 0u, 0u};
     for (int l = 0; l < a.n_layers; ++l) {
       const MegaLayer& L = a.layers[l];
       unsigned* ctr = a.tile_ctr + (size_t)l * 4;
@@ -648,9 +647,9 @@ static constexpr size_t kMegaSmem =
 
 // The grid barriers need every CTA resident at once.  Per device: opt in to the shared-memory size once, and check
 // that one CTA per SM fits (occupancy >= 1 with 288 threads + kMegaSmem); the engine falls back to the per-op path
-// otherwise.  All in-kernel waits are bounded (clock64 -> __trap), so a grid that is NOT co-resident after all (MPS, a
-// concurrent kernel of another context) ends as a kernel error, never as a hung GPU.  The launch itself is cooperative
-// (cudaLaunchAttributeCooperative; CL_MEGA_COOP=0 = plain launch): the driver guarantees co-residency or fails the launch.
+// otherwise.  The launch is cooperative (cudaLaunchAttributeCooperative): the driver guarantees co-residency or fails
+// the launch.  All in-kernel waits are bounded as well (clock64 -> __trap), so a protocol bug ends as a kernel error,
+// never as a hung GPU.
 static bool g_mega_ready[64] = {false}, g_mega_ok[64] = {false};
 bool mega_prepare_device() {
   int dev = 0;
@@ -669,20 +668,13 @@ bool mega_prepare_device() {
 
 int launch_decode_mega(const MegaArgs& a, cudaStream_t st) {
   if (!mega_prepare_device()) return -1;
-  // default on: no slower than the plain launch, and a grid that cannot be fully
-  // resident fails at launch instead of trapping in a barrier
-  static const bool coop = !(getenv("CL_MEGA_COOP") && atoi(getenv("CL_MEGA_COOP")) == 0);
-  if (coop) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(sm_count()); cfg.blockDim = dim3(288); cfg.dynamicSmemBytes = kMegaSmem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeCooperative;
-    at[0].val.cooperative = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, decode_mega_kernel, a) == cudaSuccess ? 1 : -1;
-  }
-  decode_mega_kernel<<<sm_count(), 288, kMegaSmem, st>>>(a);
-  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(sm_count()); cfg.blockDim = dim3(288); cfg.dynamicSmemBytes = kMegaSmem; cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeCooperative;
+  at[0].val.cooperative = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, decode_mega_kernel, a) == cudaSuccess ? 1 : -1;
 }
 
 }  // namespace cl

@@ -104,15 +104,12 @@ int Engine::init(const cl_engine_config& c) {
   if (max_seqs_ < max_batch_) max_seqs_ = max_batch_;
   use_graph_ = c.use_cuda_graph >= 0 && env_int("CL_GRAPH", 1) != 0;
   use_pdl_ = env_int("CL_PDL", 1) != 0;
-  pdl_early_ = env_int("CL_PDL_EARLY", 1);
   want_timeline_ = env_int("CL_TIMELINE", 0) != 0;
   gemv_variant_ = c.decode_path == 1 ? 0 : 1;
-  gemv_variant_ = env_int("CL_GEMV_VARIANT", gemv_variant_);
   q_dim_ = cfg.n_heads * cfg.head_dim;
   kv_dim_ = cfg.n_kv_heads * cfg.head_dim;
   qkv_dim_ = q_dim_ + 2 * kv_dim_;
   nsplit_ = std::max(1, std::min(64, sm_count() / cfg.n_kv_heads));
-  nsplit_ = std::max(1, std::min(64, env_int("CL_ATTN_NSPLIT", nsplit_)));
   // decided AFTER nsplit_ is final: the persistent kernel's lane-parallel combine and part buffer are sized by it
   use_mega_ = env_int("CL_MEGA", 1) != 0 &&
               mega_supported(cfg.d_model, cfg.d_ff, cfg.head_dim, cfg.n_heads, cfg.n_kv_heads, page_size_, nsplit_);
@@ -364,7 +361,6 @@ int Engine::alloc_state() {
     DMALLOC(d_timeline_, (size_t)(cfg.n_layers * 5 + 1) * 4 * 8);   // >= n_layers * 16 stamps for the megakernel view
     CL_CUDA_OK(cudaMemsetAsync(d_timeline_, 0, (size_t)(cfg.n_layers * 5 + 1) * 4 * 8, stream_));
   }
-  batch_gemm_min_ = env_int("CL_BATCH_GEMM_MIN", 2);
   // token tile of the projections = 32 / 64 / 128 rows (gemm_wgmma.cu picks it from the step's batch size)
   use_batch_gemm_ = env_int("CL_BATCH_GEMM", 1) != 0 && max_batch_ >= 2 && gemm_tc_supported(max_batch_, cfg.d_model, cfg.d_model) &&
                     max_batch_ <= 128;
@@ -656,7 +652,7 @@ void LaunchProfiler::report(const char* tag, int key_width, const std::string& h
 
 // ---- one token step for the sequences listed in d_slots_[0..B) -----------------------------------
 int Engine::enqueue_step(int B) {
-  if (B >= batch_gemm_min_ && use_batch_gemm_ && bws_) return enqueue_step_batched(B);   // from B = 2: faster than two GEMV passes
+  if (B >= 2 && use_batch_gemm_ && bws_) return enqueue_step_batched(B);   // from B = 2: faster than two GEMV passes
   const int d = cfg.d_model, F = cfg.d_ff, L_ = cfg.n_layers;
   int launches = 0;
   LaunchProfiler prof(stream_, nullptr);
@@ -668,7 +664,7 @@ int Engine::enqueue_step(int B) {
     MegaArgs m;
     m.layers = d_mega_layers_; m.n_layers = L_; m.q_dim = q_dim_; m.qkv_dim = qkv_dim_; m.n_heads = cfg.n_heads; m.n_kv = cfg.n_kv_heads;
     m.nsplit = nsplit_; m.eps = cfg.rms_eps; m.rope = rope_; m.pos = d_pos_; m.block_tables = d_bt_; m.bt_stride = max_pages_per_seq_;
-    m.slots = d_slots_; m.h = d_h_; m.q = d_q_; m.attn_x = d_attn_; m.act = d_act_; m.part = d_attn_part_; m.bars = d_sync_; m.tile_ctr = d_sync_ + (size_t)L_ * 6; m.pf_ctr = d_sync_ + (size_t)L_ * 10; m.max_flight = env_int("CL_MEGA_MAX_FLIGHT", 2); m.pause_in_barrier = env_int("CL_MEGA_PAUSE", 1); m.pf_min = env_int("CL_MEGA_PF_MIN", 900); m.pf_budget = env_int("CL_MEGA_PF_BUDGET", 4096);
+    m.slots = d_slots_; m.h = d_h_; m.q = d_q_; m.attn_x = d_attn_; m.act = d_act_; m.part = d_attn_part_; m.bars = d_sync_; m.tile_ctr = d_sync_ + (size_t)L_ * 6; m.pf_ctr = d_sync_ + (size_t)L_ * 10;
     m.tl = d_timeline_; m.tl_cta = env_int("CL_TIMELINE_CTA", 0);
     m.kv_layer_rows = (long long)n_pages_ * cfg.n_kv_heads * page_size_; m.kmap = kmap_; m.vmap = vmap_;
     CL_LAUNCH(launch_decode_mega(m, stream_));
@@ -676,7 +672,7 @@ int Engine::enqueue_step(int B) {
   for (int l = 0; l < (mega ? 0 : L_); ++l) {
     const auto& L = layers_[l];
     GemvArgs g;
-    g.slots = d_slots_; g.batch = B; g.pdl_early = pdl_early_;
+    g.slots = d_slots_; g.batch = B;
     // (1) RMSNorm + fused q|k|v projection; epilogue: RoPE + bf16 round + q out + KV append into the paged cache
     g.W = L.wqkv; g.N = qkv_dim_; g.K = d; g.h = d_h_; g.gain = L.attn_norm; g.eps = cfg.rms_eps;
     g.y = d_q_; g.x_stride = d; g.y_stride = q_dim_;
@@ -692,22 +688,22 @@ int Engine::enqueue_step(int B) {
     a.block_tables = d_bt_; a.bt_stride = max_pages_per_seq_; a.pos = d_pos_;
     a.out = d_attn_; a.out_stride = q_dim_; a.part = d_attn_part_; a.counters = d_attn_cnt_;
     a.slots = d_slots_; a.batch = B; a.n_heads = cfg.n_heads; a.n_kv = cfg.n_kv_heads; a.head_dim = cfg.head_dim;
-    a.page_size = page_size_; a.nsplit = nsplit_; a.pdl_early = pdl_early_; a.tl = tl(l, 1);
+    a.page_size = page_size_; a.nsplit = nsplit_; a.tl = tl(l, 1);
     CL_LAUNCH(launch_attn_decode(a, stream_, use_pdl_));
     // (3) o projection + residual
     GemvArgs o;
-    o.slots = d_slots_; o.batch = B; o.pdl_early = pdl_early_;
+    o.slots = d_slots_; o.batch = B;
     o.W = L.wo; o.N = d; o.K = q_dim_; o.x = d_attn_; o.x_stride = q_dim_; o.y = d_h_; o.resid = d_h_; o.y_stride = d; o.tl = tl(l, 2);
     CL_LAUNCH(launch_gemv(gemv_variant_, EPI_RESID, false, o, stream_, use_pdl_));
     // (4) RMSNorm + gate/up + SiLU*mul
     GemvArgs u;
-    u.slots = d_slots_; u.batch = B; u.pdl_early = pdl_early_;
+    u.slots = d_slots_; u.batch = B;
     u.W = L.wgu; u.N = 2 * F; u.K = d; u.h = d_h_; u.gain = L.ffn_norm; u.eps = cfg.rms_eps; u.y = d_act_;
     u.x_stride = d; u.y_stride = F; u.tl = tl(l, 3);
     CL_LAUNCH(launch_gemv(gemv_variant_, EPI_GATEUP, true, u, stream_, use_pdl_));
     // (5) down projection + residual
     GemvArgs w;
-    w.slots = d_slots_; w.batch = B; w.pdl_early = pdl_early_;
+    w.slots = d_slots_; w.batch = B;
     w.W = L.wdown; w.N = d; w.K = F; w.x = d_act_; w.x_stride = F; w.y = d_h_; w.resid = d_h_; w.y_stride = d; w.tl = tl(l, 4);
     CL_LAUNCH(launch_gemv(gemv_variant_, EPI_RESID, false, w, stream_, use_pdl_));
   }
@@ -720,7 +716,7 @@ int Engine::enqueue_step(int B) {
 // The LM head of a single-slot step or prefill: final RMSNorm + GEMV of d_h_ into d_logits_.
 int Engine::enqueue_lm_head(int B, bool pdl) {
   GemvArgs lm;
-  lm.slots = d_slots_; lm.batch = B; lm.pdl_early = pdl_early_;
+  lm.slots = d_slots_; lm.batch = B;
   lm.W = lm_head_; lm.N = cfg.vocab_size; lm.K = cfg.d_model; lm.h = d_h_; lm.gain = final_norm_; lm.eps = cfg.rms_eps;
   lm.y = d_logits_; lm.x_stride = cfg.d_model; lm.y_stride = cfg.vocab_size;
   lm.tl = d_timeline_ ? d_timeline_ + (size_t)cfg.n_layers * 5 * 4 : nullptr;
@@ -771,9 +767,7 @@ int Engine::enqueue_step_batched(int B) {
   int launches = 0;
   LaunchProfiler prof(stream_, "CL_STEP_PROFILE");   // eager launches only (CL_GRAPH=0)
   BatchWs& w = *bws_;
-  static const int batch_attn_ctas = env_int("CL_BATCH_ATTN_CTAS", sm_count());
-  static const bool bpdl_env = env_int("CL_BATCH_PDL", 1) != 0;
-  const bool bp = bpdl_env && use_pdl_;   // programmatic dependent launch between the kernels of the batched step
+  const bool bp = use_pdl_;   // programmatic dependent launch between the kernels of the batched step
   const int s_qkv = pick_splits(qkv_dim_, d), s_o = pick_splits(d, q_dim_), s_gu = pick_splits(2 * F, d), s_dn = pick_splits(d, F);
   CL_LAUNCH(launch_embed(embed_, d, d_tok_, d_h_, d, d_slots_, B, stream_));
   const float* pending = nullptr;   // split-K partials of the previous residual projection, folded into the next norm
@@ -793,10 +787,9 @@ int Engine::enqueue_step_batched(int B) {
     a.out = d_attn_; a.out_stride = q_dim_; a.out_bf16 = w.attn; a.part = d_attn_part_; a.counters = d_attn_cnt_;   // bf16 copy = X of the o-projection
     a.slots = d_slots_; a.batch = B; a.n_heads = cfg.n_heads; a.n_kv = cfg.n_kv_heads; a.head_dim = cfg.head_dim;
     // many sequences already fill the machine: fewer KV splits per sequence (cheaper combine, fewer CTAs)
-    a.page_size = page_size_; a.pdl_early = bp ? 1 : 0;
-    attn_decode_tc_plan(cfg.n_kv_heads, B, nsplit_, batch_attn_ctas, &a.nsplit, &a.tc_small);
-    static const bool attn_tc = env_int("CL_BATCH_ATTN_TC", 1) != 0;
-    if (attn_tc && have_kv_maps_ && attn_decode_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, a.nsplit))
+    a.page_size = page_size_;
+    attn_decode_tc_plan(cfg.n_kv_heads, B, nsplit_, sm_count(), &a.nsplit, &a.tc_small);
+    if (have_kv_maps_ && attn_decode_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, a.nsplit))
       CL_LAUNCH(launch_attn_decode_tc(a, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_, bp));
     else
       CL_LAUNCH(launch_attn_decode(a, stream_, bp));
@@ -852,7 +845,7 @@ bool Engine::ensure_graph(int B) {
 // (box benchmark, 64 concurrent chats: 16.6 req/s with lazy capture against 24.6 warm).  Called once when the
 // scheduler thread starts.
 void Engine::precapture_graphs() {
-  if (!use_graph_ || !env_int("CL_PRECAPTURE", 1)) return;
+  if (!use_graph_) return;
   for (int B = 1; B <= max_batch_ && !graph_failed_; ++B) ensure_graph(B);
   cudaStreamSynchronize(stream_);
 }

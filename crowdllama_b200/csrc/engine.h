@@ -24,7 +24,7 @@ namespace cl {
 constexpr int kDefaultSchedPrefillChunk = 1024; // CL_SCHED_PREFILL_CHUNK: admission token budget per scheduler iteration (0 = whole prompts); validated r2e
 constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts up to this many tokens take the split-K path (0 = off)
 constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi)
-constexpr int kDefaultSchedLingerUs = 1000;     // CL_SCHED_LINGER_US: with an empty batch, keep collecting while requests arrive within this gap (max 8x in total)
+constexpr int kSchedLingerUs = 1000;  // burst detection before a group admission into an empty batch (Engine::wait_for_work)
 
 // Speculative decoding (cl_engine_config.speculate, Engine::verify_batch, ngram_draft): the constants of the drafter.
 constexpr int kSpecMaxDraft = 15;     // drafted tokens per verify pass at most (its rows: x0 + drafts <= 16)
@@ -443,13 +443,10 @@ class Engine {
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev0_ = nullptr, ev1_ = nullptr;
   cudaEvent_t step_done_ev_ = nullptr;     // scheduler: blocking-sync event behind every batched step (scheduler.cpp)
-  bool sched_blocking_sync_ = true;
-  int sched_linger_us_ = 0;                // burst detection before a group admission into an empty batch (CL_SCHED_LINGER_US)
   bool sched_multi_prefill_ = false;       // group admission through prefill_multi (CL_SCHED_MULTI_PREFILL)
   int page_size_ = 32, max_batch_ = 8, max_seqs_ = 8, n_pages_ = 0, max_pages_per_seq_ = 0;
   int gemv_variant_ = 1, nsplit_ = 16;
   bool use_graph_ = true, use_pdl_ = true;
-  int pdl_early_ = 1;
   bool want_timeline_ = false, use_mega_ = false;
   MegaLayer* d_mega_layers_ = nullptr;
   CUtensorMap kmap_{}, vmap_{};
@@ -517,7 +514,6 @@ class Engine {
   struct BatchWs { __nv_bfloat16* xn = nullptr; __nv_bfloat16* attn = nullptr; __nv_bfloat16* act = nullptr; float* part = nullptr; float* logits = nullptr; };
   std::unique_ptr<BatchWs> bws_;
   bool use_batch_gemm_ = false;
-  int batch_gemm_min_ = 2;
   int prefill_chunk_tokens_ = 4096;
 
   std::unique_ptr<KvPool> pool_;

@@ -16,8 +16,6 @@
 // L2-resident.
 #include <cuda.h>
 
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.h"
 #include "wgmma.cuh"
@@ -256,13 +254,7 @@ cudaError_t launch_inst(const CUtensorMap& mw, const CUtensorMap& mx, const Gemm
   }
   const int tiles = ((p.T + BT - 1) / BT) * ((p.N + BM - 1) / BM) * (p.k_splits > 1 ? p.k_splits : 1);
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(384); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute la[1];
-  la[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  la[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = la; cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, mw, mx, p);
+  return launch_pdl(kern, dim3(grid), dim3(384), smem, st, pdl, mw, mx, p);
 }
 
 }  // namespace
@@ -286,9 +278,8 @@ int launch_gemm_bf16(const __nv_bfloat16* X, const __nv_bfloat16* W, float* Y, c
   CUtensorMap mw, mx;
   if (!make_map(&mw, W, N, K, BM) || !make_map(&mx, X, T, K, BT)) return -1;
   if (!gemm_splits_supported(K, k_splits) || (k_splits > 1 && resid)) return -1;
-  // PDL launches request the W tiles of the whole ring before waiting for the kernel in front (CL_GEMM_PRE stages)
-  static const int pre_env = getenv("CL_GEMM_PRE") ? atoi(getenv("CL_GEMM_PRE")) : 8;
-  GemmParams p{Y, T, N, K, N, resid ? 1 : 0, k_splits, pdl ? pre_env : 0, nullptr, 0};
+  // PDL launches request the W tiles of the whole ring (at most 8 stages) before waiting for the kernel in front
+  GemmParams p{Y, T, N, K, N, resid ? 1 : 0, k_splits, pdl ? 8 : 0, nullptr, 0};
   cudaError_t e;
   switch (BT) {
     case 128: e = launch_inst<128, 6>(mw, mx, p, st, pdl); break;

@@ -37,7 +37,6 @@ struct GemvArgs {
   int x_stride = 0, y_stride = 0;
   const int* slots = nullptr;        // blockIdx.y = b -> slot (nullptr => identity)
   int batch = 1;
-  int pdl_early = 1;                 // 1: trigger dependents at kernel start; 0: when this CTA has issued its last load
   QkvEpi qkv;                        // EPI_QKV only
   long long* tl = nullptr;           // debug timeline (CL_TIMELINE=1): 4 globaltimer stamps written by CTA 0
 };
@@ -58,7 +57,6 @@ struct AttnDecodeArgs {
   const int* slots = nullptr;
   int batch = 1;
   int n_heads = 0, n_kv = 0, head_dim = 0, page_size = 0, nsplit = 0;
-  int pdl_early = 1;
   long long* tl = nullptr;
   int ring_bytes = 0;                // filled by the launcher
   int tc_small = 0;                  // attn_decode_tc: 4-warp CTAs, two per SM (attn_decode_tc_plan)
@@ -214,9 +212,9 @@ struct MegaArgs {
   unsigned* bars = nullptr;            // [n_layers * 6] grid-barrier counters, zero at kernel start
   unsigned* tile_ctr = nullptr;        // [n_layers * 4] dynamic tile-scheduler counters, zero at kernel start
   unsigned* pf_ctr = nullptr;          // L2 lookahead frontier (one counter, zero at kernel start); nullptr = off
-  int pause_in_barrier = 0;            // producer issues no new copies while the consumers sit in a grid barrier
-  int max_flight = 6;                  // cap on bulk copies in flight per CTA (<= ring slots)
-  int pf_min = 296, pf_budget = 0;     // lookahead window in tiles ahead of a CTA's own demand position
+  // Producer issues no new copies while the consumers sit in a grid barrier.  A field rather than a constant: with the
+  // branch folded away, ptxas gives decode_mega_kernel a larger stack frame and more spill stores.
+  int pause_in_barrier = 1;
   long long* tl = nullptr;             // debug: [n_layers][16] globaltimer stamps of CTA tl_cta
   int tl_cta = 0;
   long long kv_layer_rows = 0;         // rows of one layer in the KV tensor maps (= n_pages * n_kv * page)

@@ -270,7 +270,7 @@ int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_
   a.block_tables = dbt.as<int>(); a.bt_stride = pool.bt_stride; a.pos = dpos.as<int>();
   a.out = dout.as<float>(); a.out_stride = (int)qd; a.out_bf16 = out_bf16 ? dob.as<__nv_bfloat16>() : nullptr;
   a.part = dpart.as<float>(); a.counters = dcnt.as<unsigned>(); a.slots = dslots.as<int>(); a.batch = batch;
-  a.n_heads = n_heads; a.n_kv = n_kv; a.head_dim = HD; a.page_size = P; a.nsplit = ns; a.pdl_early = 0; a.tc_small = small;
+  a.n_heads = n_heads; a.n_kv = n_kv; a.head_dim = HD; a.page_size = P; a.nsplit = ns; a.tc_small = small;
   // variant -1: the tensor-core kernel where it takes the shape and the pool's tensor maps exist, as in the engine
   const long long pool_rows = 2LL * pool.n_pages * n_kv * P;
   CUtensorMap km, vm;

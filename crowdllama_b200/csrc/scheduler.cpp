@@ -381,13 +381,9 @@ void Engine::scheduler_main() {
   cudaSetDevice(device_);
   {
     std::lock_guard<std::mutex> elk(mu_);
-    const char* v = getenv("CL_SCHED_BLOCKING_SYNC");
-    sched_blocking_sync_ = !v || atoi(v) != 0;
-    v = getenv("CL_SCHED_MULTI_PREFILL");
+    const char* v = getenv("CL_SCHED_MULTI_PREFILL");
     sched_multi_prefill_ = v ? atoi(v) != 0 : kDefaultSchedMultiPrefill != 0;
-    v = getenv("CL_SCHED_LINGER_US");
-    sched_linger_us_ = v ? atoi(v) : kDefaultSchedLingerUs;
-    if (sched_blocking_sync_ && !step_done_ev_ && cudaEventCreateWithFlags(&step_done_ev_, cudaEventBlockingSync | cudaEventDisableTiming) != cudaSuccess) {
+    if (!step_done_ev_ && cudaEventCreateWithFlags(&step_done_ev_, cudaEventBlockingSync | cudaEventDisableTiming) != cudaSuccess) {
       cudaGetLastError();
       step_done_ev_ = nullptr;
     }
@@ -415,18 +411,18 @@ void Engine::scheduler_main() {
 
 // Waits until there is work; false once the engine stops.  Burst detection while nothing is running: requests of one wave
 // reach the worker over a few milliseconds (one stream per request, pkg/peer/peer.go:177-182).  Waiting as long as new ones
-// keep arriving within sched_linger_us_ of each other (at most 8x that in total) lets group admission take them in one
-// pass instead of prefilling the first one alone; a lone request pays sched_linger_us_ once, against a prefill of several
+// keep arriving within kSchedLingerUs of each other (at most 8x that in total) lets group admission take them in one
+// pass instead of prefilling the first one alone; a lone request pays kSchedLingerUs once, against a prefill of several
 // milliseconds.
 bool Engine::wait_for_work() {
   std::unique_lock<std::mutex> lk(q_mu_);
   q_cv_.wait(lk, [&] { return stop_ || !queue_.empty() || !active_.empty() || prefilling_; });
   if (stop_) return false;
-  if (sched_multi_prefill_ && sched_linger_us_ > 0 && active_.empty() && !prefilling_ && !queue_.empty()) {
-    const auto t_end = std::chrono::steady_clock::now() + std::chrono::microseconds(8 * (int64_t)sched_linger_us_);
+  if (sched_multi_prefill_ && active_.empty() && !prefilling_ && !queue_.empty()) {
+    const auto t_end = std::chrono::steady_clock::now() + std::chrono::microseconds(8 * (int64_t)kSchedLingerUs);
     while ((int)queue_.size() < max_batch_ && std::chrono::steady_clock::now() < t_end) {
       const size_t n = queue_.size();
-      if (!q_cv_.wait_for(lk, std::chrono::microseconds(sched_linger_us_), [&] { return stop_ || queue_.size() != n; })) break;   // quiet: go
+      if (!q_cv_.wait_for(lk, std::chrono::microseconds(kSchedLingerUs), [&] { return stop_ || queue_.size() != n; })) break;   // quiet: go
       if (stop_) break;
     }
   }
@@ -647,7 +643,7 @@ int Engine::step_running() {
   // Batched steps last milliseconds: wait on a blocking-sync event instead of spinning in cudaStreamSynchronize, so that
   // eight worker processes on one box do not burn eight host cores (the box's cgroup quota is 16) while their GPUs
   // work.  Single-sequence steps (latency matters) keep the spinning wait.
-  if (B >= 2 && sched_blocking_sync_ && step_done_ev_) {
+  if (B >= 2 && step_done_ev_) {
     if (cudaEventRecord(step_done_ev_, stream_) != cudaSuccess || cudaEventSynchronize(step_done_ev_) != cudaSuccess) return CL_ERR_CUDA;
   } else if (cudaStreamSynchronize(stream_) != cudaSuccess) {
     return CL_ERR_CUDA;

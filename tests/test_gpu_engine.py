@@ -104,7 +104,6 @@ def test_batched_decode_matches_single_and_oracle(monkeypatch, batch_gemm):
     """Continuous-batching inner loop: B sequences of different lengths advance together.  CL_BATCH_GEMM=1 is
     the tensor-core path (wgmma split-K projections + glue kernels), 0 the per-sequence GEMV kernels."""
     monkeypatch.setenv("CL_BATCH_GEMM", batch_gemm)
-    monkeypatch.setenv("CL_BATCH_GEMM_MIN", "2")
     cfg = oc.PRESETS["tiny-test"]
     m = oc.Model(cfg, seed=5)
     with eng.Engine(preset="tiny-test", seed=5, max_batch=4) as e:

@@ -43,20 +43,20 @@ def gemv_sweep(f):
 
 def decode_sweep(f, preset="llama3-8b", ctx=4096, steps=128):
     bytes_per_tok = None
-    envs = [dict(CL_GEMV_VARIANT="1", CL_PDL="1"), dict(CL_GEMV_VARIANT="1", CL_PDL="0")]
+    # (decode_path, environment): decode_path 2 = TMA-ring GEMV, 1 = LDG GEMV (per-op path)
+    runs = [(2, dict(CL_PDL="1")), (2, dict(CL_PDL="0"))]
     if "full" in sys.argv:
-        envs += [dict(CL_GEMV_VARIANT="0", CL_PDL="0"), dict(CL_GEMV_VARIANT="0", CL_PDL="1"),
-                 dict(CL_GEMV_VARIANT="1", CL_PDL="1", CL_GRAPH="0")]
+        runs += [(1, dict(CL_PDL="0")), (1, dict(CL_PDL="1")), (2, dict(CL_PDL="1", CL_GRAPH="0"))]
     for spec in sys.argv:
         if "=" in spec and spec.startswith("CL_"):
-            envs = [dict(kv.split("=") for kv in spec.split(","))] + envs[:1]
-    for env in envs:
-        for k in ("CL_GEMV_VARIANT", "CL_PDL", "CL_GRAPH", "CL_ATTN_NSPLIT"):
+            runs = [(2, dict(kv.split("=") for kv in spec.split(",")))] + runs[:1]
+    for decode_path, env in runs:
+        for k in ("CL_PDL", "CL_GRAPH"):
             os.environ.pop(k, None)
         os.environ.update(env)
         try:
             t0 = time.time()
-            with eng.Engine(preset=preset, seed=1234, max_batch=1) as e:
+            with eng.Engine(preset=preset, seed=1234, max_batch=1, decode_path=decode_path) as e:
                 t_init = time.time() - t0
                 c = e.cfg
                 p_read = c["n_layers"] * ((c["n_heads"] + 2 * c["n_kv_heads"]) * c["head_dim"] * c["d_model"] +
@@ -76,12 +76,12 @@ def decode_sweep(f, preset="llama3-8b", ctx=4096, steps=128):
                 mean_ctx = ctx + steps / 2
                 bytes_per_tok = 2 * p_read + kv_tok * (mean_ctx + 1)
                 tps = steps / (ms * 1e-3)
-                emit(f, bench="decode", preset=preset, ctx=ctx, steps=steps, env=env, ms_per_tok=round(ms / steps, 4),
+                emit(f, bench="decode", preset=preset, ctx=ctx, steps=steps, decode_path=decode_path, env=env, ms_per_tok=round(ms / steps, 4),
                      tok_s=round(tps, 2), gbs=round(bytes_per_tok * tps / 1e9, 1),
                      frac=round(bytes_per_tok * tps / 1e9 / HBM, 4), init_s=round(t_init, 1), fill_s=round(t_fill, 1),
                      prefill_s=round(t_prefill, 3), fill_ms_per_tok=round(ms_fill / 64, 4), launches=e.stats()["kernel_launches"])
         except Exception as ex:  # noqa: BLE001
-            emit(f, bench="decode", env=env, error=str(ex))
+            emit(f, bench="decode", decode_path=decode_path, env=env, error=str(ex))
 
 
 def gemm_sweep(f):
