@@ -586,6 +586,16 @@ int cl_debug_seq_hidden(cl_engine* e, cl_seq_t s, int32_t what, float* out, int3
   std::lock_guard<std::mutex> lk(e->impl.mu_);
   CL_GUARD(return e->impl.debug_seq_hidden(s, what, out, n, mega_out);)
 }
+int cl_debug_pass_info(cl_engine* e, int32_t* info, int32_t* segs, int32_t max_segs) {
+  if (!e || !info) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(return e->impl.debug_pass_info(info, segs, max_segs);)
+}
+int cl_debug_pass_rows(cl_engine* e, int32_t what, int32_t row0, int32_t n, float* out) {
+  if (!e || !out) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(return e->impl.debug_pass_rows(what, row0, n, out);)
+}
 
 // ---- paged-KV allocator (host logic) ---------------------------------------------------------------
 int cl_kvpool_create(int32_t n_pages, int32_t page_size, cl_kvpool** out) {

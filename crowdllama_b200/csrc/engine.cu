@@ -911,6 +911,7 @@ int Engine::decode_step(cl_seq_t s, int32_t id, float* logits_out, int32_t* argm
 
 int Engine::prefill_tokenwise(cl_seq_t s, const int32_t* ids, int n, float* logits_out) {
   auto& q = seqs_[s];
+  pass_ = PassRecord{};   // decode steps, not a multi-row pass: debug_pass_rows must not offer an older pass's rows
   int rc = ensure_capacity(s, q.len + n);
   if (rc) return rc;
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
@@ -1060,11 +1061,16 @@ int Engine::seq_fake_fill(cl_seq_t s, int n_tokens) {
 
 int Engine::debug_kv(cl_seq_t s, int layer, int which, int t0, int n, float* out) {
   if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
-  if (layer < 0 || layer >= cfg.n_layers || t0 < 0 || n <= 0 || t0 + n > seqs_[s].len || !out) { set_last_error("debug_kv: bad range"); return CL_ERR_INVALID_ARG; }
+  // which 2 / 3: K / V up to the end of the pages the sequence holds (a verify pass's rejected rows lie past its length)
+  const long long end = which >= 2 ? (long long)pool_->pages_of(s).size() * page_size_ : seqs_[s].len;
+  if (which < 0 || which > 3 || layer < 0 || layer >= cfg.n_layers || t0 < 0 || n <= 0 || t0 + n > end || !out) {
+    set_last_error("debug_kv: bad selector or range");
+    return CL_ERR_INVALID_ARG;
+  }
   float* tmp = nullptr;
   const size_t bytes = (size_t)n * kv_dim_ * 4;
   CL_CUDA_OK(cudaMalloc(&tmp, bytes));
-  const __nv_bfloat16* pool = (which ? vpool_ : kpool_) + (size_t)layer * kv_layer_elems_;
+  const __nv_bfloat16* pool = (which & 1 ? vpool_ : kpool_) + (size_t)layer * kv_layer_elems_;
   int rc = CL_OK;
   if (launch_gather_kv(pool, d_bt_ + (size_t)s * max_pages_per_seq_, page_size_, cfg.n_kv_heads, cfg.head_dim, t0, n, tmp, stream_) < 0 ||
       cudaMemcpyAsync(out, tmp, bytes, cudaMemcpyDeviceToHost, stream_) != cudaSuccess || cudaStreamSynchronize(stream_) != cudaSuccess) {
@@ -1195,6 +1201,35 @@ int Engine::debug_seq_hidden(cl_seq_t s, int what, float* out, int n, int32_t* m
   std::vector<uint16_t> tmp((size_t)n);
   CL_CUDA_OK(cudaMemcpy(tmp.data(), (what == 4 ? bws_->attn : bws_->act) + (size_t)b * n, (size_t)n * 2, cudaMemcpyDeviceToHost));
   for (int i = 0; i < n; ++i) { const uint32_t u = (uint32_t)tmp[(size_t)i] << 16; memcpy(&out[i], &u, 4); }
+  return CL_OK;
+}
+
+int Engine::debug_pass_info(int32_t* info, int32_t* segs, int max_segs) {
+  if (pass_.T == 0) { set_last_error("debug_pass_info: no multi-row pass since the last token-wise prefill or failed pass"); return CL_ERR_INVALID_ARG; }
+  if (!info || max_segs < 0 || (max_segs > 0 && !segs)) { set_last_error("debug_pass_info: bad arguments"); return CL_ERR_INVALID_ARG; }
+  info[0] = pass_.path; info[1] = pass_.attn; info[2] = pass_.T; info[3] = (int32_t)pass_.segs.size();
+  for (int i = 0; i < max_segs && i < (int)pass_.segs.size(); ++i) {
+    const PrefillSegment& g = pass_.segs[(size_t)i];
+    segs[4 * i] = g.seq; segs[4 * i + 1] = g.row0; segs[4 * i + 2] = g.n; segs[4 * i + 3] = g.pos0;
+  }
+  return CL_OK;
+}
+
+int Engine::debug_pass_rows(int what, int row0, int n, float* out) {
+  if (pass_.T == 0) { set_last_error("debug_pass_rows: no multi-row pass since the last token-wise prefill or failed pass"); return CL_ERR_INVALID_ARG; }
+  if (what < 0 || what > 3 || row0 < 0 || n <= 0 || row0 + n > pass_.T || !out) { set_last_error("debug_pass_rows: bad selector or range"); return CL_ERR_INVALID_ARG; }
+  const bool small = pass_.path == kPassSplitK;
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  if (what == 0) {
+    const size_t w = cfg.d_model;
+    CL_CUDA_OK(cudaMemcpy(out, (small ? sws_->h : pws_->h) + (size_t)row0 * w, (size_t)n * w * 4, cudaMemcpyDeviceToHost));
+    return CL_OK;
+  }
+  const size_t w = what == 3 ? cfg.d_ff : q_dim_, cnt = (size_t)n * w;
+  const __nv_bfloat16* src = what == 1 ? (small ? sws_->q : pws_->q) : what == 2 ? (small ? sws_->attn : pws_->attn) : (small ? sws_->act : pws_->act);
+  std::vector<uint16_t> tmp(cnt);
+  CL_CUDA_OK(cudaMemcpy(tmp.data(), src + (size_t)row0 * w, cnt * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < cnt; ++i) { const uint32_t u = (uint32_t)tmp[i] << 16; memcpy(&out[i], &u, 4); }
   return CL_OK;
 }
 

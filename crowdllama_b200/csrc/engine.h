@@ -351,6 +351,8 @@ class Engine {
   int time_dominant_kernel(cl_seq_t s, int32_t first_id, int n_steps, float* kernel_ms, float* step_ms);
   int debug_hidden(float* out, int n);
   int debug_seq_hidden(cl_seq_t s, int what, float* out, int n, int32_t* mega_out);   // contract in include/clengine.h
+  int debug_pass_info(int32_t* info, int32_t* segs, int max_segs);                  // the latest multi-row pass (clengine.h)
+  int debug_pass_rows(int what, int row0, int n, float* out);                        // rows of its workspace (clengine.h)
   int debug_timeline(long long* out, int n);   // CL_TIMELINE=1: globaltimer stamps of the last step (CTA 0 of every node)
   int stats(cl_stats* out);
 
@@ -407,6 +409,14 @@ class Engine {
   // one tile-path pass of T rows made of n_segs segments; leaves the final residual rows in pws_->h
   int prefill_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, int& launches, LaunchProfiler& prof);
   int attn_prefill(const AttnPrefillArgs& a, int layer, int& launches, LaunchProfiler& prof);   // the one choice of prefill attention kernel
+  int prefill_attn_kind(int pos0, int n) const;   // the kernel attn_prefill runs for n rows from pos0: kPassAttnMma / kPassAttnWgmma
+  // What the latest multi-row pass was, on the host (debug_pass_info / debug_pass_rows); T == 0: no pass whose rows the
+  // workspace holds (none yet, a token-wise prefill since, or a failed pass).  Recording adds no device work.
+  enum { kPassSplitK = 0, kPassTile = 1 };
+  enum { kPassAttnMma = 0, kPassAttnWgmma = 1, kPassAttnVerify = 2, kPassAttnMixed = 3 };
+  struct PassRecord { int path = -1, attn = -1, T = 0; std::vector<PrefillSegment> segs; };
+  void record_pass(int path, bool multi_row, const PrefillSegment* segs, int n_segs, int T);
+  PassRecord pass_;
   int prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_out);    // short prompts: split-K projections (prefill.cu)
   int ensure_small_ws();
   // the split-K pass of prefill_small and verify_batch: T rows made of n_segs segments; leaves sws_->h and the

@@ -34,11 +34,27 @@ static int ws_alloc(std::vector<void*>& allocs, T*& p, size_t bytes) {
 // Causal attention of one prefill segment in layer l: the wgmma kernel where it applies (head_dim 128, page 32, the pool's
 // tensor maps), the mma.sync kernel otherwise.
 int Engine::attn_prefill(const AttnPrefillArgs& a, int l, int& launches, LaunchProfiler& prof) {
-  if (have_kv_maps_ && attn_prefill_tc_supported(a.n_heads, a.n_kv, a.head_dim, a.page_size, a.pos0, a.T))
+  if (prefill_attn_kind(a.pos0, a.T) == kPassAttnWgmma)
     CL_LAUNCH(launch_attn_prefill_tc(a, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_));
   else
     CL_LAUNCH(launch_attn_prefill(a, stream_));
   return CL_OK;
+}
+
+int Engine::prefill_attn_kind(int pos0, int n) const {
+  return have_kv_maps_ && attn_prefill_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, pos0, n) ? kPassAttnWgmma
+                                                                                                                     : kPassAttnMma;
+}
+
+// The record of a pass that completed: its path, its segments and the attention kernel they ran (kPassAttnMixed when the
+// segments of one pass took different prefill kernels).
+void Engine::record_pass(int path, bool multi_row, const PrefillSegment* segs, int n_segs, int T) {
+  pass_.path = path;
+  pass_.T = T;
+  pass_.segs.assign(segs, segs + n_segs);
+  pass_.attn = multi_row ? kPassAttnVerify : prefill_attn_kind(segs[0].pos0, segs[0].n);
+  for (int i = 1; i < n_segs && !multi_row; ++i)
+    if (prefill_attn_kind(segs[i].pos0, segs[i].n) != pass_.attn) pass_.attn = kPassAttnMixed;
 }
 
 // Short prompts (prefill_min_tokens_ <= n <= 256, e.g. a 128-token chat): one token tile per W row tile means only
@@ -108,6 +124,7 @@ int Engine::small_pass(const PrefillSegment* segs, int n_segs, const int* ids, i
   const int s_qkv = pick_splits_public(qkv_dim_, d), s_o = pick_splits_public(d, q_dim_), s_gu = pick_splits_public(2 * F, d), s_dn = pick_splits_public(d, F);
   SmallPrefillWs& w = *sws_;
   int rc;
+  pass_ = PassRecord{};
   AttnVerifyArgs va;
   const bool multi_row = seg_table && have_kv_maps_ && attn_verify_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_);
   if (multi_row) {
@@ -152,6 +169,7 @@ int Engine::small_pass(const PrefillSegment* segs, int n_segs, const int* ids, i
   }
   // fold the last down-projection into the residual rows; the final-norm rows it also writes feed the verify pass's head
   CL_LAUNCH(launch_batch_resid_norm(w.h, d, pending, pending_s, T, final_norm_, cfg.rms_eps, w.xn, w.iota, stream_, bp));
+  record_pass(kPassSplitK, multi_row, segs, n_segs, T);
   return CL_OK;
 }
 
@@ -341,6 +359,7 @@ int Engine::ensure_prefill_ws(int tokens) {
   int rc;
   if (!pws_) pws_.reset(new PrefillWs());
   if (pws_->cap_tokens >= tokens) return CL_OK;
+  if (pass_.path == kPassTile) pass_ = PassRecord{};   // the recorded rows stay behind in the old buffers
   const size_t T = (size_t)std::max(tokens, std::min(prefill_chunk_tokens_, cfg.max_seq_len));
   if ((rc = ws_alloc(allocs_, pws_->xn, T * d * 2)) || (rc = ws_alloc(allocs_, pws_->qkv, T * qkv_dim_ * 4)) ||
       (rc = ws_alloc(allocs_, pws_->q, T * q_dim_ * 2)) || (rc = ws_alloc(allocs_, pws_->attn, T * q_dim_ * 2)) ||
@@ -357,6 +376,7 @@ int Engine::prefill_pass(const PrefillSegment* segs, int n_segs, const int* ids,
   const int d = cfg.d_model, F = cfg.d_ff;
   PrefillWs& w = *pws_;
   int rc;
+  pass_ = PassRecord{};
   CL_LAUNCH(launch_embed_rows(embed_, d, ids, w.h, T, stream_));
   for (int l = 0; l < cfg.n_layers; ++l) {
     const auto& L = layers_[l];
@@ -381,6 +401,7 @@ int Engine::prefill_pass(const PrefillSegment* segs, int n_segs, const int* ids,
     CL_LAUNCH(launch_gemm_bf16_silu(w.xn, L.wgu, T, 2 * F, d, w.act, F, stream_));
     CL_LAUNCH(launch_gemm_bf16(w.act, L.wdown, w.h, w.h, T, d, F, stream_));
   }
+  record_pass(kPassTile, false, segs, n_segs, T);
   return CL_OK;
 }
 

@@ -89,7 +89,8 @@ EXPORTS = [
     "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_engine_set_speculate_batch", "cl_engine_set_prefix_host_cache", "cl_draft_ngram", "cl_decode_verify", "cl_decode_verify_batch", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
     "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
-    "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_seq_hidden", "cl_debug_timeline",
+    "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_seq_hidden", "cl_debug_pass_info",
+    "cl_debug_pass_rows", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
     "cl_op_attn_decode_batch", "cl_op_attn_verify", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
     "cl_op_attn_prefill_cached", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
@@ -164,6 +165,8 @@ def lib():
         "cl_debug_kv": (C.c_int, [vp, i32, i32, i32, i32, i32, vp]),
         "cl_debug_hidden": (C.c_int, [vp, vp, i32]),
         "cl_debug_seq_hidden": (C.c_int, [vp, i32, i32, vp, i32, P(i32)]),
+        "cl_debug_pass_info": (C.c_int, [vp, vp, vp, i32]),
+        "cl_debug_pass_rows": (C.c_int, [vp, i32, i32, i32, vp]),
         "cl_debug_timeline": (C.c_int, [vp, vp, i32]),
         "cl_op_gemv": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, P(f32)]),
         "cl_op_gemv_residual": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, vp, i32, i32]),
@@ -513,7 +516,9 @@ class Engine:
         _check(lib().cl_seq_fake_fill(self._h, s, n_tokens), "cl_seq_fake_fill")
 
     def debug_kv(self, s: int, layer: int, which: int, t0: int, n: int) -> np.ndarray:
-        """Cached K (which=0) / V (which=1) rows of `layer` for tokens t0..t0+n-1: [n][n_kv*head_dim] fp32."""
+        """Cached K (which=0) / V (which=1) rows of `layer` for tokens t0..t0+n-1: [n][n_kv*head_dim] fp32.  which 2 / 3:
+        K / V up to the end of the pages the sequence holds, where a verify pass leaves its rejected rows (valid until the
+        sequence's next pass or step)."""
         out = np.empty((n, self.cfg["n_kv_heads"] * self.cfg["head_dim"]), np.float32)
         _check(lib().cl_debug_kv(self._h, s, layer, which, t0, n, _ptr(out)), "cl_debug_kv")
         return out
@@ -537,6 +542,31 @@ class Engine:
         n = self.cfg["d_model"] if i == 0 else self.cfg["d_ff"] if i in (3, 5) else self.cfg["n_heads"] * self.cfg["head_dim"]
         out = np.empty(n, np.float32)
         _check(lib().cl_debug_seq_hidden(self._h, s, i, _ptr(out), n, None), "cl_debug_seq_hidden")
+        return out
+
+    PASS_PATHS = ("split-k", "tile")
+    PASS_ATTN = ("mma", "wgmma", "verify", "mixed")
+
+    def debug_pass_info(self) -> dict:
+        """cl_debug_pass_info: the latest multi-row pass.  {"path": "split-k" | "tile", "attn": "mma" | "wgmma" | "verify" |
+        "mixed", "T": rows, "segs": [(seq, row0, n, pos0), ...]}.  EngineError when none is recorded (a token-wise prefill
+        or a failed pass since)."""
+        info = np.zeros(4, np.int32)
+        _check(lib().cl_debug_pass_info(self._h, _ptr(info), None, 0), "cl_debug_pass_info")
+        segs = np.zeros((max(int(info[3]), 1), 4), np.int32)
+        _check(lib().cl_debug_pass_info(self._h, _ptr(info), _ptr(segs), int(info[3])), "cl_debug_pass_info")
+        return dict(path=self.PASS_PATHS[info[0]], attn=self.PASS_ATTN[info[1]], T=int(info[2]),
+                    segs=[tuple(int(v) for v in g) for g in segs[:int(info[3])]])
+
+    def debug_pass_rows(self, what: str, row0: int = 0, n: int = None) -> np.ndarray:
+        """cl_debug_pass_rows: rows row0 .. row0 + n - 1 (n None: to the last row) of the latest multi-row pass after its
+        last layer.  what: "h" (fp32 residual stream), "q" (roped), "attn", "act" (bf16 values as float32)."""
+        i = ("h", "q", "attn", "act").index(what)
+        if n is None:
+            n = self.debug_pass_info()["T"] - row0
+        w = self.cfg["d_model"] if i == 0 else self.cfg["d_ff"] if i == 3 else self.cfg["n_heads"] * self.cfg["head_dim"]
+        out = np.empty((max(n, 0), w), np.float32)
+        _check(lib().cl_debug_pass_rows(self._h, i, row0, n, _ptr(out) if n > 0 else None), "cl_debug_pass_rows")
         return out
 
     def runs_mega_kernel(self) -> bool:

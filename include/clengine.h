@@ -401,7 +401,10 @@ int cl_generate_ids_logprobs(cl_engine* e, const int32_t* prompt_ids, int32_t n_
  * bf16).  Lets the long-context decode kernels be compared with the oracle without a long CPU prefill. */
 int cl_seq_fake_fill(cl_engine* e, cl_seq_t seq, int32_t n_tokens);
 /* Parity aid: cached K (which = 0) / V (which = 1) rows of `layer`, tokens t0..t0+n-1 of the sequence, gathered from
- * the paged pool: out[n][n_kv_heads*head_dim] fp32 (the bf16 cache values).  Checks EVERY position of a long prefill. */
+ * the paged pool: out[n][n_kv_heads*head_dim] fp32 (the bf16 cache values).  Checks EVERY position of a long prefill.
+ * which = 2 (K) / 3 (V) read up to the end of the pages the sequence holds rather than its length: there a verify pass
+ * (cl_decode_verify*) leaves the K/V of its rejected rows.  Those rows are valid only until the sequence's next pass or
+ * step, which writes the same positions.  CL_ERR_INVALID_ARG for another `which` or a range past that end. */
 int cl_debug_kv(cl_engine* e, cl_seq_t seq, int32_t layer, int32_t which, int32_t t0, int32_t n, float* out);
 /* bench.py's roofline.dominant_kernel: n_steps greedy single-sequence steps launched eagerly with a CUDA-event pair
  * (on the launching stream) around the step's dominant kernel — decode_mega_kernel, or the per-layer kernel stack
@@ -421,6 +424,18 @@ int cl_debug_hidden(cl_engine* e, float* out, int32_t n);
  * on the sequence of the most recent single-sequence step.  CL_ERR_INVALID_ARG for a wrong n or `what`, and for 4 / 5 when
  * the sequence was not in the latest batched step. */
 int cl_debug_seq_hidden(cl_engine* e, cl_seq_t seq, int32_t what, float* out, int32_t n, int32_t* mega_out);
+/* Parity aid: the latest multi-row pass — a split-K pass (prompts of 16 .. 256 tokens, every cl_decode_verify /
+ * cl_decode_verify_batch) or a tile-path pass (longer prompts, one per chunk; cl_prefill_batch).  info[4] = {path (0 split-K,
+ * 1 tile), attention kernel (0 mma.sync prefill, 1 wgmma prefill, 2 multi-row verify, 3 segments with different prefill
+ * kernels), T (rows), n_segs}; segs[min(n_segs, max_segs)][4] = {sequence, first row, rows, position of the first row}.  A
+ * prefill longer than one chunk leaves its last chunk's pass.  CL_ERR_INVALID_ARG when no pass is recorded: none yet, or a
+ * token-wise prefill (fewer than 16 tokens) or a failed pass since. */
+int cl_debug_pass_info(cl_engine* e, int32_t* info, int32_t* segs, int32_t max_segs);
+/* Rows row0 .. row0+n-1 of that pass's workspace after its last layer, as fp32; the stream is synchronised first.  what:
+ * 0 = the fp32 residual stream (d_model; for a split-K pass after its final fold), 1 = roped q (n_heads * head_dim, bf16),
+ * 2 = attention output (n_heads * head_dim, bf16), 3 = SwiGLU activation (d_ff, bf16).  Valid until the next pass.
+ * CL_ERR_INVALID_ARG for a wrong `what`, a range outside 0 .. T - 1, or no recorded pass (cl_debug_pass_info). */
+int cl_debug_pass_rows(cl_engine* e, int32_t what, int32_t row0, int32_t n, float* out);
 /* profiling aid (engine created with env CL_TIMELINE=1): %globaltimer stamps [node][4] = {CTA start,
  * dependency satisfied, inputs loaded / pages consumed, outputs written} of CTA 0 of every kernel node of
  * the most recent token step; nodes = n_layers * {qkv, attn, o, gate|up, down} + lm_head.  Returns the

@@ -1,7 +1,7 @@
-"""Stage-by-stage float64 parity of one transformer layer as the decode step and the prefill paths run it.
+"""Stage-by-stage float64 parity of one transformer layer as the decode step, the prefill passes and the verify passes run it.
 
 What the whole-model tests only see through logits is checked here stage by stage on engines whose every weight the test
-owns (cl_engine_set_tensor), with the buffers cl_debug_seq_hidden and cl_debug_kv expose:
+owns (cl_engine_set_tensor), with the buffers cl_debug_seq_hidden, cl_debug_pass_rows and cl_debug_kv expose:
 
   1. RMSNorm -> q|k|v projection -> RoPE -> bf16 -> cache append      q, and the K / V rows written at `pos`
   2. split-KV attention + combine                                       attention output
@@ -14,10 +14,13 @@ bound of a stage holds its own rounding points only and is checked per element. 
 kernels' summation structure below; none is fitted to an observation.  The observed max(err / bound) is printed (-s).
 
 Covered: decode_mega_kernel, the per-op path with both GEMV kernels, the batched step (wgmma projections, batch_* glue,
-tensor-core attention, graph and PDL as shipped), and the K / V rows of every prefill path and of the verify passes.
-A verify pass also writes K / V of rejected rows; they lie beyond the sequence's length, where cl_debug_kv does not read,
-so only the accepted rows are checked.  The intermediates h_mid (after the o-projection) and xn are not kept by any path:
-stage 3 and 4 start from the attention output and compose the o-projection's bound.
+tensor-core attention, graph and PDL as shipped) — parts (a), (b) — and, part (d), the rows of every multi-row pass: the
+split-K pass (prompts of 16 .. 256 tokens, the verify passes) and the tile pass (longer prompts, chunk by chunk, and
+cl_prefill_batch), with the mma.sync, wgmma and multi-row verify attention kernels.  cl_debug_pass_info asserts which path
+and kernel a case ran; the rejected rows of a verify pass are read through cl_debug_kv's which 2 / 3.  Long passes are
+checked stage by stage on sampled rows, and stage 1 of K / V on every row of every pass.  The intermediates
+h_mid (after the o-projection) and xn are not kept by any path: stage 3 and 4 start from the attention output and compose
+the o-projection's bound.
 
 The CPU tests at the end feed the same checks with mutated "kernel outputs" (each must exceed its bound by the stated
 margin) and with a float32 numpy layer that sums in another order (must stay inside every bound).
@@ -28,7 +31,8 @@ import numpy as np
 import pytest
 
 from crowdllama_b200 import engine as eng
-from test_gpu_step_kernels import DECODE_C, LONGCTX_B16, _wide_lens, attn64, bf16, f32, ulp_bf16
+from test_gpu_speculative_batch import ATTN_C
+from test_gpu_step_kernels import DECODE_C, LONGCTX_B16, PREFILL_C, _wide_lens, attn64, bf16, f32, ulp_bf16
 
 gpu = pytest.mark.gpu
 U = 2.0 ** -24                                             # unit roundoff of fp32 (round to nearest)
@@ -141,14 +145,17 @@ class Net:
     def model(self, n_layers, **over):
         return dict(dict(self.shape, n_layers=n_layers, vocab_size=VOCAB, rms_eps=EPS), **over)
 
-    def engine(self, n_layers=1, **kw):
+    def engine(self, n_layers=1, zero_branch0=False, **kw):
+        """zero_branch0: layer 0's WO and WDOWN are zero, so layer 0 leaves every row's embedding unchanged (x + 0 is
+        exact in fp32) and layer 1 sees the embedding as its input."""
         e = eng.Engine(model=self.model(n_layers), **kw)
         e.set_tensor(0, "EMBED", bf16(self.embed))
         e.set_tensor(0, "LM_HEAD", bf16(self.lm_head))
         e.set_tensor(0, "FINAL_NORM", bf16(self.final_norm))
         for l in range(n_layers):
             for kind in ("ATTN_NORM", "FFN_NORM", "WQ", "WK", "WV", "WO", "WGATE", "WUP", "WDOWN"):
-                e.set_tensor(l, kind, bf16(self.layer(l)[kind]))
+                w = self.layer(l)[kind]
+                e.set_tensor(l, kind, bf16(np.zeros_like(w) if zero_branch0 and l == 0 and kind in ("WO", "WDOWN") else w))
         return e
 
 
@@ -217,22 +224,27 @@ def stage1(nt, l, h_in, pos, c):
 
 
 def check_layer(nt, l, obs, C, page=32):
-    """obs: arrays with one row per observed step — h_in, pos, q, k_new, v_new, K, V (lists: rows 0 .. pos of the cache),
-    attn, act, h_out and optionally logits.  C: c_qkv, c_o, c_gu, c_dn, c_lm.  Returns {stage: max err / bound per row}."""
+    """obs: arrays with one row per observed row — h_in, pos, q, k_new, v_new, attn, act, h_out; K, V: lists of caches,
+    rows 0 .. (at least) pos of every row that reads them, and kv_seg, each row's index into K / V (default: one cache per
+    row); optionally logits, of the rows logit_rows (default: all).  C: c_qkv, c_o, c_gu, c_dn, c_lm, and c_attn (default
+    DECODE_C), h_adds (default 1).  Returns {stage: max err / bound per row} (stage 5: 0 on rows without logits)."""
     s, L = nt.shape, nt.layer(l)
     H, G, hd = s["n_heads"], s["n_kv_heads"], s["head_dim"]
     qd, kvd = H * hd, G * hd
     h_in = np.asarray(obs["h_in"], np.float64)
+    pos = np.asarray(obs["pos"]).reshape(-1)
     out = {}
-    ref, tol = stage1(nt, l, h_in, obs["pos"], C["c_qkv"])
+    ref, tol = stage1(nt, l, h_in, pos, C["c_qkv"])
     got = np.concatenate([obs["q"], obs["k_new"], obs["v_new"]], axis=1)
     r1 = ratio(got, ref, tol)
     out["1 q"], out["1 k"], out["1 v"] = r1[:, :qd].max(1), r1[:, qd:qd + kvd].max(1), r1[:, qd + kvd:].max(1)
-    r2 = []
-    for i, p in enumerate(obs["pos"]):
-        a_ref, pv = attn64(obs["q"][i:i + 1], obs["K"][i].reshape(-1, G, hd), obs["V"][i].reshape(-1, G, hd), [p], H, G, hd, page=page)
-        r2.append(ratio(obs["attn"][i:i + 1], a_ref, ulp_bf16(a_ref) + DECODE_C * pv).max())
-    out["2 attn"] = np.array(r2)
+    kv_seg = np.asarray(obs.get("kv_seg", np.arange(len(pos))))
+    r2 = np.empty(len(pos))
+    for g in np.unique(kv_seg):                            # one float64 attention per cache, with all of its rows
+        i = np.flatnonzero(kv_seg == g)
+        a_ref, pv = attn64(obs["q"][i], obs["K"][g].reshape(-1, G, hd), obs["V"][g].reshape(-1, G, hd), pos[i], H, G, hd, page=page)
+        r2[i] = ratio(obs["attn"][i], a_ref, ulp_bf16(a_ref) + C.get("c_attn", DECODE_C) * pv).max(1)
+    out["2 attn"] = r2
     attn, act = np.asarray(obs["attn"], np.float64), np.asarray(obs["act"], np.float64)
     o, b_o = proj(L["WO"], attn, None, C["c_o"])
     h_mid = h_in + o
@@ -249,9 +261,11 @@ def check_layer(nt, l, obs, C, page=32):
     hmax = np.maximum(np.maximum(np.abs(h_in), np.abs(h_mid)), np.abs(h_ref))
     out["4 h"] = ratio(obs["h_out"], h_ref, b_o + b_d + 2 * U * hmax * C.get("h_adds", 1)).max(1)
     if "logits" in obs:
-        xn, slack = norm_round(np.asarray(obs["h_out"], np.float64), nt.final_norm)
+        lr = np.asarray(obs.get("logit_rows", np.arange(len(pos))))
+        xn, slack = norm_round(np.asarray(obs["h_out"], np.float64)[lr], nt.final_norm)
         lg, b_l = proj(nt.lm_head, xn, slack, C["c_lm"])
-        out["5 logits"] = ratio(obs["logits"], lg, b_l).max(1)
+        out["5 logits"] = np.zeros(len(pos))
+        out["5 logits"][lr] = ratio(obs["logits"], lg, b_l).max(1)
     return out
 
 
@@ -436,82 +450,305 @@ def test_batched_step_head_dim_64(monkeypatch):
     report("batched B 3 d 2048", labels, check_layer(nt, 0, obs, consts(nt.shape, "gemm")))
 
 
-# ---- GPU: K / V rows of every prefill path --------------------------------------------------------------------------------
-def kv_rows_ratio(nt, ids, pos, K, V):
-    """Rows K, V [n][kv_dim] written for tokens ids at positions pos by a one-layer engine, against stage 1 of their
-    embedding rows with the GEMM constant (the widest of the paths')."""
-    s = nt.shape
+# ---- GPU: every row of the multi-row passes (part d) ---------------------------------------------------------------------
+# The split-K pass (small_pass: prompts of 16 .. 256 tokens, every verify pass) and the tile pass (prefill_pass: longer prompts,
+# one per chunk, and cl_prefill_batch), read back through cl_debug_pass_info / cl_debug_pass_rows after the pass.
+def pass_consts(shape, info, c_lm):
+    """The wgmma constants; the tile path adds each residual projection to h once, in the GEMM epilogue (the split-K pass
+    folds up to 16 partials); the prefill kernels round P to bf16, the multi-row verify kernel does not."""
+    C = dict(consts(shape, "gemm"), c_lm=c_lm, c_attn=ATTN_C if info["attn"] == "verify" else PREFILL_C)
+    if info["path"] == "tile":
+        C["h_adds"] = 1
+    return C
+
+
+def sample_rows(info, seed):
+    """The rows checked stage by stage: every row of a pass of up to 300 rows; of a longer one the first and last row of
+    every 128-row tile and of every segment, and 64 seeded random rows.  (Stage 1 of K / V covers every row of every pass:
+    check_pass.)"""
+    T = info["T"]
+    if T <= 300:
+        return np.arange(T)
+    edges = [r for t0 in range(0, T, 128) for r in (t0, min(t0 + 127, T - 1))]
+    edges += [r for _, r0, n, _ in info["segs"] for r in (r0, r0 + n - 1)]
+    return np.unique(np.concatenate([edges, np.random.default_rng(seed).choice(T, 64, replace=False)]))
+
+
+def pass_rows(e, what, rows):
+    """Rows `rows` (sorted) of the latest pass, one cl_debug_pass_rows call per run of consecutive rows."""
+    cuts = np.flatnonzero(np.diff(rows) != 1) + 1
+    return np.concatenate([e.debug_pass_rows(what, int(run[0]), len(run)) for run in np.split(rows, cuts)])
+
+
+def kv_upto(e, s, layer, end):
+    """K, V rows 0 .. end - 1 of sequence s: below its length through debug_kv which 0 / 1, past it (the rejected rows of a
+    verify pass) through which 2 / 3."""
+    n = min(e.seq_len(s), end)
+    return [np.concatenate(([e.debug_kv(s, layer, w, 0, n)] if n else []) + ([e.debug_kv(s, layer, w + 2, n, end - n)] if end > n else []))
+            for w in (0, 1)]
+
+
+def observe_pass(e, nt, ids, layer=0, seed=0, logits=None, logit_rows=(), kept=None):
+    """The latest pass's rows (sample_rows) with the K / V of their sequences.  ids: the pass's token ids in row order;
+    logits: rows of the pass logit_rows; kept: rows of each segment its sequence kept (a verify pass), the others are
+    reported apart as rejected.  Returns obs, the label of every row group and the pass info."""
+    info = e.debug_pass_info()
+    ids = np.asarray(ids)
+    assert len(ids) == info["T"] and sum(g[2] for g in info["segs"]) == info["T"]
+    rows = sample_rows(info, seed)
+    lr = np.asarray(logit_rows, int)
+    rows = np.union1d(rows, lr).astype(int)
+    seg_of = np.concatenate([np.full(n, i) for i, (_, _, n, _) in enumerate(info["segs"])])[rows]
+    pos = np.array([info["segs"][g][3] + r - info["segs"][g][1] for g, r in zip(seg_of, rows)])
+    K, V = zip(*[kv_upto(e, q, layer, p0 + n) for q, _, n, p0 in info["segs"]])
+    group_all, labels = np.zeros(info["T"], int), []      # the group of every row of the pass
+    for i, (q, r0, n, p0) in enumerate(info["segs"]):
+        a = n if kept is None else kept[i]
+        group_all[r0:r0 + n] = len(labels)
+        labels.append(f"seq {q} rows {r0}..{r0 + min(a, n) - 1} at {p0}" + (f" ({a} kept)" if kept is not None else ""))
+        if a < n:
+            group_all[r0 + a:r0 + n] = len(labels)
+            labels.append(f"seq {q} rejected rows {r0 + a}..{r0 + n - 1} at {p0 + a}")
+    obs = dict(h_in=nt.embed[ids[rows]], pos=pos, q=pass_rows(e, "q", rows), attn=pass_rows(e, "attn", rows),
+               act=pass_rows(e, "act", rows), h_out=pass_rows(e, "h", rows), K=list(K), V=list(V), kv_seg=seg_of,
+               k_new=np.stack([K[g][p] for g, p in zip(seg_of, pos)]), v_new=np.stack([V[g][p] for g, p in zip(seg_of, pos)]),
+               group=group_all[rows], group_all=group_all)
+    if logits is not None:
+        obs["logits"], obs["logit_rows"] = np.asarray(logits).reshape(len(lr), -1), np.searchsorted(rows, lr)
+    return obs, labels, info
+
+
+def kv_rows_ratio(nt, l, ids, pos, K, V, c):
+    """Stage 1 of the K and V rows [R][kv_dim] written for tokens ids at positions pos, whose layer input is their embedding
+    row: max err / bound per row of K and of V.  Before RoPE a row depends on its id only, so the projection runs once per
+    distinct id (prompt_ids has 32), and a pass of thousands of rows is checked whole."""
+    s, L = nt.shape, nt.layer(l)
     qd = s["n_heads"] * s["head_dim"]
-    uniq, inv = np.unique(ids, return_inverse=True)         # stage 1 before RoPE depends on the id only
-    L = nt.layer(0)
+    uniq, inv = np.unique(ids, return_inverse=True)
     xn, slack = norm_round(nt.embed[uniq], L["ATTN_NORM"])
-    y, b = proj(L["WQKV"][qd:], xn, slack, gemm_c(s["d_model"]))
+    y, b = proj(L["WQKV"][qd:], xn, slack, c)
     cos, sin = rope_table(s, pos)
     ref, tol = rope_ref(y[inv], b[inv], cos, sin, s["n_kv_heads"], s["head_dim"])
     r = ratio(np.concatenate([K, V], axis=1), ref, tol + ulp_bf16(ref))
     kvd = K.shape[1]
-    return float(r[:, :kvd].max()), float(r[:, kvd:].max())
+    return r[:, :kvd].max(1), r[:, kvd:].max(1)
 
 
-def check_kv(name, nt, e, s, ids, t0=0):
-    ids = np.asarray(ids)
-    n = len(ids)
-    rk, rv = kv_rows_ratio(nt, ids, t0 + np.arange(n), e.debug_kv(s, 0, 0, t0, n), e.debug_kv(s, 0, 1, t0, n))
-    print(f"[stages] kv rows {name}: {n} rows from {t0}: K {rk:.3g}  V {rv:.3g}")
-    assert rk <= 1.0 and rv <= 1.0, f"{name}: K {rk:.3g} V {rv:.3g}"
+def check_pass(name, nt, e, ids, expect, c_lm, layer=0, seed=0, **kw):
+    """Asserts that the latest pass ran the path and attention kernel `expect`, checks every sampled row stage by stage,
+    and stage 1 of the K / V of every row of the pass ("1 K all", "1 V all")."""
+    obs, labels, info = observe_pass(e, nt, ids, layer, seed, **kw)
+    assert (info["path"], info["attn"]) == expect, f"{name}: the pass ran {info['path']} / {info['attn']}, not {expect}"
+    C = pass_consts(nt.shape, info, c_lm)
+    res = check_layer(nt, layer, obs, C)
+    grouped = {k: np.array([v[obs["group"] == g].max() for g in range(len(labels))]) for k, v in res.items()}
+    segs = info["segs"]
+    rk, rv = kv_rows_ratio(nt, layer, np.asarray(ids), np.concatenate([np.arange(p0, p0 + n) for _, _, n, p0 in segs]),
+                           np.concatenate([obs["K"][i][p0:p0 + n] for i, (_, _, n, p0) in enumerate(segs)]),
+                           np.concatenate([obs["V"][i][p0:p0 + n] for i, (_, _, n, p0) in enumerate(segs)]), C["c_qkv"])
+    grouped["1 K all"] = np.array([rk[obs["group_all"] == g].max() for g in range(len(labels))])
+    grouped["1 V all"] = np.array([rv[obs["group_all"] == g].max() for g in range(len(labels))])
+    return report(f"{name} ({info['path']}, {info['attn']}, T {info['T']}, {len(obs['pos'])} rows)", labels, grouped)
+
+
+def prefill_case(name, nt, e, ids, expect, prefix=None, layer=0):
+    """A fresh sequence (after `prefix`, prefilled first), prefilled with ids; checks the pass and the last row's logits
+    (cl_prefill's GEMV head).  A prompt longer than one chunk leaves its last chunk's pass."""
+    s = e.seq_create()
+    if prefix is not None:
+        e.prefill(s, prefix, want_logits=False)
+    lg = e.prefill(s, ids)
+    info = e.debug_pass_info()
+    T = info["T"]
+    assert info["segs"] == [(s, 0, T, e.seq_len(s) - T)]
+    check_pass(name, nt, e, np.asarray(ids)[len(ids) - T:], expect, gemv_c(nt.shape["d_model"], True), layer,
+               seed=len(ids), logits=lg, logit_rows=[T - 1])
+    e.seq_free(s)
 
 
 @gpu
-@pytest.mark.parametrize("name,page", [("llama", 32), ("llama", 16), ("llama", 64), ("llama32", 32)])
-def test_prefill_kv_rows(name, page):
-    """Token-wise (1, 2), split-K (40 .. 256) and tile (257 ..) prefill, a chunk boundary, a continuation at an unaligned
-    position, several prompts in one pass, and the verify passes: every K / V element at every position."""
-    nt = net(name)
-    full = name == "llama" and page == 32
-    sizes = [1, 2, 40, 128, 256, 257, 300, 1024, 4096] if full else [1, 40, 300]
-    with nt.engine(1, max_batch=4, page_size=page) as e:
-        for n in sizes:
-            s = e.seq_create()
-            ids = prompt_ids(n, n)
-            e.prefill(s, ids, want_logits=False)
-            check_kv(f"{name} page {page} prefill {n}", nt, e, s, ids)
-            e.seq_free(s)
-        s = e.seq_create()
+def test_split_k_pass_rows():
+    """Llama-3-8B layer: prompts of 16, 40, 128, 129 and 256 tokens, a continuation 33 + 40 and 40 rows behind 4096 cached
+    tokens, each through the split-K pass with the wgmma prefill attention."""
+    nt = net("llama")
+    with nt.engine(1, max_batch=4) as e:
+        for n in (16, 40, 128, 129, 256):
+            prefill_case(f"split-k {n}", nt, e, prompt_ids(n, n), ("split-k", "wgmma"))
+        ids = prompt_ids(9, 33 + 40)
+        prefill_case("split-k 33 + 40", nt, e, ids[33:], ("split-k", "wgmma"), prefix=ids[:33])
+        ids = prompt_ids(11, 4096 + 40)
+        prefill_case("split-k 4096 + 40", nt, e, ids[4096:], ("split-k", "wgmma"), prefix=ids[:4096])
+
+
+@gpu
+def test_tile_pass_rows():
+    """Llama-3-8B layer: prompts of 257, 300, 1024 and 4096 tokens, a continuation 33 + 300, 300 rows behind 4096 cached
+    tokens, the last chunk (700 rows at 4096) of a 4796-token prompt; Mistral-7B (theta 1e6) at 8192 with T = 300."""
+    nt = net("llama")
+    with nt.engine(1, max_batch=4) as e:
+        for n in (257, 300, 1024, 4096):
+            prefill_case(f"tile {n}", nt, e, prompt_ids(n, n), ("tile", "wgmma"))
         ids = prompt_ids(9, 33 + 300)
-        e.prefill(s, ids[:33], want_logits=False)
-        e.prefill(s, ids[33:], want_logits=False)
-        check_kv(f"{name} page {page} continuation 33 + 300", nt, e, s, ids)
-        e.seq_free(s)
-        if not full:
-            return
-        s = e.seq_create()
-        ids = prompt_ids(10, 2048 + 700)                    # longer than one chunk of prefill_chunked
-        e.prefill(s, ids, want_logits=False)
-        check_kv("llama chunk boundary", nt, e, s, ids[1900:2200], t0=1900)
-        e.seq_free(s)
+        prefill_case("tile 33 + 300", nt, e, ids[33:], ("tile", "wgmma"), prefix=ids[:33])
+        ids = prompt_ids(12, 4096 + 300)
+        prefill_case("tile 4096 + 300", nt, e, ids[4096:], ("tile", "wgmma"), prefix=ids[:4096])
+        prefill_case("tile last chunk of 4796", nt, e, prompt_ids(13, 4096 + 700), ("tile", "wgmma"))
+    nt = net("mistral")
+    with nt.engine(1, max_batch=2) as e:
+        ids = prompt_ids(14, 8192 + 300)
+        prefill_case("mistral tile 8192 + 300", nt, e, ids[8192:], ("tile", "wgmma"), prefix=ids[:8192])
+
+
+@gpu
+@pytest.mark.parametrize("name,page", [("llama", 16), ("llama", 64), ("llama32", 32)])
+def test_pass_rows_mma_prefill_attention(name, page):
+    """The mma.sync prefill kernel, which the wgmma kernel leaves to pages 16 and 64 and to head_dim 64 (Llama-3.2-1B
+    shape): a split-K and a tile pass, each behind a cached prefix."""
+    nt = net(name)
+    with nt.engine(1, max_batch=4, page_size=page) as e:
+        ids = prompt_ids(page, 33 + 300)
+        prefill_case(f"{name} page {page} split-k 40", nt, e, ids[:40], ("split-k", "mma"))
+        prefill_case(f"{name} page {page} split-k 33 + 40", nt, e, ids[33:73], ("split-k", "mma"), prefix=ids[:33])
+        prefill_case(f"{name} page {page} tile 300", nt, e, ids[:300], ("tile", "mma"))
+        prefill_case(f"{name} page {page} tile 33 + 300", nt, e, ids[33:], ("tile", "mma"), prefix=ids[:33])
+
+
+@gpu
+def test_prefill_batch_pass_rows():
+    """cl_prefill_batch of prompts of 1, 40, 300 and 1000 tokens in one tile pass (segments at rows 0, 1, 41, 341): rows of
+    every segment and the last row of each, whose logits come from the batched wgmma head."""
+    nt = net("llama")
+    with nt.engine(1, max_batch=4) as e:
         seqs = [e.seq_create() for _ in range(4)]
         prompts = [prompt_ids(20 + i, n) for i, n in enumerate((1, 40, 300, 1000))]
-        e.prefill_batch(seqs, prompts, want_logits=False)
-        for q, t in zip(seqs, prompts):
-            check_kv(f"llama prefill_batch {len(t)}", nt, e, q, t)
-        # verify passes: drafts = what greedy decoding of a twin produces, so most rows are accepted and stay readable
-        for q in seqs[2:]:
-            e.seq_free(q)
-        a, b = seqs[0], seqs[1]                             # 1 and 40 cached tokens
-        twin = e.seq_create()
-        e.prefill(twin, prompts[1], want_logits=False)
-        chain = np.concatenate([[19], e.decode_greedy(twin, 19, 17)[0]])   # b's input, then what greedy decoding emits
-        x0 = 19
-        for k in (1, 15):
-            n0 = e.seq_len(b)
-            d = chain[n0 - 40 + 1:n0 - 40 + 1 + k]
-            out, _ = e.decode_verify(b, x0, d)
-            check_kv(f"llama verify k {k} ({len(out)} rows kept)", nt, e, b, np.concatenate([[x0], d])[:len(out)], t0=n0)
-            x0 = int(out[-1])
-        n_a, n_b = e.seq_len(a), e.seq_len(b)
-        outs, _ = e.decode_verify_batch([a, b], [7, 11], [[3, 19, 35], list(range(3, 3 + 16 * 9, 16))])
-        check_kv("llama verify_batch k 3", nt, e, a, [7, 3, 19, 35][:len(outs[0])], t0=n_a)
-        check_kv("llama verify_batch k 9", nt, e, b, ([11] + list(range(3, 3 + 16 * 9, 16)))[:len(outs[1])], t0=n_b)
+        lg = e.prefill_batch(seqs, prompts)
+        last = np.cumsum([len(p) for p in prompts]) - 1
+        assert e.debug_pass_info()["segs"] == [(q, int(r - len(p) + 1), len(p), 0) for q, p, r in zip(seqs, prompts, last)]
+        check_pass("prefill_batch 1 / 40 / 300 / 1000", nt, e, np.concatenate(prompts), ("tile", "wgmma"),
+                   gemm_c(nt.shape["d_model"]), logits=lg, logit_rows=last)
+
+
+def greedy_drafts(e, ids, x0, k, wrong, salt):
+    """k drafts after x0 for a sequence holding ids: what greedy decoding of a twin emits, with draft `wrong` (if < k)
+    replaced, so that the verify pass keeps the rows before it and rejects the rest."""
+    if k == 0:
+        return []
+    twin = e.seq_create()
+    e.prefill(twin, ids, want_logits=False)
+    d = [int(t) for t in e.decode_greedy(twin, x0, k)[0]]
+    e.seq_free(twin)
+    if wrong < k:
+        d[wrong] = (d[wrong] + 16 * (1 + salt % 7)) % VOCAB
+    return d
+
+
+def verify_case(name, nt, e, lens, ks, wrong, attn, batch=True, layer=0):
+    """Sequences holding prompts of `lens` tokens, verified with ks drafts (partly wrong) in one decode_verify_batch pass, or
+    (batch False) one decode_verify pass each.  Every row is checked, rejected ones through debug_kv which 2 / 3, and every
+    row's logits (the verify pass's wgmma head).  Returns the number of rejected rows."""
+    seqs = [e.seq_create() for _ in lens]
+    prompts = [prompt_ids(100 * len(lens) + i, n) for i, n in enumerate(lens)]
+    for q, p in zip(seqs, prompts):
+        e.prefill(q, p, want_logits=False)
+    x0 = [int(p[-1]) ^ 16 for p in prompts]
+    drafts = [greedy_drafts(e, p, x, k, w, i) for i, (p, x, k, w) in enumerate(zip(prompts, x0, ks, wrong))]
+    rejected = 0
+    for grp in [list(range(len(lens)))] if batch else [[i] for i in range(len(lens))]:
+        if batch:
+            outs, lg = e.decode_verify_batch([seqs[i] for i in grp], [x0[i] for i in grp], [drafts[i] for i in grp], want_logits=True)
+        else:
+            out, lg = e.decode_verify(seqs[grp[0]], x0[grp[0]], drafts[grp[0]], want_logits=True)
+            outs = [out]
+        kept = [len(o) for o in outs]
+        rejected += sum(ks[i] + 1 - a for i, a in zip(grp, kept))
+        ids = np.concatenate([[x0[i]] + drafts[i] for i in grp])
+        check_pass(f"{name} k {[ks[i] for i in grp]}", nt, e, ids, ("split-k", attn), gemm_c(nt.shape["d_model"]), layer,
+                   logits=lg, logit_rows=np.arange(len(ids)), kept=kept)
+    for q in seqs:
+        e.seq_free(q)
+    return rejected
+
+
+@gpu
+def test_verify_pass_rows():
+    """cl_decode_verify with k = 1 and 15 (the per-segment prefill attention; rows 20 .. 35 cross a page boundary) and
+    cl_decode_verify_batch over 2 and 8 sequences (the multi-row kernel; sequences behind 4096 cached tokens take 17
+    splits), drafts right up to a wrong one: the rejected rows are checked too."""
+    nt = net("llama")
+    with nt.engine(1, max_batch=8, max_seqs=10) as e:
+        rej = verify_case("verify", nt, e, [20, 60], [15, 1], [9, 0], "wgmma", batch=False)
+        rej += verify_case("verify_batch B 2", nt, e, [40, 4096], [15, 6], [3, 4], "verify")
+        rej += verify_case("verify_batch B 8", nt, e, [4096, 40, 17, 4100, 1, 300, 33, 64], [15, 3, 0, 7, 15, 1, 4, 9],
+                           [5, 1, 0, 7, 12, 0, 2, 9], "verify")
+    assert rej > 0, "no rejected row was checked"
+
+
+@gpu
+@pytest.mark.parametrize("page", [32, 64])
+def test_pass_rows_layer_1(page):
+    """A 2-layer engine whose layer 0 has WO = WDOWN = 0: layer 1's input is the embedding and the pass buffers hold layer
+    1, so its rows check the per-layer pool offsets and tensor-map rows (l * n_pages * n_kv * page) of rope_scatter, of the
+    prefill kernel (wgmma at page 32, mma.sync at 64) and of the multi-row verify kernel."""
+    nt = net("llama")
+    kern = "wgmma" if page == 32 else "mma"
+    with nt.engine(2, zero_branch0=True, max_batch=4, page_size=page) as e:
+        ids = prompt_ids(5, 33 + 300)
+        prefill_case(f"layer 1 page {page} split-k 33 + 40", nt, e, ids[33:73], ("split-k", kern), prefix=ids[:33], layer=1)
+        prefill_case(f"layer 1 page {page} tile 33 + 300", nt, e, ids[33:], ("tile", kern), prefix=ids[:33], layer=1)
+        # the multi-row kernel takes page 32 only; at page 64 a verify pass runs the prefill kernel per segment
+        verify_case(f"layer 1 page {page} verify_batch", nt, e, [300, 40], [15, 5], [6, 2], "verify" if page == 32 else "mma", layer=1)
+
+
+@gpu
+def test_pass_rows_on_prefix_cache_pages(monkeypatch):
+    """CL_PREFIX_CACHE=1: 40- and 300-token suffixes prefilled on 256 attached tokens (split-K and tile pass)."""
+    monkeypatch.setenv("CL_PREFIX_CACHE", "1")
+    nt = net("llama")
+    with nt.engine(1, max_batch=4) as e:
+        A = prompt_ids(30, 256)
+        x = e.seq_create()
+        e.prefill(x, A, want_logits=False)
+        e.seq_free(x)
+        for n, path in ((40, "split-k"), (300, "tile")):
+            Q = prompt_ids(31 + n, n)
+            s = e.seq_create()
+            assert e.attach_prefix(s, np.concatenate([A, Q])) == 256
+            lg = e.prefill(s, Q)
+            assert e.debug_pass_info()["segs"] == [(s, 0, n, 256)]
+            check_pass(f"prefix cache 256 + {n}", nt, e, Q, (path, "wgmma"), gemv_c(nt.shape["d_model"], True),
+                       logits=lg, logit_rows=[n - 1])
+            e.seq_free(s)
+
+
+@gpu
+def test_pass_accessor_refuses():
+    """No pass yet, a token-wise prefill since the last pass, a wrong selector or row range: CL_ERR_INVALID_ARG, never
+    another pass's rows.  debug_kv which 2 / 3 stop at the end of the pages the sequence holds."""
+    nt = net("tiny")
+    with nt.engine(1, max_batch=2, page_size=16) as e:
+        s = e.seq_create()
+        for call in (e.debug_pass_info, lambda: e.debug_pass_rows("h", 0, 1)):
+            with pytest.raises(eng.EngineError) as ei:
+                call()
+            assert ei.value.status == eng.CL_ERR_INVALID_ARG
+        e.prefill(s, prompt_ids(1, 40), want_logits=False)
+        assert e.debug_pass_info()["T"] == 40
+        for what, r0, n in (("h", -1, 1), ("h", 0, 41), ("act", 40, 1), ("q", 0, 0)):
+            with pytest.raises(eng.EngineError) as ei:
+                e.debug_pass_rows(what, r0, n)
+            assert ei.value.status == eng.CL_ERR_INVALID_ARG, (what, r0, n)
+        out = np.empty(nt.shape["d_model"], np.float32)
+        assert eng.lib().cl_debug_pass_rows(e._h, 4, 0, 1, eng._ptr(out)) == eng.CL_ERR_INVALID_ARG
+        assert e.debug_kv(s, 0, 2, 40, 8).shape == (8, nt.shape["n_kv_heads"] * nt.shape["head_dim"])   # 48 = 3 pages
+        for which, t0, n in ((2, 40, 9), (3, 0, 49), (1, 40, 1), (4, 0, 1)):
+            with pytest.raises(eng.EngineError) as ei:
+                e.debug_kv(s, 0, which, t0, n)
+            assert ei.value.status == eng.CL_ERR_INVALID_ARG, (which, t0, n)
+        e.prefill(s, prompt_ids(2, 3), want_logits=False)     # token-wise: decode steps, no multi-row pass
+        for call in (e.debug_pass_info, lambda: e.debug_pass_rows("h", 0, 1)):
+            with pytest.raises(eng.EngineError) as ei:
+                call()
+            assert ei.value.status == eng.CL_ERR_INVALID_ARG
 
 
 # ---- CPU: the bounds hold for an honest float32 layer and catch every mutation -------------------------------------------
@@ -547,10 +784,14 @@ def layer32(nt, l, h_in, pos, K_prev, V_prev, mutate=None):
     y = pairwise32(L["WQKV"], xn)
     if mutate == "splitk":                                  # one of four split-K partials (k 1024 .. 2047) left out of the sum
         y = y - pairwise32(L["WQKV"][:, 1024:2048], xn[1024:2048])
-    cos, sin = rope_table(s, [pos + 1 if mutate == "rope_pos" else pos])
-    c, sn = cos[0].astype(f), sin[0].astype(f)
     yh = y.reshape(-1, hd)
-    rot = np.concatenate([yh[:H + G, :half] * c - yh[:H + G, half:] * sn, yh[:H + G, half:] * c + yh[:H + G, :half] * sn], axis=1)
+
+    def rope(p):
+        cos, sin = rope_table(s, [p])
+        c, sn = cos[0].astype(f), sin[0].astype(f)
+        return np.concatenate([yh[:H + G, :half] * c - yh[:H + G, half:] * sn, yh[:H + G, half:] * c + yh[:H + G, :half] * sn], axis=1)
+
+    rot = rope({"rope_pos": pos + 1, "rope_rel": pos - ROPE_REL_POS0}.get(mutate, pos))
     q, k_new, v_new = bf16r(rot[:H].reshape(-1)), bf16r(rot[H:].reshape(-1)), bf16r(y[qd + kvd:])
     if mutate == "q_perm":                                  # the heads of the first group in another order
         q = q.reshape(H, hd)[[1, 0] + list(range(2, H))].reshape(-1)
@@ -559,12 +800,23 @@ def layer32(nt, l, h_in, pos, K_prev, V_prev, mutate=None):
     K, V = np.concatenate([K_prev, k_new[None]]).astype(f), np.concatenate([V_prev, v_new[None]]).astype(f)
     am = {"drop_current": "current", "drop_page": "page"}.get(mutate)
     Ka, Va, qp = K, V, pos
+    if mutate == "future_key":                              # the causal mask one key late: the next row (the same id) visible
+        K, V = np.concatenate([K, bf16r(rope(pos + 1)[H:].reshape(1, -1))]), np.concatenate([V, v_new[None]])
+        Ka, Va, qp = K, V, pos + 1
+    if mutate == "other_seg":                               # another segment's sequence: its K / V rows 0 .. pos
+        Ka, Va, _ = fake_cache(nt, 77, pos + 1)
     if mutate == "drop_split":                              # the split of pages 0 .. pps - 1 never reaches the combine
         pps = -(-(-(-(pos + 1) // 32)) // 16)
         Ka, Va, qp = K[pps * 32:], V[pps * 32:], pos - pps * 32
     a64, _ = attn64(q[None], Ka.reshape(-1, G, hd), Va.reshape(-1, G, hd), [qp], H, G, hd, mutate=am)
     attn = bf16r(a64[0])
-    h_mid = h_in + pairwise32(L["WO"], attn)
+    # neighbour_row: the o-projection adds another row's residual.  In a pass, a row offset off by one reads the neighbouring
+    # token's row, which in layer 0 is the same embedding whenever the two ids agree (1 in 32 for prompt_ids), and then that
+    # row cannot show the defect; the pass's other rows do.  The mutation takes id 7, which no prompt_ids id is (3 mod 16),
+    # to stand for the rows that can show it.
+    h_mid = (np.asarray(nt.embed[7], f) if mutate == "neighbour_row" else h_in) + pairwise32(L["WO"], attn)
+    if mutate == "resid_twice":                             # Y aliases resid: the residual added twice
+        h_mid = h_mid + h_in
     xn2 = norm(h_in if mutate == "stale_xn" else h_mid, L["FFN_NORM"])
     g, u = pairwise32(L["WGATE"], xn2), pairwise32(L["WUP"], xn2)
     act = bf16r(g / (f(1) + np.exp(-g)) * u)
@@ -596,36 +848,45 @@ def fake_cache(nt, seed, n):
     return bf16r(k), bf16r(v), ids
 
 
-@pytest.mark.parametrize("name,pos", [("llama", 0), ("llama", 33), ("llama", 4096), ("tinyllama", 600), ("llama32", 32), ("tiny", 31)])
+@pytest.mark.parametrize("name,pos", [("llama", 0), ("llama", 33), ("llama", 4096), ("tinyllama", 600), ("llama32", 32), ("tiny", 31),
+                                      ("llama", 4395)])
 def test_float32_layer_stays_inside_every_bound(name, pos):
-    """Rehearsal that no bound is too tight: a float32 layer with pairwise sums against the tightest constants of any path."""
+    """Rehearsal that no bound is too tight: a float32 layer with pairwise sums against the tightest constants of any path,
+    and against the tile pass's (one residual add, the prefill attention constant: the last row of 4096 + 300)."""
     nt = net(name)
     K, V, ids = fake_cache(nt, pos, pos)
     obs = stack([layer32(nt, 0, nt.embed[ids[pos]], pos, K, V)])
-    for path in ("ring", "ldg"):
-        worst = report(f"float32 {name} {path}", [f"pos {pos}"], check_layer(nt, 0, obs, consts(nt.shape, path)))
+    tile = dict(consts(nt.shape, "gemm"), h_adds=1, c_attn=PREFILL_C)
+    for path, C in (("ring", consts(nt.shape, "ring")), ("ldg", consts(nt.shape, "ldg")), ("tile", tile)):
+        worst = report(f"float32 {name} {path}", [f"pos {pos}"], check_layer(nt, 0, obs, C))
         assert max(worst.values()) > 0.01                   # and none is idle: the bf16 stages sit near half an ulp
 
 
-# mutation -> (stage that must see it, least err / bound)
+# mutation -> (stage that must see it, least err / bound); the second line: the defects of the multi-row passes
 MUTATIONS = {
     "row_dropped": ("4 h", 10), "row_twice": ("4 h", 10), "k_slice": ("4 h", 10), "stale_xn": ("3 act", 10),
     "no_gain": ("1 q", 10), "rope_pos": ("1 k", 10), "q_perm": ("1 q", 10), "v_interleave": ("1 v", 10),
     "drop_current": ("2 attn", 4), "drop_page": ("2 attn", 4), "drop_split": ("2 attn", 4), "splitk": ("1 v", 10),
+    "future_key": ("2 attn", 4), "rope_rel": ("1 k", 10), "other_seg": ("2 attn", 4), "resid_twice": ("4 h", 10),
+    "neighbour_row": ("4 h", 10),
 }
+ROPE_REL_POS0 = 4096                                       # rope_rel: RoPE at pos - pos0, as if positions restarted per chunk
 
 
 @pytest.mark.parametrize("mutate", sorted(MUTATIONS))
 def test_bounds_catch_mutation(mutate):
-    """The widest constants of any path (the GEMM's) still put each defect outside its stage's bound by the stated factor."""
+    """The widest constants of the decode paths (the GEMM's, 16 residual adds, DECODE_C) and of the multi-row passes (the
+    same with the prefill kernels' attention constant PREFILL_C, 128 x DECODE_C) still put each defect outside its stage's
+    bound by the stated factor."""
     nt = net("llama")
     pos = 4096
     K, V, ids = fake_cache(nt, 1, pos)
     obs = stack([layer32(nt, 0, nt.embed[ids[pos]], pos, K, V, mutate=mutate)])
-    res = check_layer(nt, 0, obs, consts(nt.shape, "gemm"))
     stage, least = MUTATIONS[mutate]
-    print(f"[power] {mutate}: " + "  ".join(f"{k} {v[0]:.3g}" for k, v in res.items()))
-    assert res[stage][0] >= least, (mutate, res[stage][0])
+    for name, C in (("decode", consts(nt.shape, "gemm")), ("pass", dict(consts(nt.shape, "gemm"), c_attn=PREFILL_C))):
+        res = check_layer(nt, 0, obs, C)
+        print(f"[power] {mutate} {name}: " + "  ".join(f"{k} {v[0]:.3g}" for k, v in res.items()))
+        assert res[stage][0] >= least, (mutate, name, res[stage][0])
 
 
 def test_bounds_catch_missing_eps_at_small_norm():
@@ -650,3 +911,20 @@ def test_rope_shift_is_caught_on_the_pairs_that_can_show_it():
     r = ratio(obs["k_new"], ref[:, 4096:5120], tol[:, 4096:5120]).reshape(8, 2, 64).max(axis=(0, 1))
     assert (r[:24] > 1.0).all(), r[:24]
     assert 4096 * 5e5 ** (-2 * 31 / 128) < 2.0 ** -9 * 4096
+
+
+def test_rope_at_segment_relative_position_is_caught():
+    """K roped at pos - pos0 (positions restarting at a chunk or segment): at pos 4096, pos0 4096 pair i is off by a turn of
+    4096 theta^(-2i / head_dim) rad, which moves a value by 2 |sin(turn / 2)| (|y0| + |y1|) at most.  Every pair whose turn
+    moves it by more than 2^-5 of that must exceed the bound; that is pairs 0 .. 50 at theta 5e5 save those whose turn
+    lands near a multiple of 2 pi."""
+    nt = net("llama")
+    pos = 4096
+    K, V, ids = fake_cache(nt, 1, pos)
+    obs = stack([layer32(nt, 0, nt.embed[ids[pos]], pos, K, V, mutate="rope_rel")])
+    ref, tol = stage1(nt, 0, obs["h_in"], obs["pos"], gemm_c(4096))
+    r = ratio(obs["k_new"], ref[:, 4096:5120], tol[:, 4096:5120]).reshape(8, 2, 64).max(axis=(0, 1))
+    turn = ROPE_REL_POS0 * np.float64(np.float32(5e5)) ** (-2.0 * np.arange(64) / 128)
+    shows = 2 * np.abs(np.sin(turn / 2)) > 2.0 ** -5
+    assert shows.sum() >= 40, shows.sum()
+    assert (r[shows] > 1.0).all(), np.flatnonzero(shows & (r <= 1.0))
