@@ -541,6 +541,11 @@ int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, c
   std::lock_guard<std::mutex> lk(e->impl.mu_);
   CL_GUARD(return e->impl.decode_verify_batch(seqs, n_seqs, input_ids, drafts, ks, sp, step0, ids_out, n_out, logits_out, true);)
 }
+int cl_seq_shift(cl_engine* e, cl_seq_t s, int32_t n_keep, int32_t n_discard) {
+  if (!e) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(return e->impl.seq_shift(s, n_keep, n_discard);)
+}
 int cl_seq_set_logprobs(cl_engine* e, cl_seq_t s, int32_t top_n) {
   if (!e) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
@@ -677,6 +682,23 @@ int cl_kvpool_host_cached_pages(cl_kvpool* p) {
   if (!p) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(p->mu);
   return p->pool.host_cached_pages();
+}
+int cl_kvpool_shift(cl_kvpool* p, int32_t owner, int32_t len, int32_t n_keep, int32_t n_discard, int32_t* items, int32_t cap,
+                    int32_t* n_out) {
+  if (!p || !items || !n_out) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (cap < (int32_t)p->pool.pages_of(owner).size() + 1) return CL_ERR_INVALID_ARG;
+  std::vector<KvShiftItem> it;
+  CL_GUARD(
+    const int rc = p->pool.shift(owner, len, n_keep, n_discard, &it);
+    if (rc) return rc;
+  )
+  for (size_t i = 0; i < it.size(); ++i) {
+    const int32_t row[5] = {it[i].src, it[i].dst, it[i].off0, it[i].off1, it[i].rot};
+    memcpy(items + 5 * i, row, sizeof row);
+  }
+  *n_out = (int32_t)it.size();
+  return CL_OK;
 }
 
 }  // extern "C"

@@ -186,6 +186,12 @@ int Engine::init(const cl_engine_config& c) {
   prefill_small_max_ = std::min(256, env_int("CL_PREFILL_SMALL_MAX", kDefaultPrefillSmallMax));
   device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
   prefix_cache_ = env_int("CL_PREFIX_CACHE", c.prefix_cache) != 0;
+  context_shift_ = env_int("CL_CONTEXT_SHIFT", c.context_shift) != 0;
+  num_keep_ = env_int("CL_NUM_KEEP", c.num_keep);
+  if (context_shift_ && (num_keep_ < 0 || cfg.max_seq_len - num_keep_ < 2 * page_size_)) {
+    set_last_error("num_keep must leave at least two pages of max_seq_len to shift");
+    return CL_ERR_INVALID_ARG;
+  }
   speculate_ = env_int("CL_SPECULATE", c.speculate);
   if (speculate_ < 0 || speculate_ > kSpecMaxDraft) { set_last_error("speculate must be 0..15"); return CL_ERR_INVALID_ARG; }
   if (speculate_ > 0 && !spec_path_ok()) {
@@ -321,6 +327,7 @@ int Engine::alloc_state() {
   DMALLOC(d_tok_, S * 4);
   DMALLOC(d_pos_, S * 4);
   DMALLOC(d_bt_, S * max_pages_per_seq_ * 4);
+  DMALLOC(d_shift_items_, ((size_t)max_pages_per_seq_ + 1) * sizeof(KvShiftItem));
   DMALLOC(d_slots_, (size_t)max_batch_ * 4);
   DMALLOC(d_h_, S * d * 4);
   DMALLOC(d_q_, S * q_dim_ * 4);
@@ -530,6 +537,36 @@ int Engine::attach_prefix(cl_seq_t s, const int32_t* ids, int n, int* reused) {
   q.known = r;
   q.history.assign(ids, ids + r);
   *reused = r;
+  return CL_OK;
+}
+
+// ---- context shift --------------------------------------------------------------------------------
+int Engine::seq_shift(cl_seq_t s, int n_keep, int n_discard) {
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  auto& q = seqs_[s];
+  std::vector<KvShiftItem> items;
+  const int rc = pool_->shift(s, q.len, n_keep, n_discard, &items);
+  if (rc == CL_ERR_OOM) { set_last_error("context shift: no free page for a copy of a shared page"); return rc; }
+  if (rc) { set_last_error("context shift: n_discard must be a positive multiple of page_size and n_keep + n_discard <= len"); return rc; }
+  if (const int mrc = drain_kv_moves()) return mrc;   // a copy's page may have been spilled to the host tier first
+  const auto& pages = pool_->pages_of(s);
+  if (!pages.empty())
+    CL_CUDA_OK(cudaMemcpyAsync(d_bt_ + (size_t)s * max_pages_per_seq_, pages.data(), pages.size() * 4, cudaMemcpyHostToDevice, stream_));
+  if (!items.empty()) {
+    CL_CUDA_OK(cudaMemcpyAsync(d_shift_items_, items.data(), items.size() * sizeof(KvShiftItem), cudaMemcpyHostToDevice, stream_));
+    KvShiftArgs a;
+    a.items = d_shift_items_; a.n_items = (int)items.size();
+    a.kpool = kpool_; a.vpool = vpool_; a.layer_elems = kv_layer_elems_;
+    a.n_layers = cfg.n_layers; a.n_kv = cfg.n_kv_heads; a.head_dim = cfg.head_dim; a.page_size = page_size_;
+    a.rope_row = rope_ + (size_t)n_discard * (cfg.head_dim / 2);   // n_discard < len - n_keep <= max_seq_len when a row is kept
+    int launches = 0;
+    LaunchProfiler prof(stream_, nullptr);
+    CL_LAUNCH(launch_kv_shift(a, stream_));
+    launches_ += launches;
+  }
+  q.len -= n_discard;
+  CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &q.len, 4, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaStreamSynchronize(stream_));
   return CL_OK;
 }
 

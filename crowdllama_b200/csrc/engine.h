@@ -136,6 +136,15 @@ class KvPool {
   int lookup(const int32_t* ids, int n, int* cached_pages) const;
   // Index the owner's full pages covering ids[0..n_known) not published yet.  A page whose key is already indexed stays private.
   int publish(int owner, const int32_t* ids, int n_known);
+  // Context shift of an owner holding len tokens: tokens [n_keep, n_keep + n_discard) go, n_discard a positive multiple of
+  // the page size and n_keep + n_discard <= len.  With k0 = n_keep / P and d = n_discard / P, entries k0 + 1 .. k0 + d are
+  // released (k0 .. k0 + d - 1 when n_keep % P == 0) and the row is compacted; *items get the kernel's work (kv_shift.cu):
+  // rows [n_keep % P, P) of old entry k0 + d into entry k0, and every later page holding tokens rotated in place.  A page
+  // the shift writes (entry k0 and after) that another owner holds or the index keys is first replaced by a private page
+  // (copy-on-write: its item reads the original and writes the copy, rows [0, n_keep % P) of entry k0 copied unrotated),
+  // so the index and other owners never see the shifted rows; the original keeps its entry or goes to the cache.  The owner
+  // publishes nothing more.  CL_ERR_INVALID_ARG / CL_ERR_OOM (copies need free pages) change nothing.
+  int shift(int owner, int len, int n_keep, int n_discard, std::vector<KvShiftItem>* items);
   const std::vector<int>& pages_of(int owner);
   int free_pages() const { return (int)free_.size() + (int)lru_.size(); }   // allocatable: free + cached
   int used_pages() const { return n_pages_ - free_pages(); }                // referenced by some owner
@@ -160,7 +169,8 @@ class KvPool {
   };
   struct Entry { int loc; uint64_t uid; };   // loc >= 0: device page; loc < 0: host page ~loc
   using Index = std::map<Key, Entry>;
-  struct Chain { int published = 0; uint64_t tail = kRootUid; };   // leading pages indexed (or matched), uid of the last
+  struct Chain { int published = 0; uint64_t tail = kRootUid; bool shifted = false; };   // leading pages indexed (or matched), uid of the last
+  void unref(int p);      // one owner fewer: at 0 an indexed page becomes cached, any other free
   int walk(const int32_t* ids, int n, std::vector<int>* locs) const;   // the chain's entry locations
   int take_page();        // a free page, else the device LRU front, evicted (spilled when a host page can be had)
   int take_host_page();   // a free host page, else the host LRU front, dropped; -1 when there is none
@@ -297,6 +307,12 @@ class Engine {
   // Prefix cache (CL_PREFIX_CACHE / cl_engine_config.prefix_cache): a live sequence with len 0 takes the cached pages of
   // the longest page-aligned prefix of ids[0..n), at most n - 1 tokens; len = *reused.  A no-op (0) with the cache off.
   int attach_prefix(cl_seq_t s, const int32_t* ids, int n, int* reused);
+  // Context shift (contract in include/clengine.h, cl_seq_shift): tokens [n_keep, n_keep + n_discard) leave the cache, the
+  // kept K after them is rotated to its new position (kv_shift.cu), len and the device pos drop by n_discard.
+  int seq_shift(cl_seq_t s, int n_keep, int n_discard);
+  // the request-level switch (cl_engine_config.context_shift / num_keep) and its discard rule at length len
+  bool context_shift() const { return context_shift_; }
+  int shift_discard(int len) const { return page_size_ * ((len - num_keep_) / (2 * page_size_)); }
   bool prefix_cache() const { return prefix_cache_; }
   int prefix_stats(cl_prefix_stats* out);
   // Host tier of the prefix cache (contract in include/clengine.h, cl_engine_set_prefix_host_cache); callers hold mu_
@@ -434,6 +450,7 @@ class Engine {
   bool join(Request& r, const int32_t* ids, int n, bool admission);
   void retire(Request& r, int status, const std::string& err);
   void preempt(std::shared_ptr<Request> r);
+  int shift_request(Request& r);
   int host_next_token(Request& r, float* logits, bool read_back, const int32_t* hist, int n_hist, int32_t* next);
   int spec_round(const std::shared_ptr<Request>* rs, int n);
   int generate_sync(const std::shared_ptr<Request>& r, const TokenSink* sink);
@@ -531,6 +548,9 @@ class Engine {
   int2* d_moves_ = nullptr;           // the moves of one drain (at most 2 per pool page), uploaded for the transfer kernels
   std::vector<SeqState> seqs_;
   bool prefix_cache_ = false;         // share full KV pages across sequences with the same prefix (CL_PREFIX_CACHE)
+  bool context_shift_ = false;        // requests shift their sequence instead of stopping at max_seq_len (CL_CONTEXT_SHIFT)
+  int num_keep_ = 0;                  // leading tokens a request's shift never discards (CL_NUM_KEEP)
+  KvShiftItem* d_shift_items_ = nullptr;   // one shift's work list (at most max_pages_per_seq_ + 1 items)
   std::atomic<int64_t> prefix_lookups_{0}, prefix_tokens_looked_up_{0}, prefix_tokens_reused_{0};
   std::map<int, cudaGraphExec_t> graphs_;
   std::map<int, int> graph_nodes_;

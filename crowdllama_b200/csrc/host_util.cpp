@@ -93,13 +93,56 @@ int KvPool::release(int owner) {
   auto it = owned_.find(owner);
   if (it == owned_.end()) return CL_OK;
   // deepest page first: a chain is reachable only from its root, so the LRU must evict its leaves before its root
-  for (auto rit = it->second.rbegin(); rit != it->second.rend(); ++rit) {
-    const int p = *rit;
-    if (--ref_[p] > 0) continue;
-    if (entry_[p] != index_.end()) lru_pos_[p] = lru_.insert(lru_.end(), p);
-    else free_.push_back(p);
-  }
+  for (auto rit = it->second.rbegin(); rit != it->second.rend(); ++rit) unref(*rit);
   owned_.erase(it);
+  return CL_OK;
+}
+void KvPool::unref(int p) {
+  if (--ref_[p] > 0) return;
+  if (entry_[p] != index_.end()) lru_pos_[p] = lru_.insert(lru_.end(), p);
+  else free_.push_back(p);
+}
+int KvPool::shift(int owner, int len, int n_keep, int n_discard, std::vector<KvShiftItem>* items) {
+  items->clear();
+  auto it = owned_.find(owner);
+  const int P = page_size_;
+  if (it == owned_.end() || n_keep < 0 || n_discard <= 0 || n_discard % P || (int64_t)n_keep + n_discard > len ||
+      (int64_t)it->second.size() * P < len)
+    return CL_ERR_INVALID_ARG;
+  std::vector<int>& v = it->second;
+  const int k0 = n_keep / P, r = n_keep % P, d = n_discard / P;
+  const int used = (len + P - 1) / P;                   // entries holding tokens
+  const int head = k0 + (r ? 1 : 0), tail = head + d;   // entries [head, tail) go
+  const int part_end = r ? std::min(P, len - (k0 + d) * P) : 0;   // rows [r, part_end) of entry k0 + d move to entry k0
+  auto shared = [&](int p) { return ref_[p] > 1 || entry_[p] != index_.end(); };
+  int copies = part_end > r && shared(v[k0]) ? 1 : 0;
+  for (int j = tail; j < used; ++j) copies += shared(v[j]) ? 1 : 0;
+  if (copies > free_pages()) return CL_ERR_OOM;
+  // every copy's page is taken before any page is given back: a page this shift reads must not come back as a copy
+  std::vector<int> nv(v.begin(), v.begin() + head), gone;   // gone: old entries the owner lets go of, deepest last
+  auto writable = [&](int p, int rows_kept) {
+    if (!shared(p)) return p;
+    const int q = take_page();
+    ref_[q] = 1;
+    if (rows_kept > 0) items->push_back(KvShiftItem{p, q, 0, rows_kept, 0});
+    gone.push_back(p);
+    return q;
+  };
+  if (part_end > r) {
+    nv[k0] = writable(v[k0], r);
+    items->push_back(KvShiftItem{v[k0 + d], nv[k0], r, part_end, 1});
+  }
+  for (int j = head; j < tail; ++j) gone.push_back(v[j]);
+  for (int j = tail; j < (int)v.size(); ++j) {
+    if (j >= used) { nv.push_back(v[j]); continue; }
+    const int rows = std::min(P, len - j * P);
+    const int p = writable(v[j], 0);
+    items->push_back(KvShiftItem{v[j], p, 0, rows, 1});
+    nv.push_back(p);
+  }
+  for (auto g = gone.rbegin(); g != gone.rend(); ++g) unref(*g);
+  v.swap(nv);
+  chain_[owner].shifted = true;
   return CL_OK;
 }
 int KvPool::walk(const int32_t* ids, int n, std::vector<int>* locs) const {
@@ -169,6 +212,7 @@ int KvPool::publish(int owner, const int32_t* ids, int n_known) {
   if (it == owned_.end()) return CL_OK;
   const std::vector<int>& v = it->second;
   Chain& c = chain_[owner];
+  if (c.shifted) return CL_OK;   // its pages no longer hold the K/V of their ids at their positions
   for (int k = c.published; k < (int)v.size() && (int64_t)(k + 1) * page_size_ <= n_known; ++k) {
     Key key{c.tail, std::vector<int32_t>(ids + (size_t)k * page_size_, ids + (size_t)(k + 1) * page_size_)};
     auto f = index_.find(key);

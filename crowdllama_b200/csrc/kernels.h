@@ -186,6 +186,23 @@ struct KvMoveArgs {
 };
 int launch_kv_move(bool to_host, const KvMoveArgs& a, cudaStream_t st);
 
+// Context shift (kv_shift.cu): token rows [off0, off1) of page src move to the same rows of page dst, in every layer and kv
+// head.  rot 1: K is rotated by -delta in fp32 with rope row delta, a = a c + b s, b = b c - a s for the pair (j, j + D/2),
+// and rounded to bf16; V is copied when src != dst.  rot 0: K and V are copied unchanged.  No two items write the same row
+// and no item reads a row another one writes, so an item with src == dst rotates in place.  Never launched with PDL, and the
+// kernel does not trigger its dependents early: the decode and attention kernels load KV pages before griddepcontrol.wait.
+struct KvShiftItem { int src, dst, off0, off1, rot; };
+struct KvShiftArgs {
+  const KvShiftItem* items = nullptr;  // [n_items], device memory
+  int n_items = 0;
+  __nv_bfloat16* kpool = nullptr;      // [n_layers][n_pages][n_kv][page][head_dim]
+  __nv_bfloat16* vpool = nullptr;
+  size_t layer_elems = 0;
+  int n_layers = 0, n_kv = 0, head_dim = 0, page_size = 0;
+  const float2* rope_row = nullptr;    // [head_dim / 2] device: row delta of the RoPE table, cos / sin of delta * inv_freq(i)
+};
+int launch_kv_shift(const KvShiftArgs& a, cudaStream_t st);
+
 int launch_gather_kv(const __nv_bfloat16* pool_layer, const int* block_table, int page_size, int n_kv, int head_dim, int t0, int n,
                      float* out, cudaStream_t st);
 

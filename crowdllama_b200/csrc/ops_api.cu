@@ -398,6 +398,97 @@ int cl_op_kv_host_roundtrip(int device, int32_t n_layers, int32_t n_kv, int32_t 
   return CL_OK;
 }
 
+int cl_op_kv_shift(int device, int32_t n_layers, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t len, int32_t n_keep,
+                   int32_t n_discard, const float* rope_row, const uint16_t* k, const uint16_t* v, uint16_t* k_out, uint16_t* v_out,
+                   int32_t iters, float* ms) {
+  if (n_layers <= 0 || n_kv <= 0 || len <= 0 || iters < 0 || !rope_row || !k || !v || !k_out || !v_out ||
+      (head_dim != 64 && head_dim != 128) || (page_size != 16 && page_size != 32 && page_size != 64)) {
+    set_last_error("cl_op_kv_shift: unsupported shape");
+    return CL_ERR_INVALID_ARG;
+  }
+  int rc = check_device(device);
+  if (rc) return rc;
+  // the sequence's pages (one more than its tokens need, as after a reserve for the next token) scattered among 0..2 filler
+  // pages each, seeded; every page the sequence does not hold names the largest finite bf16 (+ K, - V)
+  const int P = page_size, np = (len + P - 1) / P + 1, n_pages = 3 * np + 2;
+  KvPool pool(n_pages, P);
+  std::mt19937 rng(0x5417);
+  int fill = 0;
+  for (int i = 0; i < np; ++i) {
+    fill += (int)(rng() % 3);
+    pool.reserve(1, fill * P);
+    pool.reserve(0, (i + 1) * P);
+  }
+  const std::vector<int> before = pool.pages_of(0);
+  const size_t blk = (size_t)n_kv * P * head_dim, layer_elems = (size_t)n_pages * blk, pool_elems = (size_t)n_layers * layer_elems;
+  const size_t row = (size_t)n_kv * head_dim;
+  auto at = [&](const std::vector<int>& pages, int l, int t, int g) {
+    return (size_t)l * layer_elems + (size_t)pages[(size_t)t / P] * blk + ((size_t)g * P + t % P) * head_dim;
+  };
+  std::vector<uint16_t> kp(pool_elems, 0x7F7F), vp(pool_elems, 0xFF7F);
+  for (int l = 0; l < n_layers; ++l)
+    for (int t = 0; t < len; ++t)
+      for (int g = 0; g < n_kv; ++g) {
+        memcpy(&kp[at(before, l, t, g)], k + ((size_t)l * len + t) * row + (size_t)g * head_dim, (size_t)head_dim * 2);
+        memcpy(&vp[at(before, l, t, g)], v + ((size_t)l * len + t) * row + (size_t)g * head_dim, (size_t)head_dim * 2);
+      }
+  std::vector<KvShiftItem> items;
+  if ((rc = pool.shift(0, len, n_keep, n_discard, &items))) {
+    set_last_error("cl_op_kv_shift: n_discard must be a positive multiple of page_size and n_keep + n_discard <= len");
+    return rc;
+  }
+  const std::vector<int> after = pool.pages_of(0);
+  DevBuf dk, dv, di, dr;
+  CL_CUDA_OK(dk.upload(kp.data(), pool_elems * 2));
+  CL_CUDA_OK(dv.upload(vp.data(), pool_elems * 2));
+  CL_CUDA_OK(di.upload(items.data(), items.size() * sizeof(KvShiftItem)));
+  CL_CUDA_OK(dr.upload(rope_row, (size_t)head_dim / 2 * sizeof(float2)));
+  KvShiftArgs a;
+  a.items = di.as<KvShiftItem>(); a.n_items = (int)items.size();
+  a.kpool = dk.as<__nv_bfloat16>(); a.vpool = dv.as<__nv_bfloat16>(); a.layer_elems = layer_elems;
+  a.n_layers = n_layers; a.n_kv = n_kv; a.head_dim = head_dim; a.page_size = P; a.rope_row = dr.as<float2>();
+  if (launch_kv_shift(a, nullptr) < 0) {
+    CL_CUDA_OK(cudaGetLastError());
+    return CL_ERR_CUDA;
+  }
+  CL_CUDA_OK(cudaDeviceSynchronize());
+  std::vector<uint16_t> k2(pool_elems), v2(pool_elems);
+  CL_CUDA_OK(cudaMemcpy(k2.data(), dk.p, pool_elems * 2, cudaMemcpyDeviceToHost));
+  CL_CUDA_OK(cudaMemcpy(v2.data(), dv.p, pool_elems * 2, cudaMemcpyDeviceToHost));
+  // the sequence's rows out, then zeroed on both sides: everything else must be the bytes it was
+  const int len2 = len - n_discard;
+  for (int l = 0; l < n_layers; ++l)
+    for (int t = 0; t < len2; ++t)
+      for (int g = 0; g < n_kv; ++g) {
+        const size_t e = at(after, l, t, g), o = ((size_t)l * len2 + t) * row + (size_t)g * head_dim;
+        memcpy(k_out + o, &k2[e], (size_t)head_dim * 2);
+        memcpy(v_out + o, &v2[e], (size_t)head_dim * 2);
+        std::fill_n(&k2[e], head_dim, 0); std::fill_n(&v2[e], head_dim, 0);
+        std::fill_n(&kp[e], head_dim, 0); std::fill_n(&vp[e], head_dim, 0);
+      }
+  if (k2 != kp || v2 != vp) {
+    set_last_error("cl_op_kv_shift: an element outside the sequence's rows changed");
+    return CL_ERR_INTERNAL;
+  }
+  if (iters > 0 && ms && !items.empty()) {
+    cudaEvent_t e0, e1;
+    CL_CUDA_OK(cudaEventCreate(&e0));
+    CL_CUDA_OK(cudaEventCreate(&e1));
+    launch_kv_shift(a, nullptr);   // warm-up
+    CL_CUDA_OK(cudaEventRecord(e0, nullptr));
+    for (int i = 0; i < iters; ++i) launch_kv_shift(a, nullptr);
+    CL_CUDA_OK(cudaEventRecord(e1, nullptr));
+    CL_CUDA_OK(cudaEventSynchronize(e1));
+    CL_CUDA_OK(cudaGetLastError());
+    float t = 0.f;
+    CL_CUDA_OK(cudaEventElapsedTime(&t, e0, e1));
+    *ms = t / (float)iters;
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+  }
+  return CL_OK;
+}
+
 int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, const uint16_t* v_cache, const int32_t* ctx_lens,
                       const int32_t* rows, int32_t n_segs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit,
                       uint16_t* out, int32_t* nsplit_used) {

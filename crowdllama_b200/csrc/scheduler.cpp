@@ -46,12 +46,17 @@ struct Request {
   std::vector<LogprobRecord> pub_lps;   // streaming: the records of `pub` (guarded by m)
   bool lp_mismatch = false;         // an id joined without its own record: the request fails with CL_ERR_INTERNAL
   int spec_backoff = 0;             // tokens to decode without drafting (after a verify pass that accepted nothing)
+  bool ctx_shift = false;           // cl_engine_config.context_shift: the sequence shifts instead of ending at max_seq_len
+  int keep = 0;                     // ... keeping its first `keep` ids
+  int shifted = 0;                  // ids after the first `keep` that shifts have discarded so far
   bool greedy() const { return sp.temperature <= 0.f; }
   bool device_next() const { return greedy() || dev_sample; }   // the next id is d_tok_ after the step: no host sampler
-  // prompt + out into `full`, reusing its storage: what an admission (re-)prefills, and the history a draft comes from
+  // prompt + out into `full`, reusing its storage: what an admission (re-)prefills, and the history a draft comes from.
+  // After context shifts, the window the sequence holds: the first `keep` ids, then those after the discarded ones.
   const std::vector<int32_t>& sync_full() {
     full.assign(prompt.begin(), prompt.end());
     full.insert(full.end(), out.begin(), out.end());
+    if (shifted) full.erase(full.begin() + keep, full.begin() + keep + shifted);
     return full;
   }
 };
@@ -77,7 +82,7 @@ static bool finished(Request& r, const Tokenizer& tok, int max_seq_len) {
   if (r.cancel.load(std::memory_order_relaxed)) { r.done_reason = "cancelled"; return true; }
   if (!r.out.empty() && !r.sp.ignore_eos && tok.is_stop(r.out.back())) { r.done_reason = "stop"; return true; }
   if ((int)r.out.size() >= r.max_new) { r.done_reason = "length"; return true; }
-  if ((int)(r.prompt.size() + r.out.size()) >= max_seq_len) { r.done_reason = "length"; return true; }
+  if (!r.ctx_shift && (int)(r.prompt.size() + r.out.size()) >= max_seq_len) { r.done_reason = "length"; return true; }
   return false;
 }
 
@@ -147,14 +152,24 @@ int Engine::admission_pages(Request& r, int* hit) {
   return ((int)full.size() + 1 + page_size_ - 1) / page_size_ - *hit / page_size_ + cached;
 }
 
-// Preempt: r gives its pages back and waits at the queue's head; its next admission recomputes prompt + out.
+// Preempt: r gives its pages back and waits at the queue's head; its next admission recomputes prompt + out (its window,
+// after context shifts).  A window that would leave no position for the next token is shifted first, on the host only.
 void Engine::preempt(std::shared_ptr<Request> r) {
+  if (r->ctx_shift && (int)r->sync_full().size() >= cfg.max_seq_len) r->shifted += shift_discard(cfg.max_seq_len);
   seq_free(r->seq);
   r->seq = -1;
   r->n_preempted++;
   preemptions_++;
   std::lock_guard<std::mutex> lk(q_mu_);
   queue_.push_front(std::move(r));
+}
+
+// Context shift of a running request whose sequence holds max_seq_len tokens: the discard rule of cl_engine_config.context_shift
+int Engine::shift_request(Request& r) {
+  const int d = shift_discard(seqs_[r.seq].len);
+  const int rc = seq_shift(r.seq, num_keep_, d);
+  if (rc == CL_OK) r.shifted += d;
+  return rc;
 }
 
 // Host next token: sample_token over the logits of r's slot (read back first with read_back, else already in `logits`), with
@@ -264,12 +279,14 @@ int Engine::generate_sync(const std::shared_ptr<Request>& rp, const TokenSink* s
   join(r, &next, 1, true);
   emit();
   while (!finished(r, *tok, cfg.max_seq_len)) {
+    if (r.ctx_shift && seqs_[r.seq].len >= cfg.max_seq_len && (rc = shift_request(r))) break;
     const int spec = spec_round(&rp, 1);
     if (spec < 0) { rc = spec; break; }
     if (spec > 0) {
       next = r.out.back();
     } else if (r.device_next()) {   // greedy or device-sampled: the token loop stays on the device
-      int room = std::min(r.max_new - (int)r.out.size(), cfg.max_seq_len - (int)(r.prompt.size() + r.out.size()));
+      const int window = r.ctx_shift ? cfg.max_seq_len - seqs_[r.seq].len : cfg.max_seq_len - (int)(r.prompt.size() + r.out.size());
+      int room = std::min(r.max_new - (int)r.out.size(), window);
       int chunk = std::min(room, sink ? 8 : 32);
       // speculating: back to drafting after the back-off, or after one step when the history had no match
       if (speculate_ > 0) chunk = std::min(chunk, std::max(1, r.spec_backoff));
@@ -299,14 +316,23 @@ int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling&
     set_last_error("logprobs: top_n must be -1..20 and the vocabulary at most 163840");
     return CL_ERR_INVALID_ARG;
   }
-  if (n_prompt >= cfg.max_seq_len) { set_last_error("prompt longer than max_seq_len"); return CL_ERR_TOO_LONG; }
+  if (n_prompt >= cfg.max_seq_len && !context_shift_) { set_last_error("prompt longer than max_seq_len"); return CL_ERR_TOO_LONG; }
   for (int i = 0; i < n_prompt; ++i)
     if (prompt[i] < 0 || prompt[i] >= cfg.vocab_size) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
   auto r = std::make_shared<Request>();
-  r->prompt.assign(prompt, prompt + n_prompt);
+  r->ctx_shift = context_shift_;
+  r->keep = num_keep_;
+  if (n_prompt >= cfg.max_seq_len) {   // context shift: the first num_keep ids and the tail, one position left to generate
+    r->prompt.assign(prompt, prompt + num_keep_);
+    r->prompt.insert(r->prompt.end(), prompt + n_prompt - (cfg.max_seq_len - 1 - num_keep_), prompt + n_prompt);
+    n_prompt = (int)r->prompt.size();
+  } else {
+    r->prompt.assign(prompt, prompt + n_prompt);
+  }
   r->sp = sp;
   r->max_new = sp.max_new_tokens > 0 ? sp.max_new_tokens : cfg.max_seq_len - n_prompt;
-  r->max_new = std::min(r->max_new, cfg.max_seq_len - n_prompt);
+  // num_predict <= 0 stays bounded by the window even with context shift: an unbounded request would hold a slot forever
+  if (!r->ctx_shift || sp.max_new_tokens <= 0) r->max_new = std::min(r->max_new, cfg.max_seq_len - n_prompt);
   r->t_arrive = now_ns();
   r->sync = !sched_started_;
   r->streaming = !r->sync && sink && sink->fn;   // the synchronous path calls the sink itself
@@ -573,11 +599,14 @@ void Engine::admitted(const std::shared_ptr<Request>& r, int32_t next) {
   else active_.push_back(r);
 }
 
-// Makes room for one more token per running request.  On an empty pool the youngest request is preempted: the one still
-// being admitted, else the running request that arrived last.  A request the pool cannot serve even alone fails.
+// Makes room for one more token per running request, first shifting a request whose sequence fills max_seq_len (context
+// shift).  On an empty pool the youngest request is preempted: the one still being admitted, else the running request that
+// arrived last.  A request the pool cannot serve even alone fails.
 void Engine::make_room() {
   for (size_t i = 0; i < active_.size();) {
-    const int rc = ensure_capacity(active_[i]->seq, seqs_[active_[i]->seq].len + 1);
+    Request& r = *active_[i];
+    int rc = r.ctx_shift && seqs_[r.seq].len >= cfg.max_seq_len ? shift_request(r) : CL_OK;
+    if (rc == CL_OK) rc = ensure_capacity(r.seq, seqs_[r.seq].len + 1);
     if (rc == CL_ERR_OOM && prefilling_) {
       preempt(prefilling_);
       prefilling_.reset();

@@ -39,7 +39,7 @@ class EngineConfig(C.Structure):
                 ("kv_pool_bytes", C.c_int64), ("page_size", C.c_int32), ("max_batch", C.c_int32),
                 ("max_seqs", C.c_int32), ("use_cuda_graph", C.c_int32), ("decode_path", C.c_int32),
                 ("start_scheduler", C.c_int32), ("prefix_cache", C.c_int32), ("speculate", C.c_int32),
-                ("reserved", C.c_int32 * 6)]
+                ("reserved", C.c_int32 * 6)]   # reserved[0], [1]: the C struct's context_shift, num_keep
 
 
 class Sampling(C.Structure):
@@ -96,7 +96,7 @@ EXPORTS = [
     "cl_op_attn_prefill_cached", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages", "cl_kvpool_set_host_pages", "cl_kvpool_take_moves",
-    "cl_kvpool_host_cached_pages", "cl_seq_set_logprobs", "cl_seq_take_logprobs", "cl_generate_ids_logprobs", "cl_op_sample_logprobs",
+    "cl_kvpool_host_cached_pages", "cl_kvpool_shift", "cl_seq_shift", "cl_op_kv_shift", "cl_seq_set_logprobs", "cl_seq_take_logprobs", "cl_generate_ids_logprobs", "cl_op_sample_logprobs",
     "cl_tokenizer_load", "cl_tokenizer_free", "cl_tokenizer_encode", "cl_tokenizer_decode", "cl_tokenizer_info", "cl_engine_load_tokenizer",
 ]
 
@@ -186,6 +186,9 @@ def lib():
         "cl_op_sample": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), vp, vp, i32, vp, vp]),
         "cl_op_sample_logprobs": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), vp, vp, i32, vp, i32, vp, vp]),
         "cl_seq_set_logprobs": (C.c_int, [vp, i32, i32]),
+        "cl_seq_shift": (C.c_int, [vp, i32, i32, i32]),
+        "cl_kvpool_shift": (C.c_int, [vp, i32, i32, i32, i32, vp, i32, P(i32)]),
+        "cl_op_kv_shift": (C.c_int, [C.c_int, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i32, P(f32)]),
         "cl_seq_take_logprobs": (C.c_int, [vp, i32, vp, i32, P(i32)]),
         "cl_generate_ids_logprobs": (C.c_int, [vp, vp, i32, P(Sampling), i32, P(Result), P(vp)]),
         "cl_op_synth_weights": (C.c_int, [C.c_int, u64, i32, i64, f32, vp]),
@@ -313,7 +316,8 @@ class Engine:
                  device: int = 0, seed: int = 1234, max_batch: int = 8, max_seqs: int | None = None,
                  page_size: int = 32, kv_pool_bytes: int = 0, use_cuda_graph: bool = True, decode_path: int = 0,
                  start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False,
-                 speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0):
+                 speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
+                 num_keep: int = 4):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -337,6 +341,8 @@ class Engine:
         cfg.start_scheduler = 1 if start_scheduler else 0
         cfg.prefix_cache = 1 if prefix_cache else 0     # env CL_PREFIX_CACHE=0|1 overrides
         cfg.speculate = speculate                       # 0 off, 1..15 drafted tokens per verify pass; env CL_SPECULATE overrides
+        cfg.reserved[0] = 1 if context_shift else 0     # cl_engine_config.context_shift; env CL_CONTEXT_SHIFT=0|1 overrides
+        cfg.reserved[1] = num_keep                      # cl_engine_config.num_keep (Ollama's documented default 4); env CL_NUM_KEEP overrides
         h = C.c_void_p()
         _check(L.cl_engine_create(C.byref(cfg), C.byref(h)), "cl_engine_create")
         self._h = h
@@ -406,6 +412,11 @@ class Engine:
         n = C.c_int32(0)
         _check(lib().cl_seq_attach_prefix(self._h, s, _ptr(ids), len(ids), C.byref(n)), "cl_seq_attach_prefix")
         return n.value
+
+    def seq_shift(self, s: int, n_keep: int, n_discard: int):
+        """cl_seq_shift: cached tokens [n_keep, n_keep + n_discard) leave the sequence (n_discard a multiple of page_size); the
+        kept K after them is rotated to its new position, len drops by n_discard."""
+        _check(lib().cl_seq_shift(self._h, s, n_keep, n_discard), "cl_seq_shift")
 
     def prefill(self, s: int, ids, want_logits: bool = True):
         ids = np.ascontiguousarray(ids, dtype=np.int32)
@@ -929,6 +940,23 @@ def op_kv_host_roundtrip(n_layers, n_kv, head_dim, page_size, n_moves, iters=0, 
     return (ms[0], ms[1]) if iters else None
 
 
+def op_kv_shift(k, v, page_size, n_keep, n_discard, rope_row, iters=0, device=0):
+    """cl_op_kv_shift: k, v uint16 (bf16) [n_layers][len][n_kv][head_dim] paged into a scattered pool, shifted by one
+    kv_shift_kernel launch with rope_row [head_dim / 2][2] (cos, sin); raises if anything outside the sequence's rows changed.
+    Returns (k_out, v_out) [n_layers][len - n_discard][n_kv][head_dim], and the ms of one launch over `iters` timed launches
+    (None when iters is 0)."""
+    k = np.ascontiguousarray(k, dtype=np.uint16)
+    v = np.ascontiguousarray(v, dtype=np.uint16)
+    L, T, KV, D = k.shape
+    cs = np.ascontiguousarray(rope_row, dtype=np.float32)
+    ko = np.zeros((L, max(T - n_discard, 0), KV, D), np.uint16)
+    vo = np.zeros_like(ko)
+    ms = C.c_float(0.0)
+    _check(lib().cl_op_kv_shift(device, L, KV, D, page_size, T, n_keep, n_discard, _ptr(cs), _ptr(k), _ptr(v), _ptr(ko), _ptr(vo),
+                                iters, C.byref(ms) if iters else None), "cl_op_kv_shift")
+    return ko, vo, (ms.value if iters else None)
+
+
 def op_synth_weights(seed, key, n, scale, device=0):
     out = np.empty(n, np.uint16)
     _check(lib().cl_op_synth_weights(device, seed, key, n, scale, _ptr(out)), "cl_op_synth_weights")
@@ -1047,3 +1075,12 @@ class KvPool:
     @property
     def host_cached_pages(self) -> int:
         return lib().cl_kvpool_host_cached_pages(self._h)
+
+    def shift(self, owner: int, length: int, n_keep: int, n_discard: int):
+        """Context shift of an owner holding `length` tokens (cl_kvpool_shift): returns (status, work items as a list of
+        (source page, destination page, first row, end row, rotate))."""
+        cap = len(self.pages_of(owner)) + 1
+        a = np.zeros((cap, 5), np.int32)
+        n = C.c_int32(0)
+        rc = lib().cl_kvpool_shift(self._h, owner, length, n_keep, n_discard, _ptr(a), cap, C.byref(n))
+        return rc, [tuple(int(x) for x in r) for r in a[:n.value]] if rc == 0 else []

@@ -74,10 +74,11 @@ class _Conn(socketserver.BaseRequestHandler):
 
 def serve(device: int, port: int, preset: str, model_name: str, max_batch: int = 8, greedy_tokens: int = 0, host="127.0.0.1",
           ready_event=None, seed: int = 1234, tokenizer: str | None = None, chat_family: str | None = None, prefix_cache: bool = False,
-          speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0):
+          speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
+          num_keep: int = 4):
     e = eng.Engine(preset=preset, model_name=model_name, device=device, seed=seed, max_batch=max_batch, start_scheduler=True,
                    prefix_cache=prefix_cache, speculate=speculate, speculate_batch=speculate_batch,
-                   prefix_cache_host_bytes=prefix_cache_host_bytes)
+                   prefix_cache_host_bytes=prefix_cache_host_bytes, context_shift=context_shift, num_keep=num_keep)
     if tokenizer:
         e.load_tokenizer(tokenizer, chat_family)      # HF tokenizer.json instead of the byte-level fallback
     sampling = eng.greedy(greedy_tokens, ignore_eos=True) if greedy_tokens > 0 else None   # None = Ollama defaults
@@ -112,13 +113,21 @@ def main():
     ap.add_argument("--prefix-cache-host-gib", type=float, default=0.0,
                     help="with --prefix-cache: GiB of pinned host memory that keeps evicted cached KV pages for reuse "
                          "(0 = off; env CL_PREFIX_CACHE_HOST_MIB overrides)")
+    ap.add_argument("--context-shift", action="store_true",
+                    help="a request that fills the context window discards half of its tokens after the first --num-keep and goes "
+                         "on generating, instead of ending with done_reason \"length\" (env CL_CONTEXT_SHIFT overrides)")
+    ap.add_argument("--num-keep", type=int, default=None,
+                    help="with --context-shift: leading tokens a shift never discards (default 4; env CL_NUM_KEEP overrides)")
     a = ap.parse_args()
     if a.prefix_cache_host_gib and not a.prefix_cache:
         ap.error("--prefix-cache-host-gib requires --prefix-cache")
+    if a.num_keep is not None and not a.context_shift:
+        ap.error("--num-keep requires --context-shift")
     print(f"worker on cuda:{a.device} port {a.port} serving {a.model_name}", flush=True)
     serve(a.device, a.port, a.preset, a.model_name, a.max_batch, a.greedy_tokens, tokenizer=a.tokenizer, chat_family=a.chat_family,
           prefix_cache=a.prefix_cache, speculate=a.speculate, speculate_batch=a.speculate_batch,
-          prefix_cache_host_bytes=int(a.prefix_cache_host_gib * 2**30))
+          prefix_cache_host_bytes=int(a.prefix_cache_host_gib * 2**30), context_shift=a.context_shift,
+          num_keep=4 if a.num_keep is None else a.num_keep)
 
 
 if __name__ == "__main__":

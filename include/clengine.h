@@ -105,7 +105,33 @@ typedef struct cl_engine_config {
                               prompt and output (cl_draft_ngram) and checks them in one pass over the weights
                               (cl_decode_verify).  The ids are the ones single steps would produce, up to near-tie flips
                               between the two kernel paths.  Model shapes without the verify path decode normally. */
-  int32_t reserved[6];
+  int32_t context_shift;   /* 1 => a request whose sequence fills max_seq_len shifts it (cl_seq_shift) and goes on generating
+                              instead of ending with done_reason "length"; 0 => off (default; env CL_CONTEXT_SHIFT=0|1
+                              overrides).  Ollama's rule, as its documentation states it (its source cannot be checked
+                              here, like the sampler order and the templates): keep the first num_keep tokens and discard
+                              half of the rest.  Here the half is rounded down to whole KV pages: before a decode step or a
+                              verify pass would write position max_seq_len, the request's sequence discards
+                                  delta = page_size * floor((max_seq_len - num_keep) / (2 * page_size))
+                              tokens after its first num_keep.  With the switch on:
+                              - num_predict > 0 may exceed max_seq_len - n_prompt.  num_predict <= 0 keeps its meaning,
+                                "until EOS or max_seq_len - n_prompt tokens", on purpose: an unbounded request would hold
+                                a slot of a shared worker forever.
+                              - A prompt of max_seq_len tokens or more keeps its first num_keep ids and its last
+                                max_seq_len - 1 - num_keep ids instead of failing with CL_ERR_TOO_LONG; cl_result.n_prompt
+                                counts what was prefilled.
+                              - A shifted request that is preempted comes back by prefilling its current window (first
+                                num_keep ids, then the ids after the discarded ones).  Those K/V are computed without the
+                                discarded context in view, so they differ from the shifted cache they replace.
+                              - Speculative rounds still draft only up to max_seq_len; the shift runs before the next round.
+                              The device loops (cl_decode_greedy*, cl_decode_sample_batch) never shift. */
+  int32_t num_keep;        /* leading tokens a context shift never discards (env CL_NUM_KEEP overrides).
+                              cl_default_engine_config leaves it 0, like the reserved ints it came from; the Python Engine
+                              and worker.py pass 4, Ollama's documented default.  A C caller that turns context_shift on
+                              should set num_keep too (4 to match Ollama): with 0, the first shift discards the BOS token
+                              and the start of the prompt.  With context_shift on, cl_engine_create
+                              fails with CL_ERR_INVALID_ARG unless 0 <= num_keep <= max_seq_len - 2 * page_size (a
+                              shift must discard at least one page). */
+  int32_t reserved[4];
 } cl_engine_config;
 
 /* Sampler.  The reference sends no options (api.go:109-118), so Ollama defaults apply upstream:
@@ -363,6 +389,22 @@ int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, c
                            const int32_t* ks, const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int32_t* n_out,
                            float* logits_out);
 
+/* Context shift, token level: the cached tokens [n_keep, n_keep + n_discard) of the sequence leave its cache.  Afterwards:
+ *   - position p < n_keep holds exactly what it held;
+ *   - position p >= n_keep holds what position p + n_discard held: V bit-identical, K = bf16(R(-n_discard) K_old), rotated
+ *     in fp32 (a c + b s, b c - a s, each product and sum rounded, for the pair of dims j and j + head_dim/2) with row
+ *     n_discard of the engine's own cos/sin table, the one prefill and decode use ("llama3" scaling included);
+ *   - len and the slot's device position drop by n_discard.  The next input id, the id history, an armed sampler's RNG step
+ *     and penalty window, and logprobs are unchanged.
+ * The kept K/V were computed with the discarded tokens in view: they are not what a prefill of the kept ids would give.
+ * Pages the shift writes that another sequence or the prefix cache holds are copied first (copy-on-write), so neither ever
+ * sees a shifted row; the sequence publishes no page to the prefix cache afterwards.  Works whatever
+ * cl_engine_config.context_shift is.  CL_ERR_INVALID_ARG unless n_discard is a positive multiple of page_size and
+ * 0 <= n_keep, n_keep + n_discard <= len; CL_ERR_OOM when a copy-on-write finds no free page.  On these errors nothing
+ * changes.  CL_ERR_CUDA (a failed copy or launch after the page list was rewritten) leaves the sequence's pages and K/V
+ * undefined, like any CUDA failure: free the sequence. */
+int cl_seq_shift(cl_engine* e, cl_seq_t seq, int32_t n_keep, int32_t n_discard);
+
 /* ---- per-token log-probabilities (Ollama's `logprobs` / `top_logprobs`) -----------------------------------------------
  * What is computed: the natural-log log_softmax of the logits row the step tail chose the id from, taken over the raw fp32
  * logits, i.e. BEFORE the repeat penalty, temperature, top-k and top-p: the model's distribution, whatever the sampler
@@ -501,6 +543,16 @@ int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, co
  * mean over iters launches of each.  head_dim 64 or 128, page_size 16, 32 or 64. */
 int cl_op_kv_host_roundtrip(int device, int32_t n_layers, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t n_moves,
                             int32_t iters, float* ms);
+/* The context shift's kernel (kv_shift_kernel, cl_seq_shift): k, v [n_layers][len][n_kv][head_dim] bf16 are the rows of a
+ * sequence paged into a scattered pool whose other pages hold the largest finite bf16 (+ K, - V).  The allocator's shift
+ * (cl_kvpool_shift, no page shared) plans the work and one launch runs it with rope_row [head_dim / 2][2] (cos, sin) as
+ * row n_discard of the RoPE table.  k_out, v_out [n_layers][len - n_discard][n_kv][head_dim] = the sequence's rows
+ * afterwards.  CL_ERR_INTERNAL if any element of the pool outside those rows changed.  iters > 0: *ms = CUDA-event time of
+ * one launch, the mean over iters more launches of the same work (rotating again).  head_dim 64 or 128, page_size 16, 32 or
+ * 64; the cl_seq_shift argument rules otherwise (CL_ERR_INVALID_ARG). */
+int cl_op_kv_shift(int device, int32_t n_layers, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t len, int32_t n_keep,
+                   int32_t n_discard, const float* rope_row, const uint16_t* k, const uint16_t* v, uint16_t* k_out, uint16_t* v_out,
+                   int32_t iters, float* ms);
 /* prefill GEMM on the tensor cores (wgmma): Y[t][n] = sum_k X[t][k] W[n][k]; X,W bf16, Y fp32 */
 int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, int32_t t,
                     int32_t n, int32_t k, int32_t iters, float* ms);
@@ -583,6 +635,18 @@ int cl_kvpool_cached_pages(cl_kvpool* p);
 int cl_kvpool_set_host_pages(cl_kvpool* p, int32_t n);
 int cl_kvpool_take_moves(cl_kvpool* p, int32_t* moves, int32_t cap, int32_t* n_out);
 int cl_kvpool_host_cached_pages(cl_kvpool* p);
+/* Context shift (what cl_seq_shift runs on): `owner` holds len tokens; tokens [n_keep, n_keep + n_discard) go.  With
+ * P = page_size, k0 = n_keep / P and d = n_discard / P, entries k0 + 1 .. k0 + d of the owner's page list are released
+ * (k0 .. k0 + d - 1 when n_keep % P == 0) and the list is compacted.  The pages the shift writes are the new entry k0 and
+ * every later one holding tokens; each that another owner holds or the index keys is first replaced by a fresh page
+ * (copy-on-write) and the original keeps its index entry or becomes cached.  The owner publishes nothing afterwards.
+ * items (cap >= the owner's page count + 1, else CL_ERR_INVALID_ARG before anything changes) receive the kernel's work as
+ * [n][5] (source page, destination page, first row, end row, rotate): rotate 1 moves rows [first, end) with K rotated by
+ * -n_discard and V copied unless source == destination; rotate 0 copies K and V unchanged (rows [0, n_keep % P) of a
+ * copied entry k0).  *n_out = n.  CL_ERR_INVALID_ARG for the cl_seq_shift argument rules or a list covering fewer than len
+ * tokens; CL_ERR_OOM when the copies find no page (free or cached).  On an error nothing changes. */
+int cl_kvpool_shift(cl_kvpool* p, int32_t owner, int32_t len, int32_t n_keep, int32_t n_discard, int32_t* items, int32_t cap,
+                    int32_t* n_out);
 
 #ifdef __cplusplus
 }
