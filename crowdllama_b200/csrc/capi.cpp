@@ -59,6 +59,15 @@ int cl_sample_token(const float* logits, int32_t vocab, const cl_sampling* s, co
   return CL_OK;
 }
 
+int cl_sample_token_ext(const float* logits, int32_t vocab, const cl_sampling* s, const cl_sampling_ext* ext, const int32_t* history,
+                        int32_t n_history, uint64_t step, int32_t* id) {
+  if (!logits || vocab <= 0 || !s || !id || n_history < 0 || (n_history > 0 && !history)) return CL_ERR_INVALID_ARG;
+  SamplerExt x;
+  if (int rc = read_sampling_ext(ext, &x, nullptr)) return rc;
+  *id = cl::sample_token(logits, vocab, *s, history, n_history, step, x);
+  return CL_OK;
+}
+
 int cl_draft_ngram(const int32_t* hist, int32_t n, int32_t k, int32_t* out, int32_t* n_out) {
   if (!out || !n_out || n < 0 || (n > 0 && !hist) || k < 1 || k > kSpecMaxDraft) return CL_ERR_INVALID_ARG;
   *n_out = cl::ngram_draft(hist, n, k, out);
@@ -172,21 +181,27 @@ int cl_generate_ids_logprobs(cl_engine* e, const int32_t* prompt_ids, int32_t n_
 }
 
 namespace {
-// incremental detokeniser: emits only text that later tokens cannot change (an incomplete UTF-8 tail is held back)
+// incremental detokeniser: emits only text that later tokens cannot change.  Held back: whatever could still begin one of
+// the stop strings (StopScan::safe), and an incomplete UTF-8 sequence before that; the text ends at a stop match.
 struct StreamText {
   const Tokenizer* tok;
+  StopScan stop;
   std::vector<int32_t> ids;
   size_t emitted = 0;       // bytes of sanitised text already handed out
   std::string feed(const int32_t* fresh, int n, bool final) {
     ids.insert(ids.end(), fresh, fresh + n);
+    if (stop.active())
+      for (int i = 0; i < n; ++i) stop.feed_id(*tok, fresh[i]);
     std::string raw = tok->decode_bytes(ids);
     size_t cut = raw.size();
+    if (stop.active() && (!final || stop.match() >= 0)) cut = (size_t)stop.safe();
     if (!final) {
-      for (size_t back = 1; back <= 3 && back <= raw.size(); ++back) {
-        const unsigned char c = (unsigned char)raw[raw.size() - back];
+      const size_t end = cut;
+      for (size_t back = 1; back <= 3 && back <= end; ++back) {
+        const unsigned char c = (unsigned char)raw[end - back];
         if ((c >> 6) == 2) continue;                                   // continuation byte: keep looking for the lead
         const size_t need = (c >> 5) == 6 ? 2 : (c >> 4) == 14 ? 3 : (c >> 3) == 30 ? 4 : 1;
-        if (need > back) cut = raw.size() - back;                      // lead byte of a sequence that is still open
+        if (need > back) cut = end - back;                             // lead byte of a sequence that is still open
         break;
       }
     }
@@ -286,11 +301,31 @@ int cl_generate_stream(cl_engine* e, const char* model, const char* prompt, size
     std::vector<int32_t> ids = prompt_ids(e, prompt, prompt_len, false);
     cl_sampling sp;
     if (s) sp = *s; else cl_default_sampling(&sp);
-    TextSinkCtx ctx{StreamText{e->impl.tok.get(), {}, 0}, cb, user};
+    TextSinkCtx ctx{StreamText{e->impl.tok.get(), StopScan(), {}, 0}, cb, user};
     Engine::TokenSink sink{text_sink, &ctx};
     const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, out, &sink);
     if (rc) return rc;
     const std::string tail = ctx.st.feed(nullptr, 0, true);   // whatever the UTF-8 hold-back kept
+    if (!tail.empty()) cb(user, tail.data(), tail.size(), nullptr, 0);
+    return CL_OK;
+  )
+}
+
+int cl_generate_ids_ext(cl_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const cl_sampling* s, const cl_sampling_ext* ext,
+                        int32_t top_n, cl_token_cb cb, void* user, cl_result* out, cl_token_logprob** lps) {
+  if (!e || !out || top_n < -1 || top_n > CL_MAX_TOP_LOGPROBS || (top_n >= 0 && !lps)) return CL_ERR_INVALID_ARG;
+  if (lps) *lps = nullptr;
+  cl_sampling sp;
+  if (s) sp = *s; else cl_default_sampling(&sp);
+  CL_GUARD(
+    SamplerExt x;
+    std::vector<std::string> stop;
+    if (int rc = read_sampling_ext(ext, &x, &stop)) return rc;
+    TextSinkCtx ctx{StreamText{e->impl.tok.get(), StopScan(stop), {}, 0}, cb, user};
+    Engine::TokenSink sink{text_sink, &ctx};
+    const int rc = e->impl.generate_ids(prompt_ids, n_prompt, sp, out, cb ? &sink : nullptr, top_n, top_n >= 0 ? lps : nullptr, &x, &stop);
+    if (rc || !cb) return rc;
+    const std::string tail = ctx.st.feed(nullptr, 0, true);   // what the UTF-8 and stop hold-backs kept
     if (!tail.empty()) cb(user, tail.data(), tail.size(), nullptr, 0);
     return CL_OK;
   )
@@ -314,7 +349,10 @@ static int handle_message_impl(cl_engine* e, const uint8_t* req, size_t req_len,
   if (int rc = check_model(e, gr.model.c_str())) return rc;
   cl_sampling sp;
   if (s) sp = *s; else cl_default_sampling(&sp);
-  apply_options(gr.opt, &sp);                                   // request options win over the worker's defaults
+  SamplerExt ext;
+  apply_options(gr.opt, &sp, &ext);                             // request options win over the worker's defaults
+  std::vector<std::string> stop = gr.opt.stop;
+  if (int rc = check_sampling_ext(ext, &stop)) return rc;
   // logprobs (Ollama's rules): top_logprobs 0..20, and more than 0 only together with logprobs
   if (gr.opt.top_logprobs < 0 || gr.opt.top_logprobs > CL_MAX_TOP_LOGPROBS || (gr.opt.top_logprobs > 0 && !gr.opt.logprobs)) {
     set_last_error("top_logprobs must be 0..20 and needs logprobs");
@@ -326,9 +364,9 @@ static int handle_message_impl(cl_engine* e, const uint8_t* req, size_t req_len,
   cl_token_logprob* lps = nullptr;
   if (gr.stream && allow_stream) {
     // streaming (SURVEY.md §8f row 4): Done=false frames carrying text deltas, then one Done=true frame
-    FrameSinkCtx ctx{StreamText{e->impl.tok.get(), {}, 0}, cb, user, gr.model, {}};
+    FrameSinkCtx ctx{StreamText{e->impl.tok.get(), StopScan(stop), {}, 0}, cb, user, gr.model, {}};
     Engine::TokenSink sink{frame_sink, &ctx, top_n >= 0 ? frame_lp_sink : nullptr};
-    const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r, &sink, top_n, top_n >= 0 ? &lps : nullptr);
+    const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r, &sink, top_n, top_n >= 0 ? &lps : nullptr, &ext, &stop);
     if (rc) return rc;
     free(lps);
     const std::string tail = ctx.st.feed(nullptr, 0, true);
@@ -337,7 +375,7 @@ static int handle_message_impl(cl_engine* e, const uint8_t* req, size_t req_len,
     cb(user, f.data(), f.size());
     return CL_OK;
   }
-  const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r, nullptr, top_n, top_n >= 0 ? &lps : nullptr);
+  const int rc = e->impl.generate_ids(ids.data(), (int)ids.size(), sp, &r, nullptr, top_n, top_n >= 0 ? &lps : nullptr, &ext, &stop);
   if (rc) return rc;
   std::vector<PbTokenLogprob> wl = lps ? wire_logprobs(*e->impl.tok, lps, (size_t)r.n_generated) : std::vector<PbTokenLogprob>();
   free(lps);
@@ -550,6 +588,13 @@ int cl_seq_set_logprobs(cl_engine* e, cl_seq_t s, int32_t top_n) {
   if (!e) return CL_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lk(e->impl.mu_);
   CL_GUARD(return e->impl.set_logprobs(s, top_n);)
+}
+int cl_seq_set_sampling_ext(cl_engine* e, cl_seq_t s, const cl_sampling_ext* ext) {
+  if (!e) return CL_ERR_INVALID_ARG;
+  SamplerExt x;
+  if (int rc = read_sampling_ext(ext, &x, nullptr)) return rc;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  CL_GUARD(return e->impl.set_sampling_ext(s, x);)
 }
 int cl_seq_take_logprobs(cl_engine* e, cl_seq_t s, cl_token_logprob* out, int32_t cap, int32_t* n_out) {
   if (!e || !n_out) return CL_ERR_INVALID_ARG;

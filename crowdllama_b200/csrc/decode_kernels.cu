@@ -790,14 +790,13 @@ struct TailHist {
   int n_extra;
 };
 
-// The draw of one logits row, called by all kTailBlocks blocks of the row: each block keys its vocabulary slice (repeat
-// penalty applied) and leaves its top-k keys in cand[blockIdx.x]; the last block to finish merges them and draws at RNG
+// The draw of one logits row, called by all kTailBlocks blocks of the row: each block keys its vocabulary slice (penalty
+// stage applied) and leaves its top-k keys in cand[blockIdx.x]; the last block to finish merges them and draws at RNG
 // step *step + step_add.  Returns the id on thread 0 of the last block, -1 on every other thread.
 __device__ __forceinline__ int tail_draw(const float* lg_row, int V, const SampleParams& sp, const TailHist& h,
                                          unsigned long long* cand_row, unsigned* counter, const unsigned long long* step,
                                          int step_add) {
   __shared__ unsigned long long keys[kSampleSliceMax];
-  __shared__ unsigned pen[kSampleSliceMax / 32];
   __shared__ unsigned long long top[kSampleTopKMax], sorted[kSampleTopKMax];
   __shared__ double p[kSampleTopKMax];
   __shared__ int n_out, is_last_s;
@@ -808,25 +807,33 @@ __device__ __forceinline__ int tail_draw(const float* lg_row, int V, const Sampl
   const int lo = blockIdx.x * slice, n = max(0, min(slice, V - lo));
   const float* lg = lg_row + lo;
 
-  for (int i = tid; i < kSampleSliceMax / 32; i += 256) pen[i] = 0u;
   if (tid == 0) n_out = 0;
+  for (int i = tid; i < n; i += 256) keys[i] = sample_key(lg[i], lo + i);
   __syncthreads();
-  if (sp.repeat_penalty != 1.0f && sp.repeat_last_n != 0) {   // the distinct in-range ids of the last repeat_last_n
+  // Penalty stage over the last repeat_last_n ids: the thread holding the first occurrence of an id of this slice counts
+  // it in the window (c) and re-keys it, repeat penalty first, then v -= c * frequency + presence.  A scan of the window
+  // instead of a count array: a slice-sized array would not leave the tail kernels 8 blocks per SM.
+  if (sp.repeat_last_n != 0 && (sp.repeat_penalty != 1.0f || sp.presence_penalty != 0.f || sp.frequency_penalty != 0.f)) {
     const int total = h.ring_len + h.n_extra;
-    const int w = sp.repeat_last_n > 0 && total > sp.repeat_last_n ? sp.repeat_last_n : total;
-    for (int j = tid; j < w; j += 256) {
-      const int idx = total - w + j;
-      const int id = idx < h.ring_len ? h.ring[idx % kSampleHistMax] : h.extra[idx - h.ring_len];
-      if (id >= lo && id < lo + n) atomicOr(&pen[(id - lo) >> 5], 1u << ((id - lo) & 31));
+    const int i0 = sp.repeat_last_n > 0 && total > sp.repeat_last_n ? total - sp.repeat_last_n : 0;   // window: ids i0 .. total - 1
+    auto at = [&](int i) { return i < h.ring_len ? h.ring[i % kSampleHistMax] : h.extra[i - h.ring_len]; };
+    for (int j = i0 + tid; j < total; j += 256) {
+      const int id = at(j);
+      if (id < lo || id >= lo + n) continue;
+      int c = 0;
+      for (int m = i0; m < total; ++m)
+        if (at(m) == id) {
+          if (m < j) { c = 0; break; }   // not the first occurrence
+          ++c;
+        }
+      if (c == 0) continue;
+      float v = lg[id - lo];
+      if (sp.repeat_penalty != 1.0f) v = v > 0.f ? __fdiv_rn(v, sp.repeat_penalty) : __fmul_rn(v, sp.repeat_penalty);
+      v = __fsub_rn(v, __fadd_rn(__fmul_rn((float)c, sp.frequency_penalty), sp.presence_penalty));
+      keys[id - lo] = sample_key(v, id);
     }
+    __syncthreads();
   }
-  __syncthreads();
-  for (int i = tid; i < n; i += 256) {
-    float v = lg[i];
-    if (pen[i >> 5] & (1u << (i & 31))) v = v > 0.f ? __fdiv_rn(v, sp.repeat_penalty) : __fmul_rn(v, sp.repeat_penalty);
-    keys[i] = sample_key(v, lo + i);
-  }
-  __syncthreads();
   const unsigned long long t1 = n > K ? block_topk_threshold([&](int i) { return keys[i]; }, n, K) : 1ull;
   unsigned long long* cand = cand_row + (size_t)blockIdx.x * kSampleTopKMax;
   for (int i = tid; i < n; i += 256)
@@ -881,6 +888,8 @@ __device__ __forceinline__ int tail_draw(const float* lg_row, int V, const Sampl
     double cum = 0.0;
     for (int i = 0; i < K; ++i) { cum = __dadd_rn(cum, q[i]); if (cum >= (double)sp.top_p) { keep = i + 1; break; } }
   }
+  if (sp.min_p > 0.f)   // min_p: the leading candidates with p_i >= min_p * p_0, and p_0 = exp(0) = 1
+    for (int i = 1; i < keep; ++i) if (p[i] < (double)sp.min_p) { keep = i; break; }
   double tot = 0.0;
   for (int i = 0; i < keep; ++i) tot = __dadd_rn(tot, p[i]);
   const double u = __dmul_rn(sample_uniform01(sp.seed, *step + (unsigned long long)step_add), tot);

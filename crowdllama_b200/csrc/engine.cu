@@ -464,11 +464,17 @@ int Engine::collect_logprobs(const cl_seq_t* ss, int n) {
   return CL_OK;
 }
 
+int Engine::set_sampling_ext(cl_seq_t s, const SamplerExt& ext) {
+  if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  if (int rc = check_sampling_ext(ext, nullptr)) return rc;
+  seqs_[s].ext = ext;
+  return CL_OK;
+}
+
 int Engine::arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist) {
-  if (!device_sampling_ok(sp, cfg.vocab_size)) { set_last_error("sampling settings need the host sampler"); return CL_ERR_INVALID_ARG; }
-  SampleParams par;
-  par.temperature = sp.temperature; par.top_p = sp.top_p; par.repeat_penalty = sp.repeat_penalty;
-  par.top_k = sp.top_k; par.repeat_last_n = sp.repeat_last_n; par.seed = sp.seed;
+  const SamplerExt& ext = seqs_[s].ext;
+  if (!device_sampling_ok(sp, cfg.vocab_size, ext)) { set_last_error("sampling settings need the host sampler"); return CL_ERR_INVALID_ARG; }
+  const SampleParams par = sample_params(sp, ext);
   std::vector<int> ring(kSampleHistMax, 0);
   for (int i = std::max(0, n_hist - kSampleHistMax); i < n_hist; ++i) ring[i % kSampleHistMax] = hist[i];
   const int mode = 1;
@@ -1060,7 +1066,7 @@ int Engine::decode_sample(const cl_seq_t* ss, int B, const int32_t* first_ids, c
   if (B <= 0 || B > max_batch_) { set_last_error("bad batch / steps"); return CL_ERR_INVALID_ARG; }
   for (int b = 0; b < B; ++b) {
     if (ss[b] < 0 || ss[b] >= max_seqs_ || !seqs_[ss[b]].live) return CL_ERR_BAD_SEQ;
-    if (sp[b].temperature > 0.f && !device_sampling_ok(sp[b], cfg.vocab_size)) {
+    if (sp[b].temperature > 0.f && !device_sampling_ok(sp[b], cfg.vocab_size, seqs_[ss[b]].ext)) {
       set_last_error("sampling settings of sequence " + std::to_string(b) + " need the host sampler");
       return CL_ERR_INVALID_ARG;
     }

@@ -203,6 +203,8 @@ class Tokenizer {
   virtual ~Tokenizer() {}
   virtual std::vector<int32_t> encode(const std::string& text, bool add_bos) const = 0;
   virtual std::string decode_bytes(const std::vector<int32_t>& ids) const = 0;   // raw surface bytes (may cut a UTF-8 sequence)
+  // What id adds to decode_bytes of a sequence when appended to it; at_start: nothing before it rendered any byte
+  virtual std::string piece_bytes(int32_t id, bool at_start) const { (void)at_start; return decode_bytes({id}); }
   std::string decode(const std::vector<int32_t>& ids) const { return sanitize(decode_bytes(ids)); }
   static std::string sanitize(const std::string& raw);              // invalid UTF-8 / control bytes -> U+FFFD
   virtual int bos() const = 0;
@@ -240,17 +242,59 @@ int model_config_from_dir(const std::string& dir, cl_model_config* out);
 // inverse rotary frequency of dimension pair i: theta^(-2i/head_dim), with the "llama3" scaling of cl_model_config when
 // rope_factor > 1 — the same expression as oracle/llama_oracle.c rope_inv_freq(), so both sides build bit-identical tables
 double rope_inv_freq(const cl_model_config& c, int i);
+// The sampler options of cl_sampling_ext (include/clengine.h) that the draw reads; all zero: cl_sampling alone
+struct SamplerExt {
+  float min_p = 0.f, presence_penalty = 0.f, frequency_penalty = 0.f;
+};
+constexpr int kMaxStops = 16;           // stop strings of one request at most
+constexpr int kMaxStopBytes = 256;      // ... each at most this long
+// Validates a caller's options: min_p in [0, 1], finite penalties, and when stop is not nullptr at most kMaxStops strings
+// of at most kMaxStopBytes each (empty ones are dropped from *stop).  CL_OK, or CL_ERR_INVALID_ARG with the last error set.
+int check_sampling_ext(const SamplerExt& x, std::vector<std::string>* stop);
+// ext == nullptr: all zero; the stop strings go to *stop when it is not nullptr (checked as check_sampling_ext does)
+int read_sampling_ext(const cl_sampling_ext* ext, SamplerExt* x, std::vector<std::string>* stop);
 int32_t sample_token(const float* logits, int32_t vocab, const cl_sampling& sp, const int32_t* history, int32_t n_history,
-                     uint64_t step);
+                     uint64_t step, const SamplerExt& ext = SamplerExt());
 // True when the step tail's device sampler draws exactly what sample_token draws for these settings: temperature > 0,
-// 1 <= top_k <= kSampleTopKMax with top_k < vocab, vocab <= kTailBlocks * kSampleSliceMax, and the repeat penalty off or
-// over a window of 1..kSampleHistMax ids.  Everything else (top_k 0, repeat_last_n -1, ...) stays on the host sampler.
-inline bool device_sampling_ok(const cl_sampling& sp, int vocab) {
+// 1 <= top_k <= kSampleTopKMax with top_k < vocab, vocab <= kTailBlocks * kSampleSliceMax, and the penalty stage (repeat,
+// presence and frequency penalties) off or over a window of 1..kSampleHistMax ids.  Everything else (top_k 0,
+// repeat_last_n -1, ...) stays on the host sampler.  min_p and the penalties' values need no more (check_sampling_ext).
+inline bool device_sampling_ok(const cl_sampling& sp, int vocab, const SamplerExt& ext = SamplerExt()) {
   if (!(sp.temperature > 0.f)) return false;
   if (sp.top_k < 1 || sp.top_k > kSampleTopKMax || sp.top_k >= vocab || vocab > kTailBlocks * kSampleSliceMax) return false;
-  const bool penalty = sp.repeat_penalty != 1.0f && sp.repeat_last_n != 0;
+  const bool penalty = sp.repeat_last_n != 0 && (sp.repeat_penalty != 1.0f || ext.presence_penalty != 0.f || ext.frequency_penalty != 0.f);
   return !penalty || (sp.repeat_last_n > 0 && sp.repeat_last_n <= kSampleHistMax);
 }
+inline SampleParams sample_params(const cl_sampling& sp, const SamplerExt& ext) {
+  SampleParams p;
+  p.temperature = sp.temperature; p.top_p = sp.top_p; p.repeat_penalty = sp.repeat_penalty;
+  p.min_p = ext.min_p; p.presence_penalty = ext.presence_penalty; p.frequency_penalty = ext.frequency_penalty;
+  p.top_k = sp.top_k; p.repeat_last_n = sp.repeat_last_n; p.seed = sp.seed;
+  return p;
+}
+
+// Stop sequences (Ollama's `stop`): the one place that decides where a response's text ends.  The generated text's bytes
+// are fed in order; the first time one of the stop strings occurs in them, match() is the offset of the earliest such
+// occurrence and the text is cut there.  safe() is how many leading bytes no later byte can cut: everything before the
+// longest tail that could still begin a stop string (match() once matched).  Each feed costs O(stops x (longest stop +
+// bytes fed)), whatever the text's length.
+class StopScan {
+ public:
+  StopScan() = default;
+  explicit StopScan(std::vector<std::string> stops);
+  bool active() const { return !stops_.empty(); }
+  void feed(const std::string& bytes);                                 // a no-op once matched
+  void feed_id(const Tokenizer& tok, int32_t id);                      // the id's bytes as they appear in decode_bytes
+  int64_t match() const { return match_; }                             // -1: no match yet
+  int64_t safe() const { return match_ >= 0 ? match_ : n_ - hold_; }
+  int64_t size() const { return n_; }
+
+ private:
+  std::vector<std::string> stops_;
+  size_t keep_ = 0;        // longest stop string - 1: the bytes a later match can start in
+  std::string tail_;       // the last keep_ bytes fed
+  int64_t n_ = 0, match_ = -1, hold_ = 0;
+};
 
 // ---- minimal protobuf codec for llama.v1.BaseMessage (pbmsg.cpp) -------------------------------
 // GenerateOptions: the proto extension SURVEY.md §8f row 3 asks for (seed / temperature / num_predict ... are
@@ -261,10 +305,12 @@ struct PbGenerateOptions {
   uint64_t seed = 0; float temperature = 0.f; int32_t top_k = 0; float top_p = 0.f; float repeat_penalty = 0.f;
   int32_t repeat_last_n = 0; int32_t num_predict = 0; bool raw = false;
   bool logprobs = false; int32_t top_logprobs = 0;   // Ollama's top-level logprobs / top_logprobs (fields 9, 10)
+  std::vector<std::string> stop;                      // fields 11 - 14: stop, min_p, presence_penalty, frequency_penalty
+  SamplerExt ext;
 };
 struct PbGenerateRequest { std::string model, prompt; bool stream = false; PbGenerateOptions opt; };
 // request options override the caller's default sampling field by field
-void apply_options(const PbGenerateOptions& o, cl_sampling* sp);
+void apply_options(const PbGenerateOptions& o, cl_sampling* sp, SamplerExt* ext);
 struct PbTokenLogprob { std::string token, bytes; float logprob = 0.f; std::vector<PbTokenLogprob> top; };
 struct PbGenerateResponse {
   std::string model, response, done_reason, worker_id;
@@ -290,6 +336,7 @@ struct SeqState {
   int known = 0;          // leading history ids that are the real tokens of the cached K/V (seq_fake_fill's are not)
   std::vector<int32_t> history;
   std::vector<LogprobRecord> lps;   // records of the ids the step tail chose while logprobs were on, not taken yet
+  SamplerExt ext;                   // cl_seq_set_sampling_ext: merged into every cl_sampling the sequence draws with
 };
 
 struct Request;  // scheduler.cpp
@@ -329,7 +376,9 @@ class Engine {
                     int n_steps, int32_t* ids_out, float* device_ms);
   // Device sampler of one slot: every later step tail of `s` draws with `sp`, the first draw at RNG step `step0`, with the
   // last kSampleHistMax ids of hist[0..n_hist) as its history.  seq_create / seq_free disarm.
+  // The sequence's SamplerExt (set_sampling_ext) joins sp.
   int arm_sampling(cl_seq_t s, const cl_sampling& sp, uint64_t step0, const int32_t* hist, int n_hist);
+  int set_sampling_ext(cl_seq_t s, const SamplerExt& ext);   // seq_create / seq_free reset it to all zero
   int disarm_sampling(cl_seq_t s);
   int read_next_token(cl_seq_t s, int32_t* out);   // d_tok_[s]: what the last step tail of `s` chose
   // Log-probabilities (contract in include/clengine.h, cl_seq_set_logprobs): top_n -1 = off, 0..kLogprobTopMax = every
@@ -379,9 +428,11 @@ class Engine {
     int (*fn)(void* user, const int32_t* ids, int n) = nullptr; void* user = nullptr;
     int (*lp_fn)(void* user, const cl_token_logprob* lps, int n) = nullptr;
   };
-  // top_n >= 0: logprobs on for the request; *lps (malloc'd, one record per generated id) when lps is not nullptr
+  // top_n >= 0: logprobs on for the request; *lps (malloc'd, one record per generated id) when lps is not nullptr.
+  // ext / stop (may be nullptr: none): checked by check_sampling_ext; a stop ends the request as StopScan decides.
   int generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink = nullptr,
-                   int top_n = -1, cl_token_logprob** lps = nullptr);
+                   int top_n = -1, cl_token_logprob** lps = nullptr, const SamplerExt* ext = nullptr,
+                   const std::vector<std::string>* stop = nullptr);
   void scheduler_main();
   void start_scheduler();
   void stop_scheduler();

@@ -321,8 +321,65 @@ double rope_inv_freq(const cl_model_config& c, int i) {
   return (1.0 - smooth) * inv / factor + smooth * inv;
 }
 
+int check_sampling_ext(const SamplerExt& x, std::vector<std::string>* stop) {
+  if (!(x.min_p >= 0.f && x.min_p <= 1.f)) { set_last_error("min_p must be in [0, 1]"); return CL_ERR_INVALID_ARG; }
+  if (!std::isfinite(x.presence_penalty) || !std::isfinite(x.frequency_penalty)) {
+    set_last_error("presence_penalty and frequency_penalty must be finite");
+    return CL_ERR_INVALID_ARG;
+  }
+  if (!stop) return CL_OK;
+  stop->erase(std::remove(stop->begin(), stop->end(), std::string()), stop->end());
+  if ((int)stop->size() > kMaxStops) { set_last_error("at most 16 stop strings"); return CL_ERR_INVALID_ARG; }
+  for (const auto& t : *stop)
+    if ((int)t.size() > kMaxStopBytes) { set_last_error("a stop string is longer than 256 bytes"); return CL_ERR_INVALID_ARG; }
+  return CL_OK;
+}
+int read_sampling_ext(const cl_sampling_ext* ext, SamplerExt* x, std::vector<std::string>* stop) {
+  *x = SamplerExt();
+  if (stop) stop->clear();
+  if (!ext) return CL_OK;
+  x->min_p = ext->min_p; x->presence_penalty = ext->presence_penalty; x->frequency_penalty = ext->frequency_penalty;
+  if (stop) {
+    if (ext->n_stop < 0 || (ext->n_stop > 0 && !ext->stop)) {
+      set_last_error("n_stop must be >= 0, with a stop array when > 0");
+      return CL_ERR_INVALID_ARG;
+    }
+    for (int i = 0; i < ext->n_stop; ++i) {
+      if (!ext->stop[i]) { set_last_error("a stop string is NULL"); return CL_ERR_INVALID_ARG; }
+      const size_t len = strnlen(ext->stop[i], kMaxStopBytes + 1);
+      stop->emplace_back(ext->stop[i], len);
+    }
+  }
+  return check_sampling_ext(*x, stop);
+}
+
+StopScan::StopScan(std::vector<std::string> stops) : stops_(std::move(stops)) {
+  stops_.erase(std::remove(stops_.begin(), stops_.end(), std::string()), stops_.end());
+  for (const auto& t : stops_) keep_ = std::max(keep_, t.size() - 1);
+}
+void StopScan::feed_id(const Tokenizer& tok, int32_t id) { feed(tok.piece_bytes(id, n_ == 0)); }
+void StopScan::feed(const std::string& bytes) {
+  if (match_ >= 0 || stops_.empty() || bytes.empty()) return;
+  const std::string w = tail_ + bytes;
+  const int64_t base = n_ - (int64_t)tail_.size();   // text offset of w[0]
+  size_t best = std::string::npos;
+  for (const auto& t : stops_) {
+    // a match ending in the tail alone would have been found by an earlier feed
+    const size_t from = tail_.size() >= t.size() ? tail_.size() - t.size() + 1 : 0;
+    const size_t at = w.find(t, from);
+    if (at != std::string::npos && at < best) best = at;
+  }
+  n_ += (int64_t)bytes.size();
+  if (best != std::string::npos) { match_ = base + (int64_t)best; return; }
+  tail_ = w.substr(w.size() > keep_ ? w.size() - keep_ : 0);
+  hold_ = 0;
+  for (size_t len = tail_.size(); len > 0 && hold_ == 0; --len)   // the longest tail that is the start of a stop string
+    for (const auto& t : stops_)
+      if (t.size() > len && t.compare(0, len, tail_, tail_.size() - len, len) == 0) { hold_ = (int64_t)len; break; }
+}
+
 int32_t sample_token(const float* logits, int32_t vocab, const cl_sampling& sp, const int32_t* history, int32_t n_history,
-                     uint64_t step) {
+                     uint64_t step, const SamplerExt& ext) {
   if (sp.temperature <= 0.f) {
     int best = 0;
     for (int i = 1; i < vocab; ++i) if (logits[i] > logits[best]) best = i;
@@ -331,14 +388,21 @@ int32_t sample_token(const float* logits, int32_t vocab, const cl_sampling& sp, 
   struct Cand { float v; int32_t id; };
   std::vector<Cand> c(vocab);
   for (int i = 0; i < vocab; ++i) c[i] = {logits[i], i};
-  if (sp.repeat_penalty != 1.0f && sp.repeat_last_n != 0 && history) {
+  // penalty stage (llama.cpp's formula) over the last repeat_last_n ids: an id occurring c > 0 times takes the repeat
+  // penalty, then v -= c * frequency_penalty + presence_penalty
+  if (sp.repeat_last_n != 0 && history && (sp.repeat_penalty != 1.0f || ext.presence_penalty != 0.f || ext.frequency_penalty != 0.f)) {
     int start = sp.repeat_last_n > 0 && n_history > sp.repeat_last_n ? n_history - sp.repeat_last_n : 0;
-    std::vector<char> seen(vocab, 0);
+    std::vector<int> count(vocab, 0);
+    for (int i = start; i < n_history; ++i)
+      if (history[i] >= 0 && history[i] < vocab) ++count[history[i]];
     for (int i = start; i < n_history; ++i) {
-      int id = history[i];
-      if (id < 0 || id >= vocab || seen[id]) continue;
-      seen[id] = 1;
-      c[id].v = c[id].v > 0.f ? c[id].v / sp.repeat_penalty : c[id].v * sp.repeat_penalty;
+      const int id = history[i];
+      if (id < 0 || id >= vocab || count[id] == 0) continue;
+      float v = c[id].v;
+      if (sp.repeat_penalty != 1.0f) v = v > 0.f ? v / sp.repeat_penalty : v * sp.repeat_penalty;
+      const float d = (float)count[id] * ext.frequency_penalty;
+      c[id].v = v - (d + ext.presence_penalty);
+      count[id] = 0;   // applied once
     }
   }
   auto cmp = [](const Cand& a, const Cand& b) { return a.v > b.v || (a.v == b.v && a.id < b.id); };
@@ -355,6 +419,8 @@ int32_t sample_token(const float* logits, int32_t vocab, const cl_sampling& sp, 
     double cum = 0.0;
     for (int i = 0; i < n; ++i) { cum += p[i] / den; if (cum >= (double)sp.top_p) { keep = i + 1; break; } }
   }
+  if (ext.min_p > 0.f)   // min_p: the leading candidates with p_i >= min_p * p_0, and p_0 = exp(0) = 1
+    for (int i = 1; i < keep; ++i) if (p[i] < (double)ext.min_p) { keep = i; break; }
   double tot = 0.0;
   for (int i = 0; i < keep; ++i) tot += p[i];
   const double u = uniform01(sp.seed, step) * tot;
@@ -374,7 +440,9 @@ int32_t sample_token(const float* logits, int32_t vocab, const cl_sampling& sp, 
 //   GenerateOptions  { optional uint64 seed = 1; optional float temperature = 2; optional int32 top_k = 3;
 //                      optional float top_p = 4; optional float repeat_penalty = 5;
 //                      optional int32 repeat_last_n = 6; optional int32 num_predict = 7; optional bool raw = 8;
-//                      optional bool logprobs = 9; optional int32 top_logprobs = 10; }      <- EXTENSION (logprobs)
+//                      optional bool logprobs = 9; optional int32 top_logprobs = 10;        <- EXTENSION (logprobs)
+//                      repeated string stop = 11; optional float min_p = 12;
+//                      optional float presence_penalty = 13; optional float frequency_penalty = 14; }  <- EXTENSION
 //   GenerateResponse { string model = 1; google.protobuf.Timestamp created_at = 2;
 //                      string response = 3; bool done = 4; string done_reason = 5;
 //                      string worker_id = 6; int64 total_duration = 7;
@@ -382,7 +450,8 @@ int32_t sample_token(const float* logits, int32_t vocab, const cl_sampling& sp, 
 //   TokenLogprob     { string token = 1; float logprob = 2; bytes bytes = 3; repeated TokenLogprob top_logprobs = 4; }
 // ================================================================================================
 enum { kReqOptions = 4, kOptSeed = 1, kOptTemperature = 2, kOptTopK = 3, kOptTopP = 4, kOptRepeatPenalty = 5, kOptRepeatLastN = 6,
-       kOptNumPredict = 7, kOptRaw = 8, kOptLogprobs = 9, kOptTopLogprobs = 10 };
+       kOptNumPredict = 7, kOptRaw = 8, kOptLogprobs = 9, kOptTopLogprobs = 10, kOptStop = 11, kOptMinP = 12,
+       kOptPresencePenalty = 13, kOptFrequencyPenalty = 14 };
 enum { kRespLogprobs = 8, kTlpToken = 1, kTlpLogprob = 2, kTlpBytes = 3, kTlpTop = 4 };
 enum { kBaseReq = 1, kBaseResp = 2, kReqModel = 1, kReqPrompt = 2, kReqStream = 3, kRespModel = 1, kRespCreated = 2,
        kRespResponse = 3, kRespDone = 4, kRespDoneReason = 5, kRespWorkerId = 6, kRespTotalDuration = 7 };
@@ -423,18 +492,30 @@ static bool decode_options(const uint8_t* q, const uint8_t* qe, PbGenerateOption
       else if (f == kOptTopLogprobs) o->top_logprobs = (int32_t)(int64_t)v;
       else o->raw = v != 0;
       o->has |= 1u << f;
-    } else if (wt == 5 && (f == kOptTemperature || f == kOptTopP || f == kOptRepeatPenalty)) {
+    } else if (wt == 5 && (f == kOptTemperature || f == kOptTopP || f == kOptRepeatPenalty || f == kOptMinP || f == kOptPresencePenalty ||
+                           f == kOptFrequencyPenalty)) {
       if (qe - q < 4) return false;
       float v;
       memcpy(&v, q, 4);
       q += 4;
-      if (f == kOptTemperature) o->temperature = v; else if (f == kOptTopP) o->top_p = v; else o->repeat_penalty = v;
+      if (f == kOptTemperature) o->temperature = v; else if (f == kOptTopP) o->top_p = v; else if (f == kOptRepeatPenalty) o->repeat_penalty = v;
+      else if (f == kOptMinP) o->ext.min_p = v; else if (f == kOptPresencePenalty) o->ext.presence_penalty = v;
+      else o->ext.frequency_penalty = v;
+      o->has |= 1u << f;
+    } else if (wt == 2 && f == kOptStop) {
+      uint64_t m;
+      if (!rd_varint(q, qe, &m) || (uint64_t)(qe - q) < m) return false;
+      o->stop.emplace_back((const char*)q, m);
+      q += m;
       o->has |= 1u << f;
     } else if (!skip_field(q, qe, wt)) return false;
   }
   return true;
 }
-void apply_options(const PbGenerateOptions& o, cl_sampling* sp) {
+void apply_options(const PbGenerateOptions& o, cl_sampling* sp, SamplerExt* ext) {
+  if (o.has & (1u << kOptMinP)) ext->min_p = o.ext.min_p;
+  if (o.has & (1u << kOptPresencePenalty)) ext->presence_penalty = o.ext.presence_penalty;
+  if (o.has & (1u << kOptFrequencyPenalty)) ext->frequency_penalty = o.ext.frequency_penalty;
   if (o.has & (1u << kOptSeed)) sp->seed = o.seed;
   if (o.has & (1u << kOptTemperature)) sp->temperature = o.temperature;
   if (o.has & (1u << kOptTopK)) sp->top_k = o.top_k;

@@ -65,11 +65,12 @@ struct AttnDecodeArgs {
 // ---- step tail: argmax or a seeded draw, then advance the sequence ----------------------------------
 constexpr int kTailBlocks = 64;          // blocks per slot; each owns a contiguous slice of the vocabulary
 constexpr int kSampleTopKMax = 128;      // device draws cover 1 <= top_k <= this
-constexpr int kSampleHistMax = 256;      // ... and a repeat-penalty window of at most this many ids
+constexpr int kSampleHistMax = 256;      // ... and a penalty window of at most this many ids
 constexpr int kSampleSliceMax = 2560;    // ... and vocab <= kTailBlocks * kSampleSliceMax (one slice's keys sit in shared memory)
 
-struct SampleParams {                    // cl_sampling fields the draw reads
+struct SampleParams {                    // cl_sampling (and cl_sampling_ext) fields the draw reads
   float temperature = 0.f, top_p = 1.f, repeat_penalty = 1.f;
+  float min_p = 0.f, presence_penalty = 0.f, frequency_penalty = 0.f;
   int top_k = 0, repeat_last_n = 0;
   unsigned long long seed = 0;
 };

@@ -621,22 +621,24 @@ int cl_op_qkv_rope_append(int device, int variant, const uint16_t* w_qkv, const 
   return CL_OK;
 }
 
-// cl_op_sample, and with top_n >= 0 cl_op_sample_logprobs (rows with temperature <= 0 then take the greedy choice)
-static int op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
-                     const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t top_n, int32_t* ids_out,
-                     cl_token_logprob* lp_out) {
+// cl_op_sample, cl_op_sample_ext (ext: [n_rows], may be nullptr) and with top_n >= 0 cl_op_sample_logprobs (rows with
+// temperature <= 0 then take the greedy choice)
+static int op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const cl_sampling_ext* ext,
+                     const int32_t* history, const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t top_n,
+                     int32_t* ids_out, cl_token_logprob* lp_out) {
   if (!logits || n_rows <= 0 || vocab <= 1 || !sp || !n_history || !step || !ids_out) return CL_ERR_INVALID_ARG;
   if (top_n >= 0 && (top_n > kLogprobTopMax || !lp_out || vocab > kTailBlocks * kSampleSliceMax)) return CL_ERR_INVALID_ARG;
   const size_t R = (size_t)n_rows;
   std::vector<SampleParams> par(R);
   std::vector<int> ring(R * kSampleHistMax, 0), hlen(R), mode(R, 1);
   for (size_t r = 0; r < R; ++r) {
+    SamplerExt x;
+    if (int rc = read_sampling_ext(ext ? ext + r : nullptr, &x, nullptr)) return rc;
     if (top_n >= 0 && !(sp[r].temperature > 0.f)) mode[r] = 0;
-    else if (!device_sampling_ok(sp[r], vocab)) { set_last_error("cl_op_sample: settings the device sampler does not cover"); return CL_ERR_INVALID_ARG; }
+    else if (!device_sampling_ok(sp[r], vocab, x)) { set_last_error("cl_op_sample: settings the device sampler does not cover"); return CL_ERR_INVALID_ARG; }
     const int n = n_history[r];
     if (n < 0 || (n > 0 && (!history || n > hist_stride))) return CL_ERR_INVALID_ARG;
-    par[r].temperature = sp[r].temperature; par[r].top_p = sp[r].top_p; par[r].repeat_penalty = sp[r].repeat_penalty;
-    par[r].top_k = sp[r].top_k; par[r].repeat_last_n = sp[r].repeat_last_n; par[r].seed = sp[r].seed;
+    par[r] = sample_params(sp[r], x);
     for (int i = std::max(0, n - kSampleHistMax); i < n; ++i) ring[r * kSampleHistMax + i % kSampleHistMax] = history[r * hist_stride + i];
     hlen[r] = n;
   }
@@ -693,14 +695,19 @@ static int op_sample(int device, const float* logits, int32_t n_rows, int32_t vo
 
 int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
                  const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out) {
-  return op_sample(device, logits, n_rows, vocab, sp, history, n_history, hist_stride, step, -1, ids_out, nullptr);
+  return op_sample(device, logits, n_rows, vocab, sp, nullptr, history, n_history, hist_stride, step, -1, ids_out, nullptr);
+}
+
+int cl_op_sample_ext(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const cl_sampling_ext* ext,
+                     const int32_t* history, const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out) {
+  return op_sample(device, logits, n_rows, vocab, sp, ext, history, n_history, hist_stride, step, -1, ids_out, nullptr);
 }
 
 int cl_op_sample_logprobs(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
                           const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t top_n, int32_t* ids_out,
                           cl_token_logprob* lp_out) {
   if (top_n < 0) return CL_ERR_INVALID_ARG;
-  return op_sample(device, logits, n_rows, vocab, sp, history, n_history, hist_stride, step, top_n, ids_out, lp_out);
+  return op_sample(device, logits, n_rows, vocab, sp, nullptr, history, n_history, hist_stride, step, top_n, ids_out, lp_out);
 }
 
 int cl_op_synth_weights(int device, uint64_t seed, int32_t tensor_key, int64_t n, float scale, uint16_t* out_bf16) {

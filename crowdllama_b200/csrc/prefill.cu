@@ -330,7 +330,7 @@ int Engine::decode_verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x
   if (n_seqs < 1 || !ss) { set_last_error("verify_batch: bad arguments"); return CL_ERR_INVALID_ARG; }
   for (int i = 0; i < n_seqs; ++i) {
     if (ss[i] < 0 || ss[i] >= max_seqs_ || !seqs_[ss[i]].live) return CL_ERR_BAD_SEQ;
-    if (sp && sp[i].temperature > 0.f && !device_sampling_ok(sp[i], cfg.vocab_size)) {
+    if (sp && sp[i].temperature > 0.f && !device_sampling_ok(sp[i], cfg.vocab_size, seqs_[ss[i]].ext)) {
       set_last_error("sampling settings need the host sampler");
       return CL_ERR_INVALID_ARG;
     }

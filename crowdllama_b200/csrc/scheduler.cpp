@@ -21,6 +21,8 @@ static int64_t now_ns() {
 struct Request {
   std::vector<int32_t> prompt;
   cl_sampling sp{};
+  SamplerExt ext;                   // min_p and the presence / frequency penalties; the sequence carries them while admitted
+  StopScan stop;                    // stop strings over the text of `out` (kept across preemptions and context shifts)
   std::vector<int32_t> out;
   cl_seq_t seq = -1;
   int max_new = 0;
@@ -67,7 +69,8 @@ static void fill_result(const Request& r, cl_result* out, const Tokenizer* tok) 
   out->n_generated = (int32_t)r.out.size();
   out->token_ids = (int32_t*)malloc(sizeof(int32_t) * std::max<size_t>(1, r.out.size()));
   if (!r.out.empty()) memcpy(out->token_ids, r.out.data(), r.out.size() * 4);
-  std::string text = tok ? tok->decode(r.out) : std::string();
+  std::string text;
+  if (tok) text = r.stop.match() >= 0 ? Tokenizer::sanitize(tok->decode_bytes(r.out).substr(0, (size_t)r.stop.match())) : tok->decode(r.out);
   out->text = (char*)malloc(text.size() + 1);
   memcpy(out->text, text.c_str(), text.size() + 1);
   out->text_len = text.size();
@@ -80,6 +83,7 @@ static void fill_result(const Request& r, cl_result* out, const Tokenizer* tok) 
 
 static bool finished(Request& r, const Tokenizer& tok, int max_seq_len) {
   if (r.cancel.load(std::memory_order_relaxed)) { r.done_reason = "cancelled"; return true; }
+  if (r.stop.match() >= 0) { r.done_reason = "stop"; return true; }
   if (!r.out.empty() && !r.sp.ignore_eos && tok.is_stop(r.out.back())) { r.done_reason = "stop"; return true; }
   if ((int)r.out.size() >= r.max_new) { r.done_reason = "length"; return true; }
   if (!r.ctx_shift && (int)(r.prompt.size() + r.out.size()) >= max_seq_len) { r.done_reason = "length"; return true; }
@@ -108,6 +112,7 @@ bool Engine::join(Request& r, const int32_t* ids, int n, bool admission) {
       r.lps.push_back(rec);
     }
     r.out.push_back(ids[joined++]);
+    if (r.stop.active()) r.stop.feed_id(*tok, r.out.back());
     if (r.streaming) {
       std::lock_guard<std::mutex> lk(r.m);
       r.pub.push_back(r.out.back());
@@ -180,7 +185,7 @@ int Engine::host_next_token(Request& r, float* logits, bool read_back, const int
     const int rc = read_logits(r.seq, logits);
     if (rc) return rc;
   }
-  *next = sample_token(logits, cfg.vocab_size, r.sp, hist, n_hist, (uint64_t)r.out.size());
+  *next = sample_token(logits, cfg.vocab_size, r.sp, hist, n_hist, (uint64_t)r.out.size(), r.ext);
   auto& pending = seqs_[r.seq].lps;
   if (r.top_n >= 0 && !pending.empty()) {   // lse and the top list are the device's; the host's id gets logit - lse as there
     LogprobRecord& rec = pending.back();
@@ -259,6 +264,7 @@ int Engine::generate_sync(const std::shared_ptr<Request>& rp, const TokenSink* s
     emitted = r.out.size();
   };
   int rc = seq_create(&r.seq);
+  if (rc == CL_OK) seqs_[r.seq].ext = r.ext;
   if (rc == CL_OK && r.top_n >= 0) rc = set_logprobs(r.seq, r.top_n);
   if (rc) return rc;
   std::vector<float> logits(cfg.vocab_size);
@@ -310,8 +316,11 @@ int Engine::generate_sync(const std::shared_ptr<Request>& rp, const TokenSink* s
 }
 
 int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling& sp, cl_result* out, const TokenSink* sink, int top_n,
-                         cl_token_logprob** lps) {
+                         cl_token_logprob** lps, const SamplerExt* ext, const std::vector<std::string>* stop) {
   if (!prompt || n_prompt <= 0 || !out) { set_last_error("empty prompt"); return CL_ERR_INVALID_ARG; }
+  std::vector<std::string> stops = stop ? *stop : std::vector<std::string>();
+  const SamplerExt x = ext ? *ext : SamplerExt();
+  if (int rc = check_sampling_ext(x, &stops)) return rc;
   if (top_n < -1 || top_n > kLogprobTopMax || (top_n >= 0 && cfg.vocab_size > kTailBlocks * kSampleSliceMax)) {
     set_last_error("logprobs: top_n must be -1..20 and the vocabulary at most 163840");
     return CL_ERR_INVALID_ARG;
@@ -330,13 +339,15 @@ int Engine::generate_ids(const int32_t* prompt, int n_prompt, const cl_sampling&
     r->prompt.assign(prompt, prompt + n_prompt);
   }
   r->sp = sp;
+  r->ext = x;
+  r->stop = StopScan(std::move(stops));
   r->max_new = sp.max_new_tokens > 0 ? sp.max_new_tokens : cfg.max_seq_len - n_prompt;
   // num_predict <= 0 stays bounded by the window even with context shift: an unbounded request would hold a slot forever
   if (!r->ctx_shift || sp.max_new_tokens <= 0) r->max_new = std::min(r->max_new, cfg.max_seq_len - n_prompt);
   r->t_arrive = now_ns();
   r->sync = !sched_started_;
   r->streaming = !r->sync && sink && sink->fn;   // the synchronous path calls the sink itself
-  r->dev_sample = device_sample_ && device_sampling_ok(sp, cfg.vocab_size);
+  r->dev_sample = device_sample_ && device_sampling_ok(sp, cfg.vocab_size, x);
   r->top_n = top_n;
   if (r->sync) {
     std::lock_guard<std::mutex> lk(mu_);
@@ -486,6 +497,7 @@ bool Engine::admit_group(int budget) {
   // every member attaches its cached prefix before any of them reserves: a reserve may evict cached pages
   for (auto& r : group) {
     rc = seq_create(&r->seq);
+    if (rc == CL_OK) seqs_[r->seq].ext = r->ext;
     int reused = 0;
     if (rc == CL_OK) rc = attach_prefix(r->seq, r->full.data(), (int)r->full.size(), &reused);
     if (rc) break;
@@ -550,6 +562,7 @@ void Engine::admit_chunked(int budget) {
           { std::lock_guard<std::mutex> lk(q_mu_); queue_.pop_front(); }
           int reused = 0;
           int rc = seq_create(&r->seq);
+          if (rc == CL_OK) seqs_[r->seq].ext = r->ext;
           if (rc == CL_OK) rc = attach_prefix(r->seq, r->full.data(), (int)r->full.size(), &reused);   // takes `hit` tokens
           if (rc == CL_OK) rc = ensure_capacity(r->seq, (int)r->full.size() + 1);   // all pages up front: a later chunk cannot run dry
           if (rc) { retire(*r, rc, get_last_error()); continue; }

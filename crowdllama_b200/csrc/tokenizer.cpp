@@ -172,7 +172,8 @@ class HfBpeTokenizer : public Tokenizer {
  public:
   bool load(const std::string& path, const std::string& chat_family, std::string* err);
   std::vector<int32_t> encode(const std::string& text, bool add_bos) const override;
-  std::string decode_bytes(const std::vector<int32_t>& ids) const override;
+  std::string decode_bytes(const std::vector<int32_t>& ids) const override { return decode_raw(ids, true); }
+  std::string piece_bytes(int32_t id, bool at_start) const override { return decode_raw({id}, at_start); }
   int bos() const override { return bos_; }
   int eos() const override { return eos_; }
   bool is_stop(int id) const override { return id == eos_ || id == eot_; }
@@ -195,6 +196,8 @@ class HfBpeTokenizer : public Tokenizer {
   int unk_ = -1, bos_ = -1, eos_ = -1, eot_ = -1, byte_tok_[256];
   std::string family_;
 
+  // strip: drop the leading space of the whole output (SentencePiece decoders with strip_leading_space_)
+  std::string decode_raw(const std::vector<int32_t>& ids, bool strip) const;
   void bpe_word(const std::string& w, std::vector<int32_t>* out) const;
   void encode_segment(const std::string& seg, bool first, std::vector<int32_t>* out) const;
   int find(const char* t) const { auto it = vocab_.find(t); return it == vocab_.end() ? -1 : it->second; }
@@ -433,7 +436,7 @@ std::vector<int32_t> HfBpeTokenizer::encode(const std::string& text, bool add_bo
   return out;
 }
 
-std::string HfBpeTokenizer::decode_bytes(const std::vector<int32_t>& ids) const {
+std::string HfBpeTokenizer::decode_raw(const std::vector<int32_t>& ids, bool strip) const {
   std::string out;
   const ByteMap& bm = byte_map();
   for (int32_t id : ids) {
@@ -454,7 +457,7 @@ std::string HfBpeTokenizer::decode_bytes(const std::vector<int32_t>& ids) const 
       else { std::string piece = t; replace_all(piece, kMeta, " "); out += piece; }
     }
   }
-  if (spm_decoder_ && strip_leading_space_ && !out.empty() && out[0] == ' ') out.erase(0, 1);
+  if (strip && spm_decoder_ && strip_leading_space_ && !out.empty() && out[0] == ' ') out.erase(0, 1);
   return out;
 }
 

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import time
 from pathlib import Path
 
 import numpy as np
@@ -46,6 +47,23 @@ class Sampling(C.Structure):
     _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("repeat_penalty", C.c_float),
                 ("repeat_last_n", C.c_int32), ("seed", C.c_uint64), ("max_new_tokens", C.c_int32),
                 ("ignore_eos", C.c_int32)]
+
+
+class SamplingExt(C.Structure):
+    """cl_sampling_ext: min_p, presence / frequency penalties and stop strings; all zero = cl_sampling alone."""
+    _fields_ = [("min_p", C.c_float), ("presence_penalty", C.c_float), ("frequency_penalty", C.c_float), ("n_stop", C.c_int32),
+                ("stop", C.POINTER(C.c_char_p)), ("reserved", C.c_int32 * 8)]
+
+
+def sampling_ext(min_p: float = 0.0, presence_penalty: float = 0.0, frequency_penalty: float = 0.0, stop=()) -> SamplingExt:
+    """A SamplingExt; stop: str or bytes items.  The ctypes array of the strings stays alive on the returned object."""
+    x = SamplingExt(min_p=min_p, presence_penalty=presence_penalty, frequency_penalty=frequency_penalty)
+    stop = [t.encode("utf-8") if isinstance(t, str) else bytes(t) for t in (stop or ())]
+    if stop:
+        x._stop_arr = (C.c_char_p * len(stop))(*stop)
+        x.stop = C.cast(x._stop_arr, C.POINTER(C.c_char_p))
+        x.n_stop = len(stop)
+    return x
 
 
 class Result(C.Structure):
@@ -97,6 +115,7 @@ EXPORTS = [
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages", "cl_kvpool_set_host_pages", "cl_kvpool_take_moves",
     "cl_kvpool_host_cached_pages", "cl_kvpool_shift", "cl_seq_shift", "cl_op_kv_shift", "cl_seq_set_logprobs", "cl_seq_take_logprobs", "cl_generate_ids_logprobs", "cl_op_sample_logprobs",
+    "cl_sample_token_ext", "cl_op_sample_ext", "cl_seq_set_sampling_ext", "cl_generate_ids_ext",
     "cl_tokenizer_load", "cl_tokenizer_free", "cl_tokenizer_encode", "cl_tokenizer_decode", "cl_tokenizer_info", "cl_engine_load_tokenizer",
 ]
 
@@ -192,6 +211,10 @@ def lib():
         "cl_seq_take_logprobs": (C.c_int, [vp, i32, vp, i32, P(i32)]),
         "cl_generate_ids_logprobs": (C.c_int, [vp, vp, i32, P(Sampling), i32, P(Result), P(vp)]),
         "cl_op_synth_weights": (C.c_int, [C.c_int, u64, i32, i64, f32, vp]),
+        "cl_sample_token_ext": (C.c_int, [vp, i32, P(Sampling), P(SamplingExt), vp, i32, u64, P(i32)]),
+        "cl_op_sample_ext": (C.c_int, [C.c_int, vp, i32, i32, P(Sampling), P(SamplingExt), vp, vp, i32, vp, vp]),
+        "cl_seq_set_sampling_ext": (C.c_int, [vp, i32, P(SamplingExt)]),
+        "cl_generate_ids_ext": (C.c_int, [vp, vp, i32, P(Sampling), P(SamplingExt), i32, TOKEN_CB, vp, P(Result), P(vp)]),
         "cl_tokenizer_load": (C.c_int, [C.c_char_p, C.c_char_p, P(vp)]),
         "cl_tokenizer_free": (None, [vp]),
         "cl_tokenizer_encode": (C.c_int, [vp, C.c_char_p, sz, i32, i32, vp, i32, P(i32)]),
@@ -280,6 +303,16 @@ def sample_token(logits, sampling: Sampling, history=(), step: int = 0) -> int:
     return int(out.value)
 
 
+def sample_token_ext(logits, sampling: Sampling, ext: SamplingExt | None, history=(), step: int = 0) -> int:
+    """cl_sample_token_ext: sample_token with min_p and the presence / frequency penalties of ext (None: all zero)."""
+    lg = np.ascontiguousarray(logits, dtype=np.float32)
+    h = np.ascontiguousarray(list(history), dtype=np.int32)
+    out = C.c_int32()
+    _check(lib().cl_sample_token_ext(_ptr(lg), lg.size, C.byref(sampling), C.byref(ext) if ext is not None else None,
+                                     _ptr(h) if h.size else None, h.size, step, C.byref(out)), "cl_sample_token_ext")
+    return int(out.value)
+
+
 def draft_ngram(hist, k: int) -> np.ndarray:
     """The prompt-lookup drafter of speculative decoding (cl_draft_ngram; no GPU involved): the up to k ids that followed
     the most recent earlier occurrence of hist's last 3 (else 2) ids; empty when there is none."""
@@ -307,6 +340,19 @@ class GenerateResult:
         self.n_prompt, self.n_generated = r.n_prompt, r.n_generated
         self.prefill_ns, self.decode_ns, self.total_ns = r.prefill_ns, r.decode_ns, r.total_ns
         self.n_preempted = r.n_preempted
+
+    @classmethod
+    def from_response(cls, text: str, done_reason: str) -> "GenerateResult":
+        """A result answered over the wire (GenerateResponse): text and done_reason, no ids or timings."""
+        g = cls.__new__(cls)
+        g.text, g.done_reason, g.token_ids = text, done_reason, np.zeros(0, np.int32)
+        g.n_prompt = g.n_generated = g.prefill_ns = g.decode_ns = g.total_ns = g.n_preempted = 0
+        return g
+
+
+def _ext_kwargs(stop=None, min_p=None, presence_penalty=None, frequency_penalty=None) -> dict:
+    return {k: v for k, v in dict(stop=stop, min_p=min_p, presence_penalty=presence_penalty, frequency_penalty=frequency_penalty).items()
+            if v is not None}
 
 
 class Engine:
@@ -391,6 +437,10 @@ class Engine:
     def set_logprobs(self, s: int, top_n: int):
         """cl_seq_set_logprobs: -1 off, 0..20 = every later step tail of s leaves a record with top_n alternatives."""
         _check(lib().cl_seq_set_logprobs(self._h, s, top_n), "cl_seq_set_logprobs")
+
+    def set_sampling_ext(self, s: int, ext: SamplingExt | None):
+        """cl_seq_set_sampling_ext: min_p and the presence / frequency penalties for every later draw of s (None: all zero)."""
+        _check(lib().cl_seq_set_sampling_ext(self._h, s, C.byref(ext) if ext is not None else None), "cl_seq_set_sampling_ext")
 
     def take_logprobs(self, s: int) -> np.ndarray:
         """cl_seq_take_logprobs: the records of the ids chosen for s since the last take (a TOKEN_LOGPROB array)."""
@@ -595,7 +645,12 @@ class Engine:
         return out.reshape(-1, 4)
 
     # ---- request level ---------------------------------------------------------------------------
-    def generate_ids(self, prompt_ids, sampling: Sampling) -> GenerateResult:
+    def generate_ids(self, prompt_ids, sampling: Sampling, stop=None, min_p=None, presence_penalty=None,
+                     frequency_penalty=None) -> GenerateResult:
+        """cl_generate_ids; with any of stop / min_p / presence_penalty / frequency_penalty, cl_generate_ids_ext."""
+        ext = _ext_kwargs(stop, min_p, presence_penalty, frequency_penalty)
+        if ext:
+            return self.generate_ids_ext(prompt_ids, sampling, sampling_ext(**ext))[0]
         ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
         r = Result()
         _check(lib().cl_generate_ids(self._h, _ptr(ids), len(ids), C.byref(sampling), C.byref(r)), "cl_generate_ids")
@@ -603,6 +658,54 @@ class Engine:
             return GenerateResult(r)
         finally:
             lib().cl_result_free(C.byref(r))
+
+    def generate_ids_ext(self, prompt_ids, sampling: Sampling, ext: SamplingExt | None, top_n: int = -1, on_text=None):
+        """cl_generate_ids_ext: (GenerateResult, records or None).  on_text(text_delta: str, ids: list[int]) streams the
+        text as cl_generate_stream does (a truthy return cancels); records: a TOKEN_LOGPROB array when top_n >= 0."""
+        ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
+        r = Result()
+        lp = C.c_void_p()
+
+        def cb(user, text, text_len, cids, n_ids):
+            try:
+                delta = C.string_at(text, text_len).decode("utf-8", "replace") if text_len else ""
+                return 1 if on_text(delta, [cids[i] for i in range(n_ids)] if n_ids else []) else 0
+            except Exception:       # never unwind through the C frames
+                return 1
+
+        cfn = TOKEN_CB(cb) if on_text else TOKEN_CB()
+        _check(lib().cl_generate_ids_ext(self._h, _ptr(ids), len(ids), C.byref(sampling), C.byref(ext) if ext is not None else None,
+                                         top_n, cfn, None, C.byref(r), C.byref(lp) if top_n >= 0 else None), "cl_generate_ids_ext")
+        try:
+            res = GenerateResult(r)
+            recs = np.frombuffer(C.string_at(lp, res.n_generated * TOKEN_LOGPROB.itemsize), TOKEN_LOGPROB).copy() if top_n >= 0 else None
+            return res, recs
+        finally:
+            lib().cl_result_free(C.byref(r))
+            if top_n >= 0:
+                lib().cl_buffer_free(lp)
+
+    def _generate_wire(self, model: str, prompt: str, sampling: Sampling | None, ext: dict, on_text=None) -> GenerateResult:
+        """generate / generate_stream with Ollama's stop, min_p or penalties: the request goes through cl_handle_message[_stream]
+        with every cl_sampling field as an explicit option, so the chat template and the stop rule are libclengine's."""
+        from .pb import BaseMessage, GenerateOptions, GenerateRequest
+        s = sampling if sampling is not None else ollama_default_sampling(seed=time.time_ns() & 0xFFFFFFFF)
+        opts = GenerateOptions(seed=s.seed, temperature=s.temperature, top_k=s.top_k, top_p=s.top_p, repeat_penalty=s.repeat_penalty,
+                               repeat_last_n=s.repeat_last_n, num_predict=s.max_new_tokens, **ext)
+        req = BaseMessage(generate_request=GenerateRequest(model=model, prompt=prompt, stream=on_text is not None, options=opts)).encode()
+        if on_text is None:
+            g = BaseMessage.decode(self.handle_message(req)).generate_response
+            return GenerateResult.from_response(g.response, g.done_reason)
+        last = {}
+
+        def on_frame(msg):
+            g = BaseMessage.decode(msg).generate_response
+            if g.done:
+                last["g"] = g
+            return bool(g.response) and bool(on_text(g.response, []))
+
+        self.handle_message_stream(req, None, on_frame)
+        return GenerateResult.from_response("", last["g"].done_reason)
 
     def generate_ids_logprobs(self, prompt_ids, sampling: Sampling, top_n: int):
         """cl_generate_ids_logprobs: (GenerateResult, records), records a TOKEN_LOGPROB array with one entry per generated id."""
@@ -619,7 +722,13 @@ class Engine:
             lib().cl_result_free(C.byref(r))
             lib().cl_buffer_free(lp)
 
-    def generate(self, model: str, prompt: str, sampling: Sampling | None = None) -> GenerateResult:
+    def generate(self, model: str, prompt: str, sampling: Sampling | None = None, stop=None, min_p=None, presence_penalty=None,
+                 frequency_penalty=None) -> GenerateResult:
+        """cl_generate.  With stop / min_p / presence_penalty / frequency_penalty the request goes over the byte-level
+        handler (_generate_wire): the result then has text and done_reason only."""
+        ext = _ext_kwargs(stop, min_p, presence_penalty, frequency_penalty)
+        if ext:
+            return self._generate_wire(model, prompt, sampling, ext)
         r = Result()
         p = prompt.encode("utf-8")
         _check(lib().cl_generate(self._h, model.encode(), p, len(p), C.byref(sampling) if sampling else None,
@@ -629,9 +738,14 @@ class Engine:
         finally:
             lib().cl_result_free(C.byref(r))
 
-    def generate_stream(self, model: str, prompt: str, sampling: Sampling | None = None, on_text=None) -> GenerateResult:
+    def generate_stream(self, model: str, prompt: str, sampling: Sampling | None = None, on_text=None, stop=None, min_p=None,
+                        presence_penalty=None, frequency_penalty=None) -> GenerateResult:
         """cl_generate_stream: on_text(text_delta: str, ids: list[int]) is called on this thread as tokens arrive;
-        a truthy return cancels the request."""
+        a truthy return cancels the request.  With stop / min_p / presence_penalty / frequency_penalty the request goes over
+        the byte-level handler (_generate_wire): ids are then [] and the result has done_reason only."""
+        ext = _ext_kwargs(stop, min_p, presence_penalty, frequency_penalty)
+        if ext:
+            return self._generate_wire(model, prompt, sampling, ext, on_text or (lambda d, i: False))
         r = Result()
         p = prompt.encode("utf-8")
 
@@ -908,6 +1022,24 @@ def op_sample(logits, samplings, histories, steps, device=0):
     out = np.empty(rows, np.int32)
     _check(lib().cl_op_sample(device, _ptr(lg), rows, lg.shape[1], sp, _ptr(hist), _ptr(nh), stride, _ptr(st), _ptr(out)),
            "cl_op_sample")
+    return out
+
+
+def op_sample_ext(logits, samplings, exts, histories, steps, device=0):
+    """cl_op_sample_ext: op_sample where row r also applies exts[r] (a SamplingExt, or None for all zero)."""
+    lg = np.ascontiguousarray(np.atleast_2d(logits), dtype=np.float32)
+    rows = lg.shape[0]
+    stride = max(1, max(len(h) for h in histories))
+    hist = np.zeros((rows, stride), np.int32)
+    for r, h in enumerate(histories):
+        hist[r, :len(h)] = np.asarray(h, np.int32)
+    nh = np.ascontiguousarray([len(h) for h in histories], dtype=np.int32)
+    st = np.ascontiguousarray(steps, dtype=np.uint64)
+    sp = (Sampling * rows)(*samplings)
+    xs = (SamplingExt * rows)(*[x if x is not None else SamplingExt() for x in exts])
+    out = np.empty(rows, np.int32)
+    _check(lib().cl_op_sample_ext(device, _ptr(lg), rows, lg.shape[1], sp, xs, _ptr(hist), _ptr(nh), stride, _ptr(st), _ptr(out)),
+           "cl_op_sample_ext")
     return out
 
 

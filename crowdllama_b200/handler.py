@@ -50,6 +50,13 @@ def merge_sampling(base: "eng.Sampling | None", options) -> "eng.Sampling | None
     return s
 
 
+def _needs_ext(options) -> bool:
+    """The request sets one of Ollama's options that cl_sampling cannot carry (cl_sampling_ext: stop, min_p, presence_penalty,
+    frequency_penalty); merge_sampling leaves them to libclengine, whose apply_options reads them off the wire."""
+    return options is not None and (bool(options.stop) or any(getattr(options, k) is not None
+                                                                for k in ("min_p", "presence_penalty", "frequency_penalty")))
+
+
 def _response(model: str, text: str, done: bool, done_reason: str = "") -> BaseMessage:
     now = time.time_ns()
     return BaseMessage(generate_response=GenerateResponse(
@@ -71,12 +78,13 @@ def worker_api_handler(engine: "eng.Engine", sampling: "eng.Sampling | None" = N
         return generate_req
 
     def _raw(generate_req) -> bool:
-        # raw = "do not apply the chat template" and logprobs: only the byte-level entry points of libclengine carry them,
-        # so such requests take that path instead of assembling frames a second way here
+        # raw = "do not apply the chat template", logprobs, stop, min_p and the presence / frequency penalties: only the
+        # byte-level entry points of libclengine carry them, so such requests take that path instead of assembling frames
+        # (and cutting text at a stop) a second way here
         o = generate_req.options
-        if o is not None and (o.logprobs or o.top_logprobs is not None):
+        if o is not None and (o.logprobs or o.top_logprobs is not None or _needs_ext(o)):
             if not hasattr(engine, "handle_message_stream"):
-                raise HandlerError("logprobs need the byte-level engine entry points")
+                raise HandlerError("logprobs, stop, min_p and the presence / frequency penalties need the byte-level engine entry points")
             return True
         return bool(o and o.raw and hasattr(engine, "handle_message_stream"))
 

@@ -17,7 +17,9 @@ FIELDS = {
     "GenerateOptions": {"seed": 1, "temperature": 2, "top_k": 3, "top_p": 4, "repeat_penalty": 5, "repeat_last_n": 6,
                         "num_predict": 7, "raw": 8,
                         # EXTENSION: Ollama's top-level `logprobs` / `top_logprobs` (0..20) of a request
-                        "logprobs": 9, "top_logprobs": 10},
+                        "logprobs": 9, "top_logprobs": 10,
+                        # EXTENSION: Ollama's stop (repeated string), min_p, presence_penalty and frequency_penalty
+                        "stop": 11, "min_p": 12, "presence_penalty": 13, "frequency_penalty": 14},
     "GenerateResponse": {"model": 1, "created_at": 2, "response": 3, "done": 4, "done_reason": 5, "worker_id": 6,
                          "total_duration": 7,
                          "logprobs": 8},          # EXTENSION: repeated TokenLogprob, one per token of this frame
@@ -81,7 +83,7 @@ def _fields(b: bytes):
 
 import struct
 
-_OPT_FLOAT = ("temperature", "top_p", "repeat_penalty")
+_OPT_FLOAT = ("temperature", "top_p", "repeat_penalty", "min_p", "presence_penalty", "frequency_penalty")
 
 
 @dataclass
@@ -97,6 +99,10 @@ class GenerateOptions:
     raw: bool | None = None
     logprobs: bool | None = None
     top_logprobs: int | None = None
+    stop: list | None = None            # of str
+    min_p: float | None = None
+    presence_penalty: float | None = None
+    frequency_penalty: float | None = None
 
     def encode(self) -> bytes:
         F, out = FIELDS["GenerateOptions"], b""
@@ -104,7 +110,10 @@ class GenerateOptions:
             v = getattr(self, name)
             if v is None:
                 continue
-            if name in _OPT_FLOAT:
+            if name == "stop":
+                for t in v:
+                    out += _ld(fno, t.encode("utf-8"))
+            elif name in _OPT_FLOAT:
                 out += _varint(fno << 3 | 5) + struct.pack("<f", float(v))
             else:
                 out += _varint(fno << 3) + _varint(int(v))
@@ -118,7 +127,9 @@ class GenerateOptions:
             name = by_no.get(f)
             if name is None:
                 continue
-            if name in _OPT_FLOAT and wt == 5:
+            if name == "stop" and wt == 2:
+                m.stop = (m.stop or []) + [v.decode("utf-8", "replace")]
+            elif name in _OPT_FLOAT and wt == 5:
                 setattr(m, name, struct.unpack("<f", v)[0])
             elif name not in _OPT_FLOAT and wt == 0:
                 if name in ("raw", "logprobs"):
@@ -141,6 +152,8 @@ class GenerateOptions:
         for k in _OPT_FLOAT:
             if d.get(k) is not None:
                 setattr(m, k, float(d[k]))
+        if d.get("stop") is not None:   # a list of strings (a lone string is taken as a list of one)
+            m.stop = [d["stop"]] if isinstance(d["stop"], str) else [str(t) for t in d["stop"]]
         return m
 
     def is_empty(self) -> bool:

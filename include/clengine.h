@@ -136,12 +136,23 @@ typedef struct cl_engine_config {
 
 /* Sampler.  The reference sends no options (api.go:109-118), so Ollama defaults apply upstream:
  * temperature 0.8, top_k 40, top_p 0.9, repeat_penalty 1.1 over the last 64 tokens, random seed.
- * temperature <= 0 selects greedy argmax with lowest-index tie-break (the parity mode).
- * Where the draw runs: with temperature > 0, 1 <= top_k <= 128, top_k < vocab_size, vocab_size <= 163840, and the repeat
- * penalty off (repeat_penalty 1 or repeat_last_n 0) or over 1..256 ids, the decode step's last kernel draws the token on
- * the GPU, so the token loop never waits for the host (Ollama's defaults qualify).  Other settings (top_k 0,
- * repeat_last_n -1, ...) run the host sampler on the step's logits.  Both draw the same id for the same logits, history,
- * seed and step (cl_sample_token is the host one; env CL_DEVICE_SAMPLE=0 sends every request to it). */
+ * temperature <= 0 selects greedy argmax with lowest-index tie-break (the parity mode) and ignores every stage below.
+ * The stages, in order (cl_sampling_ext adds the presence / frequency penalties and min_p):
+ *   1. penalty stage over the last repeat_last_n ids of the history (out-of-range ids skipped): an id occurring c > 0
+ *      times there gets v / repeat_penalty (v > 0) or v * repeat_penalty, then v -= c * frequency_penalty +
+ *      presence_penalty (llama.cpp's formula, in fp32);
+ *   2. top-k (value descending, id ascending);  3. softmax at `temperature` (p_i = exp((v_i - v_0) / T) in double);
+ *   4. top-p: the shortest leading run whose normalised mass reaches top_p;
+ *   5. min_p: of those, the leading candidates with p_i >= min_p * p_0 (the top candidate always stays);
+ *   6. one draw from the counter-based generator at (seed, step).
+ * This order follows Ollama's own sampler (top-k, temperature, softmax, top-p, min-p).  Like the rest of the chain it is
+ * unpinned: it was not checked draw for draw against Ollama's binary.
+ * Where the draw runs: with temperature > 0, 1 <= top_k <= 128, top_k < vocab_size, vocab_size <= 163840, and the penalty
+ * stage off (repeat_penalty 1 and both other penalties 0, or repeat_last_n 0) or over 1..256 ids, the decode step's last
+ * kernel draws the token on the GPU, so the token loop never waits for the host (Ollama's defaults qualify, and so does
+ * any min_p and any finite presence / frequency penalty).  Other settings (top_k 0, repeat_last_n -1, ...) run the host
+ * sampler on the step's logits.  Both draw the same id for the same logits, history, seed and step (cl_sample_token[_ext]
+ * is the host one; env CL_DEVICE_SAMPLE=0 sends every request to it). */
 typedef struct cl_sampling {
   float temperature;
   int32_t top_k;
@@ -152,6 +163,27 @@ typedef struct cl_sampling {
   int32_t max_new_tokens;  /* num_predict; <= 0 => until EOS or context full */
   int32_t ignore_eos;      /* 1 => never stop on EOS (benchmarks) */
 } cl_sampling;
+
+/* Ollama's other generation options, kept out of cl_sampling so that its layout stays what callers compiled against.  All
+ * zero is exactly the behaviour of cl_sampling alone; every entry point that takes only a cl_sampling runs with all zero.
+ *   min_p: 0..1 (0 off), stage 5 above.  presence_penalty, frequency_penalty: any finite value (0 off), stage 1 above.
+ *   stop / n_stop: request level only (cl_generate_ids_ext).  Generation ends as soon as the response text contains one of
+ *   the strings: done_reason "stop" (over "length" on the same token), cl_result.text ends just before the earliest
+ *   occurrence.  Matched against the raw bytes of the generated ids (cl_tokenizer_decode of them, never the prompt), so a
+ *   match may span tokens and start or end inside one token's bytes.  token_ids / n_generated keep every generated id up to
+ *   and including the one that completed the match, and logprob records stay one per id: only the text is cut.  Streamed
+ *   deltas hold back any text that could still begin a stop string, so they never carry a byte of one and concatenate to
+ *   cl_result.text.  At most 16 non-empty strings (empty ones are dropped) of at most 256 bytes each.
+ * CL_ERR_INVALID_ARG, with cl_last_error set, for min_p outside [0, 1], a NaN or infinite penalty, or stops past the limits.
+ * The token-level calls know nothing of text and ignore stop / n_stop. */
+typedef struct cl_sampling_ext {
+  float min_p;
+  float presence_penalty;
+  float frequency_penalty;
+  int32_t n_stop;
+  const char* const* stop;   /* n_stop NUL-terminated strings */
+  int32_t reserved[8];
+} cl_sampling_ext;
 
 typedef struct cl_result {
   char* text;            /* NUL-terminated UTF-8, malloc'd */
@@ -232,6 +264,9 @@ void cl_greedy_sampling(cl_sampling* s, int32_t max_new_tokens);
  * (tests/test_host_logic.py pins it to the HF transformers logits processors). */
 int cl_sample_token(const float* logits, int32_t vocab, const cl_sampling* s, const int32_t* history, int32_t n_history,
                     uint64_t step, int32_t* id);
+/* cl_sample_token with the stages of cl_sampling_ext (ext may be NULL: all zero; its stop strings are ignored). */
+int cl_sample_token_ext(const float* logits, int32_t vocab, const cl_sampling* s, const cl_sampling_ext* ext, const int32_t* history,
+                        int32_t n_history, uint64_t step, int32_t* id);
 int cl_model_preset(const char* name, cl_model_config* out);
 /* The prompt-lookup drafter of speculative decoding (host only, no GPU involved): the longest suffix of hist[0..n) of
  * length 3, else 2, that also occurs earlier in hist; from its most recent earlier occurrence, the up to k ids that
@@ -296,8 +331,8 @@ int cl_generate_stream(cl_engine* e, const char* model, const char* prompt, size
  * sequence of serialised BaseMessage{GenerateResponse} frames — Done=false frames carrying text deltas, then one
  * Done=true frame with done_reason — each handed to cb (the host writes them length-prefixed to the stream,
  * pbwire.go:14-33).  Without stream: exactly one Done=true frame.  GenerateRequest.options (field 4, the proto
- * extension of §8f row 3: seed, temperature, top_k, top_p, repeat_penalty, repeat_last_n, num_predict, raw)
- * override `s` field by field in both entry points. */
+ * extension of §8f row 3: seed, temperature, top_k, top_p, repeat_penalty, repeat_last_n, num_predict, raw, and
+ * stop, min_p, presence_penalty, frequency_penalty as in cl_sampling_ext) override `s` field by field in both entry points. */
 typedef int (*cl_frame_cb)(void* user, const uint8_t* msg, size_t len);
 int cl_handle_message_stream(cl_engine* e, const uint8_t* req, size_t req_len, const cl_sampling* s,
                              cl_frame_cb cb, void* user);
@@ -431,12 +466,23 @@ int cl_seq_set_logprobs(cl_engine* e, cl_seq_t seq, int32_t top_n);
  * and cl_decode_verify[_batch] (the emitted ids).  Up to cap records go to out and are removed; *n_out = how many.
  * out == NULL: *n_out = the count pending, nothing is removed. */
 int cl_seq_take_logprobs(cl_engine* e, cl_seq_t seq, cl_token_logprob* out, int32_t cap, int32_t* n_out);
+/* Arms the sequence with min_p and the presence / frequency penalties of ext (NULL: all zero; stop strings are ignored):
+ * every later token-level call that draws for it with a cl_sampling (cl_decode_sample_batch, cl_decode_verify[_batch])
+ * applies them too, on the device, and so does the prefill tail of an armed sampler.  cl_seq_create / cl_seq_free reset
+ * it to all zero.  CL_ERR_INVALID_ARG as cl_sampling_ext states. */
+int cl_seq_set_sampling_ext(cl_engine* e, cl_seq_t seq, const cl_sampling_ext* ext);
 /* cl_generate_ids with logprobs on (top_n 0..20): *lps (malloc'd, free with cl_buffer_free) = one record per generated id,
  * out->n_generated of them.  The ids equal those of the same request through cl_generate_ids.  A host-sampled request
  * (settings the device sampler does not cover) takes lse and the top list from the device and sets logprob = logit[id] - lse
  * with the same double subtraction and fp32 rounding. */
 int cl_generate_ids_logprobs(cl_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const cl_sampling* s, int32_t top_n,
                              cl_result* out, cl_token_logprob** lps);
+/* cl_generate_ids with Ollama's remaining options: ext (may be NULL: all zero) adds min_p, the presence / frequency penalties
+ * and stop strings (cl_sampling_ext); top_n -1 = logprobs off, 0..20 = on as cl_generate_ids_logprobs (*lps then one record
+ * per generated id; lps may be NULL with top_n -1); cb (may be NULL) streams text deltas as cl_generate_stream does, the
+ * last flush with ids NULL.  With an all-zero ext the ids are those of cl_generate_ids. */
+int cl_generate_ids_ext(cl_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const cl_sampling* s, const cl_sampling_ext* ext,
+                        int32_t top_n, cl_token_cb cb, void* user, cl_result* out, cl_token_logprob** lps);
 /* Parity aid: make the sequence hold n_tokens cached tokens whose K/V, in every layer, are the CPU oracle's
  * synthetic cache pattern (oracle/llama_oracle.c oc_seq_fake_fill: k[i] = (((i * 2654435761) >> 24 & 255) - 128) / 128,
  * v[i] = (((i * 40503) >> 8 & 255) - 128) / 128 with i = token * n_kv * head_dim + head * head_dim + dim; exact in
@@ -584,6 +630,9 @@ int cl_op_sample(int device, const float* logits, int32_t n_rows, int32_t vocab,
 int cl_op_sample_logprobs(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const int32_t* history,
                           const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t top_n, int32_t* ids_out,
                           cl_token_logprob* lp_out);
+/* cl_op_sample with ext[n_rows] (may be NULL: all zero; stop strings ignored): row r also applies ext[r]'s stages. */
+int cl_op_sample_ext(int device, const float* logits, int32_t n_rows, int32_t vocab, const cl_sampling* sp, const cl_sampling_ext* ext,
+                     const int32_t* history, const int32_t* n_history, int32_t hist_stride, const uint64_t* step, int32_t* ids_out);
 /* synthetic weight generator (device kernel) -> host copy, for known-answer tests */
 int cl_op_synth_weights(int device, uint64_t seed, int32_t tensor_key, int64_t n, float scale,
                         uint16_t* out_bf16);
