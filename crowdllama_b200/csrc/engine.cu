@@ -61,15 +61,9 @@ int Engine::init(const cl_engine_config& c) {
   const std::string wpath = c.weights_path ? c.weights_path : "";
   struct stat wst{};
   const bool wdir = !wpath.empty() && stat(wpath.c_str(), &wst) == 0 && S_ISDIR(wst.st_mode);
-  if (c.preset) {
-    if (cl_model_preset(c.preset, &cfg) != CL_OK) { set_last_error("unknown preset"); return CL_ERR_UNKNOWN_MODEL; }
-  } else if (c.model.n_layers == 0 && wdir) {
-    // a model directory describes itself: config.json (HF LlamaConfig / MistralConfig field names)
-    const int rc0 = model_config_from_dir(wpath, &cfg);
-    if (rc0) return rc0;
-  } else {
-    cfg = c.model;
-  }
+  int context_length = 0;
+  const int rc0 = resolve_model_config(c, &cfg, &context_length);   // preset / config.json / c.model, the window, the num_keep check
+  if (rc0) return rc0;
   model_name = c.model_name ? c.model_name : (c.preset ? c.preset : "model");
   const int rep = cfg.n_kv_heads > 0 ? cfg.n_heads / cfg.n_kv_heads : 0;
   if (cfg.n_layers <= 0 || cfg.d_model <= 0 || cfg.n_heads <= 0 || cfg.n_kv_heads <= 0 || cfg.d_ff <= 0 ||
@@ -118,6 +112,17 @@ int Engine::init(const cl_engine_config& c) {
   const size_t kv_bytes_per_token = (size_t)2 * cfg.n_layers * kv_dim_ * 2;
   int64_t pool_bytes = c.kv_pool_bytes;
   if (pool_bytes <= 0) pool_bytes = (int64_t)max_seqs_ * max_pages_per_seq_ * page_size_ * (int64_t)kv_bytes_per_token;
+  if (c.kv_pool_bytes <= 0 && context_length > 0) {
+    // a long window: max_seqs full windows rarely fit, so the pool takes what is free after the weights (and the RoPE
+    // table), less kPoolReserveBytes for the state and the lazily allocated prefill / verify workspaces
+    size_t free_b = 0, total_b = 0;
+    CL_CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+    const int64_t d = cfg.d_model, F = cfg.d_ff, V = cfg.vocab_size;
+    const int64_t weights = 2 * (2 * V * d) + (int64_t)cfg.n_layers * 2 * ((int64_t)qkv_dim_ * d + d * q_dim_ + 3 * F * d) +
+                            (int64_t)cfg.max_seq_len * cfg.head_dim * 4;
+    const int64_t avail = (int64_t)free_b - weights - kPoolReserveBytes;
+    pool_bytes = std::min(pool_bytes, std::max<int64_t>(avail, 0));
+  }
   n_pages_ = (int)(pool_bytes / ((int64_t)page_size_ * (int64_t)kv_bytes_per_token));
   if (n_pages_ < 1) { set_last_error("kv_pool_bytes too small for one page"); return CL_ERR_INVALID_ARG; }
 
@@ -187,11 +192,7 @@ int Engine::init(const cl_engine_config& c) {
   device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
   prefix_cache_ = env_int("CL_PREFIX_CACHE", c.prefix_cache) != 0;
   context_shift_ = env_int("CL_CONTEXT_SHIFT", c.context_shift) != 0;
-  num_keep_ = env_int("CL_NUM_KEEP", c.num_keep);
-  if (context_shift_ && (num_keep_ < 0 || cfg.max_seq_len - num_keep_ < 2 * page_size_)) {
-    set_last_error("num_keep must leave at least two pages of max_seq_len to shift");
-    return CL_ERR_INVALID_ARG;
-  }
+  num_keep_ = env_int("CL_NUM_KEEP", c.num_keep);   // checked against the final window by resolve_model_config
   speculate_ = env_int("CL_SPECULATE", c.speculate);
   if (speculate_ < 0 || speculate_ > kSpecMaxDraft) { set_last_error("speculate must be 0..15"); return CL_ERR_INVALID_ARG; }
   if (speculate_ > 0 && !spec_path_ok()) {

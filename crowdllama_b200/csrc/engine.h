@@ -26,6 +26,16 @@ constexpr int kDefaultPrefillSmallMax = 256;    // CL_PREFILL_SMALL_MAX: prompts
 constexpr int kDefaultSchedMultiPrefill = 1;    // CL_SCHED_MULTI_PREFILL: scheduler admits the prompts at the head of the queue in one tile-path pass (Engine::prefill_multi)
 constexpr int kSchedLingerUs = 1000;  // burst detection before a group admission into an empty batch (Engine::wait_for_work)
 
+constexpr int kMaxContext = 131072;   // longest window cl_engine_config.context_length may ask for (Llama-3.1 / 3.2's 128K)
+// Prefill segments that end past this many tokens (the longest window served before context_length) run the split-KV
+// prefill attention; shorter ones keep their kernels and bits (Engine::attn_prefill)
+constexpr int kLongPrefillFrom = 32768;
+// the attention kernel of a multi-row pass (cl_debug_pass_info; Engine::prefill_attn_kind)
+enum { kPassAttnMma = 0, kPassAttnWgmma = 1, kPassAttnVerify = 2, kPassAttnMixed = 3, kPassAttnLong = 4 };
+// Device memory a context_length > 0 engine leaves outside its KV pool when it sizes the pool itself: the per-slot state,
+// the tile-path prefill workspace at its chunk size, the verify pass's logits (128 rows x vocab fp32) and split partials,
+// and the CUDA context's own growth; 4 GiB covers them for the 8B shapes at max_batch 8 with room to spare
+constexpr int64_t kPoolReserveBytes = 4LL << 30;
 // Speculative decoding (cl_engine_config.speculate, Engine::verify_batch, ngram_draft): the constants of the drafter.
 constexpr int kSpecMaxDraft = 15;     // drafted tokens per verify pass at most (its rows: x0 + drafts <= 16)
 constexpr int kDraftNgramMax = 3;     // the drafter matches the history's last 3 ids, then its last 2
@@ -236,7 +246,8 @@ class ByteTokenizer : public Tokenizer {
 std::unique_ptr<Tokenizer> load_hf_tokenizer(const std::string& path, const std::string& chat_family, std::string* err);
 
 // HF config.json of a model directory -> cl_model_config (weights_io.cpp)
-int model_config_from_dir(const std::string& dir, cl_model_config* out);
+int model_config_from_dir(const std::string& dir, cl_model_config* out, double* limits);
+int resolve_model_config(const cl_engine_config& c, cl_model_config* out, int* context_length);   // cl_resolve_model_config
 
 // ---- sampler (host; mirrors oracle oc_sample) ---------------------------------------------------
 // inverse rotary frequency of dimension pair i: theta^(-2i/head_dim), with the "llama3" scaling of cl_model_config when
@@ -476,11 +487,11 @@ class Engine {
   // one tile-path pass of T rows made of n_segs segments; leaves the final residual rows in pws_->h
   int prefill_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, int& launches, LaunchProfiler& prof);
   int attn_prefill(const AttnPrefillArgs& a, int layer, int& launches, LaunchProfiler& prof);   // the one choice of prefill attention kernel
-  int prefill_attn_kind(int pos0, int n) const;   // the kernel attn_prefill runs for n rows from pos0: kPassAttnMma / kPassAttnWgmma
+  int prefill_attn_kind(int pos0, int n) const;   // the kernel attn_prefill runs for n rows from pos0: kPassAttnMma / Wgmma / Verify / Long
+  int ensure_long_attn_ws();                      // the split workspace of the segments that end past kLongPrefillFrom
   // What the latest multi-row pass was, on the host (debug_pass_info / debug_pass_rows); T == 0: no pass whose rows the
   // workspace holds (none yet, a token-wise prefill since, or a failed pass).  Recording adds no device work.
   enum { kPassSplitK = 0, kPassTile = 1 };
-  enum { kPassAttnMma = 0, kPassAttnWgmma = 1, kPassAttnVerify = 2, kPassAttnMixed = 3 };
   struct PassRecord { int path = -1, attn = -1, T = 0; std::vector<PrefillSegment> segs; };
   void record_pass(int path, bool multi_row, const PrefillSegment* segs, int n_segs, int T);
   PassRecord pass_;
@@ -577,6 +588,9 @@ class Engine {
   struct SmallPrefillWs { float* part = nullptr; __nv_bfloat16* xn = nullptr; __nv_bfloat16* q = nullptr; __nv_bfloat16* attn = nullptr;
                           float* h = nullptr; __nv_bfloat16* act = nullptr; int* iota = nullptr; };
   std::unique_ptr<SmallPrefillWs> sws_;
+  float* long_part_ = nullptr;        // split-KV partials of the long-context prefill kernel (lazily, attn_prefill)
+  unsigned* long_cnt_ = nullptr;      // its arrival counters, zero between launches
+  int* long_seg_ = nullptr;           // the one-segment table of a long segment run by the multi-row verify kernel
   // verify passes (allocated lazily): rows of at most kSpecMaxRows; out holds 1 + T ints per sequence, row_map [2][rows];
   // segs [rows][8], attn_part and attn_cnt: the multi-row attention's segment table, split partials and counters
   struct SpecWs { float* logits = nullptr; int* choice = nullptr; float* part_val = nullptr; int* part_idx = nullptr;

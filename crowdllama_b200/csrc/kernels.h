@@ -291,6 +291,17 @@ int launch_attn_prefill(const AttnPrefillArgs& a, cudaStream_t st);
 // wgmma variant (attn_prefill_tc.cu): head_dim 128, page 32; kmap / vmap = pool-wide 2-D tensor maps (box {64, 32})
 bool attn_prefill_tc_supported(int n_heads, int n_kv, int head_dim, int page_size, int pos0, int T);
 int launch_attn_prefill_tc(const AttnPrefillArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st);
+// split-KV wgmma variant for any length (attn_prefill_tc.cu, "variant 2"): same shapes, block table read from global memory,
+// work items (head, 128-row tile, KV split).  nsplit > 1 needs part (attn_prefill_long_part_floats(sms) floats cover every
+// automatic plan; a forced plan needs tiles x n_heads x nsplit x 128 x 130) and counters (one per tile x head, zero before
+// the first launch; the kernel re-arms them).
+constexpr int kAttnLongMinSplitBlocks = 32;   // KV blocks of 64 tokens per split, at least, in an automatic plan
+bool attn_prefill_long_supported(int n_heads, int n_kv, int head_dim, int page_size);
+int attn_prefill_long_splits(int pos0, int T, int n_heads, int sms, int force);
+size_t attn_prefill_long_part_floats(int sms);
+size_t attn_prefill_long_counters(int sms);
+int launch_attn_prefill_long(const AttnPrefillArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, int nsplit,
+                             float* part, unsigned* counters, cudaStream_t st);
 // multi-row split-KV attention (attn_verify_tc.cu): segment s holds len_s cached tokens and R_s <= kVerifyMaxRows new rows at
 // positions len_s .. len_s + R_s - 1 (their K/V already in the pages); row r sees keys < len_s + r + 1
 constexpr int kVerifyMaxRows = 16;

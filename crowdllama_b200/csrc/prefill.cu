@@ -31,19 +31,76 @@ static int ws_alloc(std::vector<void*>& allocs, T*& p, size_t bytes) {
   return CL_OK;
 }
 
-// Causal attention of one prefill segment in layer l: the wgmma kernel where it applies (head_dim 128, page 32, the pool's
-// tensor maps), the mma.sync kernel otherwise.
+// A prefill segment of at most kVerifyMaxRows rows as the one segment of the multi-row split-KV attention of verify passes
+// (attn_verify_tc.cu): every split covers split_pages pages.  seg_dev: 8 ints of device memory for the segment table;
+// part / counters: the kernel's split workspace (counters zero between launches, the kernel re-arms them).
+static int launch_attn_prefill_as_verify(const AttnPrefillArgs& a, const CUtensorMap& km, const CUtensorMap& vm, long long row0,
+                                         int split_pages, int* seg_dev, float* part, unsigned* counters, cudaStream_t st) {
+  const int pages = (a.pos0 + a.T + a.page_size - 1) / a.page_size;
+  const int ns = (pages + split_pages - 1) / split_pages;
+  const int seg[8] = {0, 0, a.T, a.pos0, 0, ns, 0, 0};   // block-table row, first row, rows, cached length, partial offset, splits
+  if (cudaMemcpyAsync(seg_dev, seg, sizeof seg, cudaMemcpyHostToDevice, st) != cudaSuccess) return -1;
+  AttnVerifyArgs va;
+  va.q = a.q; va.q_stride = a.n_heads * a.head_dim; va.segs = seg_dev; va.block_tables = a.block_table; va.bt_stride = 0;
+  va.out = a.out; va.out_stride = a.n_heads * a.head_dim; va.part = part; va.counters = counters;
+  va.n_segs = 1; va.n_heads = a.n_heads; va.n_kv = a.n_kv; va.head_dim = a.head_dim; va.page_size = a.page_size;
+  va.nsplit = ns; va.split_pages = split_pages;
+  return launch_attn_verify_tc(va, km, vm, row0, st);
+}
+
+// Causal attention of one prefill segment in layer l.  Segments that end within kLongPrefillFrom tokens run what they always
+// have: the wgmma kernel where it applies (head_dim 128, page 32, the pool's tensor maps, up to its 10240-token block-table
+// limit), the mma.sync kernel otherwise.  Segments that end past it spread over every SM: up to kVerifyMaxRows rows (a
+// single-sequence verify pass, a short prompt's last rows) through the multi-row split-KV kernel of verify passes, longer
+// ones through the split-KV wgmma prefill kernel, where the shape allows; other shapes keep the mma.sync kernel.
 int Engine::attn_prefill(const AttnPrefillArgs& a, int l, int& launches, LaunchProfiler& prof) {
-  if (prefill_attn_kind(a.pos0, a.T) == kPassAttnWgmma)
-    CL_LAUNCH(launch_attn_prefill_tc(a, kmap_, vmap_, (long long)l * n_pages_ * cfg.n_kv_heads * page_size_, stream_));
-  else
+  const long long row0 = (long long)l * n_pages_ * cfg.n_kv_heads * page_size_;
+  const int kind = prefill_attn_kind(a.pos0, a.T);
+  if (kind == kPassAttnLong || kind == kPassAttnVerify) {
+    const int rc = ensure_long_attn_ws();
+    if (rc) return rc;
+  }
+  if (kind == kPassAttnVerify) {
+    CL_LAUNCH(launch_attn_prefill_as_verify(a, kmap_, vmap_, row0, verify_split_pages(), long_seg_, long_part_, long_cnt_, stream_));
+  } else if (kind == kPassAttnLong) {
+    const int ns = attn_prefill_long_splits(a.pos0, a.T, a.n_heads, sm_count(), 0);
+    CL_LAUNCH(launch_attn_prefill_long(a, kmap_, vmap_, row0, ns, long_part_, long_cnt_, stream_));
+  } else if (kind == kPassAttnWgmma) {
+    CL_LAUNCH(launch_attn_prefill_tc(a, kmap_, vmap_, row0, stream_));
+  } else {
     CL_LAUNCH(launch_attn_prefill(a, stream_));
+  }
   return CL_OK;
 }
 
+// The rule of attn_prefill, shared with cl_op_attn_prefill_long's variant -1.  maps: the pool's K / V tensor maps exist.
+static int prefill_attn_rule(int n_heads, int n_kv, int head_dim, int page_size, int pos0, int n, bool maps) {
+  if (pos0 + n > kLongPrefillFrom) {
+    if (maps && n <= kVerifyMaxRows && attn_verify_tc_supported(n_heads, n_kv, head_dim, page_size)) return kPassAttnVerify;
+    return maps && attn_prefill_long_supported(n_heads, n_kv, head_dim, page_size) ? kPassAttnLong : kPassAttnMma;
+  }
+  return maps && attn_prefill_tc_supported(n_heads, n_kv, head_dim, page_size, pos0, n) ? kPassAttnWgmma : kPassAttnMma;
+}
+
 int Engine::prefill_attn_kind(int pos0, int n) const {
-  return have_kv_maps_ && attn_prefill_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, pos0, n) ? kPassAttnWgmma
-                                                                                                                     : kPassAttnMma;
+  return prefill_attn_rule(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, page_size_, pos0, n, have_kv_maps_);
+}
+
+// The split workspace of both long-segment kernels (they run in stream order, and each leaves its counters at zero):
+// the split-KV prefill kernel's automatic plans, and the multi-row kernel's 4 x kVerifyMaxRows rows per kv head and split.
+static size_t verify_part_floats(int n_kv, int head_dim) {
+  return (size_t)4 * kVerifyMaxRows * n_kv * attn_verify_max_splits() * (head_dim + 2);
+}
+
+int Engine::ensure_long_attn_ws() {
+  if (long_part_) return CL_OK;
+  const size_t n_cnt = std::max(attn_prefill_long_counters(sm_count()), (size_t)cfg.n_kv_heads);
+  const size_t n_part = std::max(attn_prefill_long_part_floats(sm_count()), verify_part_floats(cfg.n_kv_heads, cfg.head_dim));
+  int rc;
+  if ((rc = ws_alloc(allocs_, long_seg_, 8 * 4)) || (rc = ws_alloc(allocs_, long_cnt_, n_cnt * 4)) ||
+      (rc = ws_alloc(allocs_, long_part_, n_part * 4))) { long_part_ = nullptr; return rc; }
+  CL_CUDA_OK(cudaMemsetAsync(long_cnt_, 0, n_cnt * 4, stream_));
+  return CL_OK;
 }
 
 // The record of a pass that completed: its path, its segments and the attention kernel they ran (kPassAttnMixed when the
@@ -607,11 +664,15 @@ int cl_op_gemm_bf16(int device, const uint16_t* x, const uint16_t* w, float* y, 
 }
 
 // Causal attention of the queries at positions pos0 .. pos0 + t - 1 (q [t][n_heads * head_dim]) over keys 0 .. pos0 + t - 1
-// (k, v [pos0 + t][n_kv][head_dim]), paged by op_build_kv_pool.  variant: -1 the engine's rule (Engine::attn_prefill: the wgmma
-// kernel when it takes the shape), 0 mma.sync kernel, 1 wgmma kernel.  out [t][n_heads * head_dim] = the kernel's bf16 output.
+// (k, v [pos0 + t][n_kv][head_dim]), paged by op_build_kv_pool.  variant: -1 the engine's rule (Engine::attn_prefill; past
+// kLongPrefillFrom its multi-row kernel takes every split over max(8, ceil(pages / 64)) pages, as cl_op_attn_verify does),
+// 0 mma.sync kernel, 1 wgmma kernel, 2 split-KV wgmma kernel (nsplit 0: its own plan, > 0: forced, clamped to what the
+// shape allows).  out [t][n_heads * head_dim] = the kernel's bf16 output.  The split kernels run twice without re-arming
+// their counters and the call fails with CL_ERR_INTERNAL when the two outputs differ in any bit.
 static int attn_prefill_impl(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0, int32_t t,
-                             int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int iters, float* out, float* ms) {
-  if (!q || !k || !v || !out || t <= 0 || pos0 < 0 || variant < -1 || variant > 1) return CL_ERR_INVALID_ARG;
+                             int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int nsplit, int iters, float* out, float* ms,
+                             int32_t* nsplit_used = nullptr, int32_t* kind_used = nullptr) {
+  if (!q || !k || !v || !out || t <= 0 || pos0 < 0 || variant < -1 || variant > 2 || nsplit < 0) return CL_ERR_INVALID_ARG;
   int rc = check_device(device);
   if (rc) return rc;
   if ((head_dim != 64 && head_dim != 128) || n_kv <= 0 || n_heads % n_kv || (page_size != 16 && page_size != 32 && page_size != 64)) {
@@ -619,10 +680,18 @@ static int attn_prefill_impl(int device, int variant, const uint16_t* q, const u
     return CL_ERR_INVALID_ARG;
   }
   const int P = page_size, HD = head_dim, n_tok = pos0 + t;
+  int kind = variant == -1 ? prefill_attn_rule(n_heads, n_kv, HD, P, pos0, t, true)
+                           : variant == 2 ? kPassAttnLong : variant == 1 ? kPassAttnWgmma : kPassAttnMma;
+  if (kind == kPassAttnWgmma && !attn_prefill_tc_supported(n_heads, n_kv, HD, P, pos0, t)) {
+    set_last_error("wgmma prefill attention does not support this shape"); return CL_ERR_INVALID_ARG;
+  }
+  if (kind == kPassAttnLong && !attn_prefill_long_supported(n_heads, n_kv, HD, P)) {
+    set_last_error("split-KV prefill attention does not support this shape"); return CL_ERR_INVALID_ARG;
+  }
   OpKvPool pool;
   op_build_kv_pool(k, v, &n_tok, 1, n_kv, HD, P, &pool);
   const size_t qd = (size_t)n_heads * HD;
-  DevBuf dq, dk, dv, dbt, dout, dout32;
+  DevBuf dq, dk, dv, dbt, dout, dout32, dpart, dcnt, dseg;
   CL_CUDA_OK(dq.upload(q, (size_t)t * qd * 2));
   CL_CUDA_OK(dk.upload(pool.k.data(), pool.k.size() * 2));
   CL_CUDA_OK(dv.upload(pool.v.data(), pool.v.size() * 2));
@@ -634,14 +703,50 @@ static int attn_prefill_impl(int device, int variant, const uint16_t* q, const u
                     dbt.as<int>(), P, pos0, t, n_heads, n_kv, HD, dout.as<__nv_bfloat16>()};
   const long long pool_rows = 2LL * pool.n_pages * n_kv * P;
   CUtensorMap km, vm;
-  bool tc = variant != 0 && attn_prefill_tc_supported(n_heads, n_kv, HD, P, pos0, t);
-  if (tc) tc = make_tmap_2d_bf16(&km, dk.p, pool_rows, HD, 64, 32) && make_tmap_2d_bf16(&vm, dv.p, pool_rows, HD, 64, 32);
-  if (variant == 1 && !tc) { set_last_error("wgmma prefill attention does not support this shape"); return CL_ERR_INVALID_ARG; }
-  auto run = [&]() { return tc ? launch_attn_prefill_tc(a, km, vm, pool_rows / 2, nullptr) : launch_attn_prefill(a, nullptr); };
+  if (kind != kPassAttnMma &&
+      !(make_tmap_2d_bf16(&km, dk.p, pool_rows, HD, 64, 32) && make_tmap_2d_bf16(&vm, dv.p, pool_rows, HD, 64, 32))) {
+    if (variant != -1) { set_last_error("wgmma prefill attention does not support this shape"); return CL_ERR_INVALID_ARG; }
+    kind = kPassAttnMma;   // the engine's rule without tensor maps
+  }
+  const int pages = (n_tok + P - 1) / P;
+  const int split_pages = std::max(8, (pages + attn_verify_max_splits() - 1) / attn_verify_max_splits());
+  const int ns = kind == kPassAttnLong ? attn_prefill_long_splits(pos0, t, n_heads, sm_count(), nsplit)
+                 : kind == kPassAttnVerify ? (pages + split_pages - 1) / split_pages : 1;
+  if (kind == kPassAttnLong && ns > 1) {
+    const size_t items = (size_t)((t + 127) / 128) * n_heads;
+    CL_CUDA_OK(dpart.alloc(items * ns * 128 * (HD + 2) * 4));
+    CL_CUDA_OK(dcnt.alloc(items * 4));
+    CL_CUDA_OK(cudaMemset(dcnt.p, 0, items * 4));
+  }
+  if (kind == kPassAttnVerify) {
+    CL_CUDA_OK(dpart.alloc((size_t)4 * t * n_kv * ns * (HD + 2) * 4));
+    CL_CUDA_OK(dcnt.alloc((size_t)n_kv * 4));
+    CL_CUDA_OK(cudaMemset(dcnt.p, 0, (size_t)n_kv * 4));
+    CL_CUDA_OK(dseg.alloc(8 * 4));
+  }
+  auto run = [&]() {
+    if (kind == kPassAttnVerify)
+      return launch_attn_prefill_as_verify(a, km, vm, pool_rows / 2, split_pages, dseg.as<int>(), dpart.as<float>(), dcnt.as<unsigned>(),
+                                           nullptr);
+    if (kind == kPassAttnLong)
+      return launch_attn_prefill_long(a, km, vm, pool_rows / 2, ns, dpart.as<float>(), dcnt.as<unsigned>(), nullptr);
+    return kind == kPassAttnWgmma ? launch_attn_prefill_tc(a, km, vm, pool_rows / 2, nullptr) : launch_attn_prefill(a, nullptr);
+  };
   if (run() < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("prefill attention launch failed"); return CL_ERR_CUDA; }
   if (launch_bf16_to_f32(dout.as<__nv_bfloat16>(), dout32.as<float>(), (int64_t)t * qd, nullptr) < 0) return CL_ERR_CUDA;
   CL_CUDA_OK(cudaDeviceSynchronize());
   CL_CUDA_OK(cudaMemcpy(out, dout32.p, (size_t)t * qd * 4, cudaMemcpyDeviceToHost));
+  if (nsplit_used) *nsplit_used = ns;
+  if (kind_used) *kind_used = kind;
+  if (kind == kPassAttnLong || kind == kPassAttnVerify) {   // a second launch on counters the first one re-armed: the same bits
+    std::vector<uint16_t> first((size_t)t * qd), again((size_t)t * qd);
+    CL_CUDA_OK(cudaMemcpy(first.data(), dout.p, first.size() * 2, cudaMemcpyDeviceToHost));
+    CL_CUDA_OK(cudaMemset(dout.p, 0xff, (size_t)t * qd * 2));
+    if (run() < 0) { CL_CUDA_OK(cudaGetLastError()); set_last_error("prefill attention launch failed"); return CL_ERR_CUDA; }
+    CL_CUDA_OK(cudaDeviceSynchronize());
+    CL_CUDA_OK(cudaMemcpy(again.data(), dout.p, again.size() * 2, cudaMemcpyDeviceToHost));
+    if (first != again) { set_last_error("split-KV attention: a second launch differs from the first"); return CL_ERR_INTERNAL; }
+  }
   if (iters > 0 && ms) {
     cudaEvent_t e0, e1;
     CL_CUDA_OK(cudaEventCreate(&e0));
@@ -663,15 +768,28 @@ static int attn_prefill_impl(int device, int variant, const uint16_t* q, const u
 
 int cl_op_attn_prefill(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t, int32_t n_heads, int32_t n_kv,
                        int32_t head_dim, float* out) {
-  return attn_prefill_impl(device, -1, q, k, v, 0, t, n_heads, n_kv, head_dim, 32, 0, out, nullptr);
+  return attn_prefill_impl(device, -1, q, k, v, 0, t, n_heads, n_kv, head_dim, 32, 0, 0, out, nullptr);
 }
 int cl_op_attn_prefill_variant(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t, int32_t n_heads,
                                int32_t n_kv, int32_t head_dim, float* out, int32_t iters, float* ms) {
-  return attn_prefill_impl(device, variant, q, k, v, 0, t, n_heads, n_kv, head_dim, 32, iters, out, ms);
+  return attn_prefill_impl(device, variant, q, k, v, 0, t, n_heads, n_kv, head_dim, 32, 0, iters, out, ms);
 }
 int cl_op_attn_prefill_cached(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0, int32_t t,
                               int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, float* out) {
-  return attn_prefill_impl(device, variant, q, k, v, pos0, t, n_heads, n_kv, head_dim, page_size, 0, out, nullptr);
+  return attn_prefill_impl(device, variant, q, k, v, pos0, t, n_heads, n_kv, head_dim, page_size, 0, 0, out, nullptr);
+}
+int cl_op_attn_prefill_long(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0, int32_t t,
+                            int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit, int32_t iters, float* out,
+                            float* ms, int32_t* nsplit_used, int32_t* kind_used) {
+  return attn_prefill_impl(device, variant, q, k, v, pos0, t, n_heads, n_kv, head_dim, page_size, nsplit, iters, out, ms, nsplit_used,
+                           kind_used);
+}
+int cl_attn_prefill_long_plan(int32_t pos0, int32_t t, int32_t n_heads, int32_t sms, int32_t nsplit, int32_t* nsplit_used,
+                              int64_t* part_floats) {
+  if (!nsplit_used || t <= 0 || pos0 < 0 || n_heads <= 0 || sms <= 0 || nsplit < 0) return CL_ERR_INVALID_ARG;
+  *nsplit_used = attn_prefill_long_splits(pos0, t, n_heads, sms, nsplit);
+  if (part_floats) *part_floats = (int64_t)attn_prefill_long_part_floats(sms);
+  return CL_OK;
 }
 
 }  // extern "C"

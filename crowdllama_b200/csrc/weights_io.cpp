@@ -110,8 +110,9 @@ bool read_text(const std::string& path, std::string* out) {
 }
 }  // namespace
 
-// HF config.json -> cl_model_config (LlamaConfig / MistralConfig field names)
-int model_config_from_dir(const std::string& dir, cl_model_config* out) {
+// HF config.json -> cl_model_config (LlamaConfig / MistralConfig field names).  limits (may be NULL): the longest window
+// the checkpoint allows, {max_position_embeddings, sliding_window or 0}.
+int model_config_from_dir(const std::string& dir, cl_model_config* out, double* limits) {
   std::string text;
   if (!read_text(dir + "/config.json", &text)) { set_last_error("weights_path: no config.json in " + dir + " (pass a preset or a model config)"); return CL_ERR_IO; }
   JParser jp{text.data(), text.data() + text.size(), {}};
@@ -169,6 +170,7 @@ int model_config_from_dir(const std::string& dir, cl_model_config* out) {
   }
   const double window = num("sliding_window", 0.0);
   if (window >= 1.0 && window < (double)c.max_seq_len) c.max_seq_len = (int)window;
+  if (limits) { limits[0] = num("max_position_embeddings", 8192); limits[1] = window >= 1.0 ? window : 0.0; }
   if (c.n_layers <= 0 || c.d_model <= 0 || c.n_heads <= 0 || c.d_ff <= 0 || c.vocab_size <= 0) {
     set_last_error("config.json: missing llama-family fields (num_hidden_layers, hidden_size, num_attention_heads, intermediate_size, vocab_size)");
     return CL_ERR_IO;
@@ -303,7 +305,66 @@ int Engine::load_safetensors(const std::string& path) {
   return visit_checkpoint(path, cfg, [this](int layer, int kind, const uint16_t* bf, int64_t n) { return set_tensor(layer, kind, bf, n); });
 }
 
+// The model config and served window of an engine config (cl_engine_create / cl_resolve_model_config): the one place that
+// reads context_length and CL_CONTEXT_LENGTH.  *context_length (may be NULL): the value applied, 0 for the model's window.
+int resolve_model_config(const cl_engine_config& c, cl_model_config* out, int* context_length) {
+  cl_model_config cfg{};
+  double limits[2] = {0.0, 0.0};   // a model directory's max_position_embeddings and sliding window; 0: no limit
+  const std::string wpath = c.weights_path ? c.weights_path : "";
+  struct stat wst{};
+  const bool wdir = !wpath.empty() && stat(wpath.c_str(), &wst) == 0 && S_ISDIR(wst.st_mode);
+  if (c.preset) {
+    if (cl_model_preset(c.preset, &cfg) != CL_OK) { set_last_error("unknown preset"); return CL_ERR_UNKNOWN_MODEL; }
+  } else if (c.model.n_layers == 0 && wdir) {
+    // a model directory describes itself: config.json (HF LlamaConfig / MistralConfig field names)
+    const int rc = model_config_from_dir(wpath, &cfg, limits);
+    if (rc) return rc;
+  } else {
+    cfg = c.model;
+  }
+  const char* env = getenv("CL_CONTEXT_LENGTH");
+  const int ctx = env && *env ? atoi(env) : c.context_length;
+  const int page = c.page_size ? c.page_size : 32;
+  if (ctx != 0) {
+    if (ctx < 2 * page || ctx > kMaxContext) {
+      set_last_error("context_length " + std::to_string(ctx) + " is outside " + std::to_string(2 * page) + " .. " + std::to_string(kMaxContext));
+      return CL_ERR_INVALID_ARG;
+    }
+    if (limits[0] > 0.0 && ctx > limits[0]) {
+      set_last_error("context_length " + std::to_string(ctx) + " exceeds the model's max_position_embeddings (" + std::to_string((long long)limits[0]) + ")");
+      return CL_ERR_INVALID_ARG;
+    }
+    if (limits[1] > 0.0 && ctx > limits[1]) {
+      set_last_error("context_length " + std::to_string(ctx) + " exceeds the model's sliding_window (" + std::to_string((long long)limits[1]) + ")");
+      return CL_ERR_INVALID_ARG;
+    }
+    cfg.max_seq_len = ctx;
+  }
+  const char* shift = getenv("CL_CONTEXT_SHIFT");
+  const char* keep = getenv("CL_NUM_KEEP");
+  const bool context_shift = (shift && *shift ? atoi(shift) : c.context_shift) != 0;
+  const int num_keep = keep && *keep ? atoi(keep) : c.num_keep;
+  if (context_shift && (num_keep < 0 || cfg.max_seq_len - num_keep < 2 * page)) {
+    set_last_error("num_keep must leave at least two pages of max_seq_len to shift");
+    return CL_ERR_INVALID_ARG;
+  }
+  *out = cfg;
+  if (context_length) *context_length = ctx;
+  return CL_OK;
+}
+
 }  // namespace cl
+
+extern "C" int cl_resolve_model_config(const cl_engine_config* c, cl_model_config* out) {
+  if (!c || !out) return CL_ERR_INVALID_ARG;
+  if (c->abi_version != CL_ABI_VERSION) { cl::set_last_error("abi_version mismatch"); return CL_ERR_INVALID_ARG; }
+  try {
+    return cl::resolve_model_config(*c, out, nullptr);
+  } catch (const std::exception& ex) {
+    cl::set_last_error(ex.what());
+    return CL_ERR_INTERNAL;
+  }
+}
 
 extern "C" int cl_checkpoint_info(const char* path, cl_model_config* cfg_io, int32_t* n_tensors, int64_t* n_params) {
   using namespace cl;
@@ -312,7 +373,7 @@ extern "C" int cl_checkpoint_info(const char* path, cl_model_config* cfg_io, int
     struct stat st{};
     if (cfg_io->n_layers == 0) {
       if (stat(path, &st) != 0 || !S_ISDIR(st.st_mode)) { set_last_error("cl_checkpoint_info: a model config is needed unless path is a model directory"); return CL_ERR_INVALID_ARG; }
-      const int rc = model_config_from_dir(path, cfg_io);
+      const int rc = model_config_from_dir(path, cfg_io, nullptr);
       if (rc) return rc;
     }
     int32_t nt = 0;

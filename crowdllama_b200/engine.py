@@ -40,7 +40,7 @@ class EngineConfig(C.Structure):
                 ("kv_pool_bytes", C.c_int64), ("page_size", C.c_int32), ("max_batch", C.c_int32),
                 ("max_seqs", C.c_int32), ("use_cuda_graph", C.c_int32), ("decode_path", C.c_int32),
                 ("start_scheduler", C.c_int32), ("prefix_cache", C.c_int32), ("speculate", C.c_int32),
-                ("reserved", C.c_int32 * 6)]   # reserved[0], [1]: the C struct's context_shift, num_keep
+                ("reserved", C.c_int32 * 6)]   # reserved[0], [1], [2]: the C struct's context_shift, num_keep, context_length
 
 
 class Sampling(C.Structure):
@@ -111,7 +111,7 @@ EXPORTS = [
     "cl_debug_pass_rows", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
     "cl_op_attn_decode_batch", "cl_op_attn_verify", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
-    "cl_op_attn_prefill_cached", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
+    "cl_op_attn_prefill_cached", "cl_op_attn_prefill_long", "cl_attn_prefill_long_plan", "cl_resolve_model_config", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages", "cl_kvpool_set_host_pages", "cl_kvpool_take_moves",
     "cl_kvpool_host_cached_pages", "cl_kvpool_shift", "cl_seq_shift", "cl_op_kv_shift", "cl_seq_set_logprobs", "cl_seq_take_logprobs", "cl_generate_ids_logprobs", "cl_op_sample_logprobs",
@@ -196,6 +196,10 @@ def lib():
         "cl_op_attn_decode_batch": (C.c_int, [C.c_int, C.c_int, i32, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp,
                                               P(i32), P(i32)]),
         "cl_op_attn_verify": (C.c_int, [C.c_int, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, P(i32)]),
+        "cl_op_attn_prefill_long": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, P(f32),
+                                              P(i32), P(i32)]),
+        "cl_attn_prefill_long_plan": (C.c_int, [i32, i32, i32, i32, i32, P(i32), P(i64)]),
+        "cl_resolve_model_config": (C.c_int, [P(EngineConfig), P(ModelConfig)]),
         "cl_op_gemm_bf16": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, P(f32)]),
         "cl_op_gemm_bf16_epi": (C.c_int, [C.c_int, C.c_int, i32, C.c_int, vp, vp, vp, vp, vp, i32, i32, i32, P(i32)]),
         "cl_op_attn_prefill": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -363,7 +367,7 @@ class Engine:
                  page_size: int = 32, kv_pool_bytes: int = 0, use_cuda_graph: bool = True, decode_path: int = 0,
                  start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False,
                  speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
-                 num_keep: int = 4):
+                 num_keep: int = 4, context_length: int = 0):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -389,6 +393,7 @@ class Engine:
         cfg.speculate = speculate                       # 0 off, 1..15 drafted tokens per verify pass; env CL_SPECULATE overrides
         cfg.reserved[0] = 1 if context_shift else 0     # cl_engine_config.context_shift; env CL_CONTEXT_SHIFT=0|1 overrides
         cfg.reserved[1] = num_keep                      # cl_engine_config.num_keep (Ollama's documented default 4); env CL_NUM_KEEP overrides
+        cfg.reserved[2] = context_length                # cl_engine_config.context_length (0: the model's window); env CL_CONTEXT_LENGTH overrides
         h = C.c_void_p()
         _check(L.cl_engine_create(C.byref(cfg), C.byref(h)), "cl_engine_create")
         self._h = h
@@ -606,11 +611,11 @@ class Engine:
         return out
 
     PASS_PATHS = ("split-k", "tile")
-    PASS_ATTN = ("mma", "wgmma", "verify", "mixed")
+    PASS_ATTN = ("mma", "wgmma", "verify", "mixed", "long")
 
     def debug_pass_info(self) -> dict:
         """cl_debug_pass_info: the latest multi-row pass.  {"path": "split-k" | "tile", "attn": "mma" | "wgmma" | "verify" |
-        "mixed", "T": rows, "segs": [(seq, row0, n, pos0), ...]}.  EngineError when none is recorded (a token-wise prefill
+        "mixed" | "long" (the split-KV wgmma kernel), "T": rows, "segs": [(seq, row0, n, pos0), ...]}.  EngineError when none is recorded (a token-wise prefill
         or a failed pass since)."""
         info = np.zeros(4, np.int32)
         _check(lib().cl_debug_pass_info(self._h, _ptr(info), None, 0), "cl_debug_pass_info")
@@ -981,6 +986,21 @@ def op_attn_prefill_cached(q_bf16, k_bf16, v_bf16, pos0, n_heads, n_kv, head_dim
     _check(lib().cl_op_attn_prefill_cached(device, variant, _ptr(q), _ptr(k), _ptr(v), pos0, t, n_heads, n_kv, head_dim, page_size,
                                            _ptr(out)), "cl_op_attn_prefill_cached")
     return out
+
+
+def op_attn_prefill_long(q_bf16, k_bf16, v_bf16, pos0, n_heads, n_kv, head_dim, page_size=32, variant=2, nsplit=0, iters=0,
+                         device=0):
+    """cl_op_attn_prefill_long: cl_op_attn_prefill_cached with variant 2's split count (0: its plan, > 0: forced) and a
+    timing loop.  Returns (out [T][H*D] fp32, splits used, kernel that ran: "mma" | "wgmma" | "long", ms per launch or None)."""
+    q = np.ascontiguousarray(q_bf16, dtype=np.uint16)
+    k = np.ascontiguousarray(k_bf16, dtype=np.uint16)
+    v = np.ascontiguousarray(v_bf16, dtype=np.uint16)
+    t = q.shape[0]
+    out = np.empty((t, n_heads * head_dim), np.float32)
+    ms, ns, kind = C.c_float(0.0), C.c_int32(0), C.c_int32(-1)
+    _check(lib().cl_op_attn_prefill_long(device, variant, _ptr(q), _ptr(k), _ptr(v), pos0, t, n_heads, n_kv, head_dim, page_size,
+                                         nsplit, iters, _ptr(out), C.byref(ms), C.byref(ns), C.byref(kind)), "cl_op_attn_prefill_long")
+    return out, ns.value, Engine.PASS_ATTN[kind.value], (ms.value if iters > 0 else None)
 
 
 def op_attn_prefill(q_bf16, k_bf16, v_bf16, n_heads, n_kv, head_dim, device=0):

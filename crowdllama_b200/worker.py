@@ -75,10 +75,11 @@ class _Conn(socketserver.BaseRequestHandler):
 def serve(device: int, port: int, preset: str, model_name: str, max_batch: int = 8, greedy_tokens: int = 0, host="127.0.0.1",
           ready_event=None, seed: int = 1234, tokenizer: str | None = None, chat_family: str | None = None, prefix_cache: bool = False,
           speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
-          num_keep: int = 4):
+          num_keep: int = 4, context_length: int = 0):
     e = eng.Engine(preset=preset, model_name=model_name, device=device, seed=seed, max_batch=max_batch, start_scheduler=True,
                    prefix_cache=prefix_cache, speculate=speculate, speculate_batch=speculate_batch,
-                   prefix_cache_host_bytes=prefix_cache_host_bytes, context_shift=context_shift, num_keep=num_keep)
+                   prefix_cache_host_bytes=prefix_cache_host_bytes, context_shift=context_shift, num_keep=num_keep,
+                   context_length=context_length)
     if tokenizer:
         e.load_tokenizer(tokenizer, chat_family)      # HF tokenizer.json instead of the byte-level fallback
     sampling = eng.greedy(greedy_tokens, ignore_eos=True) if greedy_tokens > 0 else None   # None = Ollama defaults
@@ -118,6 +119,9 @@ def main():
                          "on generating, instead of ending with done_reason \"length\" (env CL_CONTEXT_SHIFT overrides)")
     ap.add_argument("--num-keep", type=int, default=None,
                     help="with --context-shift: leading tokens a shift never discards (default 4; env CL_NUM_KEEP overrides)")
+    ap.add_argument("--context-length", type=int, default=0,
+                    help="the context window in tokens, up to 131072 (Ollama's num_ctx / OLLAMA_CONTEXT_LENGTH for the whole "
+                         "worker; 0 = the model's default; env CL_CONTEXT_LENGTH overrides)")
     a = ap.parse_args()
     if a.prefix_cache_host_gib and not a.prefix_cache:
         ap.error("--prefix-cache-host-gib requires --prefix-cache")
@@ -127,7 +131,7 @@ def main():
     serve(a.device, a.port, a.preset, a.model_name, a.max_batch, a.greedy_tokens, tokenizer=a.tokenizer, chat_family=a.chat_family,
           prefix_cache=a.prefix_cache, speculate=a.speculate, speculate_batch=a.speculate_batch,
           prefix_cache_host_bytes=int(a.prefix_cache_host_gib * 2**30), context_shift=a.context_shift,
-          num_keep=4 if a.num_keep is None else a.num_keep)
+          num_keep=4 if a.num_keep is None else a.num_keep, context_length=a.context_length)
 
 
 if __name__ == "__main__":

@@ -131,7 +131,20 @@ typedef struct cl_engine_config {
                               and the start of the prompt.  With context_shift on, cl_engine_create
                               fails with CL_ERR_INVALID_ARG unless 0 <= num_keep <= max_seq_len - 2 * page_size (a
                               shift must discard at least one page). */
-  int32_t reserved[4];
+  int32_t context_length;  /* the served context window in tokens (env CL_CONTEXT_LENGTH overrides).  0 (the default) keeps
+                              the model's own: a preset's or cl_model_config's max_seq_len, and for a model directory
+                              min(max_position_embeddings, 32768), capped by sliding_window.  > 0 sets max_seq_len to it,
+                              from 2 pages up to 131072 tokens (Llama-3.1 / 3.2's 128K window); a model directory refuses
+                              it above max_position_embeddings or sliding_window.  A window cl_engine_create does not
+                              accept fails it with CL_ERR_INVALID_ARG; cl_resolve_model_config applies the same rule on the
+                              host.  With kv_pool_bytes == 0 and context_length > 0, the KV pool takes the device memory
+                              that is free after the weights, less a 4 GiB reserve for the engine's state and prefill /
+                              verify workspaces, capped at max_seqs x the window: at 131072 tokens a full batch of
+                              windows rarely fits, and a prompt whose pages exceed the whole pool fails with CL_ERR_OOM.
+                              Prefill segments that end past 32768 tokens run split-KV attention kernels for head_dim
+                              128 / page 32 (up to 16 rows: the multi-row verify kernel); shorter segments run what they
+                              always have. */
+  int32_t reserved[3];
 } cl_engine_config;
 
 /* Sampler.  The reference sends no options (api.go:109-118), so Ollama defaults apply upstream:
@@ -268,6 +281,11 @@ int cl_sample_token(const float* logits, int32_t vocab, const cl_sampling* s, co
 int cl_sample_token_ext(const float* logits, int32_t vocab, const cl_sampling* s, const cl_sampling_ext* ext, const int32_t* history,
                         int32_t n_history, uint64_t step, int32_t* id);
 int cl_model_preset(const char* name, cl_model_config* out);
+/* Host only (no GPU needed): the model config cl_engine_create derives from cfg — the preset, the model directory's
+ * config.json or cfg->model — with the served window of cfg->context_length (and CL_CONTEXT_LENGTH) in max_seq_len, and
+ * the same checks: CL_ERR_INVALID_ARG for a window it refuses or a num_keep that leaves no room to shift (context_shift on),
+ * CL_ERR_UNKNOWN_MODEL / CL_ERR_IO as cl_engine_create.  cl_checkpoint_info keeps the default window. */
+int cl_resolve_model_config(const cl_engine_config* cfg, cl_model_config* out);
 /* The prompt-lookup drafter of speculative decoding (host only, no GPU involved): the longest suffix of hist[0..n) of
  * length 3, else 2, that also occurs earlier in hist; from its most recent earlier occurrence, the up to k ids that
  * followed it, stopping at the end of hist, go to out.  *n_out = their count (0: no match).  k: 1..15. */
@@ -515,7 +533,8 @@ int cl_debug_seq_hidden(cl_engine* e, cl_seq_t seq, int32_t what, float* out, in
 /* Parity aid: the latest multi-row pass — a split-K pass (prompts of 16 .. 256 tokens, every cl_decode_verify /
  * cl_decode_verify_batch) or a tile-path pass (longer prompts, one per chunk; cl_prefill_batch).  info[4] = {path (0 split-K,
  * 1 tile), attention kernel (0 mma.sync prefill, 1 wgmma prefill, 2 multi-row verify, 3 segments with different prefill
- * kernels), T (rows), n_segs}; segs[min(n_segs, max_segs)][4] = {sequence, first row, rows, position of the first row}.  A
+ * kernels, 4 split-KV wgmma prefill: segments of more than 16 rows that end past 32768 tokens; up to 16 rows run the
+ * multi-row verify kernel there, 2), T (rows), n_segs}; segs[min(n_segs, max_segs)][4] = {sequence, first row, rows, position of the first row}.  A
  * prefill longer than one chunk leaves its last chunk's pass.  CL_ERR_INVALID_ARG when no pass is recorded: none yet, or a
  * token-wise prefill (fewer than 16 tokens) or a failed pass since. */
 int cl_debug_pass_info(cl_engine* e, int32_t* info, int32_t* segs, int32_t max_segs);
@@ -613,13 +632,30 @@ int cl_op_gemm_bf16_epi(int device, int epi, int32_t k_splits, int pdl, const ui
 int cl_op_attn_prefill(int device, const uint16_t* q, const uint16_t* k, const uint16_t* v,
                        int32_t t, int32_t n_heads, int32_t n_kv, int32_t head_dim, float* out);
 /* the same with the kernel chosen explicitly — variant 0: mma.sync kernel (prefill_kernels.cu, any head_dim 64|128),
- * 1: wgmma kernel (attn_prefill_tc.cu, head_dim 128), -1: what the engine would pick — and an optional timing loop */
+ * 1: wgmma kernel (attn_prefill_tc.cu, head_dim 128, up to 10240 tokens), 2: split-KV wgmma kernel (attn_prefill_tc.cu,
+ * head_dim 128, page 32, any length; its own split plan), -1: what the engine would pick — and an optional timing loop */
 int cl_op_attn_prefill_variant(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t t,
                                int32_t n_heads, int32_t n_kv, int32_t head_dim, float* out, int32_t iters, float* ms);
 /* the same behind a cached prefix: q [t][n_heads][d] for positions pos0 .. pos0+t-1, k,v [pos0+t][n_kv][d]; page_size 16,
  * 32 or 64.  CL_ERR_INVALID_ARG when variant 1 does not take the shape. */
 int cl_op_attn_prefill_cached(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0,
                               int32_t t, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, float* out);
+/* cl_op_attn_prefill_cached with the split count of variant 2 and a timing loop.  nsplit: 0 = the kernel's own plan (what
+ * the engine runs), > 0 = that many KV splits per (128-row tile, head), clamped to 1 .. the KV blocks (64 tokens) of the
+ * first tile.  *nsplit_used (may be NULL): the splits that ran (1 for variants 0 and 1); *kind_used (may be NULL): the kernel
+ * that ran, numbered as cl_debug_pass_info's attention kernels (0 mma.sync, 1 wgmma, 2 multi-row verify, 4 split-KV
+ * wgmma), which for variant -1 is the engine's rule: segments that end within 32768 tokens keep the kernels they ran before;
+ * past it, up to 16 rows run the multi-row verify kernel (every split over max(8, ceil(pages / 64)) pages) and more rows
+ * the split-KV wgmma kernel.  The split kernels launch twice without re-arming their counters and the call fails with
+ * CL_ERR_INTERNAL if the two outputs differ in any bit.  iters > 0: *ms = CUDA-event time of one launch over iters launches. */
+int cl_op_attn_prefill_long(int device, int variant, const uint16_t* q, const uint16_t* k, const uint16_t* v, int32_t pos0,
+                            int32_t t, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit,
+                            int32_t iters, float* out, float* ms, int32_t* nsplit_used, int32_t* kind_used);
+/* Host-only: the split plan of the split-KV prefill attention for t rows from pos0 over n_heads query heads on sms SMs
+ * (nsplit as above), and *part_floats (may be NULL) = the fp32 workspace the engine gives it, which bounds every automatic
+ * plan's partials (tiles x n_heads x splits x 128 rows x (head_dim + 2)). */
+int cl_attn_prefill_long_plan(int32_t pos0, int32_t t, int32_t n_heads, int32_t sms, int32_t nsplit, int32_t* nsplit_used,
+                              int64_t* part_floats);
 /* the decode step's device sampler (the step tail kernel) on host logits [n_rows][vocab]: row r draws with sp[r] at RNG
  * step step[r], with history row r = history + r * hist_stride, n_history[r] ids (history may be NULL when every
  * n_history[r] is 0).  ids_out[n_rows].  CL_ERR_INVALID_ARG for settings the device sampler does not cover. */
