@@ -23,7 +23,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOSTCXX = "/usr/bin/g++"
 
 SOURCES = ["decode_kernels.cu", "decode_mega.cu", "attn_decode_tc.cu", "attn_verify_tc.cu", "batch_kernels.cu", "engine.cu", "ops_api.cu", "prefill.cu", "gemm_wgmma.cu", "prefill_kernels.cu", "attn_prefill_tc.cu", "kv_host.cu", "kv_shift.cu",
-           "host_util.cpp", "tokenizer.cpp", "weights_io.cpp", "scheduler.cpp", "capi.cpp"]
+           "host_util.cpp", "tokenizer.cpp", "weights_io.cpp", "scheduler.cpp", "draft.cpp", "capi.cpp"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-ccbin", HOSTCXX,
          "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function,-fvisibility=default", "--expt-relaxed-constexpr",
          "-I", str(HERE.parent / "include")]

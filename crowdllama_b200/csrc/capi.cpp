@@ -98,14 +98,16 @@ int cl_model_preset(const char* name, cl_model_config* o) {
   return CL_ERR_UNKNOWN_MODEL;
 }
 
-int cl_engine_create(const cl_engine_config* cfg, cl_engine** out) {
+int cl_engine_create(const cl_engine_config* cfg, cl_engine** out) { return cl_engine_create_with_draft(cfg, nullptr, out); }
+
+int cl_engine_create_with_draft(const cl_engine_config* cfg, const cl_engine_config* draft, cl_engine** out) {
   if (!cfg || !out) return CL_ERR_INVALID_ARG;
   *out = nullptr;
   cl_engine* e = new (std::nothrow) cl_engine();
   if (!e) return CL_ERR_OOM;
   int rc;
   try {
-    rc = e->impl.init(*cfg);
+    rc = e->impl.init(*cfg, draft);
   } catch (const std::exception& ex) {
     set_last_error(ex.what());
     rc = CL_ERR_INTERNAL;
@@ -152,6 +154,18 @@ int cl_engine_set_prefix_host_cache(cl_engine* e, int64_t bytes) {
 int cl_engine_set_speculate_batch(cl_engine* e, int32_t n) {
   if (!e) return CL_ERR_INVALID_ARG;
   return e->impl.set_speculate_batch(n);   // an atomic the scheduler reads once per iteration, no engine lock
+}
+
+int cl_draft_model(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* const* hists, const int32_t* hist_lens,
+                   const int32_t* ks, const cl_sampling* sp, const uint64_t* step0, int32_t* drafts, int32_t* n_drafts) {
+  if (!e) return CL_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  try {
+    return e->impl.draft_tokens(seqs, n_seqs, hists, hist_lens, ks, sp, step0, drafts, n_drafts);
+  } catch (const std::exception& ex) {
+    set_last_error(ex.what());
+    return CL_ERR_INTERNAL;
+  }
 }
 
 int cl_engine_set_tensor(cl_engine* e, int32_t layer, int32_t kind, const uint16_t* data, int64_t n) {

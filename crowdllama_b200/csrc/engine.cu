@@ -56,7 +56,14 @@ Engine::~Engine() {
     ptr = reinterpret_cast<decltype(ptr)>(_p);                       \
   } while (0)
 
-int Engine::init(const cl_engine_config& c) {
+int64_t weight_bytes(const cl_model_config& m) {
+  const int64_t d = m.d_model, F = m.d_ff, V = m.vocab_size, q = (int64_t)m.n_heads * m.head_dim, kv = (int64_t)m.n_kv_heads * m.head_dim;
+  return 2 * (2 * V * d) + (int64_t)m.n_layers * 2 * ((q + 2 * kv) * d + d * q + 3 * F * d) + (int64_t)m.max_seq_len * m.head_dim * 4;
+}
+
+bool draft_engine_config(const cl_engine_config& c, const cl_engine_config* draft, cl_engine_config* out);   // draft.cpp
+
+int Engine::init(const cl_engine_config& c, const cl_engine_config* draft) {
   if (c.abi_version != CL_ABI_VERSION) { set_last_error("abi_version mismatch"); return CL_ERR_INVALID_ARG; }
   const std::string wpath = c.weights_path ? c.weights_path : "";
   struct stat wst{};
@@ -72,6 +79,19 @@ int Engine::init(const cl_engine_config& c) {
       (cfg.vocab_size & 1)) {
     set_last_error("unsupported model shape (need head_dim 64|128, heads/kv in {1,2,4,8}, d_model,d_ff %16==0, even vocab)");
     return CL_ERR_INVALID_ARG;
+  }
+  // the draft model: its config and the refusals that need no device (the rest follow once both engines exist)
+  cl_engine_config dc{};
+  cl_model_config dm{};
+  const bool want_draft = !is_draft_ && draft_engine_config(c, draft, &dc);
+  if (want_draft) {
+    dc.context_length = cfg.max_seq_len;   // the target's window, which the draft must serve
+    if (const int rc = resolve_model_config(dc, &dm, nullptr)) return rc;
+    if (dm.vocab_size != cfg.vocab_size) {
+      set_last_error("draft model: vocabulary of " + std::to_string(dm.vocab_size) + " ids, the target has " + std::to_string(cfg.vocab_size));
+      return CL_ERR_INVALID_ARG;
+    }
+    if (env_int("CL_SPECULATE", c.speculate) == 0) { set_last_error("draft model: speculate is 0, so nothing would use it"); return CL_ERR_INVALID_ARG; }
   }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
@@ -114,14 +134,13 @@ int Engine::init(const cl_engine_config& c) {
   if (pool_bytes <= 0) pool_bytes = (int64_t)max_seqs_ * max_pages_per_seq_ * page_size_ * (int64_t)kv_bytes_per_token;
   if (c.kv_pool_bytes <= 0 && context_length > 0) {
     // a long window: max_seqs full windows rarely fit, so the pool takes what is free after the weights (and the RoPE
-    // table), less kPoolReserveBytes for the state and the lazily allocated prefill / verify workspaces
+    // table), less kPoolReserveBytes for the state and the lazily allocated prefill / verify workspaces.  With a draft model
+    // both weight sets come off first, and the draft's pool, as many tokens as this one, takes its share of the rest.
     size_t free_b = 0, total_b = 0;
     CL_CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
-    const int64_t d = cfg.d_model, F = cfg.d_ff, V = cfg.vocab_size;
-    const int64_t weights = 2 * (2 * V * d) + (int64_t)cfg.n_layers * 2 * ((int64_t)qkv_dim_ * d + d * q_dim_ + 3 * F * d) +
-                            (int64_t)cfg.max_seq_len * cfg.head_dim * 4;
+    const int64_t weights = weight_bytes(cfg) + (want_draft ? weight_bytes(dm) : 0);
     const int64_t avail = (int64_t)free_b - weights - kPoolReserveBytes;
-    pool_bytes = std::min(pool_bytes, std::max<int64_t>(avail, 0));
+    pool_bytes = std::min(pool_bytes, target_pool_share(avail, (int64_t)kv_bytes_per_token, want_draft ? cl::kv_bytes_per_token(dm) : 0));
   }
   n_pages_ = (int)(pool_bytes / ((int64_t)page_size_ * (int64_t)kv_bytes_per_token));
   if (n_pages_ < 1) { set_last_error("kv_pool_bytes too small for one page"); return CL_ERR_INVALID_ARG; }
@@ -168,6 +187,7 @@ int Engine::init(const cl_engine_config& c) {
       if (!t) { set_last_error("tokenizer.json: " + err); return CL_ERR_IO; }
       if (t->vocab_size() > cfg.vocab_size) { set_last_error("tokenizer.json has more ids than the model's vocabulary"); return CL_ERR_IO; }
       tok = std::move(t);
+      hf_tok_ = true;
     }
   }
   CL_CUDA_OK(cudaStreamSynchronize(stream_));
@@ -190,11 +210,13 @@ int Engine::init(const cl_engine_config& c) {
   if (sched_prefill_chunk_ > 0 && sched_prefill_chunk_ < 16) sched_prefill_chunk_ = 16;
   prefill_small_max_ = std::min(256, env_int("CL_PREFILL_SMALL_MAX", kDefaultPrefillSmallMax));
   device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
+  if (is_draft_) return CL_OK;   // a draft serves its target's drafter only: no prefix cache, shift, speculation or scheduler
   prefix_cache_ = env_int("CL_PREFIX_CACHE", c.prefix_cache) != 0;
   context_shift_ = env_int("CL_CONTEXT_SHIFT", c.context_shift) != 0;
   num_keep_ = env_int("CL_NUM_KEEP", c.num_keep);   // checked against the final window by resolve_model_config
   speculate_ = env_int("CL_SPECULATE", c.speculate);
   if (speculate_ < 0 || speculate_ > kSpecMaxDraft) { set_last_error("speculate must be 0..15"); return CL_ERR_INVALID_ARG; }
+  if (want_draft && !spec_path_ok()) { set_last_error("draft model: the target's shape has no verify pass"); return CL_ERR_INVALID_ARG; }
   if (speculate_ > 0 && !spec_path_ok()) {
     fprintf(stderr, "[clengine] speculative decoding needs the tensor-core split-K path, which this model shape lacks: decoding normally\n");
     speculate_ = 0;
@@ -205,6 +227,27 @@ int Engine::init(const cl_engine_config& c) {
   if (const char* v = getenv("CL_PREFIX_CACHE_HOST_MIB")) {
     const int rc = set_prefix_host_cache(atoll(v) * (1LL << 20));
     if (rc) return rc;
+  }
+  if (want_draft) {
+    // same device and page size; one mirror per sequence handle; a pool of this pool's tokens; batches up to speculate_batch
+    dc.device = device_;
+    dc.page_size = page_size_;
+    dc.max_seqs = max_seqs_;
+    dc.max_batch = std::min(max_batch_, kSpecBatchMax);
+    dc.use_cuda_graph = c.use_cuda_graph;
+    dc.decode_path = c.decode_path;
+    dc.kv_pool_bytes = (int64_t)n_pages_ * page_size_ * cl::kv_bytes_per_token(dm);
+    draft_.reset(new Engine());
+    draft_->is_draft_ = true;
+    if (const int rc = draft_->init(dc)) return rc;
+    bool same = draft_->cfg.max_seq_len == cfg.max_seq_len;
+    if (hf_tok_ && draft_->hf_tok_) {
+      same = same && tok->bos() == draft_->tok->bos() && tok->eos() == draft_->tok->eos();
+      for (int id = 0; same && id < cfg.vocab_size; ++id) same = tok->is_stop(id) == draft_->tok->is_stop(id);
+      if (!same) { set_last_error("draft model: bos / eos / stop ids differ from the target's"); return CL_ERR_INVALID_ARG; }
+    }
+    if (!same) { set_last_error("draft model: cannot serve the target's window"); return CL_ERR_INVALID_ARG; }
+    mirror_.assign(max_seqs_, -1);
   }
   if (c.start_scheduler) start_scheduler();
   return CL_OK;
@@ -423,6 +466,12 @@ int Engine::seq_free(cl_seq_t s) {
   if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
   pool_->release(s);
   seqs_[s] = SeqState();
+  if (draft_ && mirror_[s] >= 0) {   // the draft's mirror of s goes with it
+    const int rc = draft_->seq_free(mirror_[s]);
+    mirror_[s] = -1;
+    draft_pages_ = draft_->pool_->used_pages();
+    if (rc) return rc;
+  }
   const int rc = disarm_sampling(s);
   return rc ? rc : upload_logprobs(s, -1);
 }
@@ -888,9 +937,9 @@ bool Engine::ensure_graph(int B) {
 // costs tens of milliseconds, which would otherwise land inside 31 separate decode steps of the first minute of traffic
 // (box benchmark, 64 concurrent chats: 16.6 req/s with lazy capture against 24.6 warm).  Called once when the
 // scheduler thread starts.
-void Engine::precapture_graphs() {
+void Engine::precapture_graphs(int max_b) {
   if (!use_graph_) return;
-  for (int B = 1; B <= max_batch_ && !graph_failed_; ++B) ensure_graph(B);
+  for (int B = 1; B <= max_b && !graph_failed_; ++B) ensure_graph(B);
   cudaStreamSynchronize(stream_);
 }
 
@@ -1286,6 +1335,9 @@ int Engine::spec_stats(cl_spec_stats* out) {
   out->tokens_accepted = spec_accepted_;
   out->tokens_emitted = spec_emitted_;
   out->multi_passes = spec_multi_passes_;
+  out->draft_rows = draft_rows_;
+  out->draft_ns = draft_ns_;
+  out->draft_pages_used = draft_pages_;
   return CL_OK;
 }
 

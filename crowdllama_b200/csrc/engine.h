@@ -352,11 +352,23 @@ struct SeqState {
 
 struct Request;  // scheduler.cpp
 
+// Device bytes of a model's weights and RoPE table, as Engine::alloc_weights allocates them
+int64_t weight_bytes(const cl_model_config& m);
+// KV bytes per token of a model: K and V of every layer, bf16
+inline int64_t kv_bytes_per_token(const cl_model_config& m) { return 2LL * m.n_layers * m.n_kv_heads * m.head_dim * 2; }
+// The target's share of `avail` bytes of KV pool when a draft model's pool must hold as many tokens as the target's: the
+// bytes are split in proportion to bytes per token (draft_tok = 0: all of it)
+inline int64_t target_pool_share(int64_t avail, int64_t target_tok, int64_t draft_tok) {
+  if (avail <= 0) return 0;
+  return draft_tok > 0 ? avail / (target_tok + draft_tok) * target_tok : avail;
+}
+
 class Engine {
  public:
   Engine() = default;
   ~Engine();
-  int init(const cl_engine_config& cfg);
+  // draft (may be nullptr: CL_DRAFT_MODEL / CL_DRAFT_SEED decide): the draft model of speculative decoding
+  int init(const cl_engine_config& cfg, const cl_engine_config* draft = nullptr);
 
   // token-level API (callers hold mu_)
   int seq_create(cl_seq_t* out);
@@ -412,6 +424,13 @@ class Engine {
   int decode_verify(cl_seq_t s, int32_t x0, const int32_t* draft, int k, const cl_sampling* sp, uint64_t step0, int32_t* ids_out,
                     int* n_out, float* logits_out);
   bool spec_path_ok() const;          // the verify pass runs on this model shape
+  // The draft model's drafter (contract in include/clengine.h, cl_draft_model): for each target sequence ss[i], its mirror in
+  // the draft engine catches up with hists[i][0..lens[i]) (the window ending with the next input x0) and drafts ks[i] ids
+  // (0..15) with sp[i] / step0[i] (both may be nullptr: greedy, step 0).  The ids of sequence i land back to back at drafts +
+  // the sum of ks[j] over j < i; n_drafts[i] = ks[i], or 0 when the draft pool has no pages for its mirror.
+  int draft_tokens(const cl_seq_t* ss, int n, const int32_t* const* hists, const int* lens, const int* ks, const cl_sampling* sp,
+                   const uint64_t* step0, int32_t* drafts, int* n_drafts);
+  bool has_draft() const { return draft_ != nullptr; }
   int speculate() const { return speculate_; }
   int speculate_batch() const { return speculate_batch_; }
   int set_speculate_batch(int n);     // 1..min(max_batch, kSpecBatchMax), else CL_ERR_INVALID_ARG
@@ -474,7 +493,7 @@ class Engine {
   int enqueue_step_tail(int B, bool push_input);
   int run_step_graph(int B);
   bool ensure_graph(int B);
-  void precapture_graphs();                       // graph launch (or eager enqueue)
+  void precapture_graphs(int max_b);              // the step graphs of batch sizes 1..max_b
   int read_logits(int slot, float* out);
   // After a call whose step tail ran once for the sequences ss[0..n): each one with logprobs on appends its record
   // (d_lp_last_) to its pending list.  Nothing is copied when none is on.  Synchronises the stream.
@@ -602,6 +621,14 @@ class Engine {
   int speculate_ = 0;                 // most drafted tokens per verify pass in the scheduler / synchronous path (0 = off)
   std::atomic<int> speculate_batch_{1};   // most sequences the scheduler verifies in one pass (1: only a request running alone)
   std::atomic<int64_t> spec_passes_{0}, spec_drafted_{0}, spec_accepted_{0}, spec_emitted_{0}, spec_multi_passes_{0};
+  // Draft model (draft.cpp): an engine of its own on the same device, with no scheduler, prefix cache or speculation, whose
+  // pool holds as many tokens as this one's.  mirror_[s]: the draft sequence that mirrors target sequence s (-1: none).
+  std::unique_ptr<Engine> draft_;
+  bool is_draft_ = false;             // this engine is another engine's draft: the env switches of serving features stay off
+  bool hf_tok_ = false;               // the tokenizer came from the model directory's tokenizer.json
+  std::vector<int> mirror_;
+  std::atomic<int64_t> draft_rows_{0}, draft_ns_{0}, draft_pages_{0};   // cl_spec_stats.draft_*; draft_pages_: the draft pool's used pages
+  void seq_rewind(cl_seq_t s, int len);  // a draft mirror: len drops to `len` (history with it), its pages stay
   int prefill_small_max_ = 0;         // prompts up to this many tokens take the split-K path (CL_PREFILL_SMALL_MAX, 0 = off)
   struct BatchWs { __nv_bfloat16* xn = nullptr; __nv_bfloat16* attn = nullptr; __nv_bfloat16* act = nullptr; float* part = nullptr; float* logits = nullptr; };
   std::unique_ptr<BatchWs> bws_;

@@ -197,8 +197,8 @@ int Engine::host_next_token(Request& r, float* logits, bool read_back, const int
 }
 
 // Speculative round of rs[0..n): a request decoding alone, or 2 .. speculate_batch running requests; every one must be
-// greedy or device-sampled.  Each drafts from its prompt and output (ngram_draft; nothing while backing off or without a
-// match), clipped so that it passes neither max_new nor max_seq_len, and one verify pass checks all the drafts.  The pass
+// greedy or device-sampled.  Each drafts from its prompt and output (the draft model's draft_tokens when the engine has one,
+// else ngram_draft; nothing while backing off or without a match), clipped so that it passes neither max_new nor max_seq_len, and one verify pass checks all the drafts.  The pass
 // holds at most kSpecMaxRows rows: every k is capped at the largest c with sum(min(k_i, c) + 1) <= kSpecMaxRows, so no
 // request loses a drafted token while another keeps more than c.  A request the pool has no pages for drafts nothing this
 // round.  A lone request keeps the per-segment attention of cl_decode_verify; several take the multi-row kernel.  Accepted
@@ -208,16 +208,38 @@ int Engine::spec_round(const std::shared_ptr<Request>* rs, int n) {
   if (speculate_ <= 0 || !std::all_of(rs, rs + n, [](const std::shared_ptr<Request>& r) { return r->device_next(); })) return 0;
   std::vector<int> ks(n, 0);
   std::vector<int32_t> drafts((size_t)n * kSpecMaxDraft);
+  int cap = kSpecMaxDraft;
+  auto rows = [&](int c) { int t = 0; for (int k : ks) t += std::min(k, c) + 1; return t; };
   for (int b = 0; b < n; ++b) {
     Request& r = *rs[b];
     if (r.spec_backoff > 0 || r.out.empty()) continue;
     const int k_max = std::min({speculate_, r.max_new - (int)r.out.size() - 1, cfg.max_seq_len - seqs_[r.seq].len - 1});
     if (k_max < 1) continue;
     const std::vector<int32_t>& hist = r.sync_full();   // ends with the next input x0
-    ks[b] = ngram_draft(hist.data(), (int)hist.size(), k_max, drafts.data() + (size_t)b * kSpecMaxDraft);
+    ks[b] = draft_ ? k_max : ngram_draft(hist.data(), (int)hist.size(), k_max, drafts.data() + (size_t)b * kSpecMaxDraft);
   }
-  int cap = kSpecMaxDraft;
-  auto rows = [&](int c) { int t = 0; for (int k : ks) t += std::min(k, c) + 1; return t; };
+  if (draft_) {
+    // the draft model drafts every id it is asked for, so the pass's row cap applies before it runs; a sampled request's
+    // draft row i draws at the RNG step of its verify row i
+    while (cap > 0 && rows(cap) > kSpecMaxRows) --cap;
+    std::vector<cl_seq_t> ss(n);
+    std::vector<const int32_t*> hists(n);
+    std::vector<int> lens(n), got(n);
+    std::vector<cl_sampling> sp(n);
+    std::vector<uint64_t> step0(n);
+    for (int b = 0; b < n; ++b) {
+      Request& r = *rs[b];
+      ks[b] = std::min(ks[b], cap);
+      ss[b] = r.seq; hists[b] = r.full.data(); lens[b] = (int)r.full.size();   // r.full: synced above when ks[b] > 0
+      sp[b] = r.sp; step0[b] = r.out.size();
+    }
+    std::vector<int32_t> packed((size_t)n * kSpecMaxDraft);
+    if (const int rc = draft_tokens(ss.data(), n, hists.data(), lens.data(), ks.data(), sp.data(), step0.data(), packed.data(), got.data())) return rc;
+    for (int b = 0, off = 0; b < n; off += ks[b], ++b) {
+      std::copy(packed.begin() + off, packed.begin() + off + got[b], drafts.begin() + (size_t)b * kSpecMaxDraft);
+    }
+    for (int b = 0; b < n; ++b) ks[b] = got[b];
+  }
   while (cap > 0 && rows(cap) > kSpecMaxRows) --cap;
   for (int b = 0; b < n; ++b) {
     ks[b] = std::min(ks[b], cap);
@@ -427,7 +449,8 @@ void Engine::scheduler_main() {
     sched_logits_.resize(cfg.vocab_size);
     sched_toks_.resize(max_seqs_);
     sched_slots_.clear();
-    precapture_graphs();   // every batch size's step graph up front, not inside the first steps that meet it
+    precapture_graphs(max_batch_);   // every batch size's step graph up front, not inside the first steps that meet it
+    if (draft_) draft_->precapture_graphs(speculate_batch_);   // and the draft's, for the batches that draft together
   }
   while (wait_for_work()) {
     std::lock_guard<std::mutex> elk(mu_);

@@ -91,7 +91,7 @@ class PrefixStats(C.Structure):
 class SpecStats(C.Structure):
     _fields_ = [("enabled", C.c_int32), ("max_draft", C.c_int32), ("verify_passes", C.c_int64), ("tokens_drafted", C.c_int64),
                 ("tokens_accepted", C.c_int64), ("tokens_emitted", C.c_int64), ("multi_passes", C.c_int64),
-                ("reserved", C.c_int64 * 3)]
+                ("reserved", C.c_int64 * 3)]   # the C struct's draft_rows, draft_ns, draft_pages_used (Engine.draft_stats)
 
 
 # cl_token_logprob (include/clengine.h): one record of the step tail's log-probabilities, 172 bytes
@@ -104,7 +104,7 @@ assert TOKEN_LOGPROB.itemsize == 172
 EXPORTS = [
     "cl_abi_version", "cl_strerror", "cl_last_error", "cl_default_engine_config", "cl_default_sampling",
     "cl_greedy_sampling", "cl_sample_token", "cl_model_preset", "cl_engine_create", "cl_engine_destroy", "cl_engine_model_config",
-    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_engine_set_speculate_batch", "cl_engine_set_prefix_host_cache", "cl_draft_ngram", "cl_decode_verify", "cl_decode_verify_batch", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
+    "cl_engine_stats", "cl_engine_prefix_stats", "cl_engine_spec_stats", "cl_engine_set_speculate_batch", "cl_engine_set_prefix_host_cache", "cl_draft_ngram", "cl_engine_create_with_draft", "cl_draft_model", "cl_decode_verify", "cl_decode_verify_batch", "cl_engine_set_tensor", "cl_checkpoint_info", "cl_generate", "cl_generate_ids", "cl_generate_stream", "cl_result_free",
     "cl_handle_message", "cl_handle_message_stream", "cl_buffer_free", "cl_tokenize", "cl_detokenize", "cl_seq_create", "cl_seq_free",
     "cl_seq_len", "cl_seq_attach_prefix", "cl_prefill", "cl_prefill_batch", "cl_decode_step", "cl_decode_greedy", "cl_decode_greedy_batch", "cl_decode_sample_batch", "cl_decode_step_batch", "cl_seq_fake_fill",
     "cl_time_dominant_kernel", "cl_debug_kv", "cl_debug_hidden", "cl_debug_seq_hidden", "cl_debug_pass_info",
@@ -152,6 +152,8 @@ def lib():
         "cl_engine_prefix_stats": (C.c_int, [vp, P(PrefixStats)]),
         "cl_engine_spec_stats": (C.c_int, [vp, P(SpecStats)]),
         "cl_draft_ngram": (C.c_int, [vp, i32, i32, vp, P(i32)]),
+        "cl_engine_create_with_draft": (C.c_int, [P(EngineConfig), P(EngineConfig), P(vp)]),
+        "cl_draft_model": (C.c_int, [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]),
         "cl_decode_verify": (C.c_int, [vp, i32, i32, vp, i32, P(Sampling), u64, vp, P(i32), vp]),
         "cl_engine_set_speculate_batch": (C.c_int, [vp, i32]),
         "cl_engine_set_prefix_host_cache": (C.c_int, [vp, i64]),
@@ -335,6 +337,27 @@ def ollama_default_sampling(seed: int = 0, max_new_tokens: int = -1) -> Sampling
     return s
 
 
+def draft_engine_config(preset: str | None, model: dict | None, weights_path: str | None, seed: int, keep: list):
+    """The draft config cl_engine_create_with_draft reads (preset / model / weights_path / weights_seed), or None when no
+    draft model is asked for.  keep: a list that holds the encoded strings alive as long as the engine."""
+    if preset is None and model is None and weights_path is None:
+        return None
+    d = EngineConfig()
+    lib().cl_default_engine_config(C.byref(d))
+    if preset is not None:
+        keep.append(preset.encode())
+        d.preset = keep[-1]
+    else:
+        d.preset = None
+    if model is not None:
+        d.model = ModelConfig(**model)
+    if weights_path is not None:
+        keep.append(str(weights_path).encode())
+        d.weights_path = keep[-1]
+    d.weights_seed = seed
+    return d
+
+
 class GenerateResult:
     def __init__(self, r: Result):
         self.text = C.string_at(r.text, r.text_len).decode("utf-8", errors="replace") if r.text else ""
@@ -367,7 +390,8 @@ class Engine:
                  page_size: int = 32, kv_pool_bytes: int = 0, use_cuda_graph: bool = True, decode_path: int = 0,
                  start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False,
                  speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
-                 num_keep: int = 4, context_length: int = 0):
+                 num_keep: int = 4, context_length: int = 0, draft_preset: str | None = None, draft_model: dict | None = None,
+                 draft_weights_path: str | None = None, draft_seed: int | None = None):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -395,7 +419,12 @@ class Engine:
         cfg.reserved[1] = num_keep                      # cl_engine_config.num_keep (Ollama's documented default 4); env CL_NUM_KEEP overrides
         cfg.reserved[2] = context_length                # cl_engine_config.context_length (0: the model's window); env CL_CONTEXT_LENGTH overrides
         h = C.c_void_p()
-        _check(L.cl_engine_create(C.byref(cfg), C.byref(h)), "cl_engine_create")
+        dcfg = draft_engine_config(draft_preset, draft_model, draft_weights_path, seed if draft_seed is None else draft_seed,
+                                   self._keep)
+        if dcfg is None:
+            _check(L.cl_engine_create(C.byref(cfg), C.byref(h)), "cl_engine_create")
+        else:   # speculative decoding with a draft model (cl_engine_create_with_draft); env CL_DRAFT_MODEL is for plain creates
+            _check(L.cl_engine_create_with_draft(C.byref(cfg), C.byref(dcfg), C.byref(h)), "cl_engine_create_with_draft")
         self._h = h
         # requests verified in one pass; env CL_SPECULATE_BATCH overrides the argument, as CL_SPECULATE does `speculate`
         if speculate_batch != 1 and "CL_SPECULATE_BATCH" not in os.environ:
@@ -565,6 +594,26 @@ class Engine:
                                             _ptr(n), _ptr(out) if want_logits else None), "cl_decode_verify_batch")
         r0 = np.concatenate([[0], np.cumsum(ks + 1)])
         return [ids[r0[i]:r0[i] + n[i]].copy() for i in range(len(seqs))], out
+
+    def draft_model(self, seqs, hists, ks, samplings=None, step0=None):
+        """cl_draft_model: the draft model's drafter.  For target sequence seqs[i], its mirror catches up with hists[i] (the
+        window ending with the next input) and drafts ks[i] ids (0..15), greedy or with samplings[i] (None, or one Sampling
+        or None per sequence) at RNG steps step0[i] + j.  Returns the list of every sequence's drafted ids."""
+        seqs = np.ascontiguousarray(seqs, dtype=np.int32)
+        hs = [np.ascontiguousarray(h, dtype=np.int32) for h in hists]
+        ptrs = (C.c_void_p * len(hs))(*[h.ctypes.data for h in hs])
+        lens = np.array([len(h) for h in hs], np.int32)
+        ks = np.ascontiguousarray(ks, dtype=np.int32)
+        sp = None
+        if samplings is not None:
+            sp = (Sampling * len(seqs))(*[s if s is not None else greedy(-1) for s in samplings])
+        st = np.ascontiguousarray(step0 if step0 is not None else np.zeros(len(seqs)), dtype=np.uint64)
+        out = np.zeros(max(int(ks.sum()), 1), np.int32)
+        n = np.zeros(len(seqs), np.int32)
+        _check(lib().cl_draft_model(self._h, _ptr(seqs), len(seqs), ptrs, _ptr(lens), _ptr(ks), sp, _ptr(st), _ptr(out), _ptr(n)),
+               "cl_draft_model")
+        off = np.concatenate([[0], np.cumsum(ks)])
+        return [out[off[i]:off[i] + n[i]].copy() for i in range(len(seqs))]
 
     def set_speculate_batch(self, n: int):
         """cl_engine_set_speculate_batch: how many running requests the scheduler may verify in one pass (1 = only a
@@ -828,6 +877,12 @@ class Engine:
         st = SpecStats()
         _check(lib().cl_engine_spec_stats(self._h, C.byref(st)), "cl_engine_spec_stats")
         return {n: getattr(st, n) for n, _ in st._fields_ if n not in ("reserved", "multi_passes")}
+
+    def draft_stats(self) -> dict:
+        """cl_spec_stats.draft_rows, draft_ns, draft_pages_used (the struct's last three fields; all zero without a draft)."""
+        st = SpecStats()
+        _check(lib().cl_engine_spec_stats(self._h, C.byref(st)), "cl_engine_spec_stats")
+        return dict(zip(("draft_rows", "draft_ns", "draft_pages_used"), st.reserved))
 
     def spec_multi_passes(self) -> int:
         """cl_spec_stats.multi_passes: verify passes that checked two or more sequences at once."""

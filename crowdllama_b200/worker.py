@@ -13,6 +13,7 @@ the Go cgo shim installs into Peer.APIHandler.
 from __future__ import annotations
 
 import argparse
+import os
 import socketserver
 import threading
 
@@ -72,14 +73,24 @@ class _Conn(socketserver.BaseRequestHandler):
                     srv.served += 1
 
 
+def draft_kwargs(draft_model: str | None, draft_seed: int | None) -> dict:
+    """Engine keywords of --draft-model PRESET|DIR and --draft-seed: a directory is a checkpoint, anything else a preset."""
+    if not draft_model:
+        return {}
+    kw = dict(draft_weights_path=draft_model) if os.path.isdir(draft_model) else dict(draft_preset=draft_model)
+    if draft_seed is not None:
+        kw["draft_seed"] = draft_seed
+    return kw
+
+
 def serve(device: int, port: int, preset: str, model_name: str, max_batch: int = 8, greedy_tokens: int = 0, host="127.0.0.1",
           ready_event=None, seed: int = 1234, tokenizer: str | None = None, chat_family: str | None = None, prefix_cache: bool = False,
           speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
-          num_keep: int = 4, context_length: int = 0):
+          num_keep: int = 4, context_length: int = 0, draft_model: str | None = None, draft_seed: int | None = None):
     e = eng.Engine(preset=preset, model_name=model_name, device=device, seed=seed, max_batch=max_batch, start_scheduler=True,
                    prefix_cache=prefix_cache, speculate=speculate, speculate_batch=speculate_batch,
                    prefix_cache_host_bytes=prefix_cache_host_bytes, context_shift=context_shift, num_keep=num_keep,
-                   context_length=context_length)
+                   context_length=context_length, **draft_kwargs(draft_model, draft_seed))
     if tokenizer:
         e.load_tokenizer(tokenizer, chat_family)      # HF tokenizer.json instead of the byte-level fallback
     sampling = eng.greedy(greedy_tokens, ignore_eos=True) if greedy_tokens > 0 else None   # None = Ollama defaults
@@ -122,16 +133,24 @@ def main():
     ap.add_argument("--context-length", type=int, default=0,
                     help="the context window in tokens, up to 131072 (Ollama's num_ctx / OLLAMA_CONTEXT_LENGTH for the whole "
                          "worker; 0 = the model's default; env CL_CONTEXT_LENGTH overrides)")
+    ap.add_argument("--draft-model", default=None,
+                    help="with --speculate: a preset name or a model directory of the same vocabulary whose drafts the served "
+                         "model verifies, in place of drafting from the request's own history (env CL_DRAFT_MODEL)")
+    ap.add_argument("--draft-seed", type=int, default=None,
+                    help="synthetic-weight seed of a preset --draft-model (default: the served model's seed)")
     a = ap.parse_args()
     if a.prefix_cache_host_gib and not a.prefix_cache:
         ap.error("--prefix-cache-host-gib requires --prefix-cache")
+    if a.draft_model and not a.speculate:
+        ap.error("--draft-model requires --speculate")
     if a.num_keep is not None and not a.context_shift:
         ap.error("--num-keep requires --context-shift")
     print(f"worker on cuda:{a.device} port {a.port} serving {a.model_name}", flush=True)
     serve(a.device, a.port, a.preset, a.model_name, a.max_batch, a.greedy_tokens, tokenizer=a.tokenizer, chat_family=a.chat_family,
           prefix_cache=a.prefix_cache, speculate=a.speculate, speculate_batch=a.speculate_batch,
           prefix_cache_host_bytes=int(a.prefix_cache_host_gib * 2**30), context_shift=a.context_shift,
-          num_keep=4 if a.num_keep is None else a.num_keep, context_length=a.context_length)
+          num_keep=4 if a.num_keep is None else a.num_keep, context_length=a.context_length, draft_model=a.draft_model,
+          draft_seed=a.draft_seed)
 
 
 if __name__ == "__main__":

@@ -104,7 +104,8 @@ typedef struct cl_engine_config {
                               drafts the ids that followed the latest earlier occurrence of its last 3 (or 2) ids in its
                               prompt and output (cl_draft_ngram) and checks them in one pass over the weights
                               (cl_decode_verify).  The ids are the ones single steps would produce, up to near-tie flips
-                              between the two kernel paths.  Model shapes without the verify path decode normally. */
+                              between the two kernel paths.  Model shapes without the verify path decode normally.  With a
+                              draft model (cl_engine_create_with_draft, env CL_DRAFT_MODEL) the drafts come from it instead. */
   int32_t context_shift;   /* 1 => a request whose sequence fills max_seq_len shifts it (cl_seq_shift) and goes on generating
                               instead of ending with done_reason "length"; 0 => off (default; env CL_CONTEXT_SHIFT=0|1
                               overrides).  Ollama's rule, as its documentation states it (its source cannot be checked
@@ -257,7 +258,10 @@ typedef struct cl_spec_stats {
   int64_t tokens_accepted;   /* of which accepted */
   int64_t tokens_emitted;    /* tokens they emitted: tokens_accepted + verify_passes */
   int64_t multi_passes;      /* passes that verified two or more sequences at once (cl_engine_set_speculate_batch) */
-  int64_t reserved[3];
+  /* draft model (cl_engine_create_with_draft; all zero without one) */
+  int64_t draft_rows;        /* rows the draft computed: catch-up rows of its prefill passes plus its decode steps */
+  int64_t draft_ns;          /* host wall time inside draft calls (cl_draft_model and the scheduler's rounds) */
+  int64_t draft_pages_used;  /* now: pages of the draft's KV pool that mirrors hold */
 } cl_spec_stats;
 
 typedef struct cl_engine cl_engine;
@@ -293,6 +297,27 @@ int cl_draft_ngram(const int32_t* hist, int32_t n, int32_t k, int32_t* out, int3
 
 /* replaces: embedded Ollama server start, /root/reference/cmd/crowdllama/main.go:283-297 */
 int cl_engine_create(const cl_engine_config* cfg, cl_engine** out);
+/* cl_engine_create with a draft model for speculative decoding: a small model of the same vocabulary drafts, the served
+ * model verifies the drafts in one pass (cl_engine_config.speculate), in place of the prompt-lookup drafter.  Only
+ * draft->preset / model / weights_path / weights_seed are read; the draft runs on the target's device with the target's
+ * page size and window (max_seq_len), a KV pool of as many tokens as the target's, no scheduler, no prefix cache and no
+ * speculation of its own.  Every emitted id stays the served model's own greedy choice or seeded draw, so output does not
+ * depend on the draft; only how many ids a pass accepts does.
+ *   - Memory: with context_length > 0 and kv_pool_bytes == 0, both weight sets come off the free memory first, and the rest
+ *     (less the 4 GiB reserve) is split in proportion to KV bytes per token, so the target's pool is smaller than it would be
+ *     alone: 128 KiB against 32 KiB per token for Llama-3-8B with Llama-3.2-1B leaves the target 4/5 of it.  Otherwise the
+ *     target's pool is what it would be alone, and the draft's pool takes as many tokens on top.
+ *   - Drafting: each target sequence that drafts has a mirror sequence in the draft, freed with it.  A round gives the
+ *     mirror the window ending with the next input x0; the mirror keeps the longest common prefix of what it holds and that
+ *     window before x0, prefills the rest in one pass (1 or 2 rows after an accepted round; the whole window on first use or
+ *     after a context shift or preemption), and takes k - 1 steps.  A greedy request drafts the draft's argmax; a
+ *     device-sampled one draws with its own settings, penalty history and RNG step, so draft row i uses the same
+ *     (seed, step) as verify row i.  A sequence whose mirror gets no pages from the draft pool drafts nothing that round.
+ * CL_ERR_INVALID_ARG, with cl_last_error set, when the vocabularies differ, both models have a tokenizer.json and their
+ * bos / eos / stop ids differ, the target shape has no verify pass, speculate is 0, or the draft cannot serve the target's
+ * window; otherwise the errors of cl_engine_create.  cl_engine_create itself takes a draft from env CL_DRAFT_MODEL (a preset
+ * name or a model directory) with the synthetic-weight seed CL_DRAFT_SEED (default: the target's weights_seed). */
+int cl_engine_create_with_draft(const cl_engine_config* cfg, const cl_engine_config* draft, cl_engine** out);
 void cl_engine_destroy(cl_engine* e);
 int cl_engine_model_config(const cl_engine* e, cl_model_config* out);
 int cl_engine_stats(cl_engine* e, cl_stats* out);
@@ -441,6 +466,20 @@ int cl_decode_verify(cl_engine* e, cl_seq_t seq, int32_t input_id, const int32_t
 int cl_decode_verify_batch(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* input_ids, const int32_t* drafts,
                            const int32_t* ks, const cl_sampling* sp, const uint64_t* step0, int32_t* ids_out, int32_t* n_out,
                            float* logits_out);
+/* Speculative decoding, token level: the draft model's drafter (cl_engine_create_with_draft), the counterpart of
+ * cl_draft_ngram.  For each i < n_seqs, the mirror of target sequence seqs[i] (a live handle; its own K/V are not touched)
+ * catches up with hists[i][0..hist_lens[i]), the window whose last id is the next input x0, and drafts ks[i] ids (0..15)
+ * after it: one prefill pass over the catch-up rows of every sequence (its tail chooses d1; several sequences share one
+ * tile-path pass when their rows fit it), then max(ks) - 1 batched draft steps for the sequences with ks[i] >= 2.  Draft row
+ * j of sequence i is the draft's greedy argmax, or with a sampled sp[i] the draft's device draw at RNG step step0[i] + j
+ * with the window (plus d1 .. dj) as its penalty history; sp and step0 may be NULL (greedy, step 0).  The ids of sequence i
+ * land back to back in `drafts` after those of the sequences before it (sum of ks[j], j < i); n_drafts[i] = ks[i], 1 when its
+ * window (or the draft pool) leaves no room for the max(ks) - 1 steps, or 0 when the draft pool has no pages for that
+ * mirror.  Afterwards the mirror holds the window plus the drafts it fed (hist_lens[i] + max(ks) - 1 tokens when it took
+ * the steps).  CL_ERR_INVALID_ARG without a draft model, for a duplicate sequence, k
+ * outside 0..15, an empty window, an id out of range or settings that need the host sampler; CL_ERR_TOO_LONG past max_seq_len. */
+int cl_draft_model(cl_engine* e, const cl_seq_t* seqs, int32_t n_seqs, const int32_t* const* hists, const int32_t* hist_lens,
+                   const int32_t* ks, const cl_sampling* sp, const uint64_t* step0, int32_t* drafts, int32_t* n_drafts);
 
 /* Context shift, token level: the cached tokens [n_keep, n_keep + n_discard) of the sequence leave its cache.  Afterwards:
  *   - position p < n_keep holds exactly what it held;
