@@ -22,20 +22,33 @@ namespace cl {
 namespace {
 
 constexpr int HD = 128, REP = 4, P = 32;
-constexpr int NW = 4, NS = 3;                 // consumer warps (one per m16 tile), 32 KB ring slots
-constexpr int ROWS = kVerifyMaxRows * REP;    // A rows (64)
+constexpr int NS = 3;                         // ring slots
 constexpr int MAXS = 64;
-constexpr uint32_t SLOT = 32 * 1024;
+constexpr uint32_t PAGE_BYTES = 16 * 1024;    // one 32-token page: K lo|hi, V lo|hi
 constexpr float LOG2E = 1.4426950408889634f;
-constexpr size_t SMEM = (size_t)NS * SLOT + 2 * NS * 8 + (2 * NW * 16 + NW * 16 * HD + 2 * MAXS * ROWS + ROWS + 4) * 4 + 1024 + 64;
+// Two instantiations.  <4, 2>: 4 consumer warps (one per m16 tile, up to kVerifyMaxRows rows per segment) and two pages
+// per ring slot, one CTA per SM.  <1, 1>: one consumer warp (segments of one row, whose 4 A rows sit in m16 tile 0) and
+// one page per slot, about 64 KB of shared memory: three CTAs per SM (launches of kVerifyOneWarpMinSegs or more
+// segments of one row).  A row's instruction sequence is the same in both:
+// the same fragments, pages in the same order each with its own online-softmax update, hi + lo P, split-order combine.
+template <int NW, int PPS>
+struct VerifyShape {
+  static constexpr int ROWS = NW * 16;        // A rows: 4 per segment row
+  static constexpr uint32_t SLOT = PPS * PAGE_BYTES;
+  static constexpr size_t SMEM = (size_t)NS * SLOT + 2 * NS * 8 + (2 * NW * 16 + NW * 16 * HD + 2 * MAXS * ROWS + ROWS + 4) * 4 + 1024 + 64;
+};
+static_assert(VerifyShape<4, 2>::ROWS == kVerifyMaxRows * REP, "the 4-warp kernel covers the largest segment");
 
 struct VerifyTcArgs {
   AttnVerifyArgs a;
   long long layer_row0;                       // first row of this layer in the pool-wide tensor maps
 };
 
-__global__ void __launch_bounds__((NW + 1) * 32, 1)
+template <int NW, int PPS>
+__global__ void __launch_bounds__((NW + 1) * 32, NW == 1 ? 3 : 1)
 attn_verify_tc_kernel(const __grid_constant__ CUtensorMap kmap, const __grid_constant__ CUtensorMap vmap, const VerifyTcArgs t) {
+  constexpr int ROWS = VerifyShape<NW, PPS>::ROWS;
+  constexpr uint32_t SLOT = VerifyShape<NW, PPS>::SLOT;
   const AttnVerifyArgs& a = t.a;
   const int g = blockIdx.x, sp = blockIdx.y, sg = blockIdx.z;
   const int4 s0 = reinterpret_cast<const int4*>(a.segs)[2 * sg], s1 = reinterpret_cast<const int4*>(a.segs)[2 * sg + 1];
@@ -65,7 +78,7 @@ attn_verify_tc_kernel(const __grid_constant__ CUtensorMap kmap, const __grid_con
   const int pg0 = sp * pps;
   const int pg1 = min(total_pages, pg0 + pps);
   const int npg = pg1 > pg0 ? pg1 - pg0 : 0;
-  const int n_tiles = (npg + 1) / 2;
+  const int n_tiles = (npg + PPS - 1) / PPS;
   const int* bt = a.block_tables + (size_t)seq * a.bt_stride;
 
   if (warp == NW) {
@@ -76,13 +89,13 @@ attn_verify_tc_kernel(const __grid_constant__ CUtensorMap kmap, const __grid_con
     for (int it = 0; it < n_tiles; ++it) {
       const int st = it % NS;
       mbar_wait(&empty[st], ((uint32_t)(it / NS) & 1u) ^ 1u);
-      const int pa = pg0 + 2 * it;
-      const bool two = pa + 1 < pg1;
+      const int pa = pg0 + PPS * it;
+      const int npage = min(PPS, pg1 - pa);
       uint8_t* dst = ring + (size_t)st * SLOT;
-      mbar_arrive_expect_tx(&full[st], two ? 32768u : 16384u);
-      for (int pgi = 0; pgi < (two ? 2 : 1); ++pgi) {
+      mbar_arrive_expect_tx(&full[st], (uint32_t)npage * PAGE_BYTES);
+      for (int pgi = 0; pgi < npage; ++pgi) {
         const long long row = t.layer_row0 + ((long long)bt[pa + pgi] * a.n_kv + g) * P;
-        uint8_t* d = dst + pgi * 16384;
+        uint8_t* d = dst + pgi * PAGE_BYTES;
         tma_load_2d(d, &kmap, 0, (int)row, &full[st]);
         tma_load_2d(d + 4096, &kmap, 64, (int)row, &full[st]);
         tma_load_2d(d + 8192, &vmap, 0, (int)row, &full[st]);
@@ -120,10 +133,10 @@ attn_verify_tc_kernel(const __grid_constant__ CUtensorMap kmap, const __grid_con
   for (int it = 0; it < n_tiles; ++it) {
     const int st = it % NS;
     mbar_wait(&full[st], (uint32_t)(it / NS) & 1u);
-    const int npage = (pg0 + 2 * it + 1 < pg1) ? 2 : 1;
+    const int npage = min(PPS, pg1 - (pg0 + PPS * it));
     for (int pgi = 0; pgi < npage && active; ++pgi) {
-      const uint32_t kb = smem_u32(ring + (size_t)st * SLOT + pgi * 16384), vb = kb + 8192;
-      const int tok0 = (pg0 + 2 * it + pgi) * P;
+      const uint32_t kb = smem_u32(ring + (size_t)st * SLOT + pgi * PAGE_BYTES), vb = kb + 8192;
+      const int tok0 = (pg0 + PPS * it + pgi) * P;
       float sacc[4][4];
 #pragma unroll
       for (int nj = 0; nj < 4; ++nj) { sacc[nj][0] = sacc[nj][1] = sacc[nj][2] = sacc[nj][3] = 0.f; }
@@ -280,20 +293,33 @@ bool attn_verify_tc_supported(int n_heads, int n_kv, int head_dim, int page_size
 
 int attn_verify_max_splits() { return MAXS; }
 
-int launch_attn_verify_tc(const AttnVerifyArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st) {
-  if (!attn_verify_tc_supported(a.n_heads, a.n_kv, a.head_dim, a.page_size) || a.nsplit < 1 || a.nsplit > MAXS || a.n_segs < 1)
-    return -1;
+namespace {
+template <int NW, int PPS>
+int launch_inst(const AttnVerifyArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st) {
+  constexpr size_t SMEM = VerifyShape<NW, PPS>::SMEM;
   static PerDeviceOnce attr;
   if (attr.pending()) {
-    if (cudaFuncSetAttribute(attn_verify_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM) != cudaSuccess) {
+    if (cudaFuncSetAttribute(attn_verify_tc_kernel<NW, PPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM) != cudaSuccess) {
       fprintf(stderr, "[clengine] attn_verify_tc: %zu B of shared memory refused\n", SMEM);
       return -1;
     }
     attr.mark();
   }
   VerifyTcArgs t{a, layer_row0};
-  attn_verify_tc_kernel<<<dim3(a.n_kv, a.nsplit, a.n_segs), (NW + 1) * 32, SMEM, st>>>(kmap, vmap, t);
+  attn_verify_tc_kernel<NW, PPS><<<dim3(a.n_kv, a.nsplit, a.n_segs), (NW + 1) * 32, SMEM, st>>>(kmap, vmap, t);
   return cudaPeekAtLastError() == cudaSuccess ? 1 : -1;   // a failed launch stays visible to the caller's report
+}
+}  // namespace
+
+int launch_attn_verify_tc(const AttnVerifyArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st) {
+  if (!attn_verify_tc_supported(a.n_heads, a.n_kv, a.head_dim, a.page_size) || a.nsplit < 1 || a.nsplit > MAXS || a.n_segs < 1 ||
+      a.max_rows < 1 || a.max_rows > kVerifyMaxRows)
+    return -1;
+  // the one-warp kernel where every segment has one row and there are enough of them to fill the SMs with its three CTAs
+  // per SM: a deterministic step of B = 8 / 64 behind 4096 tokens spends 0.96 / 0.73 of its time with it, one of B = 1
+  // 1.08 (H100 80GB HBM3, profiles/h100_deterministic.json)
+  const bool one_warp = a.max_rows == 1 && a.n_segs >= kVerifyOneWarpMinSegs;
+  return one_warp ? launch_inst<1, 1>(a, kmap, vmap, layer_row0, st) : launch_inst<4, 2>(a, kmap, vmap, layer_row0, st);
 }
 
 }  // namespace cl

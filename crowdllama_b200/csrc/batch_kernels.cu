@@ -136,4 +136,14 @@ int launch_batch_scatter_rows(const float* y, int n, float* out, int out_stride,
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
+// ids[b] = tok[slots[b]]: a step's input ids in row order, for a pass that embeds rows (deterministic mode's step)
+__global__ void gather_tok_kernel(const int* __restrict__ tok, const int* __restrict__ slots, int B, int* __restrict__ ids) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) ids[b] = tok[slots[b]];
+}
+int launch_gather_tok(const int* tok, const int* slots, int B, int* ids, cudaStream_t st) {
+  gather_tok_kernel<<<(B + 127) / 128, 128, 0, st>>>(tok, slots, B, ids);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
 }  // namespace cl

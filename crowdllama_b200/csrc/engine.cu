@@ -93,6 +93,19 @@ int Engine::init(const cl_engine_config& c, const cl_engine_config* draft) {
     }
     if (env_int("CL_SPECULATE", c.speculate) == 0) { set_last_error("draft model: speculate is 0, so nothing would use it"); return CL_ERR_INVALID_ARG; }
   }
+  // Deterministic mode runs every row through small_pass with the multi-row attention: its shapes (the split-K pass's
+  // d_model <= 8192 included), and steps of at most one pass of rows.  Refused before the device is touched.  A draft
+  // model's engine never runs it: drafts decide how many ids a pass accepts, not which ids.
+  deterministic_ = !is_draft_ && env_int("CL_DETERMINISTIC", c.deterministic) != 0;
+  if (deterministic_ && (!attn_verify_tc_supported(cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, c.page_size ? c.page_size : 32) ||
+                         cfg.d_model > 8192)) {
+    set_last_error("deterministic mode needs head_dim 128, 4 query heads per kv head and page_size 32");
+    return CL_ERR_INVALID_ARG;
+  }
+  if (deterministic_ && c.max_batch > kSpecMaxRows) {
+    set_last_error("deterministic mode takes max_batch up to " + std::to_string(kSpecMaxRows));
+    return CL_ERR_INVALID_ARG;
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
     cudaGetLastError();
@@ -125,7 +138,7 @@ int Engine::init(const cl_engine_config& c, const cl_engine_config* draft) {
   qkv_dim_ = q_dim_ + 2 * kv_dim_;
   nsplit_ = std::max(1, std::min(64, sm_count() / cfg.n_kv_heads));
   // decided AFTER nsplit_ is final: the persistent kernel's lane-parallel combine and part buffer are sized by it
-  use_mega_ = env_int("CL_MEGA", 1) != 0 &&
+  use_mega_ = !deterministic_ && env_int("CL_MEGA", 1) != 0 &&
               mega_supported(cfg.d_model, cfg.d_ff, cfg.head_dim, cfg.n_heads, cfg.n_kv_heads, page_size_, nsplit_);
   max_pages_per_seq_ = (cfg.max_seq_len + page_size_ - 1) / page_size_;
 
@@ -159,6 +172,13 @@ int Engine::init(const cl_engine_config& c, const cl_engine_config* draft) {
     const uint64_t rows = (uint64_t)cfg.n_layers * n_pages_ * cfg.n_kv_heads * page_size_;
     have_kv_maps_ = rows < (1ull << 31) && make_tmap_2d_bf16(&kmap_, kpool_, rows, cfg.head_dim, 64, 32) &&
                     make_tmap_2d_bf16(&vmap_, vpool_, rows, cfg.head_dim, 64, 32);
+  }
+  if (deterministic_) {
+    if (!spec_path_ok()) { set_last_error("deterministic mode: the model shape has no tensor-core split-K path"); return CL_ERR_INVALID_ARG; }
+    if (!have_kv_maps_) { set_last_error("deterministic mode: the KV pool is too large for its tensor maps"); return CL_ERR_INVALID_ARG; }
+    if ((rc = ensure_small_ws()) || (rc = ensure_spec_ws())) return rc;
+    DMALLOC(det_ids_, (size_t)kSpecMaxRows * 4);
+    DMALLOC(det_xn_, (size_t)kSpecMaxRows * cfg.d_model * 2);
   }
   if (use_mega_ && !have_kv_maps_) {
     fprintf(stderr, "[clengine] KV tensor maps unavailable: using the per-op decode path\n");
@@ -210,6 +230,7 @@ int Engine::init(const cl_engine_config& c, const cl_engine_config* draft) {
   if (sched_prefill_chunk_ > 0 && sched_prefill_chunk_ < 16) sched_prefill_chunk_ = 16;
   prefill_small_max_ = std::min(256, env_int("CL_PREFILL_SMALL_MAX", kDefaultPrefillSmallMax));
   device_sample_ = env_int("CL_DEVICE_SAMPLE", 1) != 0;
+  verify_one_row_ = env_int("CL_VERIFY_ONE_ROW", 1) != 0;
   if (is_draft_) return CL_OK;   // a draft serves its target's drafter only: no prefix cache, shift, speculation or scheduler
   prefix_cache_ = env_int("CL_PREFIX_CACHE", c.prefix_cache) != 0;
   context_shift_ = env_int("CL_CONTEXT_SHIFT", c.context_shift) != 0;
@@ -744,7 +765,8 @@ void LaunchProfiler::report(const char* tag, int key_width, const std::string& h
 }
 
 // ---- one token step for the sequences listed in d_slots_[0..B) -----------------------------------
-int Engine::enqueue_step(int B) {
+int Engine::enqueue_step(int B, int step_off) {
+  if (deterministic_) return det_step(B, step_off);
   if (B >= 2 && use_batch_gemm_ && bws_) return enqueue_step_batched(B);   // from B = 2: faster than two GEMV passes
   const int d = cfg.d_model, F = cfg.d_ff, L_ = cfg.n_layers;
   int launches = 0;
@@ -839,8 +861,9 @@ int Engine::enqueue_step_tail(int B, bool push_input) {
 // 9 x 13 with 5 splits.  Among the counts within 10 % of the best the smallest wins
 // (fewer partials for the consumer kernel to sum).
 int pick_splits_public(int n_rows, int K) { return pick_splits(n_rows, K); }
-static int pick_splits(int n_rows, int K) {
-  const int tiles = (n_rows + 127) / 128, nkb = (K + 63) / 64, sms = sm_count();
+static int pick_splits(int n_rows, int K) { return pick_splits_sms(n_rows, K, sm_count()); }
+int pick_splits_sms(int n_rows, int K, int sms) {
+  const int tiles = (n_rows + 127) / 128, nkb = (K + 63) / 64;
   int best_cost = 1 << 30;
   int cost_of[17];
   for (int s = 1; s <= 16; ++s) {
@@ -938,13 +961,13 @@ bool Engine::ensure_graph(int B) {
 // (box benchmark, 64 concurrent chats: 16.6 req/s with lazy capture against 24.6 warm).  Called once when the
 // scheduler thread starts.
 void Engine::precapture_graphs(int max_b) {
-  if (!use_graph_) return;
+  if (!use_graph_ || deterministic_) return;
   for (int B = 1; B <= max_b && !graph_failed_; ++B) ensure_graph(B);
   cudaStreamSynchronize(stream_);
 }
 
-int Engine::run_step_graph(int B) {
-  if (use_graph_ && !graph_failed_) {
+int Engine::run_step_graph(int B, int step_off) {
+  if (use_graph_ && !graph_failed_ && !deterministic_) {
     ensure_graph(B);
     auto it = graphs_.find(B);
     if (it != graphs_.end()) {
@@ -953,7 +976,7 @@ int Engine::run_step_graph(int B) {
       return CL_OK;
     }
   }
-  const int n = enqueue_step(B);
+  const int n = enqueue_step(B, step_off);
   if (n < 0) return n;
   launches_ += n;
   return CL_OK;
@@ -968,6 +991,7 @@ int Engine::read_logits(int slot, float* out) {
 }
 
 int Engine::set_single_slot(cl_seq_t s) {
+  h_slots_.assign(1, s);
   if (last_single_slot_ != s) {
     CL_CUDA_OK(cudaMemcpyAsync(d_slots_, &s, 4, cudaMemcpyHostToDevice, stream_));
     last_single_slot_ = s;
@@ -1042,7 +1066,9 @@ int Engine::prefill(cl_seq_t s, const int32_t* ids, int n, float* logits_out) {
     if (ids[i] < 0 || ids[i] >= cfg.vocab_size) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
   if (seqs_[s].len + n > cfg.max_seq_len) { set_last_error("sequence exceeds max_seq_len"); return CL_ERR_TOO_LONG; }
   int rc;
-  if (n >= prefill_min_tokens_ && prefill_path_ok()) {
+  if (deterministic_) {
+    rc = det_prefill(1, &s, &ids, &n, logits_out);
+  } else if (n >= prefill_min_tokens_ && prefill_path_ok()) {
     // short prompts: split-K projections so that every SM streams weights (d_model <= 8192: one 1024-thread CTA per row in the glue)
     if (n <= prefill_small_max_ && cfg.d_model <= 8192 && cfg.d_model % 4 == 0) rc = prefill_small(s, ids, n, logits_out);
     else rc = prefill_chunked(s, ids, n, logits_out);
@@ -1068,6 +1094,7 @@ int Engine::decode_greedy(const cl_seq_t* ss, int B, const int32_t* first_ids, i
     CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &seqs_[s].len, 4, cudaMemcpyHostToDevice, stream_));
   }
   CL_CUDA_OK(cudaMemcpyAsync(d_slots_, ss, (size_t)B * 4, cudaMemcpyHostToDevice, stream_));
+  h_slots_.assign(ss, ss + B);
   last_single_slot_ = B == 1 ? ss[0] : -1;
   if (B > 1) last_batch_slots_.assign(ss, ss + B);
   slots_dirty_ = true;
@@ -1077,7 +1104,7 @@ int Engine::decode_greedy(const cl_seq_t* ss, int B, const int32_t* first_ids, i
     CL_CUDA_OK(cudaMemsetAsync(d_step_counter_, 0, 4, stream_));
     CL_CUDA_OK(cudaEventRecord(ev0_, stream_));
     for (int i = 0; i < chunk; ++i) {
-      const int rc = run_step_graph(B);
+      const int rc = run_step_graph(B, done + i);
       if (rc) return rc;
     }
     CL_CUDA_OK(cudaEventRecord(ev1_, stream_));
@@ -1191,6 +1218,7 @@ int Engine::decode_step_batch(const cl_seq_t* ss, int B, const int32_t* ids, flo
     CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + s, &seqs_[s].len, 4, cudaMemcpyHostToDevice, stream_));
   }
   CL_CUDA_OK(cudaMemcpyAsync(d_slots_, ss, (size_t)B * 4, cudaMemcpyHostToDevice, stream_));
+  h_slots_.assign(ss, ss + B);
   last_single_slot_ = B == 1 ? ss[0] : -1;
   if (B > 1) last_batch_slots_.assign(ss, ss + B);
   slots_dirty_ = true;
@@ -1216,6 +1244,7 @@ int Engine::decode_step_batch(const cl_seq_t* ss, int B, const int32_t* ids, flo
 // whole-stack kernel (or, on the per-op path, the stack of per-layer kernels between the embedding and the LM head).
 int Engine::time_dominant_kernel(cl_seq_t s, int32_t first_id, int n_steps, float* kernel_ms, float* step_ms) {
   if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+  if (deterministic_) { set_last_error("time_dominant_kernel: deterministic mode has no step of the timed kernels"); return CL_ERR_INVALID_ARG; }
   if (n_steps <= 0 || n_steps > 4096 || first_id < 0 || first_id >= cfg.vocab_size) { set_last_error("bad steps / token"); return CL_ERR_INVALID_ARG; }
   int rc = ensure_capacity(s, seqs_[s].len + n_steps);
   if (rc) return rc;

@@ -43,6 +43,12 @@ constexpr int kDraftNgramMin = 2;
 constexpr int kSpecBackoff = 8;       // tokens a request decodes without drafting after a verify pass that accepted nothing
 constexpr int kSpecMaxRows = 128;     // rows of one verify pass over several sequences (Engine::verify_batch) at most
 constexpr int kSpecBatchMax = 32;     // sequences the scheduler verifies in one pass at most (cl_engine_set_speculate_batch)
+// Deterministic mode (cl_engine_config.deterministic): split-K counts are pick_splits' at this many SMs (an H100 SXM's)
+// whatever the device has, so a card with fewer SMs computes the same bits
+constexpr int kDetSms = 132;
+
+// split-K count of an n_rows x K projection on sms SMs (engine.cu: the batched step's and the split-K pass's rule)
+int pick_splits_sms(int n_rows, int K, int sms);
 
 // Prompt-lookup drafter: the longest suffix of hist[0..n) of length kDraftNgramMax .. kDraftNgramMin that also occurs
 // earlier in hist; from its most recent earlier occurrence, the up to k ids that followed it (stopping at the end of
@@ -437,6 +443,7 @@ class Engine {
   int64_t spec_multi_passes() const { return spec_multi_passes_; }
   int spec_stats(cl_spec_stats* out);
   bool device_sample() const { return device_sample_; }
+  bool deterministic() const { return deterministic_; }
   int set_tensor(int layer, int kind, const uint16_t* data, int64_t n);
   int load_safetensors(const std::string& path);   // HF llama-layout checkpoint (file or directory) -> set_tensor (weights_io.cpp)
   // parity / benchmark aids (token level)
@@ -485,13 +492,22 @@ class Engine {
   // full pages whose tokens are all known are published.  The first n_known ids are real tokens; a placeholder stops
   // publishing for the rest of the sequence.  The work that wrote the pages is already on stream_, ahead of any reader.
   void seq_advance(cl_seq_t s, const int32_t* ids, int n, int n_known);
-  int enqueue_step(int B);                         // kernels of one token step for d_slots_[0..B)
+  // kernels of one token step for d_slots_[0..B); step_off: steps already enqueued since the sequences' lengths were last
+  // advanced on the host (a device loop's step index), which deterministic mode needs for its segment table
+  int enqueue_step(int B, int step_off = 0);
   int enqueue_step_batched(int B);                 // B >= 2: wgmma projections + per-sequence glue kernels
   int enqueue_lm_head(int B, bool pdl);            // final norm + LM-head GEMV of d_h_ -> d_logits_ for d_slots_[0..B)
   // argmax (or, on armed slots, a draw) of d_logits_, advance tok / pos, id ring (step_tail_kernel); push_input: decode
   // steps, whose input token joins an armed slot's history.  Prefill tails do not push: the armed history holds the prompt.
   int enqueue_step_tail(int B, bool push_input);
-  int run_step_graph(int B);
+  int run_step_graph(int B, int step_off = 0);    // deterministic mode: enqueue_step, eagerly
+  // Deterministic mode (prefill.cu).  det_step: the step of B sequences as B one-row segments of small_pass, its LM head the
+  // pass's wgmma GEMM, then the step tail.  det_prefill: prompts of n_seqs distinct sequences as passes of at most
+  // kSpecMaxRows rows, each prompt cut into segments of at most kVerifyMaxRows rows; the last rows' logits from the same
+  // GEMM head, then the step tail without pushing its input (collect_logprobs is the caller's).
+  int det_step(int B, int step_off);
+  int det_prefill(int n_seqs, const cl_seq_t* ss, const int32_t* const* ids, const int* lens, float* logits_out);
+  int proj_splits(int N, int K) const;            // split-K count of the split-K pass's projections (kDetSms in deterministic mode)
   bool ensure_graph(int B);
   void precapture_graphs(int max_b);              // the step graphs of batch sizes 1..max_b
   int read_logits(int slot, float* out);
@@ -522,6 +538,8 @@ class Engine {
   // kernel where the shape allows it.
   int small_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, const int* row_map, const int* seg_table, int& launches,
                  LaunchProfiler& prof);
+  // row map and segment table of a small_pass over segs into spec_->row_map / spec_->segs (the multi-row attention's plan)
+  int upload_pass_tables(const PrefillSegment* segs, int n_segs, int T);
   int ensure_spec_ws();
   SpecTailArgs spec_tail_args(const PrefillSegment& g, int out_off) const;   // the spec tail of one verify segment
   bool prefill_path_ok() const;
@@ -592,6 +610,11 @@ class Engine {
   LogprobRecord* d_lp_last_ = nullptr; LogprobRecord* d_lp_ring_ = nullptr; LogprobRecord* h_lp_pinned_ = nullptr;
   std::vector<int> lp_n_;             // host mirror of d_lp_n_
   bool device_sample_ = true;         // CL_DEVICE_SAMPLE: the scheduler and the synchronous path draw on the device where they can
+  bool deterministic_ = false;        // CL_DETERMINISTIC / cl_engine_config.deterministic (det_step, det_prefill)
+  bool verify_one_row_ = true;        // CL_VERIFY_ONE_ROW: passes of one-row segments run the one-warp multi-row attention
+  std::vector<int> h_slots_;          // host copy of d_slots_[0..B) as its last upload left it (det_step's segment table)
+  int* det_ids_ = nullptr;            // det_step: the step's input ids, row order [kSpecMaxRows]
+  __nv_bfloat16* det_xn_ = nullptr;   // det_prefill: final-norm rows of the prompts' last tokens [kSpecMaxRows][d]
 
   // prefill workspace (allocated lazily)
   struct PrefillWs {

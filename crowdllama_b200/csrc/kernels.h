@@ -318,7 +318,9 @@ struct AttnVerifyArgs {
   int n_segs = 0, n_heads = 0, n_kv = 0, head_dim = 0, page_size = 0;
   int nsplit = 1;                        // grid splits: the largest of the segments' split counts
   int split_pages = 0;                   // > 0: every split covers this many pages; 0: a segment's pages spread over its splits
+  int max_rows = kVerifyMaxRows;         // rows of the launch's largest segment (1 with >= kVerifyOneWarpMinSegs segments: one warp)
 };
+constexpr int kVerifyOneWarpMinSegs = 8;   // one-row segments the one-warp instantiation needs to be the faster one
 bool attn_verify_tc_supported(int n_heads, int n_kv, int head_dim, int page_size);
 int attn_verify_max_splits();
 int launch_attn_verify_tc(const AttnVerifyArgs& a, const CUtensorMap& kmap, const CUtensorMap& vmap, long long layer_row0, cudaStream_t st);
@@ -330,5 +332,6 @@ int launch_batch_rope_append(const float* ypart, int n_split, int B, const QkvEp
 int launch_batch_silu(const float* ypart, int n_split, int B, int d_ff, __nv_bfloat16* act, cudaStream_t st, bool pdl = false);
 int launch_batch_scatter_rows(const float* y, int n, float* out, int out_stride, const int* slots, int B, cudaStream_t st);
 int launch_embed_rows(const __nv_bfloat16* table, int d, const int* ids_dev, float* h, int T, cudaStream_t st);
+int launch_gather_tok(const int* tok, const int* slots, int B, int* ids, cudaStream_t st);   // ids[b] = tok[slots[b]]
 
 }  // namespace cl

@@ -546,6 +546,7 @@ int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, co
   a.q = dq.as<__nv_bfloat16>(); a.q_stride = (int)qd; a.segs = dseg.as<int>(); a.block_tables = dbt.as<int>(); a.bt_stride = pool.bt_stride;
   a.out = dout.as<__nv_bfloat16>(); a.out_stride = (int)qd; a.part = dpart.as<float>(); a.counters = dcnt.as<unsigned>();
   a.n_segs = n_segs; a.n_heads = n_heads; a.n_kv = n_kv; a.head_dim = HD; a.page_size = P; a.nsplit = grid_splits; a.split_pages = split_pages;
+  a.max_rows = *std::max_element(rows, rows + n_segs);
   // two launches without re-arming the split counters in between must give the same bits
   std::vector<uint16_t> first((size_t)T * qd);
   for (int run = 0; run < 2; ++run) {

@@ -44,7 +44,7 @@ static int launch_attn_prefill_as_verify(const AttnPrefillArgs& a, const CUtenso
   va.q = a.q; va.q_stride = a.n_heads * a.head_dim; va.segs = seg_dev; va.block_tables = a.block_table; va.bt_stride = 0;
   va.out = a.out; va.out_stride = a.n_heads * a.head_dim; va.part = part; va.counters = counters;
   va.n_segs = 1; va.n_heads = a.n_heads; va.n_kv = a.n_kv; va.head_dim = a.head_dim; va.page_size = a.page_size;
-  va.nsplit = ns; va.split_pages = split_pages;
+  va.nsplit = ns; va.split_pages = split_pages; va.max_rows = a.T;
   return launch_attn_verify_tc(va, km, vm, row0, st);
 }
 
@@ -149,7 +149,7 @@ int Engine::prefill_small(cl_seq_t s, const int32_t* ids, int n, float* logits_o
 int Engine::ensure_small_ws() {
   if (sws_) return CL_OK;
   const int d = cfg.d_model, F = cfg.d_ff;
-  const int s_qkv = pick_splits_public(qkv_dim_, d), s_o = pick_splits_public(d, q_dim_), s_gu = pick_splits_public(2 * F, d), s_dn = pick_splits_public(d, F);
+  const int s_qkv = proj_splits(qkv_dim_, d), s_o = proj_splits(d, q_dim_), s_gu = proj_splits(2 * F, d), s_dn = proj_splits(d, F);
   sws_.reset(new SmallPrefillWs());
   const size_t Tm = 256;
   size_t part = 0;
@@ -178,7 +178,7 @@ int Engine::ensure_small_ws() {
 int Engine::small_pass(const PrefillSegment* segs, int n_segs, const int* ids, int T, const int* row_map, const int* seg_table,
                        int& launches, LaunchProfiler& prof) {
   const int d = cfg.d_model, F = cfg.d_ff;
-  const int s_qkv = pick_splits_public(qkv_dim_, d), s_o = pick_splits_public(d, q_dim_), s_gu = pick_splits_public(2 * F, d), s_dn = pick_splits_public(d, F);
+  const int s_qkv = proj_splits(qkv_dim_, d), s_o = proj_splits(d, q_dim_), s_gu = proj_splits(2 * F, d), s_dn = proj_splits(d, F);
   SmallPrefillWs& w = *sws_;
   int rc;
   pass_ = PassRecord{};
@@ -190,8 +190,11 @@ int Engine::small_pass(const PrefillSegment* segs, int n_segs, const int* ids, i
     va.n_segs = n_segs; va.n_heads = cfg.n_heads; va.n_kv = cfg.n_kv_heads; va.head_dim = cfg.head_dim; va.page_size = page_size_;
     va.split_pages = verify_split_pages();
     va.nsplit = 1;
-    for (int i = 0; i < n_segs; ++i)
+    va.max_rows = verify_one_row_ ? 1 : kVerifyMaxRows;
+    for (int i = 0; i < n_segs; ++i) {
       va.nsplit = std::max(va.nsplit, ((segs[i].pos0 + segs[i].n + page_size_ - 1) / page_size_ + va.split_pages - 1) / va.split_pages);
+      va.max_rows = std::max(va.max_rows, segs[i].n);
+    }
   }
   // programmatic dependent launch between the GEMMs and the per-row glue kernels, as in the batched decode step (the two
   // prefill kernels in between are launched normally and order the stream)
@@ -296,6 +299,7 @@ int Engine::verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, cons
                          int* n_out, float* logits_out, bool seg_table) {
   if (n_seqs < 1 || !ss || !x0 || !ks || !ids_out || !n_out) { set_last_error("verify_batch: bad arguments"); return CL_ERR_INVALID_ARG; }
   if (!spec_path_ok()) { set_last_error("verify: the model shape has no tensor-core split-K path"); return CL_ERR_INVALID_ARG; }
+  if (deterministic_) seg_table = true;   // every row of every pass through the multi-row attention
   const int V = cfg.vocab_size, d = cfg.d_model;
   std::vector<PrefillSegment> segs(n_seqs);
   std::vector<int32_t> in;
@@ -321,21 +325,7 @@ int Engine::verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x0, cons
     if ((rc = ensure_capacity(g.seq, g.pos0 + g.n))) return rc;
   if ((rc = ensure_small_ws()) || (rc = ensure_spec_ws())) return rc;
   CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, in.data(), (size_t)T * 4, cudaMemcpyHostToDevice, stream_));
-  if (seg_table) {
-    std::vector<int> row_map(2 * (size_t)T), table(8 * (size_t)n_seqs, 0);
-    const int split_pages = verify_split_pages();
-    long long part_off = 0;
-    for (int i = 0; i < n_seqs; ++i) {
-      const PrefillSegment& g = segs[i];
-      for (int r = 0; r < g.n; ++r) { row_map[g.row0 + r] = g.seq; row_map[T + g.row0 + r] = g.pos0 + r; }
-      const int pages = (g.pos0 + g.n + page_size_ - 1) / page_size_, ns = (pages + split_pages - 1) / split_pages;
-      int* e = &table[8 * (size_t)i];
-      e[0] = g.seq; e[1] = g.row0; e[2] = g.n; e[3] = g.pos0; e[4] = (int)part_off; e[5] = ns;
-      if (ns > 1) part_off += (long long)cfg.n_kv_heads * ns * 4 * g.n * (cfg.head_dim + 2);
-    }
-    CL_CUDA_OK(cudaMemcpyAsync(spec_->row_map, row_map.data(), row_map.size() * 4, cudaMemcpyHostToDevice, stream_));
-    CL_CUDA_OK(cudaMemcpyAsync(spec_->segs, table.data(), table.size() * 4, cudaMemcpyHostToDevice, stream_));
-  }
+  if (seg_table && (rc = upload_pass_tables(segs.data(), n_seqs, T))) return rc;
   int launches = 0;
   LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
   if ((rc = small_pass(segs.data(), n_seqs, d_prompt_, T, seg_table ? spec_->row_map : nullptr, seg_table ? spec_->segs : nullptr,
@@ -407,6 +397,118 @@ int Engine::decode_verify_batch(const cl_seq_t* ss, int n_seqs, const int32_t* x
     if (rc == CL_OK) rc = r2;
   }
   return rc;
+}
+
+int Engine::proj_splits(int N, int K) const { return deterministic_ ? pick_splits_sms(N, K, kDetSms) : pick_splits_public(N, K); }
+
+// Segment i gets entry i of the table: its block-table row, first row, rows, cached length, partial offset and split count
+// (verify_split_pages() pages per split), and every row its (sequence, position) in the row map.
+int Engine::upload_pass_tables(const PrefillSegment* segs, int n_segs, int T) {
+  std::vector<int> row_map(2 * (size_t)T), table(8 * (size_t)n_segs, 0);
+  const int split_pages = verify_split_pages();
+  long long part_off = 0;
+  for (int i = 0; i < n_segs; ++i) {
+    const PrefillSegment& g = segs[i];
+    for (int r = 0; r < g.n; ++r) { row_map[g.row0 + r] = g.seq; row_map[T + g.row0 + r] = g.pos0 + r; }
+    const int pages = (g.pos0 + g.n + page_size_ - 1) / page_size_, ns = (pages + split_pages - 1) / split_pages;
+    int* e = &table[8 * (size_t)i];
+    e[0] = g.seq; e[1] = g.row0; e[2] = g.n; e[3] = g.pos0; e[4] = (int)part_off; e[5] = ns;
+    if (ns > 1) part_off += (long long)cfg.n_kv_heads * ns * 4 * g.n * (cfg.head_dim + 2);
+  }
+  CL_CUDA_OK(cudaMemcpyAsync(spec_->row_map, row_map.data(), row_map.size() * 4, cudaMemcpyHostToDevice, stream_));
+  CL_CUDA_OK(cudaMemcpyAsync(spec_->segs, table.data(), table.size() * 4, cudaMemcpyHostToDevice, stream_));
+  return CL_OK;
+}
+
+// Deterministic mode's token step.  Sequence h_slots_[b] is one-row segment b of a split-K pass at its position (its
+// length plus the steps a device loop enqueued since), so its row is computed as in a verify pass or a prefill pass: the
+// same per-row kernels, split counts and split plan, whatever else shares the step.  The host knows every length, so the
+// attention's grid has exactly the splits the longest sequence needs.  Eager launches: the segment table changes every step.
+int Engine::det_step(int B, int step_off) {
+  const int V = cfg.vocab_size, d = cfg.d_model;
+  if ((int)h_slots_.size() != B) { set_last_error("deterministic step: the host slot list does not match the batch"); return CL_ERR_INTERNAL; }
+  std::vector<PrefillSegment> segs(B);
+  for (int b = 0; b < B; ++b) segs[b] = PrefillSegment{h_slots_[b], b, 1, seqs_[h_slots_[b]].len + step_off};
+  int rc = upload_pass_tables(segs.data(), B, B);
+  if (rc) return rc;
+  int launches = 0;
+  LaunchProfiler prof(stream_, "CL_STEP_PROFILE");
+  CL_LAUNCH(launch_gather_tok(d_tok_, d_slots_, B, det_ids_, stream_));
+  if ((rc = small_pass(segs.data(), B, det_ids_, B, spec_->row_map, spec_->segs, launches, prof))) return rc;
+  CL_LAUNCH(launch_gemm_bf16(sws_->xn, lm_head_, spec_->logits, nullptr, B, V, d, stream_, 1, false));
+  CL_LAUNCH(launch_batch_scatter_rows(spec_->logits, V, d_logits_, V, d_slots_, B, stream_));
+  CL_LAUNCH(enqueue_step_tail(B, true));
+  prof.report("step profile", 34, "deterministic, B=" + std::to_string(B));
+  return launches;
+}
+
+// Deterministic mode's prefill of n_seqs distinct sequences (prefill, prefill_multi): their rows back to back in passes of
+// at most kSpecMaxRows rows, each prompt cut into segments of at most kVerifyMaxRows rows at consecutive cached lengths.  A
+// segment attends to the K/V its pass wrote for the segments before it.  Every prompt's last final-norm row is kept in
+// det_xn_; one GEMM head over those rows and the step tail (no input pushed) choose each sequence's next id.
+int Engine::det_prefill(int n_seqs, const cl_seq_t* ss, const int32_t* const* ids, const int* lens, float* logits_out) {
+  const int V = cfg.vocab_size, d = cfg.d_model;
+  if (n_seqs > max_batch_) { set_last_error("prefill: more sequences than max_batch"); return CL_ERR_INVALID_ARG; }
+  for (int i = 0; i < n_seqs; ++i) {
+    const int s = ss[i];
+    if (s < 0 || s >= max_seqs_ || !seqs_[s].live) return CL_ERR_BAD_SEQ;
+    for (int c = 0; c < i; ++c) if (ss[c] == s) { set_last_error("duplicate sequence in batch"); return CL_ERR_INVALID_ARG; }
+    if (lens[i] <= 0 || !ids[i]) { set_last_error("empty prompt"); return CL_ERR_INVALID_ARG; }
+    for (int t = 0; t < lens[i]; ++t)
+      if (ids[i][t] < 0 || ids[i][t] >= V) { set_last_error("token id out of range"); return CL_ERR_INVALID_ARG; }
+    if (seqs_[s].len + lens[i] > cfg.max_seq_len) { set_last_error("sequence exceeds max_seq_len"); return CL_ERR_TOO_LONG; }
+  }
+  int rc;
+  for (int i = 0; i < n_seqs; ++i)
+    if ((rc = ensure_capacity(ss[i], seqs_[ss[i]].len + lens[i]))) return rc;
+  int launches = 0;
+  LaunchProfiler prof(stream_, "CL_PREFILL_PROFILE");
+  std::vector<PrefillSegment> segs;
+  std::vector<int32_t> in;
+  std::vector<std::pair<int, int>> lasts;   // (sequence index, pass row) of the prompts that end in the pending pass
+  int T = 0, total = 0;
+  auto run_pass = [&]() -> int {
+    CL_CUDA_OK(cudaMemcpyAsync(d_prompt_, in.data(), (size_t)T * 4, cudaMemcpyHostToDevice, stream_));
+    int r = upload_pass_tables(segs.data(), (int)segs.size(), T);
+    if (r || (r = small_pass(segs.data(), (int)segs.size(), d_prompt_, T, spec_->row_map, spec_->segs, launches, prof))) return r;
+    for (const auto& lr : lasts)
+      CL_CUDA_OK(cudaMemcpyAsync(det_xn_ + (size_t)lr.first * d, sws_->xn + (size_t)lr.second * d, (size_t)d * 2, cudaMemcpyDeviceToDevice, stream_));
+    segs.clear(); in.clear(); lasts.clear();
+    T = 0;
+    return CL_OK;
+  };
+  for (int i = 0; i < n_seqs; ++i) {
+    for (int r0 = 0; r0 < lens[i];) {
+      if (T == kSpecMaxRows && (rc = run_pass())) return rc;
+      const int n = std::min({kVerifyMaxRows, lens[i] - r0, kSpecMaxRows - T});
+      segs.push_back(PrefillSegment{ss[i], T, n, seqs_[ss[i]].len + r0});
+      in.insert(in.end(), ids[i] + r0, ids[i] + r0 + n);
+      T += n; r0 += n;
+      if (r0 == lens[i]) lasts.emplace_back(i, T - 1);
+    }
+    total += lens[i];
+  }
+  if ((rc = run_pass())) return rc;
+  // each prompt's last position -> its slot, then the head and the tail of a step over those slots
+  std::vector<int> last_pos(n_seqs);
+  for (int i = 0; i < n_seqs; ++i) {
+    last_pos[i] = seqs_[ss[i]].len + lens[i] - 1;
+    CL_CUDA_OK(cudaMemcpyAsync(d_pos_ + ss[i], &last_pos[i], 4, cudaMemcpyHostToDevice, stream_));
+  }
+  CL_CUDA_OK(cudaMemcpyAsync(d_slots_, ss, (size_t)n_seqs * 4, cudaMemcpyHostToDevice, stream_));
+  h_slots_.assign(ss, ss + n_seqs);
+  slots_dirty_ = true;
+  last_single_slot_ = n_seqs == 1 ? ss[0] : -1;
+  CL_LAUNCH(launch_gemm_bf16(det_xn_, lm_head_, spec_->logits, nullptr, n_seqs, V, d, stream_, 1, false));
+  CL_LAUNCH(launch_batch_scatter_rows(spec_->logits, V, d_logits_, V, d_slots_, n_seqs, stream_));
+  CL_LAUNCH(enqueue_step_tail(n_seqs, false));
+  prof.report("prefill profile", 32, "deterministic passes, " + std::to_string(total) + " tokens");
+  launches_ += launches;
+  for (int i = 0; i < n_seqs; ++i) seq_advance(ss[i], ids[i], lens[i], lens[i]);
+  for (int i = 0; i < n_seqs && logits_out; ++i)
+    if ((rc = read_logits(ss[i], logits_out + (size_t)i * V))) return rc;
+  if (!logits_out) CL_CUDA_OK(cudaStreamSynchronize(stream_));
+  return CL_OK;
 }
 
 // (Re)allocate the tile-path workspace for passes of up to `tokens` rows; old buffers stay in allocs_ until the engine dies
@@ -503,6 +605,10 @@ int Engine::prefill_chunked(cl_seq_t s, const int32_t* ids, int n, float* logits
 // by the summation order only (tests/test_gpu_prefill.py).
 int Engine::prefill_multi(int n_seqs, const cl_seq_t* ss, const int32_t* const* ids, const int* lens, float* logits_out) {
   if (n_seqs <= 0 || !ss || !ids || !lens) { set_last_error("prefill_multi: bad arguments"); return CL_ERR_INVALID_ARG; }
+  if (deterministic_) {
+    const int rc = det_prefill(n_seqs, ss, ids, lens, logits_out);
+    return rc ? rc : collect_logprobs(ss, n_seqs);
+  }
   if (!prefill_path_ok() || !bws_ || n_seqs > max_batch_) { set_last_error("prefill_multi: tensor-core paths unavailable or more sequences than max_batch"); return CL_ERR_INVALID_ARG; }
   const int d = cfg.d_model, V = cfg.vocab_size;
   int total = 0, rc;
@@ -789,6 +895,11 @@ int cl_attn_prefill_long_plan(int32_t pos0, int32_t t, int32_t n_heads, int32_t 
   if (!nsplit_used || t <= 0 || pos0 < 0 || n_heads <= 0 || sms <= 0 || nsplit < 0) return CL_ERR_INVALID_ARG;
   *nsplit_used = attn_prefill_long_splits(pos0, t, n_heads, sms, nsplit);
   if (part_floats) *part_floats = (int64_t)attn_prefill_long_part_floats(sms);
+  return CL_OK;
+}
+int cl_gemm_split_plan(int32_t n, int32_t k, int32_t sms, int32_t deterministic, int32_t* k_splits) {
+  if (!k_splits || n <= 0 || k <= 0 || (!deterministic && sms <= 0)) return CL_ERR_INVALID_ARG;
+  *k_splits = pick_splits_sms(n, k, deterministic ? kDetSms : sms);
   return CL_OK;
 }
 

@@ -701,6 +701,7 @@ int Engine::step_running() {
     last_single_slot_ = B == 1 ? sched_slots_[0] : -1;
     if (B > 1) last_batch_slots_ = sched_slots_;
   }
+  h_slots_ = sched_slots_;
   const int64_t t0 = now_ns();
   int rc = run_step_graph(B);
   if (rc) return rc;

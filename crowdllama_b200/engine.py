@@ -40,7 +40,7 @@ class EngineConfig(C.Structure):
                 ("kv_pool_bytes", C.c_int64), ("page_size", C.c_int32), ("max_batch", C.c_int32),
                 ("max_seqs", C.c_int32), ("use_cuda_graph", C.c_int32), ("decode_path", C.c_int32),
                 ("start_scheduler", C.c_int32), ("prefix_cache", C.c_int32), ("speculate", C.c_int32),
-                ("reserved", C.c_int32 * 6)]   # reserved[0], [1], [2]: the C struct's context_shift, num_keep, context_length
+                ("reserved", C.c_int32 * 6)]   # reserved[0] .. [3]: the C struct's context_shift, num_keep, context_length, deterministic
 
 
 class Sampling(C.Structure):
@@ -111,7 +111,7 @@ EXPORTS = [
     "cl_debug_pass_rows", "cl_debug_timeline",
     "cl_op_gemv", "cl_op_gemv_residual", "cl_op_rmsnorm_gemv", "cl_op_rmsnorm_gateup", "cl_op_qkv_rope_append", "cl_op_attn_decode",
     "cl_op_attn_decode_batch", "cl_op_attn_verify", "cl_op_gemm_bf16", "cl_op_gemm_bf16_epi", "cl_op_attn_prefill", "cl_op_attn_prefill_variant",
-    "cl_op_attn_prefill_cached", "cl_op_attn_prefill_long", "cl_attn_prefill_long_plan", "cl_resolve_model_config", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
+    "cl_op_attn_prefill_cached", "cl_op_attn_prefill_long", "cl_attn_prefill_long_plan", "cl_gemm_split_plan", "cl_resolve_model_config", "cl_op_kv_host_roundtrip", "cl_op_sample", "cl_op_synth_weights", "cl_kvpool_create", "cl_kvpool_destroy",
     "cl_kvpool_reserve", "cl_kvpool_release", "cl_kvpool_pages_of", "cl_kvpool_free_pages", "cl_kvpool_used_pages",
     "cl_kvpool_attach", "cl_kvpool_publish", "cl_kvpool_cached_pages", "cl_kvpool_set_host_pages", "cl_kvpool_take_moves",
     "cl_kvpool_host_cached_pages", "cl_kvpool_shift", "cl_seq_shift", "cl_op_kv_shift", "cl_seq_set_logprobs", "cl_seq_take_logprobs", "cl_generate_ids_logprobs", "cl_op_sample_logprobs",
@@ -201,6 +201,7 @@ def lib():
         "cl_op_attn_prefill_long": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, P(f32),
                                               P(i32), P(i32)]),
         "cl_attn_prefill_long_plan": (C.c_int, [i32, i32, i32, i32, i32, P(i32), P(i64)]),
+        "cl_gemm_split_plan": (C.c_int, [i32, i32, i32, i32, P(i32)]),
         "cl_resolve_model_config": (C.c_int, [P(EngineConfig), P(ModelConfig)]),
         "cl_op_gemm_bf16": (C.c_int, [C.c_int, vp, vp, vp, i32, i32, i32, i32, P(f32)]),
         "cl_op_gemm_bf16_epi": (C.c_int, [C.c_int, C.c_int, i32, C.c_int, vp, vp, vp, vp, vp, i32, i32, i32, P(i32)]),
@@ -391,7 +392,7 @@ class Engine:
                  start_scheduler: bool = False, weights_path: str | None = None, prefix_cache: bool = False,
                  speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
                  num_keep: int = 4, context_length: int = 0, draft_preset: str | None = None, draft_model: dict | None = None,
-                 draft_weights_path: str | None = None, draft_seed: int | None = None):
+                 draft_weights_path: str | None = None, draft_seed: int | None = None, deterministic: bool = False):
         L = lib()
         cfg = EngineConfig()
         L.cl_default_engine_config(C.byref(cfg))
@@ -418,6 +419,7 @@ class Engine:
         cfg.reserved[0] = 1 if context_shift else 0     # cl_engine_config.context_shift; env CL_CONTEXT_SHIFT=0|1 overrides
         cfg.reserved[1] = num_keep                      # cl_engine_config.num_keep (Ollama's documented default 4); env CL_NUM_KEEP overrides
         cfg.reserved[2] = context_length                # cl_engine_config.context_length (0: the model's window); env CL_CONTEXT_LENGTH overrides
+        cfg.reserved[3] = 1 if deterministic else 0     # cl_engine_config.deterministic; env CL_DETERMINISTIC=0|1 overrides
         h = C.c_void_p()
         dcfg = draft_engine_config(draft_preset, draft_model, draft_weights_path, seed if draft_seed is None else draft_seed,
                                    self._keep)

@@ -86,11 +86,12 @@ def draft_kwargs(draft_model: str | None, draft_seed: int | None) -> dict:
 def serve(device: int, port: int, preset: str, model_name: str, max_batch: int = 8, greedy_tokens: int = 0, host="127.0.0.1",
           ready_event=None, seed: int = 1234, tokenizer: str | None = None, chat_family: str | None = None, prefix_cache: bool = False,
           speculate: int = 0, speculate_batch: int = 1, prefix_cache_host_bytes: int = 0, context_shift: bool = False,
-          num_keep: int = 4, context_length: int = 0, draft_model: str | None = None, draft_seed: int | None = None):
+          num_keep: int = 4, context_length: int = 0, draft_model: str | None = None, draft_seed: int | None = None,
+          deterministic: bool = False):
     e = eng.Engine(preset=preset, model_name=model_name, device=device, seed=seed, max_batch=max_batch, start_scheduler=True,
                    prefix_cache=prefix_cache, speculate=speculate, speculate_batch=speculate_batch,
                    prefix_cache_host_bytes=prefix_cache_host_bytes, context_shift=context_shift, num_keep=num_keep,
-                   context_length=context_length, **draft_kwargs(draft_model, draft_seed))
+                   context_length=context_length, deterministic=deterministic, **draft_kwargs(draft_model, draft_seed))
     if tokenizer:
         e.load_tokenizer(tokenizer, chat_family)      # HF tokenizer.json instead of the byte-level fallback
     sampling = eng.greedy(greedy_tokens, ignore_eos=True) if greedy_tokens > 0 else None   # None = Ollama defaults
@@ -138,6 +139,9 @@ def main():
                          "model verifies, in place of drafting from the request's own history (env CL_DRAFT_MODEL)")
     ap.add_argument("--draft-seed", type=int, default=None,
                     help="synthetic-weight seed of a preset --draft-model (default: the served model's seed)")
+    ap.add_argument("--deterministic", action="store_true",
+                    help="a request's output depends only on its prompt, settings and seed, not on what else the worker runs "
+                         "(Llama-3-8B / Mistral-7B shapes; env CL_DETERMINISTIC overrides)")
     a = ap.parse_args()
     if a.prefix_cache_host_gib and not a.prefix_cache:
         ap.error("--prefix-cache-host-gib requires --prefix-cache")
@@ -150,7 +154,7 @@ def main():
           prefix_cache=a.prefix_cache, speculate=a.speculate, speculate_batch=a.speculate_batch,
           prefix_cache_host_bytes=int(a.prefix_cache_host_gib * 2**30), context_shift=a.context_shift,
           num_keep=4 if a.num_keep is None else a.num_keep, context_length=a.context_length, draft_model=a.draft_model,
-          draft_seed=a.draft_seed)
+          draft_seed=a.draft_seed, deterministic=a.deterministic)
 
 
 if __name__ == "__main__":

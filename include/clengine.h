@@ -104,7 +104,7 @@ typedef struct cl_engine_config {
                               drafts the ids that followed the latest earlier occurrence of its last 3 (or 2) ids in its
                               prompt and output (cl_draft_ngram) and checks them in one pass over the weights
                               (cl_decode_verify).  The ids are the ones single steps would produce, up to near-tie flips
-                              between the two kernel paths.  Model shapes without the verify path decode normally.  With a
+                              between the two kernel paths (none in deterministic mode, where they are the same bits).  Model shapes without the verify path decode normally.  With a
                               draft model (cl_engine_create_with_draft, env CL_DRAFT_MODEL) the drafts come from it instead. */
   int32_t context_shift;   /* 1 => a request whose sequence fills max_seq_len shifts it (cl_seq_shift) and goes on generating
                               instead of ending with done_reason "length"; 0 => off (default; env CL_CONTEXT_SHIFT=0|1
@@ -145,7 +145,23 @@ typedef struct cl_engine_config {
                               Prefill segments that end past 32768 tokens run split-KV attention kernels for head_dim
                               128 / page 32 (up to 16 rows: the multi-row verify kernel); shorter segments run what they
                               always have. */
-  int32_t reserved[3];
+  int32_t deterministic;   /* 1 => deterministic mode (env CL_DETERMINISTIC=0|1 overrides; 0, the default, changes nothing).
+                              Every token path runs one row-invariant pass: each decode step is one-row segments of the
+                              split-K pass of verify passes, every prefill is passes of at most 128 rows cut into segments of
+                              at most 16 rows, all with the multi-row split-KV attention and the pass's wgmma LM head, and
+                              the split-K counts are those of a 132-SM card whatever the device has (cl_gemm_split_plan).
+                              With the switch on, a sequence's logits, K/V, ids and logprob records are the same bits
+                                - whatever other sequences share its steps and passes (batch size, neighbours' lengths);
+                                - however its prompt is split: one call, scheduler chunks, cl_prefill_batch groups, pages
+                                  of the prefix cache or its host tier, recompute after preemption;
+                                - whether its ids come from single steps or verify passes (n-gram or draft-model drafter);
+                                - on any sm_90 GPU, for the same model, weights, page size and context_length.
+                              The one exception is context_shift's: a shifted request that is preempted recomputes its
+                              window without the discarded context.  The persistent kernel, the GEMV path, the batched step
+                              and step graphs are not used.  cl_engine_create fails with CL_ERR_INVALID_ARG for shapes the
+                              pass does not take (head_dim 128, 4 query heads per kv head and page 32 only: Llama-3 /
+                              3.1-8B, Mistral-7B) and for max_batch > 128. */
+  int32_t reserved[2];
 } cl_engine_config;
 
 /* Sampler.  The reference sends no options (api.go:109-118), so Ollama defaults apply upstream:
@@ -553,7 +569,8 @@ int cl_seq_fake_fill(cl_engine* e, cl_seq_t seq, int32_t n_tokens);
 int cl_debug_kv(cl_engine* e, cl_seq_t seq, int32_t layer, int32_t which, int32_t t0, int32_t n, float* out);
 /* bench.py's roofline.dominant_kernel: n_steps greedy single-sequence steps launched eagerly with a CUDA-event pair
  * (on the launching stream) around the step's dominant kernel — decode_mega_kernel, or the per-layer kernel stack
- * on the per-op path.  kernel_ms / step_ms (may be NULL): mean per step. */
+ * on the per-op path.  kernel_ms / step_ms (may be NULL): mean per step.  CL_ERR_INVALID_ARG in deterministic mode,
+ * whose steps run neither. */
 int cl_time_dominant_kernel(cl_engine* e, cl_seq_t seq, int32_t first_id, int32_t n_steps, float* kernel_ms, float* step_ms);
 /* debugging / parity: copy the residual stream after `layer` (or the final norm input when
  * layer == n_layers) of the most recent single-sequence step to host (d_model floats). */
@@ -635,7 +652,9 @@ int cl_op_attn_decode_batch(int device, int variant, int32_t nsplit, int32_t tc_
  * scrambled pool.  out [sum(rows)][n_heads * head_dim] bf16.  nsplit 0: the engine's split plan (every split 8 pages),
  * else every segment spreads its pages over nsplit (1..64) splits; *nsplit_used (may be NULL) = the grid's splits.  The
  * kernel launches twice without re-arming its split counters and the call fails with CL_ERR_INTERNAL if the two outputs
- * differ in any bit.  Shapes: head_dim 128, 4 query heads per kv head, page 32; others return CL_ERR_INVALID_ARG. */
+ * differ in any bit.  Shapes: head_dim 128, 4 query heads per kv head, page 32; others return CL_ERR_INVALID_ARG.  Eight or
+ * more segments of one row each run the kernel's one-warp instantiation, as the engine's steps do; its rows are the
+ * 4-warp kernel's bits. */
 int cl_op_attn_verify(int device, const uint16_t* q, const uint16_t* k_cache, const uint16_t* v_cache, const int32_t* ctx_lens,
                       const int32_t* rows, int32_t n_segs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t page_size, int32_t nsplit,
                       uint16_t* out, int32_t* nsplit_used);
@@ -695,6 +714,10 @@ int cl_op_attn_prefill_long(int device, int variant, const uint16_t* q, const ui
  * plan's partials (tiles x n_heads x splits x 128 rows x (head_dim + 2)). */
 int cl_attn_prefill_long_plan(int32_t pos0, int32_t t, int32_t n_heads, int32_t sms, int32_t nsplit, int32_t* nsplit_used,
                               int64_t* part_floats);
+/* Host-only: the split-K count of the projections of the split-K pass and the batched step for an N x K weight on sms SMs
+ * (*k_splits), the count cl_op_gemm_bf16_epi's k_splits 0 picks on such a card.  deterministic 1: the count deterministic
+ * mode uses, the same for every sms (it is evaluated at 132 SMs, an H100 SXM's). */
+int cl_gemm_split_plan(int32_t n, int32_t k, int32_t sms, int32_t deterministic, int32_t* k_splits);
 /* the decode step's device sampler (the step tail kernel) on host logits [n_rows][vocab]: row r draws with sp[r] at RNG
  * step step[r], with history row r = history + r * hist_stride, n_history[r] ids (history may be NULL when every
  * n_history[r] is 0).  ids_out[n_rows].  CL_ERR_INVALID_ARG for settings the device sampler does not cover. */
